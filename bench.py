@@ -2,7 +2,7 @@
 """bench.py — the measurement contract of the csvplus_b200 hot path.
 
 Headline workload = BASELINE.json configs[3] (north_star's target), the reference README's own pattern
-(/root/reference/README.md:34-56, csvplus.go:545-583):
+(the reference's README.md:34-56, csvplus.go:545-583):
     customers (100 M rows, 6 cols) -> SelectColumns(id,name,surname)        -> UniqueIndexOn("id")
     products  (  1 M rows, 3 cols) -> SelectColumns(prod_id,product,price)  -> UniqueIndexOn("prod_id")
     orders (125 M rows PER GPU, 5 cols) -> SelectColumns(cust_id,prod_id,qty,ts).Join(custIdx,"cust_id").Join(prodIdx)
@@ -25,6 +25,10 @@ all-gathered (NCCL) and every rank builds the full index; products (25 MB) are p
 --impl reference: the reference (pure Go) cannot be built here (no Go toolchain), so the arm times the CPU oracle port
 of the same pipeline (oracle/, kind "port") on a bounded sample whose sizes are printed in its `config`, single-threaded
 because the reference is strictly single-threaded (csvplus.go has no goroutines).
+
+--dump-outputs DIR: after the timed steps, a fixed seeded sample of what the last timed step of each device-resident
+leg returned (the joined table, the filtered people table, the sorted index rows) is written as DIR/<name>.npy, so
+that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -61,7 +65,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -178,7 +182,7 @@ def workload_config(world, ref=None):
             "people_rows_per_gpu": PEOPLE_ROWS, "index_rows": INDEX_ROWS,
             "parallelism": f"probe row-range shards x{world}; customers parsed 1/{world} per rank and all-gathered (NCCL); "
                            "index built on every rank" if world > 1 else "single GPU",
-            "l2": "inputs (>= 25 MB products, otherwise >= 0.5 GB per pass) exceed or stream through the 126 MB L2; no flush needed"}
+            "l2": "inputs (>= 25 MB products, otherwise >= 0.5 GB per pass) exceed or stream through the 50 MB L2; no flush needed"}
 
 
 def run_reference(args, rank):
@@ -208,28 +212,6 @@ def run_reference(args, rank):
         "e2e": {"value": value, "unit": "rows/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     print(json.dumps(line), flush=True)
-
-
-def ncu_traffic(paths):
-    """mean dram__bytes_read.sum + dram__bytes_write.sum per csv_scan launch from the committed ncu metrics pass of this
-    bench command's join step; (None, None) if no file is present"""
-    import csv
-    for path in paths:
-        try:
-            per_id = {}
-            with open(path) as f:
-                rows = [r for r in csv.reader(f) if len(r) > 14]
-            hdr = rows[0]
-            ki, mi, ui, vi, ii = (hdr.index(x) for x in ("Kernel Name", "Metric Name", "Metric Unit", "Metric Value", "ID"))
-            for r in rows[1:]:
-                if "csv_scan" in r[ki] and r[mi] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[r[ui]]
-                    per_id[r[ii]] = per_id.get(r[ii], 0.0) + float(r[vi].replace(",", "")) * scale
-            if per_id:
-                return sum(per_id.values()) / len(per_id), os.path.relpath(path, ROOT)
-        except Exception:
-            continue
-    return None, None
 
 
 def bind_to_gpu_numa_node(local: int):
@@ -310,6 +292,8 @@ def main():
     ap.add_argument("--e2e-batches", type=int, default=24)
     ap.add_argument("--e2e-workers", type=int, default=8)
     ap.add_argument("--e2e-sweep", default="", help="e.g. 8x4,16x8: time these (batches x workers) settings of the e2e leg, report the best")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write a seeded sample of the last timed step's outputs as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     ORD_ROWS, CUST_ROWS, PROD_ROWS, PEOPLE_ROWS, INDEX_ROWS = args.orders, args.customers, args.products, args.people, args.index_rows
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
@@ -344,17 +328,15 @@ def main():
     d_orders = ctx.gen_csv("orders", (rank * ORD_ROWS, (rank + 1) * ORD_ROWS), seed=SEED, n_cust=CUST_ROWS, n_prod=PROD_ROWS, header=True)
     d_people = ctx.gen_csv("people", (rank * PEOPLE_ROWS, (rank + 1) * PEOPLE_ROWS), seed=SEED, header=True)
     ctx.sync()
-    # the step's tables, index structures and scratch (~35 GB at the default sizes, more with the gathered build side) come
-    # out of memory the pool maps once, here, instead of growing it over the first iterations (measured at N = 2 without
-    # it: steps of 200 ms until the sixth iteration, 56 ms after)
+    # the step's tables, index structures and scratch come out of memory the pool maps once, here, instead of growing
+    # it over the first iterations (growing it costs whole steps at N > 1)
     free_b, _total_b = torch.cuda.mem_get_info(local)
     reserve_b = int(min(0.45 * free_b, 56e9))
     reserved = ctx.reserve(reserve_b)
 
     # Python's cyclic collector: a full collection walks every object torch's import created (hundreds of ms) and its
-    # schedule depends only on allocation counts, so it hits every rank at the same step (measured at N = 2: steps of
-    # 55 ms with one of 150-780 ms every ~14 calls).  Everything alive now is long-lived: park it where collections
-    # do not look.
+    # schedule depends only on allocation counts, so it hits every rank at the same step.  Everything alive now is
+    # long-lived: park it where collections do not look.
     import gc
     gc.collect()
     gc.freeze()
@@ -404,7 +386,9 @@ def main():
     sync0 = [0, 0]
     per_step = []
 
-    def timed(fn, steps, warmup, sampler_dev=None):
+    dumped = {}  # name -> the last timed step's result (kept only with --dump-outputs)
+
+    def timed(fn, steps, warmup, sampler_dev=None, dump_as=None):
         sampler = ClockSampler(sampler_dev) if sampler_dev is not None and not os.environ.get("BENCH_NO_SAMPLER") else None  # polls through warm-up + timed steps
         for _ in range(warmup):
             r = fn(); del r
@@ -420,8 +404,11 @@ def main():
         e0.record(stream)
         rows = 0
         marks = []
-        for _ in range(steps):
-            r = fn(); rows = len(r); del r
+        for i in range(steps):
+            r = fn(); rows = len(r)
+            if dump_as and args.dump_outputs and i == steps - 1:
+                dumped[dump_as] = r
+            del r
             ev = torch.cuda.Event(enable_timing=True); ev.record(stream); marks.append(ev)
         e1.record(stream)
         sync0[1] = ctx.host_syncs() - sync0[0]
@@ -442,15 +429,21 @@ def main():
         return ms / steps, rows, stats, ctx.kernel_launches() - l0, clocks
 
     # ---------------- device-resident timing (value)
-    ms_join, out_rows, st_join, launches, clocks = timed(lambda: join_step(d_cust, d_prod, d_orders), args.steps, args.warmup, local)
+    ms_join, out_rows, st_join, launches, clocks = timed(lambda: join_step(d_cust, d_prod, d_orders), args.steps, args.warmup, local,
+                                                         dump_as="join")
     join_syncs = sync0[1] / args.steps
     join_per_step = list(per_step)
     assert out_rows == ORD_ROWS, (out_rows, ORD_ROWS)  # every order matches exactly one customer and one product
-    ms_parse, parse_rows, st_parse, _, _ = timed(lambda: parse_step(d_people), args.steps, args.warmup)
+    if rank == 0 and "join" in dumped:
+        dump_table(args.dump_outputs, "join", dumped.pop("join"))
+    dumped.clear()
+    ms_parse, parse_rows, st_parse, _, _ = timed(lambda: parse_step(d_people), args.steps, args.warmup, dump_as="csv_parse")
+    if rank == 0 and "csv_parse" in dumped:
+        dump_table(args.dump_outputs, "csv_parse", dumped.pop("csv_parse"))
+    dumped.clear()
     peak, peak_kind = hbm_peak()
-    traffic, traffic_src = ncu_traffic([os.path.join(ROOT, "profiles", f) for f in ("r2_traffic_csv_scan.csv", "r1_traffic_csv_scan.csv")])
 
-    def roof(st, traffic=None):
+    def roof(st):
         s = st.get("csv_scan")
         if not s or not s["launches"]:
             return None
@@ -458,7 +451,6 @@ def main():
         per_launch_ms = s["ms"] / s["launches"]
         ach = per_launch_bytes / (per_launch_ms * 1e-3) / 1e9
         return {"bound": "hbm", "kernel": "csv_scan", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": traffic, "traffic_unit": "bytes/launch (ncu dram read+write, %s)" % traffic_src if traffic else None,
                 "peak_kind": f"of {peak_kind}", "launches": s["launches"], "ms_per_launch": per_launch_ms,
                 "algo_bytes_per_launch": per_launch_bytes}
 
@@ -496,7 +488,10 @@ def main():
             ix.table()
             return ix
 
-        ms_ix, ix_rows, st_ix, _, _ = timed(lambda: index_step(t_ix), args.steps, args.warmup)
+        ms_ix, ix_rows, st_ix, _, _ = timed(lambda: index_step(t_ix), args.steps, args.warmup, dump_as="index_on")
+        if rank == 0 and "index_on" in dumped:
+            dump_table(args.dump_outputs, "index_on", dumped.pop("index_on").table())
+        dumped.clear()
 
         def resolve_path(tab):
             w0 = time.perf_counter()
@@ -772,7 +767,7 @@ def main():
             "kernel_ms_per_step": kernel_ms / args.steps, "host_gap_ms_per_step": ms_join - kernel_ms / args.steps,
             "host_syncs_per_step": join_syncs, "per_step_ms_rank0": join_per_step,
             "e2e": e2e,
-            "roofline": roof(st_join, traffic if world == 1 else None),
+            "roofline": roof(st_join),
             "csv_parse": {"metric": "CSV parse GB/s (configs[1]: parse+SelectColumns(name,surname,id)+Filter(Like name=Amelia))",
                           "value": world * d_people.nbytes / (ms_parse * 1e-3) / 1e9, "unit": "GB/s", "ms_per_step": ms_parse,
                           "rows_per_s": world * PEOPLE_ROWS / (ms_parse * 1e-3), "rows_out_per_gpu": parse_rows,
@@ -784,6 +779,38 @@ def main():
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_BLOCKS, DUMP_BLOCK_ROWS = 16, 256  # sample: 16 seeded blocks of 256 consecutive rows per table
+
+
+def dump_table(out_dir, name, table):
+    """Writes a fixed, seeded sample of `table` as float arrays: <name>_rows (the sampled row numbers, float64),
+    <name>_num_rows, and per column <name>.<col>_len (value lengths, float64) and <name>.<col>_bytes (the value bytes,
+    float32 [rows, longest sampled value], zero padded).  The sample depends only on the row count."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(table)
+    nblk = min(DUMP_BLOCKS, max(1, n // DUMP_BLOCK_ROWS))
+    rng = np.random.default_rng(SEED)
+    starts = np.sort(rng.choice(max(1, n - DUMP_BLOCK_ROWS + 1), size=nblk, replace=False)) if n > DUMP_BLOCK_ROWS else np.zeros(1, np.int64)
+    blocks = [(int(a), int(min(n, a + DUMP_BLOCK_ROWS))) for a in starts]
+    rows = np.concatenate([np.arange(a, b) for a, b in blocks]) if n else np.zeros(0, np.int64)
+    np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, f"{name}_num_rows.npy"), np.array([n], np.float64))
+    for c in table.columns:
+        lens, vals = [], []
+        for a, b in blocks:
+            off, data = table.column(c, a, b) if n else (np.zeros(1, np.int64), np.zeros(0, np.uint8))
+            off = off - off[0]
+            lens.append(np.diff(off))
+            vals += [data[off[i]:off[i + 1]] for i in range(len(off) - 1)]
+        ln = np.concatenate(lens).astype(np.int64)
+        mat = np.zeros((len(vals), int(ln.max()) if len(ln) else 0), np.float32)
+        for i, v in enumerate(vals):
+            mat[i, :len(v)] = v
+        np.save(os.path.join(out_dir, f"{name}.{c}_len.npy"), ln.astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}.{c}_bytes.npy"), mat)
 
 
 class C_u64:

@@ -1,6 +1,6 @@
-"""csvplus_b200 — B200-native columnar CSV ETL hot path with the csvplus API names.
+"""csvplus_b200 — H100-native columnar CSV ETL hot path with the csvplus API names.
 
-Product path = csvplus_b200/libcsvplus_b200.so (hand-written sm_100a CUDA kernels behind the C ABI
+Product path = csvplus_b200/libcsvplus_b200.so (hand-written sm_90a CUDA kernels behind the C ABI
 of include/csvplus_b200.h).  This package is the thin host mirror of the reference's Go API
 (csvplus.go) over that ABI; it never computes results on the CPU and fails loudly when the CUDA
 library or a GPU is missing.

@@ -1,8 +1,8 @@
-"""Builds csvplus_b200/libcsvplus_b200.so (sm_100a only) in-tree with nvcc.
+"""Builds csvplus_b200/libcsvplus_b200.so (sm_90a only, i.e. H100) in-tree with nvcc.
 
     python -m csvplus_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the objects under _obj/ are build products and git-ignored.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ LIB = os.path.join(HERE, "libcsvplus_b200.so")
 SOURCES = ["abi.cu", "parse.cu", "parse_general.cu", "gather.cu", "sort.cu", "join.cu", "write.cu", "gen.cu", "comm.cu", "subst.cu"]
 HEADERS = ["core.hpp", "util.cuh", "pred.cuh", "parse_kernels.cuh", "subst.hpp", os.path.join("..", "..", "include", "csvplus_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--extended-lambda"]
 
 

@@ -159,13 +159,15 @@ int cpb_init(int device, cpb_ctx** out) {
         CPB_CUDA(cudaSetDevice(device));
         // CPB_BLOCKING_SYNC=1: host waits sleep on an interrupt instead of spinning.  One process per GPU on a shared host:
         // N spinning ranks (+ NCCL's proxy threads) can run a cgroup into its CPU quota, and a throttled rank stalls all
-        // the others at the next collective (measured: steps of 55 ms with sporadic 150-750 ms ones at N = 2).
+        // the others at the next collective.
         if (const char* bs = getenv("CPB_BLOCKING_SYNC")) {
             if (bs[0] == '1') { cudaSetDeviceFlags(cudaDeviceScheduleBlockingSync); cudaGetLastError(); }
         }
         cudaDeviceProp prop;
         CPB_CUDA(cudaGetDeviceProperties(&prop, device));
-        if (prop.major < 10) throw ArgError{CPB_ERR_UNSUPPORTED, "csvplus_b200 kernels are built for sm_100a only"};
+        // sm_90a code runs on compute capability 9.0 only (the "a" features do not carry forward)
+        if (prop.major != 9 || prop.minor != 0)
+            throw ArgError{CPB_ERR_UNSUPPORTED, "csvplus_b200 kernels are built for sm_90a (H100) only"};
         c->sm_count = prop.multiProcessorCount;
         c->smem_optin = prop.sharedMemPerBlockOptin;
         CPB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));

@@ -2,7 +2,7 @@
 // that every rank can build the full Index (csvplus.go:707-767) and join its own probe shard against it, plus the
 // tiny metadata all-gather that byte-range shards of one file need (quote parity, record counts).
 //
-// NCCL (NVLink 5 / NVSwitch) is the transport.  The library is bound at run time (dlopen of libnccl.so.2 — the very
+// NCCL (NVLink / NVSwitch) is the transport.  The library is bound at run time (dlopen of libnccl.so.2 — the very
 // instance torch already mapped when the host is Python) so that single-GPU users need no NCCL at all.
 //
 // all-gather-v of a table, per column:
@@ -174,7 +174,7 @@ void job_data_collective(GatherJob& j) {  // inside ncclGroupStart/End
         col.offsets = dev_alloc(c, (row_base[R] + 1) * 4);
         col.data = dev_alloc(c, bb[R] + 16);
         // all-gather-v as grouped point-to-point transfers: my segment goes straight to its place in every peer's final
-        // buffers over NVLink (a grouped set of ncclBroadcast — one ring per root — measured 25 GB/s at N = 2), my own
+        // buffers over NVLink (a grouped set of ncclBroadcast — one ring per root — was much slower), my own
         // copy is a device-to-device memcpy
         const int me = c->rank;
         const uint64_t my_first = j.meta[(size_t)me * M + 1 + 2 * k];

@@ -161,7 +161,7 @@ struct Ctx {
     bool own_pool = false;
     std::mutex mu;              // one call in flight per ctx
     std::string last_error;
-    int sm_count = 148;
+    int sm_count = 132;
     size_t smem_optin = 0;
     // stats
     bool stats_on = false;

@@ -238,8 +238,8 @@ Column materialize(Ctx* c, const Column& col, int64_t nrows) { return gather_col
 
 // ------------------------------------------------------------------ row slots: one random access per gathered index row
 // A join reads index rows in probe order, i.e. at random: per output column that is one access to the offsets and
-// one to the bytes, each a 64-byte DRAM granule once the index outgrows L2 (measured: 9 GB of DRAM reads to gather
-// 0.7 GB).  Short rows are therefore re-laid once per index as fixed-size slots (all output columns back to back) +
+// one to the bytes, each a 64-byte DRAM granule once the index outgrows L2 (many times the
+// DRAM traffic of the bytes gathered).  Short rows are therefore re-laid once per index as fixed-size slots (all output columns back to back) +
 // one packed word of lengths; a gather then costs one L2-friendly 4-byte read (lengths -> offsets of all columns in
 // one scan) and one slot read (bytes of all columns in one pass).
 constexpr int RS_MAXC = 4;       // columns per slot set (lengths are 8 bits each in one word)
@@ -418,7 +418,7 @@ __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t*
                 uint8_t* q = stage + sh + (d - d0);
                 for (uint32_t k = 0; k < len; k++) q[k] = sp[k];
                 __syncwarp();
-                uint8_t* gb = dst + (d0 - sh);  // (warp_store_stage measured slower here: 4.25 vs 3.94 ms per 100 M rows)
+                uint8_t* gb = dst + (d0 - sh);  // (warp_store_stage was slower here)
                 for (uint32_t x = lane * 16; x < sh + total; x += 32 * 16) {
                     if (x >= sh && x + 16 <= sh + total) *reinterpret_cast<uint4*>(gb + x) = *reinterpret_cast<const uint4*>(stage + x);
                     else for (uint32_t y = x; y < x + 16; y++) if (y >= sh && y < sh + total) gb[y] = stage[y];

@@ -15,7 +15,7 @@
 //   g_rec_count    one thread per record: the exact sequential machine (options aware; seq_parse_record_gen lives in
 //                  parse_kernels.cuh, the scan's guarded instantiations use it too) -> lengths, Like terms, errors
 //   g_rec_emit     offsets + unescaped field bytes
-// Exact sizes are known before anything is written (multi-pass: this path trades bandwidth for generality: ≈ 44 GB/s).
+// Exact sizes are known before anything is written (multi-pass: this path trades bandwidth for generality).
 // Delimiter / comment are single bytes here: multi-byte runes and the multi-byte Unicode spaces arrive as stand-in bytes.
 #include <algorithm>
 

@@ -20,26 +20,18 @@
 #include "subst.hpp"
 #include "util.cuh"
 
-// Variants measured on B200 and removed (tools/time_parse.py, 20 M rows): drawing the next tile's ticket early lengthens the
-// look-back distance (656 vs 720 GB/s); word-wise staging copies lose to the byte loop on short fields (510 vs 528 GB/s).
-// Also measured and rejected (40 M rows; filter / orders / all-columns GB/s, baseline 738 / 555 / 371):
-//   * one stage for all columns, owners copy their rows, direct offset stores (2 barriers per tile instead of 4 per
-//     column): 691 / 583 / 377 -- the barriers are not the cost, the byte loop is;
-//   * folding the parity verification and the any-slow vote into the block scan's barrier: 548 / 420 / 292;
-//   * 16 KiB tiles with 128-thread CTAs (-DCPB_TILE=16384 -DCPB_THREADS=128, 6 CTAs/SM): 650 / 551 / 393 against
-//     714 / 582 / 406 for the 32 KiB / 256-thread default in the same run -- the per-tile fixed costs win.
-// Round 2, measured and rejected (40 M rows; filter / orders / all-columns GB/s of input; this kernel: 712 / 582 / 408):
-//   * line-end list + per-line walk of the structural bitmap instead of the flat index (no sidx expansion):
-//     682 / 576 / 391 — the same 895 M warp-instructions per 20 M order rows: the per-line ffs walk costs what the
-//     expansion + O(1) look-ups cost, with longer dependent chains;
-//   * a separate "lean" path for quote-free regular tiles (thread owns the lines starting in its 128-byte slice, 16-bit
-//     packed scans, per-warp output staging, no row lists): parity-green but 501 / 484 / 347 — slice ownership gives
-//     threads 2 or 3 lines (19 of 32 lanes active), and fully unrolled it was 19 K instructions (instruction-cache
-//     misses), rolled it still executed more warp-instructions (755 M vs 632 M on the filter shape) than this kernel;
-//   * the tile body as a __noinline__ function: 421 / 400 / 255 — shared memory and kernel parameters are then reached
-//     through generic pointers.
-// The profile of this kernel is flat (top line 13 % of the instructions); what would move it is fewer bytes through
-// the LSU per input byte, not a different control structure.
+// Variants tried and removed because they were slower (timings taken on an earlier GPU target; not re-measured on H100):
+//   * drawing the next tile's ticket early (it lengthens the look-back distance);
+//   * word-wise staging copies instead of the byte loop (short fields);
+//   * one stage for all columns with direct offset stores -- the barriers are not the cost, the byte loop is;
+//   * folding the parity verification and the any-slow vote into the block scan's barrier;
+//   * 16 KiB tiles with 128-thread CTAs (-DCPB_TILE=16384 -DCPB_THREADS=128) -- the per-tile fixed costs win;
+//   * a line-end list + per-line walk of the structural bitmap instead of the flat index: the per-line ffs walk costs
+//     what the expansion + O(1) look-ups cost, with longer dependent chains;
+//   * a separate "lean" path for quote-free regular tiles (thread owns the lines starting in its 128-byte slice): slice
+//     ownership leaves most lanes idle and the unrolled body overflows the instruction cache;
+//   * the tile body as a __noinline__ function: shared memory and kernel parameters are then reached through generic
+//     pointers.
 namespace cpb {
 
 #ifndef CPB_TILE
@@ -591,7 +583,7 @@ __device__ __forceinline__ bool flat_line(const ParseParams& P, const ParseSmem&
                         if (len == P.pred.term_len[t]) {
                             const bool eq = lits_in_smem ? field_eq_smem(sm.data, PRE + fb, sm.lits, P.pred.term_off[t], len)
                                                          : bytes_eq(sm.data + PRE + fb, lits + P.pred.term_off[t], len);
-                            if (eq) r.eq |= 1u << t;  // (inline: an out-of-line compare measured 708 vs 729 GB/s)
+                            if (eq) r.eq |= 1u << t;  // (inline: an out-of-line compare was slower)
                         }
                     }
                 }
@@ -1071,7 +1063,7 @@ __global__ void __launch_bounds__(THREADS, KMAX <= 8 ? 768 / THREADS : 1) csv_sc
                 const uint64_t row_base = sm.tile_prefix[1];
                 const uint32_t osh = (uint32_t)(row_base & 3);
                 if (nrow != 0 && row == 0) P.result->first_row_ordinal = rec0 + first_surv_rec;
-                // (a run-time column loop -- one copy of the staging code instead of KMAX -- measured slower: 679 vs 736 GB/s)
+                // (a run-time column loop -- one copy of the staging code instead of KMAX -- was slower)
 #pragma unroll
                 for (int k = 0; k < KMAX; k++) {
                     if (k < (EXACT ? KMAX : P.nsel)) {

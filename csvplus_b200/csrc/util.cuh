@@ -1,4 +1,4 @@
-// util.cuh — device-side helpers (sm_100a): mbarrier + bulk-async (TMA 1-D) staging, gpu-scope
+// util.cuh — device-side helpers (sm_90a): mbarrier + bulk-async (TMA 1-D) staging, gpu-scope
 // acquire/release for the decoupled look-back chains, warp scans.
 #pragma once
 #include <cuda_runtime.h>

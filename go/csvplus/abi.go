@@ -1,4 +1,4 @@
-// Package csvplus — cgo binding of the B200 hot path behind the csvplus API names (maxim2266/csvplus).
+// Package csvplus — cgo binding of the H100 hot path behind the csvplus API names (maxim2266/csvplus).
 //
 // SOURCE ONLY: this image has no Go toolchain, so these files have never been compiled.  They are the Go layer
 // INTEGRATION.md describes: the public names, signatures, panics and error texts of the reference, lowered to the C ABI
@@ -48,8 +48,8 @@ var (
 	defaultOnce sync.Once
 )
 
-// NewContext creates a context on the given CUDA device.  There is no CPU fallback: without a usable sm_100a
-// device this fails.
+// NewContext creates a context on the given CUDA device.  There is no CPU fallback: without a usable sm_90a
+// (H100) device this fails.
 func NewContext(device int) (*Context, error) {
 	var h *C.cpb_ctx
 	if st := C.cpb_init(C.int(device), &h); st != C.CPB_OK {

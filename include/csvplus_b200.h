@@ -1,4 +1,4 @@
-/* csvplus_b200.h — C ABI of the B200-native csvplus hot path.
+/* csvplus_b200.h — C ABI of the H100-native (sm_90a) csvplus hot path.
  *
  * The reference (maxim2266/csvplus, pure Go, single file csvplus.go) has no FFI seam;
  * its only boundary is the Go API (SURVEY.md §8b).  These entry points are exactly what a

@@ -14,7 +14,7 @@
 //
 // Every function cites the reference lines it restates (csvplus.go = the single
 // source file of the reference; "encoding/csv" = Go 1.23 stdlib, go.mod:3, which
-// is not vendored under /root/reference — its published algorithm is restated).
+// is not vendored with the reference — its published algorithm is restated).
 //
 // Data model mirrors the reference: Row = hash map string->string
 // (csvplus.go:59), a DataSource result = vector of Rows + optional error

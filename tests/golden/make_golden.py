@@ -4,7 +4,7 @@
 
 The reference itself (Go) cannot run in this image, so these files pin the ORACLE's behaviour (and through the parity
 tests the CUDA path's) on fixed inputs: any later change of either side that alters an output shows up as a diff of a
-committed file.  Inputs are committed next to the expected outputs; nothing here reads /root/reference."""
+committed file.  Inputs are committed next to the expected outputs; nothing here reads the reference's sources."""
 import json
 import os
 import random

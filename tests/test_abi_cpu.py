@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports every
+"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports every
 symbol include/csvplus_b200.h declares; without a GPU every compute entry fails loudly (no CPU fallback)."""
 import ctypes as C
 import os

@@ -1,31 +1,11 @@
-"""Host-side helpers of bench.py that must not depend on a GPU: the ncu traffic reader behind roofline.traffic, the
-NUMA binding (best effort, never raises) and the clock-sample filter."""
+"""Host-side helpers of bench.py that must not depend on a GPU: the NUMA binding (best effort, never raises), the
+workload description, the duplicate resolver and the output dump."""
 import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
-
-
-def test_ncu_traffic_reads_committed_profile():
-    t, src = bench.ncu_traffic([os.path.join(ROOT, "profiles", "does_not_exist.csv"), os.path.join(ROOT, "profiles", "r1_traffic_csv_scan.csv")])
-    # mean of the customers (0.69 GB) and orders (10.87 GB) csv_scan launches of one round-1 join step
-    assert t is not None and 5.5e9 < t < 6.1e9 and src.endswith("r1_traffic_csv_scan.csv")
-    assert bench.ncu_traffic([os.path.join(ROOT, "profiles", "does_not_exist.csv")]) == (None, None)
-
-
-def test_ncu_traffic_units_and_kernel_filter(tmp_path):
-    p = tmp_path / "t.csv"
-    hdr = '"ID","Process ID","Process Name","Host Name","Kernel Name","Context","Stream","Block Size","Grid Size","Device","CC","Section Name","Metric Name","Metric Unit","Metric Value"\n'
-    row = '"{i}","1","p","h","{k}","1","7","(256, 1, 1)","(444, 1, 1)","0","10.0","s","{m}","{u}","{v}"\n'
-    p.write_text("==PROF== noise\n" + hdr
-                 + row.format(i=0, k="void csv_scan_kernel<4, 1, 0>(ParseParams)", m="dram__bytes_read.sum", u="Gbyte", v="1.5")
-                 + row.format(i=0, k="void csv_scan_kernel<4, 1, 0>(ParseParams)", m="dram__bytes_write.sum", u="Mbyte", v="500")
-                 + row.format(i=0, k="void csv_scan_kernel<4, 1, 0>(ParseParams)", m="gpu__time_duration.sum", u="ns", v="9000")
-                 + row.format(i=1, k="other_kernel()", m="dram__bytes_read.sum", u="byte", v="7")
-                 + row.format(i=2, k="void csv_scan_kernel<3, 1, 0>(ParseParams)", m="dram__bytes_read.sum", u="byte", v="1000000000"))
-    assert bench.ncu_traffic([str(p)])[0] == (2.0e9 + 1.0e9) / 2
 
 
 def test_numa_binding_is_best_effort():
@@ -59,3 +39,35 @@ def test_min_id_resolver_keeps_bytewise_smallest():
     # bytewise: "10" < "100" < "9" ; "2" < "20" < "21"
     assert keep.tolist() == [1, 6]
     assert bench.index_sides(10_000_000) == 3794
+
+
+def test_dump_table_writes_a_fixed_float_sample(tmp_path):
+    import numpy as np
+
+    class FakeTable:
+        columns = ["k", "v"]
+
+        def __init__(self, n):
+            self.vals = {"k": [b"%d" % i for i in range(n)], "v": [b"x" * (i % 5) for i in range(n)]}
+
+        def __len__(self):
+            return len(self.vals["k"])
+
+        def column(self, name, lo, hi):
+            vals = self.vals[name][lo:hi]
+            off = np.zeros(len(vals) + 1, np.int64); off[1:] = np.cumsum([len(v) for v in vals])
+            return off, np.frombuffer(b"".join(vals), np.uint8)
+    for run in ("a", "b"):
+        bench.dump_table(str(tmp_path / run), "t", FakeTable(10_000))
+    files = sorted(p.name for p in (tmp_path / "a").iterdir())
+    assert files == ["t.k_bytes.npy", "t.k_len.npy", "t.v_bytes.npy", "t.v_len.npy", "t_num_rows.npy", "t_rows.npy"]
+    for f in files:
+        x, y = np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f)
+        assert x.dtype in (np.float32, np.float64) and np.array_equal(x, y)
+    rows = np.load(tmp_path / "a" / "t_rows.npy").astype(np.int64)
+    assert len(rows) == bench.DUMP_BLOCKS * bench.DUMP_BLOCK_ROWS and rows.max() < 10_000
+    k = np.load(tmp_path / "a" / "t.k_bytes.npy"); kl = np.load(tmp_path / "a" / "t.k_len.npy").astype(np.int64)
+    for i in (0, 777, len(rows) - 1):
+        assert bytes(k[i, :kl[i]].astype(np.uint8)) == b"%d" % rows[i]
+    bench.dump_table(str(tmp_path / "small"), "t", FakeTable(3))
+    assert np.load(tmp_path / "small" / "t_rows.npy").tolist() == [0, 1, 2]

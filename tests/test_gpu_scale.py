@@ -170,7 +170,7 @@ def test_composite_index_and_resolve_duplicates_vs_oracle(n_rows):
 def test_two_rank_allgathered_three_way_join():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     env = dict(os.environ, PYTHONPATH=ROOT)
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
                         "--master-port", "29617", os.path.join(ROOT, "tests", "dist_gpu_worker.py")], env=env, capture_output=True, text=True,

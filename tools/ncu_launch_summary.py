@@ -1,5 +1,5 @@
 """Summarise an ncu launch list (--metrics gpu__time_duration.sum --csv) per kernel:
-python tools/ncu_launch_summary.py launches.csv "<command line that was profiled>" > profiles/rN_launches_summary.csv"""
+python tools/ncu_launch_summary.py launches.csv "<command line that was profiled>" > launches_summary.csv"""
 import csv, re, sys, collections
 rows = [r for r in csv.reader(open(sys.argv[1])) if len(r) > 14]
 hdr = rows[0]

@@ -1,4 +1,4 @@
-"""Markdown summary of bench.py JSON lines: python tools/summarize_bench.py profiles/r2_bench_n1.json [more.json ...]"""
+"""Markdown summary of bench.py JSON lines: python tools/summarize_bench.py bench_n1.json [more.json ...]"""
 import json
 import sys
 
