@@ -249,7 +249,7 @@ struct SlotOut { uint32_t* off[RS_MAXC]; uint8_t* data[RS_MAXC]; };
 
 // (`perm`: slot r holds source row perm[r] — the slots are laid out in sorted order straight from the unsorted rows
 // of the index source; null = identity)
-__global__ void slot_lens_kernel(SlotCols sc, const uint32_t* __restrict__ perm, uint64_t n, uint32_t* lens, uint32_t* stat) {  // stat: [0] max row bytes, [1] a value > 255 bytes
+__global__ void __launch_bounds__(256) slot_lens_kernel(SlotCols sc, const uint32_t* __restrict__ perm, uint64_t n, uint32_t* lens, uint32_t* stat) {  // stat: [0] max row bytes, [1] a value > 255 bytes
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t tot = 0, packed = 0, bad = 0;
     if (r < n) {
@@ -262,9 +262,18 @@ __global__ void slot_lens_kernel(SlotCols sc, const uint32_t* __restrict__ perm,
         }
         lens[r] = packed;
     }
+    // one global atomic per block (every block hits the same word: same-address atomics serialise in L2)
+    __shared__ uint32_t s_max[8], s_bad[8];
     tot = __reduce_max_sync(0xffffffffu, tot);
     bad = __any_sync(0xffffffffu, bad);
-    if ((threadIdx.x & 31) == 0) { atomicMax(&stat[0], tot); if (bad) stat[1] = 1u; }
+    if ((threadIdx.x & 31) == 0) { s_max[threadIdx.x >> 5] = tot; s_bad[threadIdx.x >> 5] = bad; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const bool in = threadIdx.x < (blockDim.x >> 5);
+        tot = __reduce_max_sync(0xffffffffu, in ? s_max[threadIdx.x] : 0u);
+        bad = __any_sync(0xffffffffu, in && s_bad[threadIdx.x]);
+        if (threadIdx.x == 0) { atomicMax(&stat[0], tot); if (bad) stat[1] = 1u; }
+    }
 }
 // one block lays out 256 consecutive slots in shared memory (row stride padded to an odd number of words: no bank
 // conflicts) and writes them with coalesced 16-byte stores
@@ -380,57 +389,131 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const uint32_t*
     }
 }
 
+// Stores bytes [lo, hi) (lo < hi <= 16) of the vector v to gb (16-byte aligned) with naturally aligned 8/4/2/1-byte
+// stores (at most 6): the partial first / last vector of a warp's destination range, whose other bytes belong to the
+// neighbouring groups.
+__device__ __forceinline__ void store_part16(uint8_t* gb, uint4 v, uint32_t lo, uint32_t hi) {
+    const unsigned long long h0 = ((unsigned long long)v.y << 32) | v.x, h1 = ((unsigned long long)v.w << 32) | v.z;
+    for (uint32_t x = lo; x < hi;) {
+        const unsigned long long w = (x < 8 ? h0 : h1) >> (8 * (x & 7));
+        if ((x & 7) == 0 && x + 8 <= hi) { *reinterpret_cast<unsigned long long*>(gb + x) = w; x += 8; }
+        else if ((x & 3) == 0 && x + 4 <= hi) { *reinterpret_cast<uint32_t*>(gb + x) = (uint32_t)w; x += 4; }
+        else if ((x & 1) == 0 && x + 2 <= hi) { *reinterpret_cast<uint16_t*>(gb + x) = (uint16_t)w; x += 2; }
+        else { gb[x] = (uint8_t)w; x += 1; }
+    }
+}
+// ORs the len bytes at slot[pos..] into the zeroed stage at byte q, one aligned 4-byte word at a time: each word is
+// two slot words funnel-shifted into place and masked to the value's bytes.  A word the value shares with its
+// neighbours' values is completed by their ORs.  Reads the slot word before and after the value (never used).
+__device__ __forceinline__ void or_value(uint8_t* stage, uint32_t q, const uint8_t* slot, uint32_t pos, uint32_t len) {
+    if (len == 0) return;
+    const uint32_t b = q & 3u, e = (pos & 3u) + 4u - b;  // target word j = slot bytes from (pos & ~3) + 4j + e - 4
+    const uint32_t* sw = reinterpret_cast<const uint32_t*>(slot + (pos & ~3u)) + (e >> 2) - 1;
+    uint32_t* tw = reinterpret_cast<uint32_t*>(stage + (q & ~3u));
+    const uint32_t shift = 8 * (e & 3u), nw = (b + len + 3) >> 2, endb = b + len - 4 * (nw - 1);  // endb in 1..4
+    uint32_t cur = sw[0];
+    for (uint32_t j = 0; j < nw; j++) {
+        const uint32_t nxt = sw[j + 1];
+        uint32_t m = j == 0 ? 0xffffffffu << (8 * b) : 0xffffffffu;
+        if (j == nw - 1 && endb < 4) m &= (1u << (8 * endb)) - 1u;
+        atomicOr(tw + j, __funnelshift_r(cur, nxt, shift) & m);
+        cur = nxt;
+    }
+}
 // One warp gathers 32 consecutive output rows: every lane pulls its row's slot into shared memory with 16-byte
-// loads (the one random access), then, column by column, the warp lays the values out like the destination in the
-// staging buffer and writes it with aligned 16-byte stores (as gather_copy_kernel does).
-template <int NC>
+// loads (the one random access).  The lanes then OR their values, word by word, into a zeroed staging buffer laid
+// out like the destination (all columns of the group, one 16-byte aligned region each), and the warp writes every
+// column's region in ONE pass of aligned 16-byte stores, the partial first / last vector of a column with a few
+// aligned narrower stores.  No lane loops over the bytes of a value.  A column whose region does not fit the stage
+// any more is copied straight to its destination.
+constexpr uint32_t SC_STRIDE_PAD = 12;  // slot stride S + 12 bytes: an odd number of words, and room for or_value's over-read
+template <int NC, int SV>  // SV: 16-byte vectors held per prefetched slot (S <= 16 SV)
 __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
                                                                   SlotOut out, uint64_t n) {
-    __shared__ __align__(16) uint8_t slot_sm[GW_WARPS][32 * (RS_MAXS + RS_PAD)];
-    __shared__ __align__(16) uint8_t stage_all[GW_WARPS][GW_STAGE + 16];
+    // (16 bytes ahead of the first slot: or_value may read the word before a value)
+    __shared__ __align__(16) uint8_t slot_sm[16 + GW_WARPS * 32 * (RS_MAXS + SC_STRIDE_PAD)];
+    __shared__ __align__(16) uint8_t stage_all[GW_WARPS][GW_STAGE];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint8_t* stage = stage_all[warp];
-    uint8_t* myslot = slot_sm[warp] + lane * (S + RS_PAD);  // odd word stride: conflict-free byte reads
+    uint8_t* myslot = slot_sm + 16 + (warp * 32 + lane) * (S + SC_STRIDE_PAD);
     const uint64_t nwarps = (uint64_t)gridDim.x * GW_WARPS;
-    for (uint64_t g = (uint64_t)blockIdx.x * GW_WARPS + warp; g * 32 < n; g += nwarps) {
+    // the slot and the destination offsets of a lane's row are fetched one round ahead, so that the random slot read
+    // of the next group is in flight while this group is laid out and stored
+    uint4 v[SV];
+    uint32_t nd[NC], nlen[NC];
+    auto fetch = [&](uint64_t g) {
+        const uint64_t i = g * 32 + lane;
+#pragma unroll
+        for (int c = 0; c < NC; c++) { nd[c] = 0; nlen[c] = 0; }
+        if (i < n) {
+            const uint4* sp = reinterpret_cast<const uint4*>(slots + (uint64_t)ids[i] * S);
+#pragma unroll
+            for (int j = 0; j < SV; j++) if (j < (int)(S / 16)) v[j] = __ldg(sp + j);
+#pragma unroll
+            for (int c = 0; c < NC; c++) { nd[c] = out.off[c][i]; nlen[c] = out.off[c][i + 1] - nd[c]; }
+        }
+    };
+    uint64_t g = (uint64_t)blockIdx.x * GW_WARPS + warp;
+    fetch(g);
+    for (; g * 32 < n; g += nwarps) {
         const uint64_t i = g * 32 + lane;
         const bool valid = i < n;
         if (valid) {
-            const uint4* sp = reinterpret_cast<const uint4*>(slots + (uint64_t)ids[i] * S);
-            for (uint32_t j = 0; j < S / 16; j++) {
-                const uint4 v = __ldg(sp + j);
-                uint32_t* w = reinterpret_cast<uint32_t*>(myslot) + 4 * j;
-                w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
-            }
+#pragma unroll
+            for (int j = 0; j < SV; j++)
+                if (j < (int)(S / 16)) {
+                    uint32_t* w = reinterpret_cast<uint32_t*>(myslot) + 4 * j;
+                    w[0] = v[j].x; w[1] = v[j].y; w[2] = v[j].z; w[3] = v[j].w;
+                }
         }
+        // per column: this lane's destination offset and length; the group's stage region [base, base + 16 nv), head
+        // shift sh (stage byte sh = destination byte d0) and byte count
+        uint32_t d[NC], len[NC], d0[NC], sh[NC], total[NC], base[NC], nv[NC];
+#pragma unroll
+        for (int c = 0; c < NC; c++) { d[c] = nd[c]; len[c] = nlen[c]; }
+        fetch(g + nwarps);
         const uint64_t last = (g * 32 + 31 < n ? g * 32 + 31 : n - 1) - g * 32;
+        uint32_t used = 0;
+#pragma unroll
+        for (int c = 0; c < NC; c++) {
+            d0[c] = __shfl_sync(0xffffffffu, d[c], 0);
+            total[c] = __shfl_sync(0xffffffffu, d[c] + len[c], (int)last) - d0[c];
+            sh[c] = d0[c] & 15u;
+            nv[c] = total[c] ? (sh[c] + total[c] + 15) / 16 : 0;
+            base[c] = used;
+            if (used + nv[c] * 16 <= GW_STAGE) used += nv[c] * 16;
+            else nv[c] = ~0u;  // direct
+        }
+        for (uint32_t x = lane * 16; x < used; x += 32 * 16) *reinterpret_cast<uint4*>(stage + x) = make_uint4(0, 0, 0, 0);
+        __syncwarp();
         uint32_t pos = 0;
 #pragma unroll
         for (int c = 0; c < NC; c++) {
-            uint32_t d = 0, len = 0;
-            if (valid) { d = out.off[c][i]; len = out.off[c][i + 1] - d; }
-            const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
-            const uint32_t dl = __shfl_sync(0xffffffffu, d + len, (int)last);
-            const uint32_t total = dl - d0, sh = d0 & 15u;
-            const uint8_t* sp = myslot + pos;
-            uint8_t* dst = out.data[c];
-            if (sh + total <= GW_STAGE) {
-                uint8_t* q = stage + sh + (d - d0);
-                for (uint32_t k = 0; k < len; k++) q[k] = sp[k];
-                __syncwarp();
-                uint8_t* gb = dst + (d0 - sh);  // (warp_store_stage was slower here)
-                for (uint32_t x = lane * 16; x < sh + total; x += 32 * 16) {
-                    if (x >= sh && x + 16 <= sh + total) *reinterpret_cast<uint4*>(gb + x) = *reinterpret_cast<const uint4*>(stage + x);
-                    else for (uint32_t y = x; y < x + 16; y++) if (y >= sh && y < sh + total) gb[y] = stage[y];
-                }
-                __syncwarp();
+            if (nv[c] != ~0u) {
+                or_value(stage, base[c] + sh[c] + (d[c] - d0[c]), myslot, pos, len[c]);
             } else {
-                uint8_t* dp = dst + d;
-                for (uint32_t k = 0; k < len; k++) dp[k] = sp[k];
+                uint8_t* dp = out.data[c] + d[c];
+                for (uint32_t k = 0; k < len[c]; k++) dp[k] = myslot[pos + k];
             }
-            pos += len;
+            pos += len[c];
         }
-        __syncwarp();  // the slots are overwritten by the next round
+        __syncwarp();
+        for (uint32_t x = lane * 16; x < used; x += 32 * 16) {
+            uint8_t* gb = nullptr;
+            uint32_t lo = 0, hi = 0;
+#pragma unroll
+            for (int c = 0; c < NC; c++)
+                if (nv[c] != ~0u && x >= base[c] && x < base[c] + nv[c] * 16) {
+                    const uint32_t r = x - base[c];  // vector r / 16 of column c's region
+                    gb = out.data[c] + (d0[c] - sh[c]) + r;
+                    lo = sh[c] > r ? sh[c] - r : 0;
+                    hi = min(sh[c] + total[c] - r, 16u);
+                }
+            const uint4 v = *reinterpret_cast<const uint4*>(stage + x);
+            if (lo == 0 && hi == 16) *reinterpret_cast<uint4*>(gb) = v;
+            else store_part16(gb, v, lo, hi);
+        }
+        __syncwarp();  // the slots and the stage are overwritten by the next round
     }
 }
 
@@ -475,6 +558,10 @@ static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& col
 }
 
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, bool by_src) {
+    if (cols.empty()) {  // nothing to gather (a join whose index columns are all key columns): no slots, no sorted rows
+        auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = ix.schema().first_line;
+        return r;
+    }
     auto plain = [&]() {  // per-column gather: from the source rows (ids = source rows), or from the physically sorted rows
         std::shared_ptr<Table> keep = by_src ? ix.src : sorted_table(c, ix);
         const Table& st = *keep;
@@ -530,9 +617,11 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
     {
         KernelTimer kt(c, "slot_copy", 2 * all + n * (4 + 4 * (uint64_t)nc));
         const uint32_t gblocks = (uint32_t)std::min<uint64_t>((n + GW_WARPS * 32 - 1) / (GW_WARPS * 32), (uint64_t)c->sm_count * 16);
-#define CPB_SC(NC) slot_copy_kernel<NC><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(rs.slots->as<uint8_t>(), rs.S, ids, so, n)
+#define CPB_SC2(NC, SV) slot_copy_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(rs.slots->as<uint8_t>(), rs.S, ids, so, n)
+#define CPB_SC(NC) (rs.S <= 16 ? CPB_SC2(NC, 1) : rs.S <= 32 ? CPB_SC2(NC, 2) : CPB_SC2(NC, 4))
         switch (nc) { case 1: CPB_SC(1); break; case 2: CPB_SC(2); break; case 3: CPB_SC(3); break; default: CPB_SC(4); break; }
 #undef CPB_SC
+#undef CPB_SC2
         CPB_CUDA(cudaGetLastError());
     }
     for (int k = 0; k < nc; k++) r->cols.push_back(out[k]);

@@ -385,13 +385,32 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     }
     // output schema: mergeRows(indexRow, probeRow) — probe wins name collisions (csvplus.go:571-583)
     std::vector<const Column*> icols, pcols;
-    std::vector<int> icol_idx;
+    // An index column that is one of the nk joined key columns is not gathered: a match means equal key images, and
+    // equal images mean equal bytes (value zero-padded to the index's width, then its length), so the index value IS
+    // the probe value.  icol_key[j] = k takes output column j from probe key column pidx[k]; -1 gathers it from the
+    // index (gather_idx: those index columns, in order).
+    std::vector<int> icol_key, gather_idx;
     const Table& ischema = ix.schema();  // names only: the sorted columns may not be materialised
-    if (!anti) for (size_t q = 0; q < ischema.cols.size(); q++)
-        if (probe.find(ischema.cols[q].name) < 0) { icols.push_back(&ischema.cols[q]); icol_idx.push_back((int)q); }
+    if (!anti) for (size_t q = 0; q < ischema.cols.size(); q++) {
+        if (probe.find(ischema.cols[q].name) >= 0) continue;
+        int key = -1;
+        for (int k = 0; k < nk && key < 0; k++) if (ix.key_col_idx[k] == (int)q) key = k;
+        icols.push_back(&ischema.cols[q]);
+        icol_key.push_back(key);
+        if (key < 0) gather_idx.push_back((int)q);
+    }
     for (auto& col : probe.cols) pcols.push_back(&col);
 
     auto out = std::make_shared<Table>(); out->ctx = c; out->first_line = probe.first_line;
+    // appends the index-side output columns: the gathered ones in order from `gi`, the key columns as keycol(k)
+    auto put_index_cols = [&](const Table& gi, auto keycol) {
+        size_t g = 0;
+        for (size_t j = 0; j < icols.size(); j++) {
+            Column col = icol_key[j] >= 0 ? keycol(icol_key[j]) : gi.cols[g++];
+            col.name = icols[j]->name;
+            out->cols.push_back(col);
+        }
+    };
     auto empty_result = [&]() {
         Table e; e.ctx = c; e.nrows = 0;
         for (auto* p : icols) e.cols.push_back(*p);
@@ -435,9 +454,9 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     if (m > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "join result exceeds 2^32-2 rows; probe in smaller batches"};
     if (m == 0) return empty_result();
     if (probe_identity) {
-        auto gi = gather_index_rows(c, ix, icol_idx, lo->as<uint32_t>(), (int64_t)m, by_src);  // lo[i] is the single matching index row
+        auto gi = gather_index_rows(c, ix, gather_idx, lo->as<uint32_t>(), (int64_t)m, by_src);  // lo[i] is the single matching index row
         out->nrows = (int64_t)m;
-        for (auto& col : gi->cols) out->cols.push_back(col);
+        put_index_cols(*gi, [&](int k) { return probe.cols[pidx[k]]; });
         for (auto* p : pcols) out->cols.push_back(*p);
         return out;
     }
@@ -452,10 +471,10 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     }
     Table pt; pt.ctx = c; pt.nrows = (int64_t)np;
     for (auto* p : pcols) pt.cols.push_back(*p);
-    auto gi = gather_index_rows(c, ix, icol_idx, iid->as<uint32_t>(), (int64_t)m, by_src);
+    auto gi = gather_index_rows(c, ix, gather_idx, iid->as<uint32_t>(), (int64_t)m, by_src);
     auto gp = gather_rows(c, pt, pid->as<uint32_t>(), (int64_t)m);
     out->nrows = (int64_t)m;
-    for (auto& col : gi->cols) out->cols.push_back(col);
+    put_index_cols(*gi, [&](int k) { return gp->cols[pidx[k]]; });
     for (auto& col : gp->cols) out->cols.push_back(col);
     return out;
 }
