@@ -3,6 +3,7 @@
 //	go run ./golden ../../tests/golden /tmp/golden_from_reference
 //	for f in people_amelia orders_join_people orders_without_customer nasty_roundtrip; do
 //	    cmp ../../tests/golden/$f.csv /tmp/golden_from_reference/$f.csv; done
+//	cmp ../../tests/golden/json_escapes.json /tmp/golden_from_reference/json_escapes.json
 //
 // Never compiled here (no Go toolchain in this image).  orders_sorted_prod_qty.csv depends on the order of rows
 // with equal keys: the reference sorts with sort.Sort (unstable, SURVEY §Q2) while the oracle and the CUDA path keep
@@ -52,4 +53,7 @@ func main() {
 
 	// reader quoting / CRLF / blank lines -> writer
 	must(csvplus.Take(csvplus.FromFile(p("nasty.csv"))).ToCsvFile(o("nasty_roundtrip.csv"), "c0", "c1", "c2", "c3"))
+
+	// every byte class of encoding/json's string encoding, in values and keys (\b and \f since go 1.22)
+	must(csvplus.Take(csvplus.FromFile(p("json_escapes.csv"))).ToJSONFile(o("json_escapes.json")))
 }

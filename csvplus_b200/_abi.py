@@ -52,6 +52,7 @@ SYMBOLS = [
     "cpb_index_build", "cpb_index_num_rows", "cpb_index_num_keys", "cpb_index_table", "cpb_index_find", "cpb_index_sub",
     "cpb_index_dup_groups", "cpb_index_dedup_apply", "cpb_index_dedup_apply2", "cpb_free", "cpb_index_free",
     "cpb_join", "cpb_except", "cpb_table_to_csv", "cpb_table_to_csv_device", "cpb_table_to_csv_into",
+    "cpb_table_to_json", "cpb_table_to_json_device", "cpb_table_to_json_into",
     "cpb_comm_unique_id", "cpb_comm_init_rank", "cpb_init_multi", "cpb_comm_size", "cpb_comm_rank", "cpb_allgather_table",
     "cpb_allgather_tables", "cpb_allgather_u64", "cpb_allgather_layout",
     "cpb_stats_enable", "cpb_stats_reset", "cpb_stats_get", "cpb_kernel_launches", "cpb_host_syncs", "cpb_gen_csv",
@@ -122,6 +123,9 @@ def load():
         "cpb_table_to_csv": (i32, [vp, vp, P(Str), i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_csv_device": (i32, [vp, vp, P(Str), i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_csv_into": (i32, [vp, vp, P(Str), i32, i32, vp, u64, P(u64), P(Error)]),
+        "cpb_table_to_json": (i32, [vp, vp, i32, i32, P(vp), P(u64), P(Error)]),
+        "cpb_table_to_json_device": (i32, [vp, vp, i32, i32, P(vp), P(u64), P(Error)]),
+        "cpb_table_to_json_into": (i32, [vp, vp, i32, i32, vp, u64, P(u64), P(Error)]),
         "cpb_comm_unique_id": (i32, [vp]),
         "cpb_comm_init_rank": (i32, [vp, i32, i32, vp]),
         "cpb_init_multi": (i32, [P(i32), i32, P(vp)]),

@@ -23,6 +23,10 @@ from . import _abi
 
 Row = dict  # map[string]string, csvplus.go:59 (values are str; bytes survive via surrogateescape)
 
+# rows per cpb_table_to_json_into call when DataSource.ToJSON writes a device table: one call produces < 4 GiB, and
+# about 2.4 GB for joined rows of ~150 B.  A batch that is still too large is split in halves.
+JSON_BATCH_ROWS = 1 << 24
+
 
 def _enc(s) -> bytes:
     return s if isinstance(s, (bytes, bytearray)) else str(s).encode("utf-8", "surrogateescape")
@@ -33,8 +37,8 @@ def _dec(b: bytes) -> str:
 
 
 def _go_json_string(s) -> bytes:
-    """encoding/json's string encoding with HTML escaping off: `"` `\\` and control characters escaped (\\n \\r \\t, else
-    \\u00xx), U+2028 / U+2029 escaped, every invalid UTF-8 byte replaced by \\ufffd, everything else verbatim"""
+    """encoding/json's string encoding with HTML escaping off: `"` `\\` and control characters escaped (\\n \\r \\t \\b \\f,
+    else \\u00xx), U+2028 / U+2029 escaped, every invalid UTF-8 byte replaced by \\ufffd, everything else verbatim"""
     b = _enc(s)
     out = bytearray(b'"')
     i, n = 0, len(b)
@@ -46,6 +50,8 @@ def _go_json_string(s) -> bytes:
             elif c == 0x0A: out += b"\\n"
             elif c == 0x0D: out += b"\\r"
             elif c == 0x09: out += b"\\t"
+            elif c == 0x08: out += b"\\b"
+            elif c == 0x0C: out += b"\\f"
             elif c < 0x20: out += b"\\u00" + b"%02x" % c
             else: out.append(c)
             i += 1
@@ -475,6 +481,38 @@ class Table:
         """ToCsv with the serialised bytes left in HBM (cpb_table_to_csv_device)"""
         a, keep = _strs(cols); p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
         st = self.ctx.lib.cpb_table_to_csv_device(self.ctx.h, self.h, a, len(cols), C.byref(p), C.byref(n), C.byref(e))
+        if st:
+            _raise(st, e, self.ctx)
+        b = DeviceBuffer.__new__(DeviceBuffer)
+        b.ctx, b.nbytes, b.ptr = self.ctx, n.value, p.value
+        return b
+
+    def to_json(self, first: bool = True, last: bool = True) -> bytes:
+        """DataSource.ToJSON of every column (cpb_table_to_json); first / last: the batch opens / closes the array"""
+        p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
+        st = self.ctx.lib.cpb_table_to_json(self.ctx.h, self.h, int(first), int(last), C.byref(p), C.byref(n), C.byref(e))
+        if st:
+            _raise(st, e, self.ctx)
+        out = C.string_at(p.value, n.value)
+        self.ctx.lib.cpb_host_free(self.ctx.h, p)
+        return out
+
+    def to_json_into(self, dst: "HostBuffer | None", offset: int = 0, first: bool = True, last: bool = True) -> int:
+        """one batch of a streamed ToJSON into pinned host memory (cpb_table_to_json_into).  Returns the batch's size in
+        bytes; when that exceeds the room left in dst (or dst is None), nothing is written."""
+        n = C.c_uint64(); e = _abi.Error()
+        ptr, cap = (dst.ptr + offset, dst.nbytes - offset) if dst is not None else (None, 0)
+        st = self.ctx.lib.cpb_table_to_json_into(self.ctx.h, self.h, int(first), int(last), C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
+        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
+            return n.value
+        if st:
+            _raise(st, e, self.ctx)
+        return n.value
+
+    def to_json_device(self, first: bool = True, last: bool = True) -> "DeviceBuffer":
+        """ToJSON with the serialised bytes left in HBM (cpb_table_to_json_device)"""
+        p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
+        st = self.ctx.lib.cpb_table_to_json_device(self.ctx.h, self.h, int(first), int(last), C.byref(p), C.byref(n), C.byref(e))
         if st:
             _raise(st, e, self.ctx)
         b = DeviceBuffer.__new__(DeviceBuffer)
@@ -917,16 +955,23 @@ class DataSource:
 
     def ToJSON(self, out: io.IOBase):  # csvplus.go:446-474
         """all rows as a JSON array, formatted the way the reference's json.Encoder (SetEscapeHTML(false), no indent) writes
-        it: `[`, then per row the object with its keys sorted and a newline, a `,` before every row but the first, `]`."""
+        it: `[`, then per row the object with its keys sorted and a newline, a `,` before every row but the first, `]`.
+        A device table is serialised by the GPU in row-range batches; rows left on the host (after an opaque Map or
+        Filter(func), or TakeRows of rows with different columns) are encoded here.  On a source error nothing is written."""
+        state, err = self._evaluate()
+        if err is not None:
+            raise err
+        if state[0] == "table":
+            if state[1] is None:
+                out.write(b"[]")
+            else:
+                _json_batches(state[1], out)
+            return
         parts = [b"["]
-        first = [True]
-
-        def fn(row):
-            if not first[0]:
+        for i, row in enumerate(state[1]):
+            if i:
                 parts.append(b",")
-            first[0] = False
             parts.append(b"{" + b",".join(_go_json_string(k) + b":" + _go_json_string(row[k]) for k in sorted(row, key=_enc)) + b"}\n")
-        self(fn)
         parts.append(b"]")
         out.write(b"".join(parts))
 
@@ -956,6 +1001,36 @@ class DataSource:
         if t is None:
             t = Table.from_rows(self._ctx(), [], list(columns))
         return t.index_on(*columns, unique=unique)
+
+
+def _json_batches(t: Table, out: io.IOBase):
+    """ToJSON of a device table: row-range slices of at most JSON_BATCH_ROWS rows, each serialised into one reused pinned
+    buffer that grows to the size a batch reports, then written to out"""
+    n = len(t)
+    buf, lo, step = None, 0, JSON_BATCH_ROWS
+    try:
+        while True:
+            hi = min(n, lo + step)
+            part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
+            try:
+                w = part.to_json_into(buf, 0, lo == 0, hi == n)
+            except CsvPlusError as e:
+                if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
+                    raise
+                step = (hi - lo) // 2
+                continue
+            if buf is None or w > buf.nbytes:
+                if buf is not None:
+                    buf.free()
+                buf = HostBuffer(t.ctx, w + w // 4 + 64)
+                continue
+            out.write(memoryview(buf.array()[:w]))
+            lo = hi
+            if lo >= n:
+                return
+    finally:
+        if buf is not None:
+            buf.free()
 
 
 def Take(src) -> DataSource:  # csvplus.go:252-256

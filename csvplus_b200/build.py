@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libcsvplus_b200.so")
-SOURCES = ["abi.cu", "parse.cu", "parse_general.cu", "gather.cu", "sort.cu", "join.cu", "write.cu", "gen.cu", "comm.cu", "subst.cu"]
+SOURCES = ["abi.cu", "parse.cu", "parse_general.cu", "gather.cu", "sort.cu", "join.cu", "write.cu", "json.cu", "gen.cu", "comm.cu", "subst.cu"]
 HEADERS = ["core.hpp", "util.cuh", "pred.cuh", "parse_kernels.cuh", "subst.hpp", os.path.join("..", "..", "include", "csvplus_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -738,6 +738,51 @@ int cpb_table_to_csv_device(cpb_ctx* h, const cpb_table* t, const cpb_str* cols,
     return to_csv_common(h, t, cols, n, false, bytes, nbytes, err);
 }
 
+// ------------------------------------------------------------------ ToJSON
+// to_host / into host_dst / left on the device, as ToCsv
+static int to_json_common(cpb_ctx* h, const cpb_table* t, int first, int last, int mode, void** bytes, void* host_dst, uint64_t cap,
+                          uint64_t* nbytes, cpb_error* err) {
+    if (!h || !t || !nbytes || (mode != 1 && !bytes) || (mode == 1 && cap && !host_dst)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    uint64_t total = 0;
+    Buf out = table_to_json(c, *t->t, first != 0, last != 0, &total);
+    *nbytes = total;
+    if (mode == 0) {
+        void* hp = nullptr;
+        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
+        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        *bytes = hp;
+    } else if (mode == 1) {
+        if (total > cap) throw ArgError{CPB_ERR_ARG, "ToJSON destination too small"};
+        if (total) {
+            KernelTimer kt(c, "d2h_output", total, 0);
+            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        }
+        sync_stream(c);
+    } else {
+        void* dp = nullptr;
+        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
+        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
+        *bytes = dp;
+    }
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_table_to_json(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void** bytes, uint64_t* nbytes, cpb_error* err) {
+    return to_json_common(h, t, first_batch, last_batch, 0, bytes, nullptr, 0, nbytes, err);
+}
+int cpb_table_to_json_into(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void* host_dst, uint64_t cap,
+                           uint64_t* nbytes, cpb_error* err) {
+    return to_json_common(h, t, first_batch, last_batch, 1, nullptr, host_dst, cap, nbytes, err);
+}
+int cpb_table_to_json_device(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void** bytes, uint64_t* nbytes,
+                             cpb_error* err) {
+    return to_json_common(h, t, first_batch, last_batch, 2, bytes, nullptr, 0, nbytes, err);
+}
+
 // ------------------------------------------------------------------ stats
 int cpb_stats_enable(cpb_ctx* h, int on) { DeviceGuard g(&h->c); h->c.stats_on = on != 0; return CPB_OK; }
 int cpb_stats_reset(cpb_ctx* h) {

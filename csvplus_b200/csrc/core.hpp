@@ -274,6 +274,8 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep, bool
 // write.cu
 Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names,
                  uint64_t* nbytes, uint64_t* header_bytes);
+// json.cu: ToJSON of every column (keys in bytewise order); '[' before the first row when first, ']' appended when last
+Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbytes);
 
 }  // namespace cpb
 

@@ -517,34 +517,135 @@ func (src DataSource) ToCsvFile(name string, columns ...string) error {
 	return writeFile(name, func(w io.Writer) error { return src.ToCsv(w, columns...) })
 }
 
+// jsonBatchRows is the number of rows per cpb_table_to_json_into call: one call produces less than 4 GiB.
+const jsonBatchRows = 1 << 24
+
 // ToJSON writes all rows as a JSON array of objects, one object per line (csvplus.go:446-474: json.Encoder with
-// SetEscapeHTML(false), a comma before every element but the first).
+// SetEscapeHTML(false), a comma before every element but the first).  A device-resident result is serialised by the
+// GPU in row-range batches (cpb_table_to_json_into) through one reused pinned buffer; host rows (after an opaque
+// closure) go through encoding/json.  When the source fails after some rows, out receives what the reference would
+// have flushed before the error, and no closing ']'.
 func (src DataSource) ToJSON(out io.Writer) error {
+	p := planOf(src)
+	res := p.eval()
+	if res.onHost {
+		return rowsToJSON(out, res.rows, res.err)
+	}
+	c := p.context()
+	if res.table == nil {
+		if res.err != nil {
+			return res.err
+		}
+		_, err := out.Write([]byte("[]"))
+		return err
+	}
+	n := res.table.NumRows()
+	var buf unsafe.Pointer
+	var capacity C.uint64_t
+	defer func() {
+		if buf != nil {
+			C.cpb_host_free(c.h, buf)
+		}
+	}()
+	var pending []byte
+	for lo := int64(0); ; {
+		hi := lo + jsonBatchRows
+		if hi > n {
+			hi = n
+		}
+		var part *C.cpb_table
+		if st := C.cpb_table_slice(c.h, res.table.h, C.int64_t(lo), C.int64_t(hi), &part); st != C.CPB_OK {
+			return errors.New("csvplus: cpb_table_slice failed")
+		}
+		first, last := C.int(0), C.int(0)
+		if lo == 0 {
+			first = 1
+		}
+		if hi == n && res.err == nil {
+			last = 1
+		}
+		var w C.uint64_t
+		var e C.cpb_error
+		st := C.cpb_table_to_json_into(c.h, part, first, last, buf, capacity, &w, &e)
+		C.cpb_table_free(part)
+		if st == C.CPB_ERR_ARG && w > capacity { // grow the buffer to the size the batch needs and repeat it
+			if buf != nil {
+				C.cpb_host_free(c.h, buf)
+				buf, capacity = nil, 0
+			}
+			if C.cpb_host_alloc(c.h, w+w/4, &buf) != C.CPB_OK {
+				return errors.New("csvplus: cpb_host_alloc failed")
+			}
+			capacity = w + w/4
+			continue
+		}
+		if st != C.CPB_OK {
+			return mapErr(C.int(st), &e)
+		}
+		chunk := unsafe.Slice((*byte)(buf), int(w))
+		if res.err == nil {
+			if _, err := out.Write(chunk); err != nil {
+				return err
+			}
+		} else {
+			var err error
+			if pending, err = writeFlushed(out, pending, chunk); err != nil {
+				return err
+			}
+		}
+		if lo = hi; lo >= n {
+			break
+		}
+	}
+	return res.err
+}
+
+// writeFlushed writes what the reference flushes of these rows when the source fails after them: its buffer goes out
+// after every row that leaves more than 10 000 bytes pending.  A raw '\n' only ever ends a row, because the encoder
+// escapes every newline inside a string.  Returns the bytes still pending.
+func writeFlushed(out io.Writer, pending, chunk []byte) ([]byte, error) {
+	for len(chunk) > 0 {
+		i := bytes.IndexByte(chunk, '\n')
+		if i < 0 {
+			return append(pending, chunk...), nil
+		}
+		pending = append(pending, chunk[:i+1]...)
+		chunk = chunk[i+1:]
+		if len(pending) > 10000 {
+			if _, err := out.Write(pending); err != nil {
+				return nil, err
+			}
+			pending = pending[:0]
+		}
+	}
+	return pending, nil
+}
+
+// rowsToJSON is the reference's ToJSON over rows left on the host, ended by srcErr.
+func rowsToJSON(out io.Writer, rows []Row, srcErr error) error {
 	var buff bytes.Buffer
 	buff.WriteByte('[')
 	enc := json.NewEncoder(&buff)
 	enc.SetIndent("", "")
 	enc.SetEscapeHTML(false)
-	first := true
-	err := src(func(row Row) error {
-		if !first {
+	for i, row := range rows {
+		if i > 0 {
 			buff.WriteByte(',')
 		}
-		first = false
 		if e := enc.Encode(row); e != nil {
 			return e
 		}
 		if buff.Len() > 10000 {
-			_, e := buff.WriteTo(out)
-			return e
+			if _, e := buff.WriteTo(out); e != nil {
+				return e
+			}
 		}
-		return nil
-	})
-	if err != nil {
-		return err
+	}
+	if srcErr != nil {
+		return srcErr
 	}
 	buff.WriteByte(']')
-	_, err = buff.WriteTo(out)
+	_, err := buff.WriteTo(out)
 	return err
 }
 

@@ -6,6 +6,7 @@
 // and the rows are uploaded again with TakeRows semantics — exactly what the cgo wrapper does for Go
 // closures (INTEGRATION.md).  There is no CPU fallback: without a GPU every sink throws.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <functional>
@@ -253,6 +254,35 @@ public:
         detail::check(cpb_table_to_csv(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), &bytes, &n, &e), e);
         out.write((const char*)bytes, (std::streamsize)n); cpb_host_free(detail::ctx(), bytes);
         if (err) throw *err;
+    }
+    // ToJSON, csvplus.go:446-474: the GPU serialises the result in row-range batches (each < 4 GiB) into one reused
+    // pinned buffer; on a source error nothing is written
+    void ToJSON(std::ostream& out) const {
+        std::unique_ptr<DataSourceError> err; Table t = run(&err);
+        if (err) throw *err;
+        const int64_t n = t.size(), step = int64_t(1) << 24;
+        void* buf = nullptr; uint64_t cap = 0;
+        try {
+            for (int64_t lo = 0;;) {
+                const int64_t hi = std::min(n, lo + step);
+                cpb_table* part = nullptr; cpb_error e{};
+                detail::check(cpb_table_slice(detail::ctx(), t.get(), lo, hi, &part), e);
+                Table p(part); uint64_t w = 0;
+                int st = cpb_table_to_json_into(detail::ctx(), p.get(), lo == 0, hi == n, buf, cap, &w, &e);
+                if (st == CPB_ERR_ARG && w > cap) {  // grow the buffer to the size the batch needs and repeat it
+                    if (buf) cpb_host_free(detail::ctx(), buf);
+                    buf = nullptr; cap = 0;
+                    if (cpb_host_alloc(detail::ctx(), w + w / 4, &buf) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+                    cap = w + w / 4;
+                    continue;
+                }
+                detail::check(st, e);
+                out.write((const char*)buf, (std::streamsize)w);
+                lo = hi;
+                if (lo >= n) break;
+            }
+        } catch (...) { if (buf) cpb_host_free(detail::ctx(), buf); throw; }
+        if (buf) cpb_host_free(detail::ctx(), buf);
     }
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }

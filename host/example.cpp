@@ -1,6 +1,7 @@
 // example.cpp — the reference's README / test scenarios through the C++ host mirror (host/csvplus.hpp).
-// Mirrors TestSimpleDataSource (csvplus_test.go:118-151), TestSimpleUniqueJoin (:368-452), TestErrors (:808-909)
-// and TestWriteFile (:172-196) on fixtures generated like csvplus_test.go:1207-1333.  Exit code 0 = all checks hold.
+// Mirrors TestSimpleDataSource (csvplus_test.go:118-151), TestSimpleUniqueJoin (:368-452), TestErrors (:808-909),
+// TestWriteFile (:172-196) and TestJSONStruct (:1016-1048) on fixtures generated like csvplus_test.go:1207-1333.
+// Exit code 0 = all checks hold.
 #include <cstdio>
 #include <cstdlib>
 #include <iostream>
@@ -48,6 +49,15 @@ int main() {
         std::ostringstream out;
         Take(FromString(people).SelectColumns({"id", "name", "surname", "born"})).ToCsv(out, {"id", "name", "surname", "born"});
         CHECK(out.str() == people);
+        // TestJSONStruct (csvplus_test.go:1016): SelectColumns -> ToJSON, keys sorted, one object per line
+        std::ostringstream js, want_js;
+        Take(FromString(people).SelectColumns({"name", "surname", "born"})).ToJSON(js);
+        want_js << '[';
+        for (int i = 0; i < 10; i++) for (int j = 0; j < 12; j++)
+            want_js << (i || j ? "," : "") << "{\"born\":\"" << 1916 + (i * 37 + j * 11) % 90 << "\",\"name\":\"" << names[i]
+                    << "\",\"surname\":\"" << surnames[j] << "\"}\n";
+        want_js << ']';
+        CHECK(js.str() == want_js.str());
         // TestErrors
         try { Take(FromString(people).SelectColumns({"id", "name", "xxx"})).ToRows(); CHECK(false); }
         catch (const DataSourceError& e) { CHECK(std::string(e.what()) == "row 1: column not found: xxx"); }

@@ -233,6 +233,19 @@ int cpb_table_to_csv_device(cpb_ctx* ctx, const cpb_table* t, const cpb_str* col
 int cpb_table_to_csv_into(cpb_ctx* ctx, const cpb_table* t, const cpb_str* cols, int n, int with_header, void* host_dst,
                           uint64_t cap, uint64_t* nbytes, cpb_error* err);
 
+/* ------------------------------------------------------------------ ToJSON
+ * DataSource.ToJSON (csvplus.go:446-474) of one table or one batch of a streamed result: every column, keys sorted
+ * bytewise, encoding/json's string escaping with SetEscapeHTML(false), one object per line.
+ * first_batch: the first row is preceded by '[' (else ','); last_batch: ']' is appended.  first=last=1 on an empty
+ * table gives "[]".  One call produces less than 4 GiB (else CPB_ERR_DATA / CPB_E_TOO_LARGE: write row-range batches). */
+int cpb_table_to_json(cpb_ctx* ctx, const cpb_table* t, int first_batch, int last_batch, void** bytes, uint64_t* nbytes,
+                      cpb_error* err); /* pinned host bytes: release with cpb_host_free */
+int cpb_table_to_json_device(cpb_ctx* ctx, const cpb_table* t, int first_batch, int last_batch, void** dev_bytes,
+                             uint64_t* nbytes, cpb_error* err); /* device bytes: release with cpb_device_free */
+/* into caller-owned (pinned) host memory; cap too small: CPB_ERR_ARG with *nbytes = the size needed, nothing written */
+int cpb_table_to_json_into(cpb_ctx* ctx, const cpb_table* t, int first_batch, int last_batch, void* host_dst, uint64_t cap,
+                           uint64_t* nbytes, cpb_error* err);
+
 /* ------------------------------------------------------------------ multi-GPU (SURVEY §8e)
  * The probe stream shards by row range with no data-path collective; the one exchange step is the all-gather of the
  * build-side columns (each rank parses 1/N of the build file) so that every rank can build the full Index
