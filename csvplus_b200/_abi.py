@@ -53,6 +53,7 @@ SYMBOLS = [
     "cpb_index_dup_groups", "cpb_index_dedup_apply", "cpb_index_dedup_apply2", "cpb_free", "cpb_index_free",
     "cpb_join", "cpb_except", "cpb_table_to_csv", "cpb_table_to_csv_device", "cpb_table_to_csv_into",
     "cpb_table_to_json", "cpb_table_to_json_device", "cpb_table_to_json_into",
+    "cpb_table_column_as_int64", "cpb_table_column_as_float64",
     "cpb_comm_unique_id", "cpb_comm_init_rank", "cpb_init_multi", "cpb_comm_size", "cpb_comm_rank", "cpb_allgather_table",
     "cpb_allgather_tables", "cpb_allgather_u64", "cpb_allgather_layout",
     "cpb_stats_enable", "cpb_stats_reset", "cpb_stats_get", "cpb_kernel_launches", "cpb_host_syncs", "cpb_gen_csv",
@@ -126,6 +127,8 @@ def load():
         "cpb_table_to_json": (i32, [vp, vp, i32, i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_json_device": (i32, [vp, vp, i32, i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_json_into": (i32, [vp, vp, i32, i32, vp, u64, P(u64), P(Error)]),
+        "cpb_table_column_as_int64": (i32, [vp, vp, Str, vp, vp, P(u64), P(Error)]),
+        "cpb_table_column_as_float64": (i32, [vp, vp, Str, vp, vp, P(u64), P(Error)]),
         "cpb_comm_unique_id": (i32, [vp]),
         "cpb_comm_init_rank": (i32, [vp, i32, i32, vp]),
         "cpb_init_multi": (i32, [P(i32), i32, P(vp)]),

@@ -519,6 +519,47 @@ class Table:
         b.ctx, b.nbytes, b.ptr = self.ctx, n.value, p.value
         return b
 
+    def values_as_int(self, name: str, strict: bool = True):
+        """Row.ValueAsInt (strconv.Atoi, csvplus.go:165-183) of every row of a column, as an int64 CUDA tensor on the
+        ctx's device.  strict: the first failing row raises CsvPlusError with the reference's text (.row = its index), as
+        a RowFunc returning the helper's error does; else -> (values, status uint8: 0 ok, 1 ErrSyntax, 2 ErrRange), the
+        values being what Go returns alongside each error."""
+        return self._values_as(name, False, strict)
+
+    def values_as_float64(self, name: str, strict: bool = True):
+        """Row.ValueAsFloat64 (strconv.ParseFloat(s, 64), csvplus.go:187-205): as values_as_int, float64 values"""
+        return self._values_as(name, True, strict)
+
+    def _values_as(self, name: str, is_float: bool, strict: bool):
+        values, status, err = self._convert(name, is_float)
+        if err is not None and (strict or err.kind == 10):  # CPB_E_MISSING_COLUMN fails in both modes
+            raise err
+        return values if strict else (values, status)
+
+    def _convert(self, name: str, is_float: bool):
+        """-> (values, status, CsvPlusError of the first failing row or None); one host synchronisation"""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        n = len(self)
+        values = torch.empty(n, dtype=torch.float64 if is_float else torch.int64, device=dev)
+        status = torch.empty(n, dtype=torch.uint8, device=dev)
+        # the ctx stream writes into memory torch's current stream allocated: it waits for that stream first; the
+        # synchronisation inside the call orders the way back
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(dev))
+        torch.cuda.ExternalStream(self.ctx.stream, device=dev).wait_event(ev)
+        b = _enc(name); nbad = C.c_uint64(); e = _abi.Error()
+        fn = self.ctx.lib.cpb_table_column_as_float64 if is_float else self.ctx.lib.cpb_table_column_as_int64
+        st = fn(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), C.c_void_p(status.data_ptr()), C.byref(nbad),
+                C.byref(e))
+        if st == 1:
+            err = CsvPlusError(e.msg.decode("utf-8", "replace"), st, e.kind)
+            err.row = e.line
+            return values, status, err
+        if st:
+            _raise(st, e, self.ctx)
+        return values, status, None
+
     @staticmethod
     def concat(parts: list["Table"]) -> "Table":
         ctx = parts[0].ctx
@@ -983,6 +1024,35 @@ class DataSource:
             if os.path.exists(name):
                 os.remove(name)
             raise
+
+    def ToTensors(self, columns: dict) -> dict:
+        """{name: "int" | "float64"} -> {name: CUDA tensor}: Row.ValueAsInt / ValueAsFloat64 of every row of each column,
+        converted on the GPU (an extension beyond the reference API, like TakeTable).  The plan is evaluated once.  The
+        error raised is the one a RowFunc converting the columns in dict order would meet first: the lowest failing row,
+        ties to the earlier column (CsvPlusError, .row = the row).  When no row fails, a pending source error is raised:
+        the table only holds the rows delivered before it."""
+        kinds = {}
+        for name, kind in columns.items():
+            if kind not in ("int", "float64"):
+                raise ValueError(f"ToTensors: unknown type {kind!r} for column {name!r} (want 'int' or 'float64')")
+            kinds[name] = kind == "float64"
+        t, err = self._table()
+        if t is None:
+            import torch
+            dev = torch.device("cuda", self._ctx().device)
+            out = {name: torch.empty(0, dtype=torch.float64 if f else torch.int64, device=dev) for name, f in kinds.items()}
+        else:
+            out, first = {}, None
+            for name, is_float in kinds.items():
+                values, _, e = t._convert(name, is_float)
+                out[name] = values
+                if e is not None and (first is None or e.row < first.row):
+                    first = e
+            if first is not None:
+                raise first
+        if err is not None:
+            raise err
+        return out
 
     def IndexOn(self, *columns) -> Index:  # csvplus.go:529-531
         return self._index(columns, False)

@@ -783,6 +783,39 @@ int cpb_table_to_json_device(cpb_ctx* h, const cpb_table* t, int first_batch, in
     return to_json_common(h, t, first_batch, last_batch, 2, bytes, nullptr, 0, nbytes, err);
 }
 
+// ------------------------------------------------------------------ numeric columns
+// Row.ValueAsInt / ValueAsFloat64 (csvplus.go:163-205) of every row; the error is the first failing row's
+static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, bool is_float, void* values, uint8_t* status,
+                            uint64_t* nbad, cpb_error* err) {
+    if (!h || !t || !nbad || (!values && t->t->nrows > 0)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    *nbad = 0;
+    CPB_TRY(c, err)
+    const std::string name = to_string(column);
+    const int k = t->t->find(name);
+    if (t->t->nrows == 0) return CPB_OK;
+    if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // :170, :192
+    NumResult r = column_as_number(c, *t->t, k, is_float, values, status);
+    *nbad = r.nbad;
+    if (r.nbad) {
+        const bool range = r.first_status == CPB_NUM_RANGE;
+        throw DataError{range ? CPB_E_NUM_RANGE : CPB_E_NUM_SYNTAX, -1, r.first_row, false,
+                        "column " + go_quote(name) + ": cannot convert " + go_quote(r.first_value) + (is_float ? " to float: " : " to integer: ") +
+                            (range ? "value out of range" : "invalid syntax")};  // :176, :198
+    }
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_table_column_as_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, int64_t* values, uint8_t* status, uint64_t* nbad,
+                              cpb_error* err) {
+    return column_as_common(h, t, column, false, values, status, nbad, err);
+}
+int cpb_table_column_as_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, double* values, uint8_t* status, uint64_t* nbad,
+                                cpb_error* err) {
+    return column_as_common(h, t, column, true, values, status, nbad, err);
+}
+
 // ------------------------------------------------------------------ stats
 int cpb_stats_enable(cpb_ctx* h, int on) { DeviceGuard g(&h->c); h->c.stats_on = on != 0; return CPB_OK; }
 int cpb_stats_reset(cpb_ctx* h) {

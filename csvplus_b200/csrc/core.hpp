@@ -276,6 +276,14 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
                  uint64_t* nbytes, uint64_t* header_bytes);
 // json.cu: ToJSON of every column (keys in bytewise order); '[' before the first row when first, ']' appended when last
 Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbytes);
+// numeric.cu: strconv.Atoi / ParseFloat(s, 64) of every row of column `col` into device values (+ nullable status)
+struct NumResult {
+    uint64_t nbad = 0, nrare = 0;  // failing rows, rows the exact (rare) path converted
+    uint64_t first_row = 0;        // lowest failing row, its status and (up to 480 of) its bytes
+    int first_status = 0;
+    std::string first_value;
+};
+NumResult column_as_number(Ctx* c, const Table& t, int col, bool is_float, void* values, uint8_t* status);
 
 }  // namespace cpb
 

@@ -137,7 +137,26 @@ public:
         if (cpb_table_from_host(detail::ctx(), (int)cols.size(), names.v.data(), op.data(), dp.data(), (int64_t)rows.size(), &h) != CPB_OK) throw Error("from_host failed");
         return Table(h);
     }
+    // Row.ValueAsInt / ValueAsFloat64 (csvplus.go:163-205: strconv.Atoi / ParseFloat(s, 64)) of every row of a column,
+    // converted on the GPU into caller-owned device memory: values[size()] (Go's value on error too), status[size()]
+    // nullable (CPB_NUM_OK / _SYNTAX / _RANGE).  Returns the failing rows; strict: the first one throws Error with the
+    // reference's text, as a RowFunc returning the helper's error.  An absent column throws in both modes.
+    uint64_t ValuesAsInt(const std::string& column, int64_t* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
+        return convert(column, false, dev_values, dev_status, strict);
+    }
+    uint64_t ValuesAsFloat64(const std::string& column, double* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
+        return convert(column, true, dev_values, dev_status, strict);
+    }
 private:
+    uint64_t convert(const std::string& column, bool is_float, void* values, uint8_t* status, bool strict) const {
+        cpb_error e{}; uint64_t nbad = 0;
+        const cpb_str c{column.data(), column.size()};
+        const int st = is_float ? cpb_table_column_as_float64(detail::ctx(), h_.get(), c, (double*)values, status, &nbad, &e)
+                                : cpb_table_column_as_int64(detail::ctx(), h_.get(), c, (int64_t*)values, status, &nbad, &e);
+        if (st == CPB_ERR_DATA && (strict || e.kind == CPB_E_MISSING_COLUMN)) throw Error(e.msg);
+        if (st != CPB_OK && st != CPB_ERR_DATA) throw Error(e.msg[0] ? e.msg : cpb_last_error(detail::ctx()));
+        return nbad;
+    }
     std::shared_ptr<cpb_table> h_;
 };
 
@@ -247,6 +266,9 @@ public:
     // sinks
     void operator()(const RowFunc& fn) const { std::unique_ptr<DataSourceError> err; Table t = run(&err); for (auto& r : t.rows()) fn(r); if (err) throw *err; }
     std::vector<Row> ToRows() const { std::vector<Row> out; (*this)([&](const Row& r) { out.push_back(r); }); return out; }
+    // the plan's rows as a device table (an extension beyond the reference API, like TakeTable): the input of
+    // Table::ValuesAsInt / ValuesAsFloat64.  A source error is thrown.
+    Table ToTable() const { std::unique_ptr<DataSourceError> err; Table t = run(&err); if (err) throw *err; return t; }
     void ToCsv(std::ostream& out, const std::vector<std::string>& columns) const {
         if (columns.empty()) throw std::logic_error("empty column list in ToCsv() function");
         std::unique_ptr<DataSourceError> err; Table t = run(&err);

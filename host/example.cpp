@@ -1,6 +1,7 @@
 // example.cpp — the reference's README / test scenarios through the C++ host mirror (host/csvplus.hpp).
 // Mirrors TestSimpleDataSource (csvplus_test.go:118-151), TestSimpleUniqueJoin (:368-452), TestErrors (:808-909),
-// TestWriteFile (:172-196) and TestJSONStruct (:1016-1048) on fixtures generated like csvplus_test.go:1207-1333.
+// TestWriteFile (:172-196), TestJSONStruct (:1016-1048) and TestSimpleTotals (:516-571) on fixtures generated like
+// csvplus_test.go:1207-1333.
 // Exit code 0 = all checks hold.
 #include <cstdio>
 #include <cstdlib>
@@ -58,6 +59,35 @@ int main() {
                     << "\",\"surname\":\"" << surnames[j] << "\"}\n";
         want_js << ']';
         CHECK(js.str() == want_js.str());
+        // TestSimpleTotals (csvplus_test.go:516): orders x products, cust_id / qty / price converted on the GPU
+        std::string stock = "prod_id,product,price\n";
+        const double prices[8] = {1.25, 10.5, 3.75, 99.99, 0.5, 12.5, 7.3, 100.01};
+        for (int i = 0; i < 8; i++) { char b[64]; snprintf(b, sizeof b, "%d,item%d,%g\n", i, i, prices[i]); stock += b; }
+        auto prod = Take(FromString(stock).SelectColumns({"prod_id", "price"})).UniqueIndexOn({"prod_id"});
+        Table jt = Take(FromString(orders).SelectColumns({"cust_id", "prod_id", "qty"})).Join(prod).ToTable();
+        const int64_t jn = jt.size();
+        CHECK(jn == 10000);
+        void *d_id = nullptr, *d_qty = nullptr, *d_price = nullptr;
+        CHECK(cpb_device_alloc(detail::ctx(), jn * 8, &d_id) == CPB_OK && cpb_device_alloc(detail::ctx(), jn * 8, &d_qty) == CPB_OK &&
+              cpb_device_alloc(detail::ctx(), jn * 8, &d_price) == CPB_OK);
+        CHECK(jt.ValuesAsInt("cust_id", (int64_t*)d_id) == 0);
+        CHECK(jt.ValuesAsInt("qty", (int64_t*)d_qty) == 0);
+        CHECK(jt.ValuesAsFloat64("price", (double*)d_price) == 0);
+        std::vector<int64_t> hid(jn), hqty(jn); std::vector<double> hprice(jn);
+        CHECK(cpb_memcpy_d2h(detail::ctx(), hid.data(), d_id, jn * 8) == CPB_OK && cpb_memcpy_d2h(detail::ctx(), hqty.data(), d_qty, jn * 8) == CPB_OK &&
+              cpb_memcpy_d2h(detail::ctx(), hprice.data(), d_price, jn * 8) == CPB_OK);
+        std::vector<double> totals(120, 0), want_totals(120, 0);
+        for (int64_t i = 0; i < jn; i++) { CHECK(hid[i] >= 0 && hid[i] < 120); totals[hid[i]] = hprice[i] * (double)hqty[i]; }
+        for (int i = 0; i < 10000; i++) want_totals[cust[i]] = prices[i % 8] * (double)qty[i];
+        CHECK(totals == want_totals);
+        // a failing row: the reference's text, strict and not
+        try { jt.ValuesAsInt("price", (int64_t*)d_id); CHECK(false); }
+        catch (const Error& e) { CHECK(std::string(e.what()).find("column \"price\": cannot convert \"") == 0 &&
+                                       std::string(e.what()).find("\" to integer: invalid syntax") != std::string::npos); }
+        CHECK(jt.ValuesAsInt("price", (int64_t*)d_id, nullptr, false) == 10000);
+        try { jt.ValuesAsFloat64("xxx", (double*)d_price); CHECK(false); }
+        catch (const Error& e) { CHECK(std::string(e.what()) == "missing column \"xxx\""); }
+        cpb_device_free(detail::ctx(), d_id); cpb_device_free(detail::ctx(), d_qty); cpb_device_free(detail::ctx(), d_price);
         // TestErrors
         try { Take(FromString(people).SelectColumns({"id", "name", "xxx"})).ToRows(); CHECK(false); }
         catch (const DataSourceError& e) { CHECK(std::string(e.what()) == "row 1: column not found: xxx"); }

@@ -65,7 +65,9 @@ typedef enum cpb_err_kind {
     CPB_E_DUPLICATE_KEY = 12,   /* csvplus.go:751 */
     CPB_E_TOO_LARGE = 13,       /* a column/batch exceeds the 4 GiB-per-column batch limit (DESIGN.md) */
     CPB_E_CUDA = 14,
-    CPB_E_UNSUPPORTED = 15
+    CPB_E_UNSUPPORTED = 15,
+    CPB_E_NUM_SYNTAX = 16,      /* csvplus.go:176/:198  cannot convert %q to integer|float: invalid syntax */
+    CPB_E_NUM_RANGE = 17        /* csvplus.go:176/:198  ...: value out of range */
 } cpb_err_kind;
 
 typedef struct cpb_error {
@@ -245,6 +247,20 @@ int cpb_table_to_json_device(cpb_ctx* ctx, const cpb_table* t, int first_batch, 
 /* into caller-owned (pinned) host memory; cap too small: CPB_ERR_ARG with *nbytes = the size needed, nothing written */
 int cpb_table_to_json_into(cpb_ctx* ctx, const cpb_table* t, int first_batch, int last_batch, void* host_dst, uint64_t cap,
                            uint64_t* nbytes, cpb_error* err);
+
+/* ------------------------------------------------------------------ numeric columns
+ * Row.ValueAsInt / Row.ValueAsFloat64 (csvplus.go:163-205: strconv.Atoi / strconv.ParseFloat(s, 64), Go 1.23) of every
+ * row of one column, into caller-owned device memory, stream-ordered on the ctx stream; returns after one host
+ * synchronisation.  values[nrows] is always written (Go's value on error too: 0 for a syntax error, the clamped integer
+ * or +-Inf for a range error); status[nrows] is nullable (CPB_NUM_*); *nbad = failing rows.
+ * nbad > 0: CPB_ERR_DATA, kind CPB_E_NUM_SYNTAX / CPB_E_NUM_RANGE of the first failing row, err->line = that row
+ * (0-based), has_line = 0, msg = the reference's text.  An absent column on a non-empty table: CPB_ERR_DATA,
+ * CPB_E_MISSING_COLUMN, line 0, has_line = 0.  A float column converts at most 2^32 - 1 rows per call. */
+enum { CPB_NUM_OK = 0, CPB_NUM_SYNTAX = 1, CPB_NUM_RANGE = 2 };
+int cpb_table_column_as_int64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, int64_t* values, uint8_t* status,
+                              uint64_t* nbad, cpb_error* err);
+int cpb_table_column_as_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, double* values, uint8_t* status,
+                                uint64_t* nbad, cpb_error* err);
 
 /* ------------------------------------------------------------------ multi-GPU (SURVEY §8e)
  * The probe stream shards by row range with no data-path collective; the one exchange step is the all-gather of the
