@@ -7,8 +7,9 @@ library or a GPU is missing.
 """
 from .api import (All, Any, Context, CsvPlusError, DataSource, DataSourceError, DeviceBuffer, FromBytes, FromFile,  # noqa: F401
                   FromReadCloser, FromReader, HostBuffer, Index, Like, Not, Predicate, Reader, Row, StopIterationEOF, Table,
-                  Take, TakeRows, TakeTable, csv_quote_parity, parse_csv, parse_csv_shard)
+                  Take, TakeRows, TakeTable, csv_quote_parity, csv_stream_cut, parse_csv, parse_csv_shard)
 
 __all__ = ["All", "Any", "Context", "CsvPlusError", "DataSource", "DataSourceError", "DeviceBuffer", "FromBytes", "FromFile",
            "FromReadCloser", "FromReader", "HostBuffer", "Index", "Like", "Not", "Predicate", "Reader", "Row",
-           "StopIterationEOF", "Table", "Take", "TakeRows", "TakeTable", "csv_quote_parity", "parse_csv", "parse_csv_shard"]
+           "StopIterationEOF", "Table", "Take", "TakeRows", "TakeTable", "csv_quote_parity", "csv_stream_cut", "parse_csv",
+           "parse_csv_shard"]

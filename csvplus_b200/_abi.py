@@ -42,9 +42,10 @@ class KStat(C.Structure):
 
 # every symbol include/csvplus_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [
-    "cpb_abi_version", "cpb_init", "cpb_shutdown", "cpb_ctx_stream", "cpb_sync", "cpb_pool_reserve", "cpb_last_error",
+    "cpb_abi_version", "cpb_init", "cpb_shutdown", "cpb_ctx_stream", "cpb_sync", "cpb_pool_reserve", "cpb_pool_used_high", "cpb_last_error",
     "cpb_host_alloc", "cpb_host_free", "cpb_device_alloc", "cpb_device_free", "cpb_memcpy_h2d", "cpb_memcpy_d2h",
-    "cpb_parse_csv", "cpb_csv_quote_parity", "cpb_parse_csv_shard", "cpb_table_col_field", "cpb_table_record_fields",
+    "cpb_parse_csv", "cpb_stream_open", "cpb_stream_push", "cpb_stream_next", "cpb_stream_free", "cpb_csv_stream_cut",
+    "cpb_csv_quote_parity", "cpb_parse_csv_shard", "cpb_table_col_field", "cpb_table_record_fields",
     "cpb_table_num_rows", "cpb_table_num_cols", "cpb_table_col_name", "cpb_table_find_col", "cpb_table_col_bytes",
     "cpb_table_fetch_column", "cpb_table_column_device", "cpb_table_from_host", "cpb_table_from_device",
     "cpb_table_concat", "cpb_table_select", "cpb_table_drop", "cpb_table_filter", "cpb_table_first_false", "cpb_table_slice",
@@ -80,6 +81,7 @@ def load():
         "cpb_sync": (i32, [vp]),
         "cpb_pool_reserve": (i32, [vp, u64]),
         "cpb_last_error": (C.c_char_p, [vp]),
+        "cpb_pool_used_high": (i32, [vp, i32, P(u64)]),
         "cpb_host_alloc": (i32, [vp, u64, P(vp)]),
         "cpb_host_free": (i32, [vp, vp]),
         "cpb_device_alloc": (i32, [vp, u64, P(vp)]),
@@ -87,6 +89,11 @@ def load():
         "cpb_memcpy_h2d": (i32, [vp, vp, vp, u64]),
         "cpb_memcpy_d2h": (i32, [vp, vp, vp, u64]),
         "cpb_parse_csv": (i32, [vp, vp, u64, i32, P(ReaderOpts), P(HeaderCol), i32, P(Pred), P(vp), P(Error)]),
+        "cpb_stream_open": (i32, [vp, P(ReaderOpts), P(HeaderCol), i32, P(Pred), P(vp), P(Error)]),
+        "cpb_stream_push": (i32, [vp, vp, u64, i32]),
+        "cpb_stream_next": (i32, [vp, P(vp), P(i32), P(Error)]),
+        "cpb_stream_free": (None, [vp]),
+        "cpb_csv_stream_cut": (i32, [vp, vp, u64, i32, P(ReaderOpts), P(u64)]),
         "cpb_table_col_field": (i32, [vp, i32]),
         "cpb_table_record_fields": (i32, [vp]),
         "cpb_csv_quote_parity": (i32, [vp, vp, u64, i32, P(C.c_uint32)]),

@@ -26,6 +26,11 @@ Row = dict  # map[string]string, csvplus.go:59 (values are str; bytes survive vi
 # rows per cpb_table_to_json_into call when DataSource.ToJSON writes a device table: one call produces < 4 GiB, and
 # about 2.4 GB for joined rows of ~150 B.  A batch that is still too large is split in halves.
 JSON_BATCH_ROWS = 1 << 24
+# bytes per host push of a streamed input (FromFile / FromReader / host FromBytes, cpb_stream_*): one batch is parsed per
+# push, so every column of a batch stays far below the 4 GiB a column of one table may hold.  An input of at most this
+# size is parsed in one cpb_parse_csv call.  128 MiB: on an H100 the streamed orders join of DESIGN §3.7 ran as fast as
+# at 64 MiB with half the host synchronisations, and slower with larger batches (less copy / compute overlap).
+STREAM_BATCH_BYTES = 128 << 20
 
 
 def _enc(s) -> bytes:
@@ -143,6 +148,15 @@ class Context:
     def reserve(self, nbytes: int) -> bool:
         """cpb_pool_reserve: map `nbytes` of device memory into this context's pool ahead of time (False: not available)"""
         return self.lib.cpb_pool_reserve(self.h, int(nbytes)) == 0
+
+    def pool_used_high(self, reset: bool = False) -> int:
+        """cpb_pool_used_high: the most device memory this context's pool has had allocated at once since the last reset
+        (reset=True starts a new window at the current use)"""
+        out = C.c_uint64()
+        st = self.lib.cpb_pool_used_high(self.h, int(reset), C.byref(out))
+        if st:
+            _raise(st, None, self)
+        return out.value
 
     @property
     def stream(self) -> int:
@@ -631,6 +645,19 @@ def csv_quote_parity(ctx: Context, data, *, nbytes=None, on_device=False) -> int
     return out.value
 
 
+def csv_stream_cut(ctx: Context, data, *, nbytes=None, on_device=False, delimiter=",", comment="", lazy_quotes=False,
+                   trim_leading_space=False) -> int:
+    """cpb_csv_stream_cut: the end of the last complete record of data (0: none), the cut of one stream batch"""
+    opts = _abi.ReaderOpts(ord(delimiter), ord(comment) if comment else 0, 0, int(lazy_quotes), int(trim_leading_space), 1, 0)
+    keep = []
+    ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
+    out = C.c_uint64()
+    st = ctx.lib.cpb_csv_stream_cut(ctx.h, C.c_void_p(ptr), n, int(dev), C.byref(opts), C.byref(out))
+    if st:
+        _raise(st, None, ctx)
+    return out.value
+
+
 def parse_csv_shard(ctx: Context, data, *, own_bytes: int, shard_index: int, is_last: bool, initial_parity: int, nbytes=None, on_device=False,
                     delimiter=",", num_fields=0, header_from_first_row=True, spec: list | None = None, pred: Predicate | None = None):
     """cpb_parse_csv_shard.  Returns (Table, records owned by the shard, DataSourceError | None) — the error's Line is the
@@ -749,8 +776,12 @@ class Index:
 
 # ------------------------------------------------------------------ Reader (csvplus.go:922-1146)
 class Reader:
-    def __init__(self, source: Callable[[], bytes | np.ndarray | DeviceBuffer | HostBuffer], ctx: Context | None = None):
-        self._source, self._ctx = source, ctx
+    def __init__(self, source: Callable[[], bytes | np.ndarray | DeviceBuffer | HostBuffer], ctx: Context | None = None,
+                 chunks: Callable[[], Iterable] | None = None):
+        """source: the whole input for one cpb_parse_csv call.  chunks: when given, -> None if the input fits one batch
+        (then `source` is parsed), else an iterator of (host piece as numpy uint8, is the last piece), each piece left
+        untouched until the next one is asked for."""
+        self._source, self._ctx, self._chunks = source, ctx, chunks
         self.delimiter, self.comment = ",", ""
         self.numFields, self.lazyQuotes, self.trimLeadingSpace = 0, False, False
         self.header: dict | None = None
@@ -803,8 +834,187 @@ class Reader:
                          lazy_quotes=self.lazyQuotes, trim_leading_space=self.trimLeadingSpace,
                          header_from_first_row=self.headerFromFirstRow, spec=spec, pred=pred)
 
+    def _batches(self, pred: Predicate | None = None):
+        """-> (Table, DataSourceError | None, streamed) per batch; the error comes with the last batch.  An input that fits
+        one batch is one cpb_parse_csv call (streamed = False); a larger one goes through cpb_stream_*.  Closing the
+        generator early stops reading the input."""
+        pieces = self._chunks() if self._chunks is not None else None
+        if pieces is None:
+            t, err = self._parse(pred)
+            yield t, err, False
+            return
+        st = _Stream(self.ctx, self, pred)
+        try:
+            # one cpb_stream_next per push parses every complete record pushed so far.  A batch is delivered after the
+            # next piece has been pushed: that piece's host-to-device copy (the stream's copy stream) overlaps what the
+            # consumer does with the batch on the context's stream, and it is parsed only after the batch was delivered.
+            pending, finished = None, False
+            for piece, last in pieces:
+                st.push(piece, last)
+                if pending is not None:
+                    yield pending
+                    pending = None
+                t, err, done = st.next()
+                if t is not None or err is not None:
+                    pending = (t, err, True)
+                if done or err is not None:
+                    finished = True
+                    break
+            if not finished:
+                st.push(None, True)
+                if pending is not None:
+                    yield pending
+                    pending = None
+                t, err, done = st.next()
+                if t is not None or err is not None:
+                    pending = (t, err, True)
+            if pending is not None:
+                yield pending
+        finally:
+            st.free()
+            close = getattr(pieces, "close", None)
+            if close is not None:
+                close()
+
     def Iterate(self, fn):  # csvplus.go:1080
         return Take(self)(fn)
+
+
+class _Stream:
+    """cpb_stream: one input parsed in batches of whole records"""
+
+    def __init__(self, ctx: Context, r: Reader, pred: Predicate | None):
+        self.ctx, self._keep, self._pushed = ctx, [], None
+        opts = _abi.ReaderOpts(ord(r.delimiter), ord(r.comment) if r.comment else 0, r.numFields, int(r.lazyQuotes),
+                               int(r.trimLeadingSpace), int(r.headerFromFirstRow), 0)
+        spec = list(r.header.items()) if r.header else []
+        sa = (_abi.HeaderCol * max(1, len(spec)))()
+        for i, (name, idx) in enumerate(spec):
+            nb = _enc(name); self._keep.append(nb)
+            sa[i].name.ptr, sa[i].name.len, sa[i].index = nb, len(nb), idx
+        pp = None
+        if pred is not None:
+            pc = pred._c(self._keep); self._keep.append(pc); pp = C.byref(pc)  # borrowed by the stream until it is freed
+        self._keep += [opts, sa]
+        h = C.c_void_p(); e = _abi.Error()
+        st = ctx.lib.cpb_stream_open(ctx.h, C.byref(opts), sa, len(spec), pp, C.byref(h), C.byref(e))
+        if st:
+            _raise(st, e, ctx)
+        self.h = h
+
+    def push(self, piece, last: bool):
+        if piece is None:
+            ptr, n = None, 0
+        else:
+            a = piece if isinstance(piece, np.ndarray) else np.frombuffer(piece, np.uint8)
+            ptr, n = a.ctypes.data, a.size
+        self._pushed = piece  # untouched until the next cpb_stream_next returns
+        st = self.ctx.lib.cpb_stream_push(self.h, C.c_void_p(ptr), n, int(last))
+        if st:
+            _raise(st, None, self.ctx)
+
+    def next(self):
+        h = C.c_void_p(); done = C.c_int(); e = _abi.Error()
+        st = self.ctx.lib.cpb_stream_next(self.h, C.byref(h), C.byref(done), C.byref(e))
+        t = Table(self.ctx, h) if h.value else None
+        if st == 1 and t is not None:
+            return t, DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind), True
+        if st:
+            _raise(st, e, self.ctx)
+        return t, None, bool(done.value)
+
+    def free(self):
+        if self.h:
+            self.ctx.lib.cpb_stream_free(self.h)
+            self.h = None
+
+
+def _file_pieces(name: str, ctx_of: Callable[[], Context]):
+    """None when the file fits one batch (or is not a regular file: read whole, as before); else a generator of the file's
+    pieces, read by a helper thread into two pinned host buffers: piece k+1 is read while piece k is being parsed"""
+    try:
+        size = os.stat(name).st_size
+        regular = os.path.isfile(name)
+    except OSError:
+        return None  # the open error is raised by the one-shot source
+    if not regular or size <= STREAM_BATCH_BYTES:
+        return None
+    return _pinned_pieces(name, ctx_of())
+
+
+def _pinned_pieces(name: str, ctx: Context):
+    from concurrent.futures import ThreadPoolExecutor
+    step = STREAM_BATCH_BYTES
+    bufs = [HostBuffer(ctx, step), HostBuffer(ctx, step)]
+    views = [b.array() for b in bufs]
+    ex = ThreadPoolExecutor(1)
+    try:
+        with open(name, "rb", buffering=0) as f:
+            def fill(k):
+                n, v = 0, memoryview(views[k])
+                while n < step:
+                    got = f.readinto(v[n:])
+                    if not got:
+                        break
+                    n += got
+                return n
+            k = 0
+            fut = ex.submit(fill, 0)
+            while True:
+                n = fut.result()
+                if n == 0:
+                    return
+                # the other buffer held the piece before this one: its parse has returned by now
+                fut = ex.submit(fill, k ^ 1) if n == step else None
+                yield views[k][:n], fut is None
+                if fut is None:
+                    return
+                k ^= 1
+    finally:
+        ex.shutdown(wait=True)
+        for b in bufs:
+            b.free()
+
+
+def _reader_pieces(inp):
+    """pieces of an io reader, read with readinto (or read(n)); None (and the bytes as the one-shot input) when the
+    first piece is the whole input"""
+    step = STREAM_BATCH_BYTES
+
+    def read_piece():
+        a = np.empty(step, np.uint8)
+        n = 0
+        if hasattr(inp, "readinto"):
+            v = memoryview(a)
+            while n < step:
+                got = inp.readinto(v[n:])
+                if not got:
+                    break
+                n += got
+        else:
+            while n < step:
+                b = inp.read(step - n)
+                if not b:
+                    break
+                a[n:n + len(b)] = np.frombuffer(b, np.uint8); n += len(b)
+        return a[:n]
+
+    first = read_piece()
+    if first.size < step:
+        return first, None
+    second = read_piece()
+    if second.size == 0:
+        return first, None
+
+    def gen():
+        yield first, False
+        yield second, False
+        while True:
+            p = read_piece()
+            if p.size == 0:
+                return  # the stream is closed by an empty last push
+            yield p, False
+    return None, gen()
 
 
 def FromFile(name: str, ctx: Context | None = None) -> Reader:  # csvplus.go:950
@@ -813,19 +1023,40 @@ def FromFile(name: str, ctx: Context | None = None) -> Reader:  # csvplus.go:950
             return np.fromfile(name, dtype=np.uint8)
         except OSError as e:  # mapError's *os.PathError branch, csvplus.go:1216-1220
             raise DataSourceError(1, f"open: {e.strerror.lower() if e.strerror else e}") from None
-    return Reader(src, ctx)
+    r = Reader(src, ctx)
+    r._chunks = lambda: _file_pieces(name, lambda: r.ctx)
+    return r
 
 
 def FromReader(inp: io.IOBase, ctx: Context | None = None) -> Reader:  # csvplus.go:936
-    return Reader(lambda: inp.read(), ctx)
+    whole = []
+
+    def chunks():
+        first, gen = _reader_pieces(inp)
+        whole[:] = [first]
+        return gen
+    return Reader(lambda: whole.pop() if whole else inp.read(), ctx, chunks)
 
 
 FromReadCloser = FromReader
 
 
 def FromBytes(data, ctx: Context | None = None) -> Reader:
-    """bytes / numpy / HostBuffer / DeviceBuffer already in memory"""
-    return Reader(lambda: data, ctx)
+    """bytes / numpy / HostBuffer / DeviceBuffer already in memory.  Host memory larger than STREAM_BATCH_BYTES is parsed
+    in batches (cpb_stream_*); a DeviceBuffer is always parsed in one call."""
+    def chunks():
+        if isinstance(data, DeviceBuffer):
+            return None
+        if isinstance(data, HostBuffer):
+            a = data.array()
+        elif isinstance(data, np.ndarray):
+            a = np.ascontiguousarray(data, np.uint8).reshape(-1)
+        else:
+            a = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.frombuffer(bytes(data), np.uint8)
+        if a.size <= STREAM_BATCH_BYTES:
+            return None
+        return ((a[i:i + STREAM_BATCH_BYTES], i + STREAM_BATCH_BYTES >= a.size) for i in range(0, a.size, STREAM_BATCH_BYTES))
+    return Reader(lambda: data, ctx, chunks)
 
 
 # ------------------------------------------------------------------ DataSource (csvplus.go:207-608)
@@ -877,23 +1108,40 @@ class DataSource:
             return s[1].ctx
         return Context.default()
 
-    def _evaluate(self):
-        """-> (state, pending error).  state: ("table", Table) or ("rows", list[Row])."""
+    def _batches(self):
+        """-> (state, pending error, streamed) per batch of the source; state: ("table", Table | None) or ("rows", list[Row]).
+        A Reader over a large host input yields one batch per parsed batch (streamed = True), every other source one.
+        Top / Drop / TakeWhile / DropWhile carry their counters across batches; when one of them has pulled all it will
+        ever deliver, the input is no longer read."""
         ops = list(self._ops)
-        err = None
         s = self._src
+        carry: dict = {}
         if isinstance(s, Reader):
             pred = None
             if ops and ops[0][0] == "filter" and isinstance(ops[0][1], Predicate) and ops[0][1].lowerable():
                 pred = ops.pop(0)[1]  # fused into the parse kernel
-            t, err = s._parse(pred)
-            state = ("table", t)
-        elif s[0] == "table":
+            src = s._batches(pred)
+            try:
+                for t, err, streamed in src:
+                    state, err, stop = self._apply(("table", t), err, ops, carry)
+                    yield state, err, streamed
+                    if stop or err is not None:
+                        return
+            finally:
+                src.close()
+            return
+        if s[0] == "table":
             state = ("table", s[1])
         else:
             state = ("rows", [dict(r) for r in s[1]])  # iterate() clones, csvplus.go:230
+        state, err, _ = self._apply(state, None, ops, carry)
+        yield state, err, False
+
+    def _apply(self, state, err, ops, carry: dict):
+        """the operations over one batch -> (state, err, stop); carry: per-operation state across batches"""
         ctx = self._ctx()
-        for op in ops:
+        stop = False
+        for i, op in enumerate(ops):
             kind = op[0]
             device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop")
                          or (kind in ("filter", "takewhile", "dropwhile") and isinstance(op[1], Predicate) and op[1].lowerable()))
@@ -909,26 +1157,38 @@ class DataSource:
                     elif kind == "filter": t = t.filter(op[1])
                     elif kind == "join": t = t.join(op[1], *op[2])
                     elif kind == "except": t = t.join(op[1], *op[2], anti=True)
-                    elif kind == "top": t = t.slice(0, op[1])  # note: the reference pulls one extra row (SURVEY §Q8)
-                    elif kind == "drop": t = t.slice(op[1], len(t))
+                    elif kind == "top":  # note: the reference pulls one extra row (SURVEY §Q8)
+                        seen = carry.get(i, 0)
+                        t = t.slice(0, min(len(t), max(0, op[1] - seen)))
+                    elif kind == "drop":
+                        seen = carry.get(i, 0)
+                        t = t.slice(min(len(t), max(0, op[1] - seen)), len(t))
+                        carry[i] = seen + len(state[1])
                     elif kind == "takewhile":  # csvplus.go:346-358: io.EOF at the first failing row — a later error is never met
                         cut = t.first_false(op[1])
                         if cut < len(t):
-                            err = None
+                            err = None; stop = True
                         t = t.slice(0, cut)
-                    elif kind == "dropwhile": t = t.slice(t.first_false(op[1]), len(t))  # :361-374
+                    elif kind == "dropwhile":  # :361-374
+                        if carry.get(i, True):
+                            k = t.first_false(op[1])
+                            if k < len(t):
+                                carry[i] = False
+                            t = t.slice(k, len(t))
                 except DataSourceError as e:
                     if err is None or kind in ("select", "join", "except"):
-                        return ("rows", []), e
+                        return ("rows", []), e, True
                     raise
-                if kind == "top" and err is not None and len(state[1]) > op[1]:
-                    err = None  # Top(n) pulls n+1 rows then stops (io.EOF): the failing record is never reached
+                if kind == "top":
+                    carry[i] = carry.get(i, 0) + len(state[1])
+                    if carry[i] > op[1]:  # Top(n) pulls n+1 rows then stops (io.EOF): the failing record is never reached
+                        err = None; stop = True
                 state = ("table", t)
             else:
                 rows = state[1].rows() if state[0] == "table" and state[1] is not None else (state[1] or [])
-                out, stop = [], False
+                out = []
                 fn = op[1]
-                dropping = True
+                dropping = carry.get(i, True)
                 for r in rows:
                     if kind == "filter":
                         if fn(r): out.append(r)
@@ -947,26 +1207,39 @@ class DataSource:
                     elif kind == "dropwhile":
                         dropping = dropping and fn(r)
                         if not dropping: out.append(r)
+                carry[i] = dropping
                 state = ("rows", out)
-        return state, err
+        return state, err, stop
+
+    def _evaluate(self):
+        """-> (state, pending error) of the whole plan: the batches' tables concatenated"""
+        parts, err = [], None
+        for state, err, _ in self._batches():
+            parts.append(state)
+        if len(parts) == 1:
+            return parts[0], err
+        t = _concat([self._as_table(st) for st in parts])
+        return ("table", t), err
+
+    def _as_table(self, state):
+        if state[0] == "rows":
+            return Table.from_rows(self._ctx(), state[1]) if state[1] else None
+        return state[1]
 
     def _table(self) -> tuple:
         state, err = self._evaluate()
-        if state[0] == "rows":
-            t = Table.from_rows(self._ctx(), state[1]) if state[1] else None
-            return t, err
-        return state[1], err
+        return self._as_table(state), err
 
     def __call__(self, fn: Callable[[Row], None]):
-        state, err = self._evaluate()
-        rows = state[1].rows() if state[0] == "table" and state[1] is not None else (state[1] or [])
-        for r in rows:
-            try:
-                fn(r)
-            except StopIterationEOF:
-                return
-        if err is not None:
-            raise err
+        for state, err, _ in self._batches():  # each batch is delivered before the next one is parsed
+            rows = state[1].rows() if state[0] == "table" and state[1] is not None else (state[1] or [])
+            for r in rows:
+                try:
+                    fn(r)
+                except StopIterationEOF:
+                    return
+            if err is not None:
+                raise err
 
     # ---- sinks
     def ToRows(self) -> list[Row]:  # csvplus.go:483-490
@@ -977,13 +1250,24 @@ class DataSource:
     def ToCsv(self, out: io.IOBase, *columns):  # csvplus.go:379-406
         if len(columns) == 0:
             raise ValueError("empty column list in ToCsv() function")
-        t, err = self._table()
-        if t is None:
-            out.write((",".join(columns) + "\n").encode())
-        else:
-            out.write(t.to_csv(*columns))
-        if err is not None:
-            raise err
+        wrote_header = False
+        hold: list = []  # the pinned buffer the batches of a streamed input are serialised into
+        try:
+            for state, err, streamed in self._batches():
+                t = self._as_table(state)
+                if t is None:
+                    if not wrote_header:
+                        out.write((",".join(columns) + "\n").encode())
+                elif not streamed:
+                    out.write(t.to_csv(*columns))
+                else:  # the csv.Writer writes the header once, before the first batch (csvplus.go:387)
+                    _csv_into(t, out, columns, not wrote_header, hold)
+                wrote_header = True
+                if err is not None:
+                    raise err
+        finally:
+            for b in hold:
+                b.free()
 
     def ToCsvFile(self, name: str, *columns):  # csvplus.go:411-443: the file is removed on error
         try:
@@ -998,23 +1282,40 @@ class DataSource:
         """all rows as a JSON array, formatted the way the reference's json.Encoder (SetEscapeHTML(false), no indent) writes
         it: `[`, then per row the object with its keys sorted and a newline, a `,` before every row but the first, `]`.
         A device table is serialised by the GPU in row-range batches; rows left on the host (after an opaque Map or
-        Filter(func), or TakeRows of rows with different columns) are encoded here.  On a source error nothing is written."""
-        state, err = self._evaluate()
-        if err is not None:
-            raise err
-        if state[0] == "table":
-            if state[1] is None:
-                out.write(b"[]")
-            else:
-                _json_batches(state[1], out)
-            return
-        parts = [b"["]
-        for i, row in enumerate(state[1]):
-            if i:
-                parts.append(b",")
-            parts.append(b"{" + b",".join(_go_json_string(k) + b":" + _go_json_string(row[k]) for k in sorted(row, key=_enc)) + b"}\n")
-        parts.append(b"]")
-        out.write(b"".join(parts))
+        Filter(func), or TakeRows of rows with different columns) are encoded here.  On a source error nothing is written
+        when the input was parsed in one batch; a streamed input keeps what its earlier batches wrote (a prefix of the
+        array, without `]`), as the reference's encoder has flushed them."""
+        hold: list = []  # the pinned buffer the batches of a streamed input are serialised into
+        try:
+            self._to_json(out, hold)
+        finally:
+            for b in hold:
+                b.free()
+
+    def _to_json(self, out, hold: list):
+        opened = False
+        for state, err, streamed in self._batches():
+            if not streamed:  # one batch: the whole document at once
+                if err is not None:
+                    raise err
+                if state[0] == "table":
+                    if state[1] is None:
+                        out.write(b"[]")
+                    else:
+                        _json_batches(state[1], out)
+                    return
+                out.write(_json_rows(state[1], True, True))
+                return
+            if state[0] == "table":
+                if state[1] is not None and len(state[1]):
+                    _json_batches(state[1], out, first=not opened, last=False, hold=hold)
+                    opened = True
+            elif state[1]:
+                out.write(_json_rows(state[1], not opened, False))
+                opened = True
+            if err is not None:
+                raise err
+        out.write(b"]" if opened else b"[]")
 
     def ToJSONFile(self, name: str):  # csvplus.go:477-479
         try:
@@ -1073,17 +1374,59 @@ class DataSource:
         return t.index_on(*columns, unique=unique)
 
 
-def _json_batches(t: Table, out: io.IOBase):
+def _concat(tables: list) -> "Table | None":
+    """the batches' tables as one (cpb_table_concat); None when no batch has a table"""
+    parts = [t for t in tables if t is not None]
+    if not parts:
+        return None
+    return parts[0] if len(parts) == 1 else Table.concat(parts)
+
+
+def _json_rows(rows: list, first: bool, last: bool) -> bytes:
+    """host rows as (a piece of) the JSON array: `[` when first, `,` before every other row, `]` when last"""
+    parts = [b"["] if first else []
+    for i, row in enumerate(rows):
+        if i or not first:
+            parts.append(b",")
+        parts.append(b"{" + b",".join(_go_json_string(k) + b":" + _go_json_string(row[k]) for k in sorted(row, key=_enc)) + b"}\n")
+    if last:
+        parts.append(b"]")
+    return b"".join(parts)
+
+
+def _csv_into(t: Table, out: io.IOBase, columns, header: bool, hold: list):
+    """one batch of a streamed ToCsv: serialised into the pinned buffer hold[0] (grown to the size the batch reports and
+    kept for the next batch), then written to out"""
+    a, keep = _strs(columns)
+    while True:
+        buf = hold[0] if hold else None
+        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
+        n = C.c_uint64(); e = _abi.Error()
+        st = t.ctx.lib.cpb_table_to_csv_into(t.ctx.h, t.h, a, len(columns), int(header), C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
+        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
+            if buf is not None:
+                buf.free()
+            hold[:] = [HostBuffer(t.ctx, n.value + n.value // 4 + 64)]
+            continue
+        if st:
+            _raise(st, e, t.ctx)
+        if n.value:
+            out.write(memoryview(buf.array()[:n.value]))
+        return
+
+
+def _json_batches(t: Table, out: io.IOBase, first: bool = True, last: bool = True, hold: list | None = None):
     """ToJSON of a device table: row-range slices of at most JSON_BATCH_ROWS rows, each serialised into one reused pinned
-    buffer that grows to the size a batch reports, then written to out"""
+    buffer that grows to the size a batch reports, then written to out.  first / last: the table opens / closes the
+    array.  hold: a list that keeps the buffer for the next table (the caller frees it)."""
     n = len(t)
-    buf, lo, step = None, 0, JSON_BATCH_ROWS
+    buf, lo, step = (hold[0] if hold else None), 0, JSON_BATCH_ROWS
     try:
         while True:
             hi = min(n, lo + step)
             part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
             try:
-                w = part.to_json_into(buf, 0, lo == 0, hi == n)
+                w = part.to_json_into(buf, 0, first and lo == 0, last and hi == n)
             except CsvPlusError as e:
                 if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
                     raise
@@ -1093,13 +1436,15 @@ def _json_batches(t: Table, out: io.IOBase):
                 if buf is not None:
                     buf.free()
                 buf = HostBuffer(t.ctx, w + w // 4 + 64)
+                if hold is not None:
+                    hold[:] = [buf]
                 continue
             out.write(memoryview(buf.array()[:w]))
             lo = hi
             if lo >= n:
                 return
     finally:
-        if buf is not None:
+        if buf is not None and hold is None:
             buf.free()
 
 

@@ -234,6 +234,18 @@ int cpb_pool_reserve(cpb_ctx* h, uint64_t nbytes) {
     CPB_CATCH(c, nullptr)
 }
 
+int cpb_pool_used_high(cpb_ctx* h, int reset, uint64_t* bytes) {
+    if (!h || !bytes) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    CPB_TRY(c, nullptr)
+    uint64_t v = 0;  // the attribute is a cuuint64_t (64-bit unsigned)
+    if (reset) CPB_CUDA(cudaMemPoolSetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
+    CPB_CUDA(cudaMemPoolGetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
+    *bytes = (uint64_t)v;
+    return CPB_OK;
+    CPB_CATCH(c, nullptr)
+}
+
 int cpb_host_alloc(cpb_ctx* h, uint64_t n, void** out) {
     Ctx* c = &h->c; DeviceGuard g(c);
     CPB_TRY(c, nullptr)
@@ -314,6 +326,53 @@ int cpb_parse_csv(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device,
     CPB_CATCH(c, err)
 }
 
+// ------------------------------------------------------------------ streamed input (stream.cu)
+int cpb_stream_open(cpb_ctx* h, const cpb_reader_opts* opts, const cpb_header_col* spec, int nspec, const cpb_pred* filter,
+                    cpb_stream** out, cpb_error* err) {
+    if (!h || !out || !opts || nspec < 0) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    *out = nullptr;
+    CPB_TRY(c, err)
+    std::vector<std::pair<std::string, int>> sp;
+    for (int i = 0; i < nspec; i++) {
+        std::string nm = to_string(spec[i].name);
+        for (auto& s : sp) if (s.first == nm) throw ArgError{CPB_ERR_ARG, "header spec: duplicate column name: " + nm};  // csvplus.go:1047-1049
+        sp.emplace_back(nm, spec[i].index);
+    }
+    *out = new cpb_stream{stream_open(c, *opts, std::move(sp), filter)};
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_stream_push(cpb_stream* st, const void* bytes, uint64_t nbytes, int is_last) {
+    if (!st || (nbytes && !bytes)) return CPB_ERR_ARG;
+    Ctx* c = stream_ctx(st->s); DeviceGuard g(c);
+    CPB_TRY(c, nullptr)
+    stream_push(st->s, bytes, nbytes, is_last != 0);
+    return CPB_OK;
+    CPB_CATCH(c, nullptr)
+}
+int cpb_stream_next(cpb_stream* st, cpb_table** out, int* done, cpb_error* err) {
+    if (!st || !out || !done) return CPB_ERR_ARG;
+    Ctx* c = stream_ctx(st->s); DeviceGuard g(c);
+    clear_error(err);
+    *out = nullptr; *done = 0;
+    CPB_TRY(c, err)
+    bool had_error = false, fin = false; DataError de{};
+    auto t = stream_next(st->s, &had_error, &de, &fin);
+    *done = fin ? 1 : 0;
+    if (t) *out = wrap(t);
+    if (had_error) { fill_error(err, de.kind, de.column_index, de.line, de.has_line, de.msg); return CPB_ERR_DATA; }
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+void cpb_stream_free(cpb_stream* st) {
+    if (!st) return;
+    Ctx* c = stream_ctx(st->s); DeviceGuard g(c);
+    stream_free(st->s);
+    delete st;
+}
+
 // ------------------------------------------------------------------ byte-range shards of one file (SURVEY §8e)
 static const uint8_t* stage_input(Ctx* c, const void* bytes, uint64_t nbytes, int on_device, Buf& staged) {
     if (on_device) return (const uint8_t*)bytes;
@@ -333,6 +392,22 @@ int cpb_csv_quote_parity(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_
     const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
     if ((reinterpret_cast<uintptr_t>(dev) & 15) != 0) throw ArgError{CPB_ERR_ARG, "device input must be 16-byte aligned"};
     *parity = quote_parity(c, dev, nbytes);
+    return CPB_OK;
+    CPB_CATCH(c, nullptr)
+}
+int cpb_csv_stream_cut(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts, uint64_t* cut) {
+    if (!h || !cut || !opts || (nbytes && !bytes)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    CPB_TRY(c, nullptr)
+    Buf staged;
+    const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
+    if ((reinterpret_cast<uintptr_t>(dev) & 15) != 0) throw ArgError{CPB_ERR_ARG, "device input must be 16-byte aligned"};
+    Buf out = dev_alloc(c, 16);
+    stream_cut(c, dev, nbytes, *opts, out->as<uint64_t>());
+    uint64_t* hp = (uint64_t*)c->pinned_scratch(8);
+    CPB_CUDA(cudaMemcpyAsync(hp, out->p, 8, cudaMemcpyDeviceToHost, c->stream));
+    sync_stream(c);
+    *cut = *hp;
     return CPB_OK;
     CPB_CATCH(c, nullptr)
 }

@@ -232,10 +232,23 @@ struct ShardArgs {  // byte-range shard of one file (cpb_parse_csv_shard)
     uint32_t pin0;       // parity of the quote bytes of the file before this buffer
     uint64_t* records;   // out: records owned by this shard (before filtering)
 };
+struct BatchArgs {       // one batch of a streamed input (cpb_stream): it starts at a record boundary of the input
+    uint64_t line_base;  // DataSourceError.Line of the batch's first data record
+    uint64_t* records;   // out: data records of the batch (before filtering)
+    bool* no_record;     // out: the batch holds no record at all (only blank or comment lines)
+};
 std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* dev_bytes, uint64_t n, const cpb_reader_opts& o,
                                  const std::vector<std::pair<std::string, int>>& spec, const cpb_pred* filter,
-                                 bool* had_error, DataError* derr, const ShardArgs* sh = nullptr);
+                                 bool* had_error, DataError* derr, const ShardArgs* sh = nullptr, const BatchArgs* ba = nullptr);
 uint32_t quote_parity(Ctx* c, const uint8_t* dev_bytes, uint64_t n);
+// stream.cu: batches of whole records (cpb_stream_*)
+struct Stream;
+void stream_cut(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o, uint64_t* cut_dev);  // enqueued, 8 bytes
+Stream* stream_open(Ctx* c, const cpb_reader_opts& o, std::vector<std::pair<std::string, int>> spec, const cpb_pred* filter);
+void stream_push(Stream* s, const void* bytes, uint64_t n, bool is_last);
+std::shared_ptr<Table> stream_next(Stream* s, bool* had_error, DataError* derr, bool* done);
+void stream_free(Stream* s);
+Ctx* stream_ctx(Stream* s);
 // gather.cu
 void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, uint64_t* total_dev);  // out[n] = total
 Column gather_column(Ctx* c, const Column& src, const uint32_t* row_ids, int64_t nout);
@@ -293,3 +306,4 @@ extern "C" void cpb_comm_release(cpb::Ctx* c);  // comm.cu
 struct cpb_ctx { cpb::Ctx c; };
 struct cpb_table { std::shared_ptr<cpb::Table> t; };
 struct cpb_index { std::shared_ptr<cpb::Index> ix; };
+struct cpb_stream { cpb::Stream* s; };

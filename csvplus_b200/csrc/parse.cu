@@ -108,7 +108,7 @@ uint32_t quote_parity(Ctx* c, const uint8_t* in, uint64_t n) {
 
 std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, const cpb_reader_opts& o_arg,
                                  const std::vector<std::pair<std::string, int>>& spec, const cpb_pred* filter,
-                                 bool* had_error, DataError* derr, const ShardArgs* sh) {
+                                 bool* had_error, DataError* derr, const ShardArgs* sh, const BatchArgs* ba) {
     const uint8_t* in = in_arg;
     uint64_t n = n_arg;
     cpb_reader_opts o = o_arg;
@@ -187,7 +187,10 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
     // only the fixed part + what is needed: copy the whole struct (≈80 KB) — small next to the input
     CPB_CUDA(cudaMemcpyAsync(h, hbuf->p, sizeof(HeaderOut), cudaMemcpyDeviceToHost, c->stream));
     sync_stream(c);
-    if (h->truncated) throw ArgError{CPB_ERR_UNSUPPORTED, "header row larger than 16 KiB / 1024 fields"};
+    // the first record's bytes are kept only for its names: its field count and end are exact at any size, so a long first
+    // record matters only when it is the header row (not for AssumeHeader, nor for a later batch of a stream)
+    if (h->truncated && o.header_from_first_row) throw ArgError{CPB_ERR_UNSUPPORTED, "header row larger than 16 KiB / 1024 fields"};
+    if (ba) { *ba->records = 0; *ba->no_record = h->eof != 0; }
 
     // ---- header resolution: makeHeader, csvplus.go:1149-1206
     std::vector<std::pair<std::string, int>> cols;  // output columns (name, field index)
@@ -239,7 +242,8 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
     }
     std::vector<std::string> names;
     for (auto& cc : cols) names.push_back(cc.first);
-    const uint64_t line_base = hdr ? 2 : 1;  // DataSourceError.Line of data record 0 (csvplus.go:1102-1109)
+    // DataSourceError.Line of data record 0 (csvplus.go:1102-1109); a later batch of a stream continues the count
+    const uint64_t line_base = ba ? ba->line_base : (hdr ? 2 : 1);
 
     // ---- slots: distinct field indices, ascending
     std::vector<int> fields;
@@ -285,7 +289,7 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
                 members.push_back(next);
             }
             bool he = false; DataError de{};
-            auto part = parse_csv(c, in_arg, n_arg, o_arg, group, filter, &he, &de, sh);
+            auto part = parse_csv(c, in_arg, n_arg, o_arg, group, filter, &he, &de, sh, ba);
             if (first_pass) {
                 *had_error = he; *derr = de;
                 merged->ctx = c; merged->nrows = part->nrows; merged->first_line = part->first_line; merged->record_fields = part->record_fields;
@@ -334,7 +338,13 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
     P.trim = optimistic && o.trim_leading_space ? 1u : 0u;
     P.comment = optimistic ? o.comment : 0u;
 
-    if (P.ntiles == 0) { if (sh && sh->records) *sh->records = 0; return empty_table(names); }
+    if (P.ntiles == 0) {
+        if (sh && sh->records) *sh->records = 0;
+        auto t = empty_table(names);
+        for (auto& cc : cols) t->src_field.push_back(cc.second);
+        t->record_fields = first_nfields;
+        return t;
+    }
 
     Buf lits = dev_alloc(c, comp.lits.size() + 16);
     if (!comp.lits.empty())  // pageable source: the runtime stages it before returning
@@ -346,8 +356,9 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
         GenResult gr;
         P.subs = subs_dev; P.trim = 0; P.comment = 0;
         general_parse(c, P, o, &sub, data_start, &gr);
+        if (ba) *ba->records = gr.nrec;
         auto t = std::make_shared<Table>();
-        t->ctx = c; t->nrows = (int64_t)gr.rows; t->first_line = line_base;
+        t->ctx = c; t->nrows = (int64_t)gr.rows; t->first_line = line_base; t->record_fields = first_nfields;
         if (gr.err_key != ~0ull) {
             uint64_t ordinal = gr.err_key >> 16;
             int kind = (int)((gr.err_key >> 8) & 0xff), slot = (int)(gr.err_key & 0xff);
@@ -360,6 +371,7 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
         for (size_t i = 0; i < cols.size(); i++) {
             Column col; col.name = cols[i].first; col.offsets = gr.offs[col_slot[i]]; col.data = gr.datas[col_slot[i]];
             t->cols.push_back(col);
+            t->src_field.push_back(cols[i].second);
         }
         return t;
     };
@@ -447,6 +459,7 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
         row_cap = res.totals[1] + 1;
         for (int k = 0; k < nsel; k++) data_cap[k] = res.totals[2 + k];
     }
+    if (ba) *ba->records = res.totals[0];
     if (sh) {
         if (sh->records) *sh->records = res.totals[0];
         if (!sh->is_last && res.eof_hit)

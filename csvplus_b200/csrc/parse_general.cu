@@ -15,6 +15,8 @@
 //   g_rec_count    one thread per record: the exact sequential machine (options aware; seq_parse_record_gen lives in
 //                  parse_kernels.cuh, the scan's guarded instantiations use it too) -> lengths, Like terms, errors
 //   g_rec_emit     offsets + unescaped field bytes
+//   g_cut_chunk / g_cut_pick   the stream cut under CommentChar / LazyQuotes (stream.cu, general_cut): per chunk and
+//                  entry state the last line end, then the one of the chunk's true entry state
 // Exact sizes are known before anything is written (multi-pass: this path trades bandwidth for generality).
 // Delimiter / comment are single bytes here: multi-byte runes and the multi-byte Unicode spaces arrive as stand-in bytes.
 #include <algorithm>
@@ -30,6 +32,12 @@ enum { S_RS = 0, S_RSR = 1, S_CM = 2, S_FS = 3, S_UQ = 4, S_QF = 5, S_QQ = 6, S_
 enum { C_Q = 0, C_D = 1, C_N = 2, C_R = 3, C_C = 4, C_S = 5, C_O = 6, NCLASS = 7 };
 constexpr int GCHUNK = 1024;
 constexpr int GBLOCK = 256;  // chunks per block vector
+
+struct CutTokens {  // multi-byte runes the stream cut matches as byte sequences (general_cut)
+    int n;
+    uint8_t len[MAX_SUB_SEQ], cls[MAX_SUB_SEQ];
+    uint8_t b[MAX_SUB_SEQ][4];
+};
 
 struct GenOpts {
     uint8_t delim, comment, lazy, trim;
@@ -241,6 +249,7 @@ void general_parse(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substi
     uint64_t first = 0;
     if (data_start > 0 && nstarts > 0) first = 1;  // exactly one record (the header) starts before data_start
     const uint64_t nrec = nstarts - first;
+    out->nrec = nrec;
     const int nsel = P.nsel;
     out->offs.resize(nsel); out->datas.resize(nsel);
     Buf res = dev_alloc(c, sizeof(ParseResult));
@@ -284,6 +293,93 @@ void general_parse(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substi
         CPB_CUDA(cudaGetLastError());
     }
     sync_stream(c);
+}
+
+// ------------------------------------------------------------------ stream cut (stream.cu) under CommentChar / LazyQuotes
+// The end of the last complete record of a buffer that starts at a record start: 1 + the position of the last '\n' after
+// which the machine above is at a record start.  A multi-byte Delimiter / CommentChar / Unicode space (TrimLeadingSpace)
+// is matched as its byte sequence: its first byte takes the rune's class and the rest of the sequence is skipped, which
+// is what the transcoding of subst.cu gives the general parse.
+__device__ __forceinline__ int cut_token_at(const uint8_t* __restrict__ in, uint64_t n, uint64_t i, const CutTokens& tk) {
+    for (int q = 0; q < tk.n; q++) {
+        if (tk.b[q][0] != in[i] || i + tk.len[q] > n) continue;
+        bool ok = true;
+        for (int j = 1; j < tk.len[q]; j++) ok = ok && in[i + j] == tk.b[q][j];
+        if (ok) return q;
+    }
+    return -1;
+}
+// per chunk: its transition vector, and per entry state 1 + the chunk offset of the last '\n' that ends a line (0: none)
+__global__ void g_cut_chunk(const uint8_t* __restrict__ in, uint64_t n, GenOpts o, CutTokens tk, uint32_t* vec, uint16_t* last) {
+    const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t lo = c * GCHUNK;
+    if (lo >= n) return;
+    const uint64_t hi = lo + GCHUNK < n ? lo + GCHUNK : n;
+    uint64_t i = lo;
+    for (uint64_t back = 1; back <= 3 && back <= lo && tk.n; back++) {  // a sequence that started before the chunk covers its first bytes
+        const int q = in[lo - back] >= 0x80 ? cut_token_at(in, n, lo - back, tk) : -1;
+        if (q >= 0 && lo - back + tk.len[q] > i) i = lo - back + tk.len[q];
+    }
+    uint32_t v = VEC_ID;
+    uint16_t l[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    while (i < hi) {
+        const uint8_t b = in[i];
+        int cl, step = 1;
+        const int q = (b >= 0x80 && tk.n) ? cut_token_at(in, n, i, tk) : -1;
+        if (q >= 0) { cl = tk.cls[q]; step = tk.len[q]; }
+        else cl = gen_class(b, o);
+        v = vec_compose(v, o.T[cl]);
+        if (cl == C_N) {
+#pragma unroll
+            for (int s = 0; s < 8; s++) if (((v >> (3 * s)) & 7) == S_RS) l[s] = (uint16_t)(i - lo + 1);
+        }
+        i += step;
+    }
+    vec[c] = v;
+#pragma unroll
+    for (int s = 0; s < 8; s++) last[c * 8 + s] = l[s];
+}
+__global__ void g_cut_pick(const uint16_t* __restrict__ last, uint64_t nchunks, const uint8_t* __restrict__ cstate, unsigned long long* cut) {
+    const uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nchunks) return;
+    const uint16_t l = last[c * 8 + cstate[c]];
+    if (l) atomicMax(cut, (unsigned long long)(c * GCHUNK + l));
+}
+
+void general_cut(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o, uint64_t* cut_dev) {
+    GenOpts g{};
+    g.delim = o.delimiter < 0x80 ? (uint8_t)o.delimiter : (uint8_t)'"';  // '"' classifies first: a multi-byte delimiter is a token
+    g.comment = o.comment < 0x80 ? (uint8_t)o.comment : 0;
+    g.lazy = o.lazy_quotes; g.trim = o.trim_leading_space;
+    for (int cl = 0; cl < NCLASS; cl++) {
+        uint32_t v = 0;
+        for (int s = 0; s < 8; s++) v |= (uint32_t)gen_delta(s, (cl == C_C && !o.comment) ? C_O : cl, g.trim) << (3 * s);
+        g.T[cl] = v;
+    }
+    CutTokens tk{};
+    auto add = [&](uint32_t r, int cls) {
+        if (r < 0x80 || tk.n >= MAX_SUB_SEQ) return;
+        const std::string u = utf8_rune(r);
+        tk.len[tk.n] = (uint8_t)u.size();
+        for (size_t j = 0; j < u.size(); j++) tk.b[tk.n][j] = (uint8_t)u[j];
+        tk.cls[tk.n++] = (uint8_t)cls;
+    };
+    add(o.delimiter, C_D);
+    add(o.comment, C_C);
+    if (o.trim_leading_space)
+        for (uint32_t r : kUnicodeSpaces) if (r != o.delimiter && r != o.comment) add(r, C_S);
+    CPB_CUDA(cudaMemsetAsync(cut_dev, 0, 8, c->stream));
+    if (n == 0) return;
+    const uint64_t nchunks = (n + GCHUNK - 1) / GCHUNK, nblocks = (nchunks + GBLOCK - 1) / GBLOCK;
+    Buf vec = dev_alloc(c, nchunks * 4), last = dev_alloc(c, nchunks * 16), bvec = dev_alloc(c, nblocks * 4), bstate = dev_alloc(c, nblocks + 1),
+        cstate = dev_alloc(c, nchunks);
+    KernelTimer kt(c, "stream_cut_dfa", n, 5);
+    g_cut_chunk<<<nblk(nchunks, 128), 128, 0, c->stream>>>(in, n, g, tk, vec->as<uint32_t>(), last->as<uint16_t>());
+    g_block_vec<<<nblk(nblocks, 128), 128, 0, c->stream>>>(vec->as<uint32_t>(), nchunks, bvec->as<uint32_t>());
+    g_chain<<<1, 1, 0, c->stream>>>(bvec->as<uint32_t>(), nblocks, bstate->as<uint8_t>());
+    g_chunk_state<<<nblk(nblocks, 128), 128, 0, c->stream>>>(vec->as<uint32_t>(), nchunks, bstate->as<uint8_t>(), cstate->as<uint8_t>());
+    g_cut_pick<<<nblk(nchunks, 128), 128, 0, c->stream>>>(last->as<uint16_t>(), nchunks, cstate->as<uint8_t>(), (unsigned long long*)cut_dev);
+    CPB_CUDA(cudaGetLastError());
 }
 
 }  // namespace cpb

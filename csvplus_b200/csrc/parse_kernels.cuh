@@ -1191,6 +1191,7 @@ __global__ void __launch_bounds__(THREADS, KMAX <= 8 ? 768 / THREADS : 1) csv_sc
 // ------------------------------------------------------------------ general reader path (parse_general.cu)
 struct GenResult {
     uint64_t nrec_eff = 0, rows = 0;
+    uint64_t nrec = 0;  // data records of the input (before filtering)
     unsigned long long err_key = ~0ull;
     std::vector<Buf> offs, datas;
 };

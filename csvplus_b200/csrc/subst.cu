@@ -76,7 +76,9 @@ __global__ void subst_kernel(const uint8_t* __restrict__ in, uint64_t n, SeqDev 
     if (!WRITE) counts[c] = k;
 }
 
-std::string utf8(uint32_t r) {
+}  // namespace
+
+std::string utf8_rune(uint32_t r) {
     std::string s;
     if (r < 0x80) s += (char)r;
     else if (r < 0x800) { s += (char)(0xC0 | (r >> 6)); s += (char)(0x80 | (r & 0x3F)); }
@@ -84,8 +86,6 @@ std::string utf8(uint32_t r) {
     else { s += (char)(0xF0 | (r >> 18)); s += (char)(0x80 | ((r >> 12) & 0x3F)); s += (char)(0x80 | ((r >> 6) & 0x3F)); s += (char)(0x80 | (r & 0x3F)); }
     return s;
 }
-
-}  // namespace
 
 bool needs_substitution(const cpb_reader_opts& o) { return o.delimiter >= 0x80 || o.comment >= 0x80 || o.trim_leading_space; }
 
@@ -96,13 +96,10 @@ Substitution substitute_runes(Ctx* c, const uint8_t* in, uint64_t n, const cpb_r
     r.delimiter = o.delimiter; r.comment = o.comment;
     struct Want { std::string seq; int kind; };  // kind 0 delimiter, 1 comment, 2 space
     std::vector<Want> want;
-    if (o.delimiter >= 0x80) want.push_back({utf8(o.delimiter), 0});
-    if (o.comment >= 0x80) want.push_back({utf8(o.comment), 1});
-    if (o.trim_leading_space) {
-        static const uint32_t spaces[] = {0x85, 0xA0, 0x1680, 0x2000, 0x2001, 0x2002, 0x2003, 0x2004, 0x2005, 0x2006, 0x2007, 0x2008,
-                                          0x2009, 0x200A, 0x2028, 0x2029, 0x202F, 0x205F, 0x3000};
-        for (uint32_t s : spaces) if (s != o.delimiter && s != o.comment) want.push_back({utf8(s), 2});
-    }
+    if (o.delimiter >= 0x80) want.push_back({utf8_rune(o.delimiter), 0});
+    if (o.comment >= 0x80) want.push_back({utf8_rune(o.comment), 1});
+    if (o.trim_leading_space)
+        for (uint32_t s : kUnicodeSpaces) if (s != o.delimiter && s != o.comment) want.push_back({utf8_rune(s), 2});
     if (want.empty()) return r;
     // ---- which byte values occur
     Buf hist = dev_alloc(c, 256 * 8);

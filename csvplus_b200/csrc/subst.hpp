@@ -22,6 +22,10 @@ struct Substitution {
     SubTable host_table{};
 };
 bool needs_substitution(const cpb_reader_opts& o);
+std::string utf8_rune(uint32_t r);
+// the multi-byte runes unicode.IsSpace accepts: what TrimLeadingSpace trims besides ASCII white space
+constexpr uint32_t kUnicodeSpaces[] = {0x85, 0xA0, 0x1680, 0x2000, 0x2001, 0x2002, 0x2003, 0x2004, 0x2005, 0x2006,
+                                       0x2007, 0x2008, 0x2009, 0x200A, 0x2028, 0x2029, 0x202F, 0x205F, 0x3000};
 Substitution substitute_runes(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o);
 
 }  // namespace cpb

@@ -1,6 +1,6 @@
 package csvplus
 
-// reader.go: the Reader and its options (csvplus.go:922-1076) lowered to cpb_parse_csv.
+// reader.go: the Reader and its options (csvplus.go:922-1076) lowered to cpb_stream_* (cpb_parse_csv-compatible batches).
 
 /*
 #include <stdlib.h>
@@ -9,16 +9,23 @@ package csvplus
 import "C"
 
 import (
+	"bytes"
 	"errors"
 	"io"
 	"os"
+	"runtime"
 	"unsafe"
 )
 
-type sourceFn func() (data []byte, err error)
+type sourceFn func() (io.ReadCloser, error)
 
-// Reader is an iterable csv reader.  Its options have the reference's names and panics; Iterate parses the whole
-// input on the GPU (cpb_parse_csv) and then hands the rows to the callback.
+// StreamBatchBytes is the size of one piece of input pushed to the GPU (cpb_stream_push): the input is parsed in
+// batches of whole records and never held whole in host memory.
+var StreamBatchBytes = 128 << 20
+
+// Reader is an iterable csv reader.  Its options have the reference's names and panics; Iterate reads the input in
+// pieces of StreamBatchBytes, parses them on the GPU in batches of whole records (cpb_stream_*) and then hands the rows
+// to the callback.
 type Reader struct {
 	source                       sourceFn
 	delimiter, comment           rune
@@ -36,20 +43,17 @@ func makeReader(src sourceFn) *Reader {
 // FromFile binds a reader to a file; the file is opened on every iteration, so the source is re-iterable
 // (csvplus.go:950-959).
 func FromFile(name string) *Reader {
-	return makeReader(func() ([]byte, error) { return os.ReadFile(name) })
+	return makeReader(func() (io.ReadCloser, error) { return os.Open(name) })
 }
 
 // FromReader constructs a reader over an io.Reader (one shot, csvplus.go:936).
 func FromReader(input io.Reader) *Reader {
-	return makeReader(func() ([]byte, error) { return io.ReadAll(input) })
+	return makeReader(func() (io.ReadCloser, error) { return io.NopCloser(input), nil })
 }
 
 // FromReadCloser is FromReader that also closes the input when the iteration ends (csvplus.go:943).
 func FromReadCloser(input io.ReadCloser) *Reader {
-	return makeReader(func() ([]byte, error) {
-		defer input.Close()
-		return io.ReadAll(input)
-	})
+	return makeReader(func() (io.ReadCloser, error) { return input, nil })
 }
 
 // OnContext makes the reader parse on the given context instead of the default one (not in the reference).
@@ -128,16 +132,27 @@ func (r *Reader) context() *Context {
 	return ctx()
 }
 
-// parse lowers Reader.Iterate (+ an optional recognised predicate that directly follows it) to cpb_parse_csv.
-// On a data error the table holds the rows the streaming reference would have delivered before failing.
+// parse lowers Reader.Iterate (+ an optional recognised predicate that directly follows it) to cpb_parse_csv when the
+// input fits one batch, else to cpb_stream_*: the input is pushed in pinned pieces of StreamBatchBytes, each push parses the complete records received so far, and the batches'
+// tables are concatenated (cpb_table_concat).  On a data error the table holds the rows the streaming reference would
+// have delivered before failing.
 func (r *Reader) parse(pred *predSpec) (*Table, error) {
-	data, err := r.source()
-	if err != nil { // csvplus.go:1216-1220: *os.PathError is reported as "op: err", everything is row 1
+	pathErr := func(err error) error { // csvplus.go:1216-1220: *os.PathError is reported as "op: err", everything is row 1
 		var pe *os.PathError
 		if errors.As(err, &pe) {
-			return nil, &DataSourceError{Line: 1, Err: errors.New(pe.Op + ": " + pe.Err.Error())}
+			return &DataSourceError{Line: 1, Err: errors.New(pe.Op + ": " + pe.Err.Error())}
 		}
-		return nil, &DataSourceError{Line: 1, Err: err}
+		return &DataSourceError{Line: 1, Err: err}
+	}
+	input, err := r.source()
+	if err != nil {
+		return nil, pathErr(err)
+	}
+	defer input.Close()
+	// an input that fits one batch is parsed in one cpb_parse_csv call, staged at its own size
+	first, err := io.ReadAll(io.LimitReader(input, int64(StreamBatchBytes)+1))
+	if err != nil {
+		return nil, pathErr(err)
 	}
 	opts := C.cpb_reader_opts{delimiter: C.uint32_t(r.delimiter), comment: C.uint32_t(r.comment), num_fields: C.int32_t(r.numFields)}
 	if r.lazyQuotes {
@@ -166,23 +181,90 @@ func (r *Reader) parse(pred *predSpec) (*Table, error) {
 		cpred = cp.root
 	}
 	c := r.context()
-	// pinned staging memory filled by the host, as INTEGRATION.md describes
-	var staging unsafe.Pointer
-	if len(data) > 0 {
-		if st := C.cpb_host_alloc(c.h, C.uint64_t(len(data)), &staging); st != C.CPB_OK {
-			return nil, errors.New("csvplus: cpb_host_alloc failed")
+	var e C.cpb_error
+	if len(first) <= StreamBatchBytes {
+		var staging unsafe.Pointer // pinned staging memory filled by the host, as INTEGRATION.md describes
+		if len(first) > 0 {
+			if s := C.cpb_host_alloc(c.h, C.uint64_t(len(first)), &staging); s != C.CPB_OK {
+				return nil, errors.New("csvplus: cpb_host_alloc failed")
+			}
+			defer C.cpb_host_free(c.h, staging)
+			C.memcpy(staging, unsafe.Pointer(&first[0]), C.size_t(len(first)))
 		}
-		defer C.cpb_host_free(c.h, staging)
-		C.memcpy(staging, unsafe.Pointer(&data[0]), C.size_t(len(data)))
+		var out *C.cpb_table
+		s := C.cpb_parse_csv(c.h, staging, C.uint64_t(len(first)), 0, &opts, &spec[0], C.int(len(names)), cpred, &out, &e)
+		var t *Table
+		if out != nil {
+			t = newTable(c, out)
+		}
+		return t, mapErr(C.int(s), &e)
+	}
+	src := io.MultiReader(bytes.NewReader(first), input)
+	var st *C.cpb_stream
+	if s := C.cpb_stream_open(c.h, &opts, &spec[0], C.int(len(names)), cpred, &st, &e); s != C.CPB_OK {
+		return nil, mapErr(C.int(s), &e)
+	}
+	defer C.cpb_stream_free(st)
+	// pinned staging memory filled by the host (io.ReadFull), as INTEGRATION.md describes; a piece stays untouched
+	// until the cpb_stream_next after its push has returned
+	var staging unsafe.Pointer
+	if s := C.cpb_host_alloc(c.h, C.uint64_t(StreamBatchBytes), &staging); s != C.CPB_OK {
+		return nil, errors.New("csvplus: cpb_host_alloc failed")
+	}
+	defer C.cpb_host_free(c.h, staging)
+	buf := unsafe.Slice((*byte)(staging), StreamBatchBytes)
+	var parts []*Table
+	collect := func() (bool, error) { // one cpb_stream_next per push; false: the stream is done
+		var out *C.cpb_table
+		var done C.int
+		s := C.cpb_stream_next(st, &out, &done, &e)
+		if out != nil {
+			parts = append(parts, newTable(c, out))
+		}
+		if s != C.CPB_OK {
+			return false, mapErr(C.int(s), &e)
+		}
+		return done == 0, nil
+	}
+	var serr error
+	for more := true; more; {
+		n, rerr := io.ReadFull(src, buf)
+		last := rerr == io.EOF || rerr == io.ErrUnexpectedEOF
+		if rerr != nil && !last {
+			return nil, pathErr(rerr)
+		}
+		if s := C.cpb_stream_push(st, staging, C.uint64_t(n), boolToInt(last)); s != C.CPB_OK {
+			return nil, errors.New("csvplus: cpb_stream_push failed")
+		}
+		more, serr = collect()
+		more = more && !last
+		if serr != nil {
+			break
+		}
+	}
+	if len(parts) <= 1 {
+		if len(parts) == 0 {
+			return nil, serr
+		}
+		return parts[0], serr
+	}
+	hs := make([]*C.cpb_table, len(parts)+1)
+	for i, p := range parts {
+		hs[i] = p.h
 	}
 	var out *C.cpb_table
-	var e C.cpb_error
-	st := C.cpb_parse_csv(c.h, staging, C.uint64_t(len(data)), 0, &opts, &spec[0], C.int(len(names)), cpred, &out, &e)
-	var t *Table
-	if out != nil {
-		t = newTable(c, out)
+	if s := C.cpb_table_concat(c.h, &hs[0], C.int(len(parts)), &out); s != C.CPB_OK {
+		return nil, errors.New("csvplus: cpb_table_concat failed")
 	}
-	return t, mapErr(C.int(st), &e)
+	runtime.KeepAlive(parts)
+	return newTable(c, out), serr
+}
+
+func boolToInt(b bool) C.int {
+	if b {
+		return 1
+	}
+	return 0
 }
 
 // Iterate reads the input, converts every record to a Row and calls fn (csvplus.go:1080).  Rows delivered before a

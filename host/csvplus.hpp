@@ -6,12 +6,17 @@
 // and the rows are uploaded again with TakeRows semantics — exactly what the cgo wrapper does for Go
 // closures (INTEGRATION.md).  There is no CPU fallback: without a GPU every sink throws.
 #pragma once
+#include <sys/stat.h>
+
 #include <algorithm>
+#include <cerrno>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <functional>
 #include <map>
 #include <memory>
+#include <fstream>
 #include <ostream>
 #include <stdexcept>
 #include <string>
@@ -51,6 +56,10 @@ struct Strs {
     explicit Strs(const std::vector<std::string>& s) : keep(s) { for (auto& x : keep) v.push_back(cpb_str{x.data(), x.size()}); if (v.empty()) v.push_back(cpb_str{nullptr, 0}); }
 };
 }  // namespace detail
+
+// bytes per push of a streamed input (cpb_stream_*): FromFile / FromString inputs larger than this are parsed in batches
+// of whole records, smaller ones in one cpb_parse_csv call
+inline uint64_t& StreamBatchBytes() { static uint64_t v = 128ull << 20; return v; }
 
 // maps nbytes of device memory into the context's pool ahead of time (cpb_pool_reserve); optional
 inline void Reserve(uint64_t nbytes) { if (cpb_pool_reserve(detail::ctx(), nbytes) != CPB_OK) throw Error(cpb_last_error(detail::ctx())); }
@@ -120,6 +129,11 @@ public:
             for (size_t i = 0; i < out.size(); i++) out[i][cols[c]] = std::string((const char*)data.data() + off[i], (size_t)(off[i + 1] - off[i]));
         }
         return out;
+    }
+    Table slice(int64_t lo, int64_t hi) const {  // a row-range view (cpb_table_slice)
+        cpb_table* out = nullptr;
+        if (cpb_table_slice(detail::ctx(), h_.get(), lo, hi, &out) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+        return Table(out);
     }
     static Table from_rows(const std::vector<Row>& rows) {  // TakeRows, csvplus.go:218
         std::vector<std::string> cols;
@@ -197,7 +211,12 @@ private:
 // ---------------------------------------------------------------- Reader (csvplus.go:922-1076)
 class Reader {
 public:
-    explicit Reader(std::function<std::string()> source) : source_(std::move(source)) {}
+    // fills the next piece of the input; false at its end
+    using Pieces = std::function<bool(std::string&)>;
+    // source: the whole input, parsed in one cpb_parse_csv call.  pieces: null, or a function that returns null when the
+    // input fits one batch (then `source` is parsed) and else the input's pieces (cpb_stream_*)
+    explicit Reader(std::function<std::string()> source, std::function<Pieces()> pieces = nullptr)
+        : source_(std::move(source)), pieces_(std::move(pieces)) {}
     Reader& Delimiter(char32_t c) { delimiter_ = c; return *this; }
     Reader& CommentChar(char32_t c) { comment_ = c; return *this; }
     Reader& LazyQuotes() { lazy_ = true; return *this; }
@@ -220,27 +239,84 @@ public:
         for (auto& kv : spec) if (kv.second < 0) throw std::logic_error("header spec: negative index for column " + kv.first);
         header_.assign(spec.begin(), spec.end()); from_first_row_ = false; return *this;
     }
-    // Reader.Iterate lowered to cpb_parse_csv; *err receives the DataSourceError raised after the delivered rows
-    Table parse(const Predicate* pred, std::unique_ptr<DataSourceError>* err) const {
-        std::string data = source_();
+    // one batch of Reader.Iterate: its rows, the DataSourceError raised after them (last batch only) and whether the
+    // input is parsed in several batches.  fn returns false to stop reading the input.
+    using BatchFn = std::function<bool(Table, std::unique_ptr<DataSourceError>, bool streamed)>;
+    // Reader.Iterate lowered to cpb_parse_csv (an input that fits one batch) or to cpb_stream_* (a larger one)
+    void batches(const Predicate* pred, const BatchFn& fn) const {
+        Pieces next = pieces_ ? pieces_() : nullptr;
         cpb_reader_opts o{}; o.delimiter = delimiter_; o.comment = comment_; o.num_fields = num_fields_;
         o.lazy_quotes = lazy_; o.trim_leading_space = trim_; o.header_from_first_row = from_first_row_;
         std::vector<cpb_header_col> spec;
         for (auto& h : header_) spec.push_back(cpb_header_col{cpb_str{h.first.data(), h.first.size()}, h.second, 0});
         std::unique_ptr<detail::CPred> cp; if (pred) cp.reset(new detail::CPred(*pred));
         cpb_table* t = nullptr; cpb_error e{};
-        int st = cpb_parse_csv(detail::ctx(), data.data(), data.size(), 0, &o, spec.data(), (int)spec.size(), cp ? &cp->p : nullptr, &t, &e);
-        if (st == CPB_ERR_DATA && t && e.has_line) { err->reset(new DataSourceError(e.line, e.msg)); return Table(t); }
-        detail::check(st, e);
-        return Table(t);
+        if (!next) {
+            std::string data = source_();
+            int st = cpb_parse_csv(detail::ctx(), data.data(), data.size(), 0, &o, spec.data(), (int)spec.size(), cp ? &cp->p : nullptr, &t, &e);
+            if (st == CPB_ERR_DATA && t && e.has_line) { fn(Table(t), std::unique_ptr<DataSourceError>(new DataSourceError(e.line, e.msg)), false); return; }
+            detail::check(st, e);
+            fn(Table(t), nullptr, false);
+            return;
+        }
+        cpb_stream* sp = nullptr;
+        detail::check(cpb_stream_open(detail::ctx(), &o, spec.data(), (int)spec.size(), cp ? &cp->p : nullptr, &sp, &e), e);
+        std::unique_ptr<cpb_stream, void (*)(cpb_stream*)> st(sp, cpb_stream_free);
+        // One cpb_stream_next per push parses every complete record pushed so far.  A batch is delivered after the next
+        // piece has been pushed: that piece's host-to-device copy (the stream's copy stream) overlaps what fn does with
+        // the batch on the context's stream, and it is parsed only after fn has returned.
+        Table pending; bool have = false;
+        auto deliver = [&]() -> bool { if (!have) return true; have = false; return fn(pending, nullptr, true); };
+        enum { GO, DONE, STOP };
+        auto step = [&]() -> int {
+            cpb_table* bt = nullptr; int done = 0;
+            const int s = cpb_stream_next(st.get(), &bt, &done, &e);
+            if (s == CPB_ERR_DATA && bt && e.has_line) {
+                Table failed(bt);
+                if (deliver()) fn(failed, std::unique_ptr<DataSourceError>(new DataSourceError(e.line, e.msg)), true);
+                return STOP;
+            }
+            if (s != CPB_OK) detail::check(s, e);
+            if (bt) { pending = Table(bt); have = true; }
+            return done ? DONE : GO;
+        };
+        auto push = [&](const void* p, uint64_t n, int last) {
+            if (cpb_stream_push(st.get(), p, n, last) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+        };
+        std::string piece;  // untouched until the cpb_stream_next after its push has returned
+        int r = GO;
+        while (r == GO && next(piece)) {
+            push(piece.data(), piece.size(), 0);
+            if (!deliver()) return;
+            if ((r = step()) == STOP) return;
+        }
+        if (r == GO) {
+            push(nullptr, 0, 1);
+            if (!deliver()) return;
+            if (step() == STOP) return;
+        }
+        deliver();
     }
 private:
     std::function<std::string()> source_;
+    std::function<Pieces()> pieces_;
     uint32_t delimiter_ = ',', comment_ = 0; int num_fields_ = 0; bool lazy_ = false, trim_ = false, from_first_row_ = true;
     std::vector<std::pair<std::string, int>> header_;
 };
 Reader FromFile(const std::string& name);  // csvplus.go:950 (defined below)
-inline Reader FromString(std::string data) { return Reader([data] { return data; }); }
+inline Reader FromString(std::string data) {
+    auto d = std::make_shared<std::string>(std::move(data));
+    return Reader([d] { return *d; }, [d]() -> Reader::Pieces {
+        if (d->size() <= StreamBatchBytes()) return nullptr;
+        auto pos = std::make_shared<size_t>(0);
+        return [d, pos](std::string& piece) {
+            if (*pos >= d->size()) return false;
+            piece.assign(*d, *pos, (size_t)StreamBatchBytes());
+            *pos += piece.size();
+            return true;
+        };
+    });
+}
 
 // ---------------------------------------------------------------- DataSource (csvplus.go:207-608)
 class DataSource {
@@ -263,34 +339,78 @@ public:
         if (c.size() > ix.columns().size()) throw std::logic_error("too many source columns in Except()");
         Op o{EXCEPT}; o.cols = c; o.index.reset(new Index(ix)); return with(std::move(o));
     }
-    // sinks
-    void operator()(const RowFunc& fn) const { std::unique_ptr<DataSourceError> err; Table t = run(&err); for (auto& r : t.rows()) fn(r); if (err) throw *err; }
+    // sinks: each batch of a streamed input is delivered before the next one is parsed
+    void operator()(const RowFunc& fn) const {
+        each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool) {
+            for (auto& r : t.rows()) fn(r);
+            if (err) throw *err;
+            return true;
+        });
+    }
     std::vector<Row> ToRows() const { std::vector<Row> out; (*this)([&](const Row& r) { out.push_back(r); }); return out; }
     // the plan's rows as a device table (an extension beyond the reference API, like TakeTable): the input of
     // Table::ValuesAsInt / ValuesAsFloat64.  A source error is thrown.
     Table ToTable() const { std::unique_ptr<DataSourceError> err; Table t = run(&err); if (err) throw *err; return t; }
+    // ToCsv, csvplus.go:379-406: the header line once, then every batch's rows; delivered rows are written before a source
+    // error is thrown
     void ToCsv(std::ostream& out, const std::vector<std::string>& columns) const {
         if (columns.empty()) throw std::logic_error("empty column list in ToCsv() function");
-        std::unique_ptr<DataSourceError> err; Table t = run(&err);
-        detail::Strs c(columns); void* bytes = nullptr; uint64_t n = 0; cpb_error e{};
-        detail::check(cpb_table_to_csv(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), &bytes, &n, &e), e);
-        out.write((const char*)bytes, (std::streamsize)n); cpb_host_free(detail::ctx(), bytes);
-        if (err) throw *err;
+        detail::Strs c(columns);
+        bool header = false;
+        void* buf = nullptr; uint64_t cap = 0;  // pinned: the batches of a streamed input are serialised into it
+        try {
+            each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool streamed) {
+                cpb_error e{};
+                if (!streamed) {
+                    void* bytes = nullptr; uint64_t n = 0;
+                    detail::check(cpb_table_to_csv(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), &bytes, &n, &e), e);
+                    out.write((const char*)bytes, (std::streamsize)n); cpb_host_free(detail::ctx(), bytes);
+                } else {
+                    for (;;) {  // the header line once, before the first batch (csvplus.go:387)
+                        uint64_t n = 0;
+                        const int st = cpb_table_to_csv_into(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), !header, buf, cap, &n, &e);
+                        if (st == CPB_ERR_ARG && n > cap) {  // grow to the size the batch needs and repeat it
+                            if (buf) cpb_host_free(detail::ctx(), buf);
+                            buf = nullptr; cap = 0;
+                            if (cpb_host_alloc(detail::ctx(), n + n / 4 + 64, &buf) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+                            cap = n + n / 4 + 64;
+                            continue;
+                        }
+                        detail::check(st, e);
+                        out.write((const char*)buf, (std::streamsize)n);
+                        break;
+                    }
+                }
+                header = true;
+                if (err) throw *err;
+                return true;
+            });
+        } catch (...) { if (buf) cpb_host_free(detail::ctx(), buf); throw; }
+        if (buf) cpb_host_free(detail::ctx(), buf);
+    }
+    // ToCsvFile, csvplus.go:411-443: the file is removed on error
+    void ToCsvFile(const std::string& name, const std::vector<std::string>& columns) const {
+        try {
+            std::ofstream f(name, std::ios::binary | std::ios::trunc);
+            if (!f) throw Error("open " + name + ": " + strerror(errno));
+            ToCsv(f, columns);
+            f.close();
+            if (!f) throw Error("write " + name + " failed");
+        } catch (...) { std::remove(name.c_str()); throw; }
     }
     // ToJSON, csvplus.go:446-474: the GPU serialises the result in row-range batches (each < 4 GiB) into one reused
-    // pinned buffer; on a source error nothing is written
+    // pinned buffer.  On a source error nothing is written when the input was parsed in one batch; a streamed input keeps
+    // what its earlier batches wrote (a prefix of the array without ']'), as the reference's encoder has flushed it.
     void ToJSON(std::ostream& out) const {
-        std::unique_ptr<DataSourceError> err; Table t = run(&err);
-        if (err) throw *err;
-        const int64_t n = t.size(), step = int64_t(1) << 24;
         void* buf = nullptr; uint64_t cap = 0;
-        try {
+        bool opened = false;
+        auto json = [&](const Table& t, bool first, bool last) {
+            const int64_t n = t.size(), step = int64_t(1) << 24;
             for (int64_t lo = 0;;) {
                 const int64_t hi = std::min(n, lo + step);
-                cpb_table* part = nullptr; cpb_error e{};
-                detail::check(cpb_table_slice(detail::ctx(), t.get(), lo, hi, &part), e);
-                Table p(part); uint64_t w = 0;
-                int st = cpb_table_to_json_into(detail::ctx(), p.get(), lo == 0, hi == n, buf, cap, &w, &e);
+                cpb_error e{}; uint64_t w = 0;
+                Table p = t.slice(lo, hi);
+                int st = cpb_table_to_json_into(detail::ctx(), p.get(), first && lo == 0, last && hi == n, buf, cap, &w, &e);
                 if (st == CPB_ERR_ARG && w > cap) {  // grow the buffer to the size the batch needs and repeat it
                     if (buf) cpb_host_free(detail::ctx(), buf);
                     buf = nullptr; cap = 0;
@@ -303,8 +423,23 @@ public:
                 lo = hi;
                 if (lo >= n) break;
             }
+        };
+        try {
+            each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool streamed) {
+                if (!streamed) {
+                    if (err) throw *err;
+                    json(t, true, true);
+                    opened = true;
+                    return true;
+                }
+                if (t.size()) { json(t, !opened, false); opened = true; }
+                if (err) throw *err;
+                return true;
+            });
         } catch (...) { if (buf) cpb_host_free(detail::ctx(), buf); throw; }
         if (buf) cpb_host_free(detail::ctx(), buf);
+        if (!opened) out << "[]";
+        else if (streamed_) out << ']';
     }
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }
@@ -318,32 +453,67 @@ private:
         detail::check(cpb_index_build(detail::ctx(), t.get(), c.v.data(), (int)cols.size(), unique, &ix, &e), e);
         return Index(ix, cols);
     }
+    // the batches' tables concatenated (cpb_table_concat); *err: the source error after them
     Table run(std::unique_ptr<DataSourceError>* err) const {
-        size_t first = 0; Table t;
+        std::vector<Table> parts;
+        each([&](Table& t, std::unique_ptr<DataSourceError>& e, bool) { parts.push_back(t); *err = std::move(e); return true; });
+        if (parts.size() == 1) return parts[0];
+        std::vector<const cpb_table*> hs;
+        for (auto& p : parts) hs.push_back(p.get());
+        cpb_table* out = nullptr;
+        if (cpb_table_concat(detail::ctx(), hs.data(), (int)hs.size(), &out) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+        return Table(out);
+    }
+    // the operations over every batch of the source, in order: fn(rows, error after them, streamed) returns false to stop.
+    // Top / Drop count rows across batches; once Top has pulled n + 1 rows the input is no longer read.
+    using EachFn = std::function<bool(Table&, std::unique_ptr<DataSourceError>&, bool)>;
+    void each(const EachFn& fn) const {
+        size_t first = 0;
+        std::vector<uint64_t> seen(ops_.size(), 0);
+        streamed_ = false;
+        auto apply = [&](Table t, std::unique_ptr<DataSourceError> err, bool streamed) -> bool {
+            streamed_ = streamed;
+            bool stop = false;
+            for (size_t i = first; i < ops_.size(); i++) {
+                const Op& o = ops_[i]; cpb_table* out = nullptr; cpb_error e{}; detail::Strs c(o.cols);
+                const uint64_t n = (uint64_t)t.size();
+                switch (o.kind) {
+                    case FILTER:
+                        if (o.pred.lowerable()) { detail::CPred cp(o.pred); detail::check(cpb_table_filter(detail::ctx(), t.get(), &cp.p, &out), e); }
+                        else { std::vector<Row> keep; for (auto& r : t.rows()) if (o.pred(r)) keep.push_back(r); t = Table::from_rows(keep); continue; }
+                        break;
+                    case MAP: { std::vector<Row> m; for (auto& r : t.rows()) m.push_back(o.map(r)); t = Table::from_rows(m); continue; }
+                    case SELECT: detail::check(cpb_table_select(detail::ctx(), t.get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
+                    case DROPCOLS: detail::check(cpb_table_drop(detail::ctx(), t.get(), c.v.data(), (int)o.cols.size(), &out), e); break;
+                    case JOIN: detail::check(cpb_join(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
+                    case EXCEPT: detail::check(cpb_except(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
+                    case TOP: {  // the reference pulls n + 1 rows then stops (io.EOF): a later error is never met
+                        const uint64_t keep = o.n > seen[i] ? std::min(n, o.n - seen[i]) : 0;
+                        seen[i] += n;
+                        if (seen[i] > o.n) { err.reset(); stop = true; }
+                        detail::check(cpb_table_slice(detail::ctx(), t.get(), 0, (int64_t)keep, &out), e);
+                        break;
+                    }
+                    case DROP: {
+                        const uint64_t lo = o.n > seen[i] ? std::min(n, o.n - seen[i]) : 0;
+                        seen[i] += n;
+                        detail::check(cpb_table_slice(detail::ctx(), t.get(), (int64_t)lo, (int64_t)n, &out), e);
+                        break;
+                    }
+                }
+                t = Table(out);
+            }
+            const bool failed = err != nullptr;
+            return fn(t, err, streamed) && !stop && !failed;
+        };
         if (reader_) {
             const Predicate* fused = (!ops_.empty() && ops_[0].kind == FILTER && ops_[0].pred.lowerable()) ? &ops_[0].pred : nullptr;
-            t = reader_->parse(fused, err); if (fused) first = 1;
-        } else t = *table_;
-        for (size_t i = first; i < ops_.size(); i++) {
-            const Op& o = ops_[i]; cpb_table* out = nullptr; cpb_error e{}; detail::Strs c(o.cols);
-            switch (o.kind) {
-                case FILTER:
-                    if (o.pred.lowerable()) { detail::CPred cp(o.pred); detail::check(cpb_table_filter(detail::ctx(), t.get(), &cp.p, &out), e); }
-                    else { std::vector<Row> keep; for (auto& r : t.rows()) if (o.pred(r)) keep.push_back(r); t = Table::from_rows(keep); continue; }
-                    break;
-                case MAP: { std::vector<Row> m; for (auto& r : t.rows()) m.push_back(o.map(r)); t = Table::from_rows(m); continue; }
-                case SELECT: detail::check(cpb_table_select(detail::ctx(), t.get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
-                case DROPCOLS: detail::check(cpb_table_drop(detail::ctx(), t.get(), c.v.data(), (int)o.cols.size(), &out), e); break;
-                case JOIN: detail::check(cpb_join(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
-                case EXCEPT: detail::check(cpb_except(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
-                case TOP: if (*err && (uint64_t)t.size() > o.n) err->reset(); detail::check(cpb_table_slice(detail::ctx(), t.get(), 0, (int64_t)o.n, &out), e); break;
-                case DROP: detail::check(cpb_table_slice(detail::ctx(), t.get(), (int64_t)o.n, t.size(), &out), e); break;
-            }
-            t = Table(out);
-        }
-        return t;
+            if (fused) first = 1;
+            reader_->batches(fused, apply);
+        } else apply(*table_, nullptr, false);
     }
     std::shared_ptr<Reader> reader_; std::shared_ptr<Table> table_; std::vector<Op> ops_;
+    mutable bool streamed_ = false;  // the last each() parsed its input in several batches
 };
 
 inline DataSource Take(const Reader& r) { return DataSource(r); }                          // csvplus.go:252
@@ -355,14 +525,28 @@ inline DataSource Index::Find(const std::vector<std::string>& values) const {
     if (cpb_index_find(detail::ctx(), h_.get(), v.v.data(), (int)values.size(), &t) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
     return DataSource(Table(t));
 }
+// a file that fits one batch is read whole and parsed in one call; a larger one is read and parsed one batch at a time
 inline Reader FromFile(const std::string& name) {
-    return Reader([name] {
+    auto whole = [name] {
         FILE* f = fopen(name.c_str(), "rb");
         if (!f) throw DataSourceError(1, std::string("open: ") + strerror(errno));  // mapError, csvplus.go:1216-1220
         std::string s; char buf[1 << 16]; size_t n;
         while ((n = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, n);
         fclose(f); return s;
-    });
+    };
+    auto pieces = [name]() -> Reader::Pieces {
+        struct stat sb;
+        if (stat(name.c_str(), &sb) != 0 || !S_ISREG(sb.st_mode) || (uint64_t)sb.st_size <= StreamBatchBytes()) return nullptr;
+        std::shared_ptr<FILE> f(fopen(name.c_str(), "rb"), [](FILE* p) { if (p) fclose(p); });
+        if (!f) throw DataSourceError(1, std::string("open: ") + strerror(errno));
+        return [f](std::string& piece) {
+            piece.resize((size_t)StreamBatchBytes());
+            const size_t n = fread(&piece[0], 1, piece.size(), f.get());
+            piece.resize(n);
+            return n > 0;
+        };
+    };
+    return Reader(whole, pieces);
 }
 
 }  // namespace csvplus

@@ -3,8 +3,11 @@
 // TestWriteFile (:172-196), TestJSONStruct (:1016-1048) and TestSimpleTotals (:516-571) on fixtures generated like
 // csvplus_test.go:1207-1333.
 // Exit code 0 = all checks hold.
+#include <unistd.h>
+
 #include <cstdio>
 #include <cstdlib>
+#include <fstream>
 #include <iostream>
 #include <cstring>
 #include <sstream>
@@ -50,6 +53,38 @@ int main() {
         std::ostringstream out;
         Take(FromString(people).SelectColumns({"id", "name", "surname", "born"})).ToCsv(out, {"id", "name", "surname", "born"});
         CHECK(out.str() == people);
+        // TestWriteFile streamed: FromFile -> ToCsvFile with the input parsed in batches of 64 bytes (a few records each)
+        {
+            char in_name[] = "/tmp/csvplus_example_XXXXXX";
+            const int fd = mkstemp(in_name);
+            CHECK(fd >= 0);
+            CHECK(write(fd, people.data(), people.size()) == (ssize_t)people.size());
+            close(fd);
+            const std::string out_name = std::string(in_name) + ".out";
+            const uint64_t saved = StreamBatchBytes();
+            StreamBatchBytes() = 64;
+            Take(FromFile(in_name).SelectColumns({"id", "name", "surname", "born"})).ToCsvFile(out_name, {"id", "name", "surname", "born"});
+            std::ifstream back(out_name, std::ios::binary);
+            std::stringstream got; got << back.rdbuf();
+            CHECK(got.str() == people);
+            // a join over batches, and a source error in a later batch: the file is removed
+            std::ostringstream streamed_js;
+            Take(FromString(orders).SelectColumns({"order_id", "cust_id", "qty"})).Join(idx, {"cust_id"}).Top(3).ToJSON(streamed_js);
+            long sjoined = 0;
+            Take(FromString(orders).SelectColumns({"order_id", "cust_id", "qty"})).Join(idx, {"cust_id"})([&](const Row&) { sjoined++; });
+            CHECK(sjoined == 10000);
+            try {
+                Take(FromString(people + "1,2\n")).ToCsvFile(out_name, {"id"});
+                CHECK(false);
+            } catch (const DataSourceError& e) { CHECK(std::string(e.what()) == "row 122: wrong number of fields"); }
+            std::ifstream gone(out_name);
+            CHECK(!gone.good());
+            StreamBatchBytes() = saved;
+            std::ostringstream whole_js;
+            Take(FromString(orders).SelectColumns({"order_id", "cust_id", "qty"})).Join(idx, {"cust_id"}).Top(3).ToJSON(whole_js);
+            CHECK(streamed_js.str() == whole_js.str() && whole_js.str().size() > 100);
+            std::remove(in_name);
+        }
         // TestJSONStruct (csvplus_test.go:1016): SelectColumns -> ToJSON, keys sorted, one object per line
         std::ostringstream js, want_js;
         Take(FromString(people).SelectColumns({"name", "surname", "born"})).ToJSON(js);

@@ -33,6 +33,7 @@ extern "C" {
 typedef struct cpb_ctx cpb_ctx;
 typedef struct cpb_table cpb_table; /* columnar batch of rows: Arrow-style string columns in HBM */
 typedef struct cpb_index cpb_index; /* csvplus Index (csvplus.go:610-614): table sorted on key columns */
+typedef struct cpb_stream cpb_stream; /* an input parsed in batches of whole records */
 
 typedef struct cpb_str {
     const char* ptr;
@@ -127,6 +128,9 @@ int cpb_sync(cpb_ctx* ctx);
  * iterations of a loop pay for the growth).  There is no counterpart in csvplus.go (Go's heap grows the same way). */
 int cpb_pool_reserve(cpb_ctx* ctx, uint64_t nbytes);
 const char* cpb_last_error(cpb_ctx* ctx); /* last CUDA / argument error text of this ctx */
+/* *bytes = the most device memory the ctx's pool has had allocated at once since the last reset (reset != 0 then starts
+ * a new window at the current use): the peak memory of a step, a stream, a test */
+int cpb_pool_used_high(cpb_ctx* ctx, int reset, uint64_t* bytes);
 
 /* Staging memory.  Host: pinned, the Go side fills it with io.ReadFull (replaces the 4 KB bufio reads
  * under csvplus.go:1091).  Device: zero-padded input buffer for callers that produce CSV bytes on the GPU. */
@@ -148,6 +152,30 @@ int cpb_memcpy_d2h(cpb_ctx* ctx, void* dst_host, const void* src_dev, uint64_t n
  * Column order of the table = spec order (or file header order when nspec=0). */
 int cpb_parse_csv(cpb_ctx* ctx, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts,
                   const cpb_header_col* spec, int nspec, const cpb_pred* filter, cpb_table** out, cpb_error* err);
+
+/* ------------------------------------------------------------------ streamed parse
+ * Reader.Iterate over an input of any size (csvplus.go:1080-1146 pulls one record at a time): the input is pushed in
+ * host pieces and parsed in batches of whole records, cut on the GPU at the end of the last complete record; the tail
+ * is carried to the front of the next batch.  Concatenating the batches' tables gives cpb_parse_csv's rows, and the
+ * first error and its line are cpb_parse_csv's (every line number and table first_line is global).
+ *   open : reader options, header spec and fused filter as cpb_parse_csv; `filter` is borrowed until cpb_stream_free.
+ *   push : appends bytes behind the carried tail; the host->device copy is enqueued on the stream's own copy stream and
+ *          the call returns; host_bytes must stay untouched until the next cpb_stream_next returns.  is_last marks the
+ *          end of the input (nbytes may be 0).
+ *   next : parses the complete records pushed so far.  *out = NULL when there is none yet (push more); CPB_ERR_DATA with
+ *          the rows before the error as in cpb_parse_csv; *done = 1 after the last batch or an error.  One host
+ *          synchronisation for the cut, besides the parse's own.
+ * The first batch must hold the whole first record (header): it grows until it does.  Device memory: two staging slots
+ * of about one batch plus the longest record, and one batch's tables.  With CommentChar or LazyQuotes the cut takes the
+ * record-boundary DFA of the general reader path. */
+int cpb_stream_open(cpb_ctx* ctx, const cpb_reader_opts* opts, const cpb_header_col* spec, int nspec, const cpb_pred* filter,
+                    cpb_stream** out, cpb_error* err);
+int cpb_stream_push(cpb_stream* s, const void* host_bytes, uint64_t nbytes, int is_last);
+int cpb_stream_next(cpb_stream* s, cpb_table** out, int* done, cpb_error* err);
+void cpb_stream_free(cpb_stream* s);
+/* the cut alone: the end of the last complete record of `bytes` (which start at a record start), 0 when there is none —
+ * what cpb_stream_next parses of a buffer that is not the last (tests / timing) */
+int cpb_csv_stream_cut(cpb_ctx* ctx, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts, uint64_t* cut);
 
 /* ------------------------------------------------------------------ tables */
 int64_t cpb_table_num_rows(const cpb_table* t);
