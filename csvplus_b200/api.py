@@ -15,6 +15,7 @@ from __future__ import annotations
 import ctypes as C
 import io
 import os
+import stat
 from typing import Callable, Iterable
 
 import numpy as np
@@ -26,10 +27,10 @@ Row = dict  # map[string]string, csvplus.go:59 (values are str; bytes survive vi
 # rows per cpb_table_to_json_into call when DataSource.ToJSON writes a device table: one call produces < 4 GiB, and
 # about 2.4 GB for joined rows of ~150 B.  A batch that is still too large is split in halves.
 JSON_BATCH_ROWS = 1 << 24
-# bytes per host push of a streamed input (FromFile / FromReader / host FromBytes, cpb_stream_*): one batch is parsed per
-# push, so every column of a batch stays far below the 4 GiB a column of one table may hold.  An input of at most this
-# size is parsed in one cpb_parse_csv call.  128 MiB: on an H100 the streamed orders join of DESIGN §3.7 ran as fast as
-# at 64 MiB with half the host synchronisations, and slower with larger batches (less copy / compute overlap).
+# bytes per host push of an input (FromFile / FromReader / host FromBytes, cpb_stream_*): one batch is parsed per push, so
+# every column of a batch stays far below the 4 GiB a column of one table may hold.  An input of at most this size is one
+# push.  128 MiB: on an H100 the streamed orders join of DESIGN §3.7 ran as fast as at 64 MiB with half the host
+# synchronisations, and slower with larger batches (less copy / compute overlap).
 STREAM_BATCH_BYTES = 128 << 20
 
 
@@ -482,11 +483,15 @@ class Table:
         self.ctx.lib.cpb_host_free(self.ctx.h, p)
         return out
 
-    def to_csv_into(self, dst: "HostBuffer", offset: int, *cols, header: bool = True) -> int:
-        """one batch of a streamed ToCsv into pinned host memory (cpb_table_to_csv_into); returns the bytes written"""
+    def to_csv_into(self, dst: "HostBuffer | None", offset: int, *cols, header: bool = True) -> int:
+        """one batch of ToCsv into pinned host memory (cpb_table_to_csv_into).  Returns the batch's size in bytes; when
+        that exceeds the room left in dst (or dst is None), nothing is written."""
         a, keep = _strs(cols); n = C.c_uint64(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_to_csv_into(self.ctx.h, self.h, a, len(cols), int(header), C.c_void_p(dst.ptr + offset),
-                                                dst.nbytes - offset, C.byref(n), C.byref(e))
+        ptr, cap = (dst.ptr + offset, dst.nbytes - offset) if dst is not None else (None, 0)
+        st = self.ctx.lib.cpb_table_to_csv_into(self.ctx.h, self.h, a, len(cols), int(header), C.c_void_p(ptr), cap, C.byref(n),
+                                                C.byref(e))
+        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
+            return n.value
         if st:
             _raise(st, e, self.ctx)
         return n.value
@@ -588,21 +593,28 @@ def parse_csv(ctx: Context, data, *, on_device=False, nbytes=None, delimiter=","
               trim_leading_space=False, header_from_first_row=True, spec: list | None = None, pred: Predicate | None = None):
     """cpb_parse_csv.  data: bytes / numpy uint8 / HostBuffer (host) or DeviceBuffer / int pointer (device).
     Returns (Table, DataSourceError | None): the table holds the rows delivered before the error."""
-    opts = _abi.ReaderOpts(ord(delimiter), ord(comment) if comment else 0, num_fields, int(lazy_quotes), int(trim_leading_space),
-                           int(header_from_first_row), 0)
+    opts = _reader_opts(delimiter, comment, num_fields, lazy_quotes, trim_leading_space, header_from_first_row)
     keep = []
-    if isinstance(data, DeviceBuffer):
-        ptr, n, on_device = data.ptr, data.nbytes if nbytes is None else nbytes, True
-    elif isinstance(data, HostBuffer):
-        ptr, n = data.ptr, data.nbytes if nbytes is None else nbytes
-    elif isinstance(data, np.ndarray):
-        a = np.ascontiguousarray(data, np.uint8); keep.append(a)
-        ptr, n = a.ctypes.data, a.size if nbytes is None else nbytes
-    elif isinstance(data, int):
-        ptr, n = data, nbytes
-    else:
-        b = bytes(data); keep.append(b)
-        ptr, n = C.cast(C.c_char_p(b), C.c_void_p).value, len(b)
+    ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
+    sa, nspec, pp = _spec_and_pred(spec, pred, keep)
+    h = C.c_void_p(); e = _abi.Error()
+    st = ctx.lib.cpb_parse_csv(ctx.h, C.c_void_p(ptr), n, int(dev), C.byref(opts), sa, nspec, pp, C.byref(h), C.byref(e))
+    if st == 1 and h.value:
+        return Table(ctx, h), DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
+    if st:
+        _raise(st, e, ctx)
+    return Table(ctx, h), None
+
+
+def _reader_opts(delimiter=",", comment="", num_fields=0, lazy_quotes=False, trim_leading_space=False,
+                 header_from_first_row=True) -> _abi.ReaderOpts:
+    return _abi.ReaderOpts(ord(delimiter), ord(comment) if comment else 0, num_fields, int(lazy_quotes), int(trim_leading_space),
+                           int(header_from_first_row), 0)
+
+
+def _spec_and_pred(spec: list | None, pred: Predicate | None, keep: list) -> tuple:
+    """-> (HeaderCol array of spec's (name, index) pairs, their count, pointer to pred's cpb_pred tree or None); keep
+    holds what they point to"""
     spec = spec or []
     sa = (_abi.HeaderCol * max(1, len(spec)))()
     for i, (name, idx) in enumerate(spec):
@@ -611,13 +623,8 @@ def parse_csv(ctx: Context, data, *, on_device=False, nbytes=None, delimiter=","
     pp = None
     if pred is not None:
         pc = pred._c(keep); keep.append(pc); pp = C.byref(pc)
-    h = C.c_void_p(); e = _abi.Error()
-    st = ctx.lib.cpb_parse_csv(ctx.h, C.c_void_p(ptr), n, int(on_device), C.byref(opts), sa, len(spec), pp, C.byref(h), C.byref(e))
-    if st == 1 and h.value:
-        return Table(ctx, h), DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
-    if st:
-        _raise(st, e, ctx)
-    return Table(ctx, h), None
+    keep.append(sa)
+    return sa, len(spec), pp
 
 
 def _input_ptr(data, nbytes, on_device, keep):
@@ -648,7 +655,7 @@ def csv_quote_parity(ctx: Context, data, *, nbytes=None, on_device=False) -> int
 def csv_stream_cut(ctx: Context, data, *, nbytes=None, on_device=False, delimiter=",", comment="", lazy_quotes=False,
                    trim_leading_space=False) -> int:
     """cpb_csv_stream_cut: the end of the last complete record of data (0: none), the cut of one stream batch"""
-    opts = _abi.ReaderOpts(ord(delimiter), ord(comment) if comment else 0, 0, int(lazy_quotes), int(trim_leading_space), 1, 0)
+    opts = _reader_opts(delimiter, comment, 0, lazy_quotes, trim_leading_space)
     keep = []
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
     out = C.c_uint64()
@@ -662,20 +669,13 @@ def parse_csv_shard(ctx: Context, data, *, own_bytes: int, shard_index: int, is_
                     delimiter=",", num_fields=0, header_from_first_row=True, spec: list | None = None, pred: Predicate | None = None):
     """cpb_parse_csv_shard.  Returns (Table, records owned by the shard, DataSourceError | None) — the error's Line is the
     LOCAL 0-based ordinal of the failing record among the shard's records."""
-    opts = _abi.ReaderOpts(ord(delimiter), 0, num_fields, 0, 0, int(header_from_first_row), 0)
+    opts = _reader_opts(delimiter, num_fields=num_fields, header_from_first_row=header_from_first_row)
     keep = []
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
-    spec = spec or []
-    sa = (_abi.HeaderCol * max(1, len(spec)))()
-    for i, (name, idx) in enumerate(spec):
-        nb = _enc(name); keep.append(nb)
-        sa[i].name.ptr, sa[i].name.len, sa[i].index = nb, len(nb), idx
-    pp = None
-    if pred is not None:
-        pc = pred._c(keep); keep.append(pc); pp = C.byref(pc)
+    sa, nspec, pp = _spec_and_pred(spec, pred, keep)
     h = C.c_void_p(); e = _abi.Error(); recs = C.c_uint64()
     st = ctx.lib.cpb_parse_csv_shard(ctx.h, C.c_void_p(ptr), n, int(dev), own_bytes, shard_index, int(is_last), initial_parity, C.byref(opts), sa,
-                                     len(spec), pp, C.byref(h), C.byref(recs), C.byref(e))
+                                     nspec, pp, C.byref(h), C.byref(recs), C.byref(e))
     if st == 1 and h.value:
         return Table(ctx, h), recs.value, DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
     if st:
@@ -776,12 +776,10 @@ class Index:
 
 # ------------------------------------------------------------------ Reader (csvplus.go:922-1146)
 class Reader:
-    def __init__(self, source: Callable[[], bytes | np.ndarray | DeviceBuffer | HostBuffer], ctx: Context | None = None,
-                 chunks: Callable[[], Iterable] | None = None):
-        """source: the whole input for one cpb_parse_csv call.  chunks: when given, -> None if the input fits one batch
-        (then `source` is parsed), else an iterator of (host piece as numpy uint8, is the last piece), each piece left
-        untouched until the next one is asked for."""
-        self._source, self._ctx, self._chunks = source, ctx, chunks
+    def __init__(self, pieces: Callable[[], Iterable], ctx: Context | None = None):
+        """pieces: -> an iterator of (piece, is the last piece), each host piece (numpy uint8) left untouched until the
+        next one is asked for; a DeviceBuffer is the whole input as one piece"""
+        self._pieces, self._ctx = pieces, ctx
         self.delimiter, self.comment = ",", ""
         self.numFields, self.lazyQuotes, self.trimLeadingSpace = 0, False, False
         self.header: dict | None = None
@@ -827,51 +825,47 @@ class Reader:
     def NumFieldsAuto(self): return self.NumFields(0)
     def NumFieldsAny(self): return self.NumFields(-1)
 
-    def _parse(self, pred: Predicate | None = None):
-        data = self._source()
-        spec = list(self.header.items()) if self.header else []
-        return parse_csv(self.ctx, data, delimiter=self.delimiter, comment=self.comment, num_fields=self.numFields,
-                         lazy_quotes=self.lazyQuotes, trim_leading_space=self.trimLeadingSpace,
-                         header_from_first_row=self.headerFromFirstRow, spec=spec, pred=pred)
+    def _options(self) -> dict:
+        """the reader's options and header spec as keyword arguments of parse_csv"""
+        return dict(delimiter=self.delimiter, comment=self.comment, num_fields=self.numFields, lazy_quotes=self.lazyQuotes,
+                    trim_leading_space=self.trimLeadingSpace, header_from_first_row=self.headerFromFirstRow,
+                    spec=list(self.header.items()) if self.header else [])
 
     def _batches(self, pred: Predicate | None = None):
-        """-> (Table, DataSourceError | None, streamed) per batch; the error comes with the last batch.  An input that fits
-        one batch is one cpb_parse_csv call (streamed = False); a larger one goes through cpb_stream_*.  Closing the
-        generator early stops reading the input."""
-        pieces = self._chunks() if self._chunks is not None else None
-        if pieces is None:
-            t, err = self._parse(pred)
-            yield t, err, False
-            return
-        st = _Stream(self.ctx, self, pred)
+        """-> (Table, DataSourceError | None, several) per batch, several: the input was pushed in more than one piece;
+        the error comes with the last batch.  Host pieces go through cpb_stream_*: one piece is one push, parsed as one
+        batch.  Closing the generator early stops reading the input."""
+        pieces = iter(self._pieces())
+        st = None
         try:
+            piece, last = next(pieces, (None, True))
+            if isinstance(piece, DeviceBuffer):  # device memory cannot be pushed: one cpb_parse_csv call
+                t, err = parse_csv(self.ctx, piece, pred=pred, **self._options())
+                yield t, err, False
+                return
+            st = _Stream(self.ctx, pred, **self._options())
             # one cpb_stream_next per push parses every complete record pushed so far.  A batch is delivered after the
             # next piece has been pushed: that piece's host-to-device copy (the stream's copy stream) overlaps what the
             # consumer does with the batch on the context's stream, and it is parsed only after the batch was delivered.
-            pending, finished = None, False
-            for piece, last in pieces:
+            # An iterator that ends without a last piece is closed by an empty last push.
+            several = not last  # known from the first piece, so every batch, the first one included, reports it
+            pending = None
+            while True:
                 st.push(piece, last)
                 if pending is not None:
-                    yield pending
+                    yield (*pending, several)
                     pending = None
                 t, err, done = st.next()
                 if t is not None or err is not None:
-                    pending = (t, err, True)
-                if done or err is not None:
-                    finished = True
+                    pending = (t, err)
+                if last or done or err is not None:
                     break
-            if not finished:
-                st.push(None, True)
-                if pending is not None:
-                    yield pending
-                    pending = None
-                t, err, done = st.next()
-                if t is not None or err is not None:
-                    pending = (t, err, True)
+                piece, last = next(pieces, (None, True))
             if pending is not None:
-                yield pending
+                yield (*pending, several)
         finally:
-            st.free()
+            if st is not None:
+                st.free()
             close = getattr(pieces, "close", None)
             if close is not None:
                 close()
@@ -883,21 +877,13 @@ class Reader:
 class _Stream:
     """cpb_stream: one input parsed in batches of whole records"""
 
-    def __init__(self, ctx: Context, r: Reader, pred: Predicate | None):
+    def __init__(self, ctx: Context, pred: Predicate | None, spec: list | None = None, **opts):
+        """opts: the reader options of parse_csv"""
         self.ctx, self._keep, self._pushed = ctx, [], None
-        opts = _abi.ReaderOpts(ord(r.delimiter), ord(r.comment) if r.comment else 0, r.numFields, int(r.lazyQuotes),
-                               int(r.trimLeadingSpace), int(r.headerFromFirstRow), 0)
-        spec = list(r.header.items()) if r.header else []
-        sa = (_abi.HeaderCol * max(1, len(spec)))()
-        for i, (name, idx) in enumerate(spec):
-            nb = _enc(name); self._keep.append(nb)
-            sa[i].name.ptr, sa[i].name.len, sa[i].index = nb, len(nb), idx
-        pp = None
-        if pred is not None:
-            pc = pred._c(self._keep); self._keep.append(pc); pp = C.byref(pc)  # borrowed by the stream until it is freed
-        self._keep += [opts, sa]
+        o = _reader_opts(**opts)
+        sa, nspec, pp = _spec_and_pred(spec, pred, self._keep)  # the predicate is borrowed by the stream until it is freed
         h = C.c_void_p(); e = _abi.Error()
-        st = ctx.lib.cpb_stream_open(ctx.h, C.byref(opts), sa, len(spec), pp, C.byref(h), C.byref(e))
+        st = ctx.lib.cpb_stream_open(ctx.h, C.byref(o), sa, nspec, pp, C.byref(h), C.byref(e))
         if st:
             _raise(st, e, ctx)
         self.h = h
@@ -929,27 +915,16 @@ class _Stream:
             self.h = None
 
 
-def _file_pieces(name: str, ctx_of: Callable[[], Context]):
-    """None when the file fits one batch (or is not a regular file: read whole, as before); else a generator of the file's
-    pieces, read by a helper thread into two pinned host buffers: piece k+1 is read while piece k is being parsed"""
-    try:
-        size = os.stat(name).st_size
-        regular = os.path.isfile(name)
-    except OSError:
-        return None  # the open error is raised by the one-shot source
-    if not regular or size <= STREAM_BATCH_BYTES:
-        return None
-    return _pinned_pieces(name, ctx_of())
-
-
-def _pinned_pieces(name: str, ctx: Context):
+def _pinned_pieces(f, ctx: Context):
+    """the pieces of the open file f, read by a helper thread into two pinned host buffers: piece k+1 is read while piece
+    k is being parsed.  Closes f."""
     from concurrent.futures import ThreadPoolExecutor
     step = STREAM_BATCH_BYTES
     bufs = [HostBuffer(ctx, step), HostBuffer(ctx, step)]
     views = [b.array() for b in bufs]
     ex = ThreadPoolExecutor(1)
     try:
-        with open(name, "rb", buffering=0) as f:
+        with f:
             def fill(k):
                 n, v = 0, memoryview(views[k])
                 while n < step:
@@ -977,8 +952,8 @@ def _pinned_pieces(name: str, ctx: Context):
 
 
 def _reader_pieces(inp):
-    """pieces of an io reader, read with readinto (or read(n)); None (and the bytes as the one-shot input) when the
-    first piece is the whole input"""
+    """the pieces of an io reader, read with readinto (or read(n)); a piece is known to be the last one when it is short
+    or the next one is empty"""
     step = STREAM_BATCH_BYTES
 
     def read_piece():
@@ -999,64 +974,62 @@ def _reader_pieces(inp):
                 a[n:n + len(b)] = np.frombuffer(b, np.uint8); n += len(b)
         return a[:n]
 
-    first = read_piece()
-    if first.size < step:
-        return first, None
-    second = read_piece()
-    if second.size == 0:
-        return first, None
-
-    def gen():
-        yield first, False
-        yield second, False
-        while True:
-            p = read_piece()
-            if p.size == 0:
-                return  # the stream is closed by an empty last push
-            yield p, False
-    return None, gen()
+    p = read_piece()
+    while True:
+        q = read_piece() if p.size == step else None
+        last = q is None or q.size == 0
+        yield p, last
+        if last:
+            return
+        p = q
 
 
 def FromFile(name: str, ctx: Context | None = None) -> Reader:  # csvplus.go:950
-    def src():
+    """a regular file that fits one piece is read whole into pageable memory; a larger one is read by a helper thread
+    into two pinned buffers; any other file (a FIFO, a character device) is read as FromReader reads it"""
+    def pieces():
         try:
-            return np.fromfile(name, dtype=np.uint8)
+            f = open(name, "rb", buffering=0)
         except OSError as e:  # mapError's *os.PathError branch, csvplus.go:1216-1220
             raise DataSourceError(1, f"open: {e.strerror.lower() if e.strerror else e}") from None
-    r = Reader(src, ctx)
-    r._chunks = lambda: _file_pieces(name, lambda: r.ctx)
+        st = os.fstat(f.fileno())
+        if not stat.S_ISREG(st.st_mode):
+            return _closing(f, _reader_pieces(f))
+        if st.st_size > STREAM_BATCH_BYTES:
+            return _pinned_pieces(f, r.ctx)
+        with f:
+            return [(np.fromfile(f, dtype=np.uint8), True)]
+    r = Reader(pieces, ctx)
     return r
 
 
-def FromReader(inp: io.IOBase, ctx: Context | None = None) -> Reader:  # csvplus.go:936
-    whole = []
+def _closing(f, pieces):
+    with f:
+        yield from pieces
 
-    def chunks():
-        first, gen = _reader_pieces(inp)
-        whole[:] = [first]
-        return gen
-    return Reader(lambda: whole.pop() if whole else inp.read(), ctx, chunks)
+
+def FromReader(inp: io.IOBase, ctx: Context | None = None) -> Reader:  # csvplus.go:936
+    return Reader(lambda: _reader_pieces(inp), ctx)
 
 
 FromReadCloser = FromReader
 
 
 def FromBytes(data, ctx: Context | None = None) -> Reader:
-    """bytes / numpy / HostBuffer / DeviceBuffer already in memory.  Host memory larger than STREAM_BATCH_BYTES is parsed
-    in batches (cpb_stream_*); a DeviceBuffer is always parsed in one call."""
-    def chunks():
+    """bytes / numpy / HostBuffer / DeviceBuffer already in memory.  Host memory is pushed in pieces of STREAM_BATCH_BYTES
+    (one piece when it fits); a DeviceBuffer is parsed in one call."""
+    def pieces():
         if isinstance(data, DeviceBuffer):
-            return None
+            return [(data, True)]
         if isinstance(data, HostBuffer):
             a = data.array()
         elif isinstance(data, np.ndarray):
             a = np.ascontiguousarray(data, np.uint8).reshape(-1)
         else:
             a = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.frombuffer(bytes(data), np.uint8)
-        if a.size <= STREAM_BATCH_BYTES:
-            return None
-        return ((a[i:i + STREAM_BATCH_BYTES], i + STREAM_BATCH_BYTES >= a.size) for i in range(0, a.size, STREAM_BATCH_BYTES))
-    return Reader(lambda: data, ctx, chunks)
+        step = STREAM_BATCH_BYTES
+        return ((a[i:i + step], i + step >= a.size) for i in range(0, max(a.size, 1), step))
+    return Reader(pieces, ctx)
 
 
 # ------------------------------------------------------------------ DataSource (csvplus.go:207-608)
@@ -1109,8 +1082,9 @@ class DataSource:
         return Context.default()
 
     def _batches(self):
-        """-> (state, pending error, streamed) per batch of the source; state: ("table", Table | None) or ("rows", list[Row]).
-        A Reader over a large host input yields one batch per parsed batch (streamed = True), every other source one.
+        """-> (state, pending error, several) per batch of the source; state: ("table", Table | None) or ("rows", list[Row]).
+        A Reader yields one batch per parsed batch (several: its input was pushed in more than one piece), every other
+        source one.
         Top / Drop / TakeWhile / DropWhile carry their counters across batches; when one of them has pulled all it will
         ever deliver, the input is no longer read."""
         ops = list(self._ops)
@@ -1122,9 +1096,9 @@ class DataSource:
                 pred = ops.pop(0)[1]  # fused into the parse kernel
             src = s._batches(pred)
             try:
-                for t, err, streamed in src:
+                for t, err, several in src:
                     state, err, stop = self._apply(("table", t), err, ops, carry)
-                    yield state, err, streamed
+                    yield state, err, several
                     if stop or err is not None:
                         return
             finally:
@@ -1251,17 +1225,14 @@ class DataSource:
         if len(columns) == 0:
             raise ValueError("empty column list in ToCsv() function")
         wrote_header = False
-        hold: list = []  # the pinned buffer the batches of a streamed input are serialised into
+        hold: list = []  # the pinned buffer every batch is serialised into
         try:
-            for state, err, streamed in self._batches():
+            for state, err, _ in self._batches():
                 t = self._as_table(state)
-                if t is None:
-                    if not wrote_header:
-                        out.write((",".join(columns) + "\n").encode())
-                elif not streamed:
-                    out.write(t.to_csv(*columns))
-                else:  # the csv.Writer writes the header once, before the first batch (csvplus.go:387)
-                    _csv_into(t, out, columns, not wrote_header, hold)
+                if t is not None:  # the csv.Writer writes the header once, before the first batch (csvplus.go:387)
+                    _write_into(out, hold, t.ctx, lambda buf: t.to_csv_into(buf, 0, *columns, header=not wrote_header))
+                elif not wrote_header:
+                    out.write((",".join(columns) + "\n").encode())
                 wrote_header = True
                 if err is not None:
                     raise err
@@ -1283,39 +1254,27 @@ class DataSource:
         it: `[`, then per row the object with its keys sorted and a newline, a `,` before every row but the first, `]`.
         A device table is serialised by the GPU in row-range batches; rows left on the host (after an opaque Map or
         Filter(func), or TakeRows of rows with different columns) are encoded here.  On a source error nothing is written
-        when the input was parsed in one batch; a streamed input keeps what its earlier batches wrote (a prefix of the
+        when the input was pushed in one piece; an input pushed in several keeps what its batches wrote (a prefix of the
         array, without `]`), as the reference's encoder has flushed them."""
-        hold: list = []  # the pinned buffer the batches of a streamed input are serialised into
+        hold: list = []  # the pinned buffer every batch is serialised into
+        opened = False
         try:
-            self._to_json(out, hold)
+            for state, err, several in self._batches():
+                if err is not None and not several:
+                    raise err
+                if state[0] == "table":
+                    if state[1] is not None and len(state[1]):
+                        _json_batches(state[1], out, not opened, hold)
+                        opened = True
+                elif state[1]:
+                    out.write(_json_rows(state[1], not opened, False))
+                    opened = True
+                if err is not None:
+                    raise err
+            out.write(b"]" if opened else b"[]")
         finally:
             for b in hold:
                 b.free()
-
-    def _to_json(self, out, hold: list):
-        opened = False
-        for state, err, streamed in self._batches():
-            if not streamed:  # one batch: the whole document at once
-                if err is not None:
-                    raise err
-                if state[0] == "table":
-                    if state[1] is None:
-                        out.write(b"[]")
-                    else:
-                        _json_batches(state[1], out)
-                    return
-                out.write(_json_rows(state[1], True, True))
-                return
-            if state[0] == "table":
-                if state[1] is not None and len(state[1]):
-                    _json_batches(state[1], out, first=not opened, last=False, hold=hold)
-                    opened = True
-            elif state[1]:
-                out.write(_json_rows(state[1], not opened, False))
-                opened = True
-            if err is not None:
-                raise err
-        out.write(b"]" if opened else b"[]")
 
     def ToJSONFile(self, name: str):  # csvplus.go:477-479
         try:
@@ -1394,58 +1353,37 @@ def _json_rows(rows: list, first: bool, last: bool) -> bytes:
     return b"".join(parts)
 
 
-def _csv_into(t: Table, out: io.IOBase, columns, header: bool, hold: list):
-    """one batch of a streamed ToCsv: serialised into the pinned buffer hold[0] (grown to the size the batch reports and
-    kept for the next batch), then written to out"""
-    a, keep = _strs(columns)
+def _write_into(out: io.IOBase, hold: list, ctx: Context, serialise: Callable[["HostBuffer | None"], int]):
+    """serialise(buf) writes one batch into the pinned buffer buf and returns its size, or writes nothing when the size
+    exceeds buf (or buf is None).  The buffer hold[0] is grown to the size reported and the batch serialised again, then
+    the batch is written to out; hold keeps the buffer for the next batch (the caller frees it)."""
     while True:
         buf = hold[0] if hold else None
-        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
-        n = C.c_uint64(); e = _abi.Error()
-        st = t.ctx.lib.cpb_table_to_csv_into(t.ctx.h, t.h, a, len(columns), int(header), C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
-        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
-            if buf is not None:
-                buf.free()
-            hold[:] = [HostBuffer(t.ctx, n.value + n.value // 4 + 64)]
-            continue
-        if st:
-            _raise(st, e, t.ctx)
-        if n.value:
-            out.write(memoryview(buf.array()[:n.value]))
-        return
-
-
-def _json_batches(t: Table, out: io.IOBase, first: bool = True, last: bool = True, hold: list | None = None):
-    """ToJSON of a device table: row-range slices of at most JSON_BATCH_ROWS rows, each serialised into one reused pinned
-    buffer that grows to the size a batch reports, then written to out.  first / last: the table opens / closes the
-    array.  hold: a list that keeps the buffer for the next table (the caller frees it)."""
-    n = len(t)
-    buf, lo, step = (hold[0] if hold else None), 0, JSON_BATCH_ROWS
-    try:
-        while True:
-            hi = min(n, lo + step)
-            part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
-            try:
-                w = part.to_json_into(buf, 0, first and lo == 0, last and hi == n)
-            except CsvPlusError as e:
-                if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
-                    raise
-                step = (hi - lo) // 2
-                continue
-            if buf is None or w > buf.nbytes:
-                if buf is not None:
-                    buf.free()
-                buf = HostBuffer(t.ctx, w + w // 4 + 64)
-                if hold is not None:
-                    hold[:] = [buf]
-                continue
-            out.write(memoryview(buf.array()[:w]))
-            lo = hi
-            if lo >= n:
-                return
-    finally:
-        if buf is not None and hold is None:
+        n = serialise(buf)
+        if n <= (buf.nbytes if buf is not None else 0):
+            if n:
+                out.write(memoryview(buf.array()[:n]))
+            return
+        if buf is not None:
             buf.free()
+        hold[:] = [HostBuffer(ctx, n + n // 4 + 64)]
+
+
+def _json_batches(t: Table, out: io.IOBase, first: bool, hold: list):
+    """ToJSON of a device table with rows, without the closing `]`: row-range slices of at most JSON_BATCH_ROWS rows, each
+    written through the pinned buffer of hold (_write_into).  first: the table opens the array."""
+    n, lo, step = len(t), 0, JSON_BATCH_ROWS
+    while lo < n:
+        hi = min(n, lo + step)
+        part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
+        try:
+            _write_into(out, hold, t.ctx, lambda buf: part.to_json_into(buf, 0, first and lo == 0, False))
+        except CsvPlusError as e:
+            if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
+                raise
+            step = (hi - lo) // 2
+            continue
+        lo = hi
 
 
 def Take(src) -> DataSource:  # csvplus.go:252-256

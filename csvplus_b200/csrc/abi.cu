@@ -295,6 +295,29 @@ int cpb_memcpy_d2h(cpb_ctx* h, void* dst, const void* src, uint64_t n) {
 }
 
 // ------------------------------------------------------------------ parse
+// host input is copied into a device buffer (32 MiB size classes: batches reuse pool blocks) followed by at least 16 zero
+// bytes; device input is used in place
+static const uint8_t* stage_input(Ctx* c, const void* bytes, uint64_t nbytes, int on_device, Buf& staged) {
+    if (on_device) return (const uint8_t*)bytes;
+    staged = dev_alloc(c, (nbytes + 32 + (32u << 20) - 1) / (32u << 20) * (32u << 20));  // holds the zeroed 32 bytes too
+    CPB_CUDA(cudaMemsetAsync(staged->as<uint8_t>() + (nbytes & ~15ull), 0, 32, c->stream));
+    if (nbytes) {
+        KernelTimer kt(c, "h2d_input", nbytes, 0);
+        CPB_CUDA(cudaMemcpyAsync(staged->p, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
+    }
+    return staged->as<uint8_t>();
+}
+// the (name, index) pairs of a reader's header spec; a name given twice is an error (csvplus.go:1047-1049)
+static std::vector<std::pair<std::string, int>> header_spec(const cpb_header_col* spec, int nspec) {
+    std::vector<std::pair<std::string, int>> sp;
+    for (int i = 0; i < nspec; i++) {
+        std::string nm = to_string(spec[i].name);
+        for (auto& s : sp) if (s.first == nm) throw ArgError{CPB_ERR_ARG, "header spec: duplicate column name: " + nm};
+        sp.emplace_back(nm, spec[i].index);
+    }
+    return sp;
+}
+
 int cpb_parse_csv(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts,
                   const cpb_header_col* spec, int nspec, const cpb_pred* filter, cpb_table** out, cpb_error* err) {
     if (!h || !out || !opts || (nbytes && !bytes) || nspec < 0) return CPB_ERR_ARG;
@@ -302,22 +325,9 @@ int cpb_parse_csv(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device,
     clear_error(err);
     *out = nullptr;
     CPB_TRY(c, err)
-    std::vector<std::pair<std::string, int>> sp;
-    for (int i = 0; i < nspec; i++) {
-        std::string nm = to_string(spec[i].name);
-        for (auto& s : sp) if (s.first == nm) throw ArgError{CPB_ERR_ARG, "header spec: duplicate column name: " + nm};  // csvplus.go:1047-1049
-        sp.emplace_back(nm, spec[i].index);
-    }
+    auto sp = header_spec(spec, nspec);
     Buf staged;
-    const uint8_t* dev = (const uint8_t*)bytes;
-    if (!on_device) {
-        staged = dev_alloc(c, (nbytes + (32u << 20)) / (32u << 20) * (32u << 20));  // size class: batches reuse pool blocks
-        if (nbytes) {
-            KernelTimer kt(c, "h2d_input", nbytes, 0);
-            CPB_CUDA(cudaMemcpyAsync(staged->p, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
-        }
-        dev = staged->as<uint8_t>();
-    }
+    const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
     bool had_error = false; DataError de{};
     auto t = parse_csv(c, dev, nbytes, *opts, sp, filter, &had_error, &de);
     *out = wrap(t);
@@ -334,13 +344,7 @@ int cpb_stream_open(cpb_ctx* h, const cpb_reader_opts* opts, const cpb_header_co
     clear_error(err);
     *out = nullptr;
     CPB_TRY(c, err)
-    std::vector<std::pair<std::string, int>> sp;
-    for (int i = 0; i < nspec; i++) {
-        std::string nm = to_string(spec[i].name);
-        for (auto& s : sp) if (s.first == nm) throw ArgError{CPB_ERR_ARG, "header spec: duplicate column name: " + nm};  // csvplus.go:1047-1049
-        sp.emplace_back(nm, spec[i].index);
-    }
-    *out = new cpb_stream{stream_open(c, *opts, std::move(sp), filter)};
+    *out = new cpb_stream{stream_open(c, *opts, header_spec(spec, nspec), filter)};
     return CPB_OK;
     CPB_CATCH(c, err)
 }
@@ -374,16 +378,6 @@ void cpb_stream_free(cpb_stream* st) {
 }
 
 // ------------------------------------------------------------------ byte-range shards of one file (SURVEY §8e)
-static const uint8_t* stage_input(Ctx* c, const void* bytes, uint64_t nbytes, int on_device, Buf& staged) {
-    if (on_device) return (const uint8_t*)bytes;
-    staged = dev_alloc(c, (nbytes + (32u << 20)) / (32u << 20) * (32u << 20));
-    CPB_CUDA(cudaMemsetAsync(staged->as<uint8_t>() + (nbytes & ~15ull), 0, 32, c->stream));
-    if (nbytes) {
-        KernelTimer kt(c, "h2d_input", nbytes, 0);
-        CPB_CUDA(cudaMemcpyAsync(staged->p, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
-    }
-    return staged->as<uint8_t>();
-}
 int cpb_csv_quote_parity(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, uint32_t* parity) {
     if (!h || !parity || (nbytes && !bytes)) return CPB_ERR_ARG;
     Ctx* c = &h->c; DeviceGuard g(c);
@@ -744,8 +738,12 @@ int cpb_except(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cp
 }
 
 // ------------------------------------------------------------------ ToCsv
-static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, bool to_host, void** bytes, uint64_t* nbytes,
-                         cpb_error* err) {
+// mode 0: into new pinned host memory, 1: into caller-owned (ideally pinned) host memory of cap bytes, with the header
+// line only when asked for (a csv.Writer writes it once, before the first batch: csvplus.go:387), 2: left on the device.
+// A destination that is too small gets nothing: the call fails with CPB_ERR_ARG and *nbytes = the size needed.
+static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, int mode, void** bytes,
+                         void* host_dst, uint64_t cap, uint64_t* nbytes, cpb_error* err) {
+    if (!h || !t || !nbytes || (mode != 1 && !bytes) || (mode == 1 && cap && !host_dst)) return CPB_ERR_ARG;
     Ctx* c = &h->c; DeviceGuard g(c);
     clear_error(err);
     CPB_TRY(c, err)
@@ -759,14 +757,21 @@ static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, in
         idx.push_back(k);
     }
     uint64_t total = 0;
-    Buf out = table_to_csv(c, *t->t, idx, names, &total, nullptr);
+    Buf out = table_to_csv(c, *t->t, idx, names, with_header != 0, mode == 1 ? cap : UINT64_MAX, &total);
     *nbytes = total;
-    if (to_host) {
+    if (mode == 0) {
         void* hp = nullptr;
         CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
         if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
         sync_stream(c);
         *bytes = hp;
+    } else if (mode == 1) {
+        if (total > cap) throw ArgError{CPB_ERR_ARG, "ToCsv destination too small"};
+        if (total) {
+            KernelTimer kt(c, "d2h_output", total, 0);
+            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        }
+        sync_stream(c);
     } else {
         void* dp = nullptr;
         CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
@@ -776,41 +781,15 @@ static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, in
     return CPB_OK;
     CPB_CATCH(c, err)
 }
-// ToCsv of one batch of a streamed result into caller-owned (ideally pinned) host memory: no allocation per call,
-// the header line only when asked for (a csv.Writer writes it once, before the first batch: csvplus.go:387).
 int cpb_table_to_csv_into(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, void* host_dst,
                           uint64_t cap, uint64_t* nbytes, cpb_error* err) {
-    if (!h || !t || !nbytes || (cap && !host_dst)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    if (n <= 0) throw ArgError{CPB_ERR_ARG, "empty column list in ToCsv() function"};  // csvplus.go:380-382
-    auto names = str_list(cols, n);
-    std::vector<int> idx;
-    for (int i = 0; i < n; i++) {
-        int k = t->t->find(names[i]);
-        if (k < 0 && t->t->nrows > 0)
-            throw DataError{CPB_E_MISSING_COLUMN, i, t->t->first_line, true, "missing column " + go_quote(names[i])};  // :392, :145
-        idx.push_back(k);
-    }
-    uint64_t total = 0, hdr = 0;
-    Buf out = table_to_csv(c, *t->t, idx, names, &total, &hdr);
-    const uint64_t skip = with_header ? 0 : hdr;
-    *nbytes = total - skip;
-    if (*nbytes > cap) throw ArgError{CPB_ERR_ARG, "ToCsv destination too small"};
-    if (*nbytes) {
-        KernelTimer kt(c, "d2h_output", *nbytes, 0);
-        CPB_CUDA(cudaMemcpyAsync(host_dst, out->as<uint8_t>() + skip, *nbytes, cudaMemcpyDeviceToHost, c->stream));
-    }
-    sync_stream(c);
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return to_csv_common(h, t, cols, n, with_header, 1, nullptr, host_dst, cap, nbytes, err);
 }
 int cpb_table_to_csv(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, void** bytes, uint64_t* nbytes, cpb_error* err) {
-    return to_csv_common(h, t, cols, n, true, bytes, nbytes, err);
+    return to_csv_common(h, t, cols, n, 1, 0, bytes, nullptr, 0, nbytes, err);
 }
 int cpb_table_to_csv_device(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, void** bytes, uint64_t* nbytes, cpb_error* err) {
-    return to_csv_common(h, t, cols, n, false, bytes, nbytes, err);
+    return to_csv_common(h, t, cols, n, 1, 2, bytes, nullptr, 0, nbytes, err);
 }
 
 // ------------------------------------------------------------------ ToJSON
@@ -822,7 +801,7 @@ static int to_json_common(cpb_ctx* h, const cpb_table* t, int first, int last, i
     clear_error(err);
     CPB_TRY(c, err)
     uint64_t total = 0;
-    Buf out = table_to_json(c, *t->t, first != 0, last != 0, &total);
+    Buf out = table_to_json(c, *t->t, first != 0, last != 0, mode == 1 ? cap : UINT64_MAX, &total);
     *nbytes = total;
     if (mode == 0) {
         void* hp = nullptr;

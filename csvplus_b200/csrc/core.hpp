@@ -284,11 +284,13 @@ void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi);
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep, bool bug_compatible, const Table* repl = nullptr);
-// write.cu
-Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names,
-                 uint64_t* nbytes, uint64_t* header_bytes);
-// json.cu: ToJSON of every column (keys in bytewise order); '[' before the first row when first, ']' appended when last
-Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbytes);
+// write.cu: ToCsv of columns cols under the header line of names (when with_header).  room: the most bytes the caller can
+// take; when *nbytes exceeds it, null is returned after the length pass, before any output is allocated or written.
+Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, bool with_header,
+                 uint64_t room, uint64_t* nbytes);
+// json.cu: ToJSON of every column (keys in bytewise order); '[' before the first row when first, ']' appended when last;
+// room as table_to_csv
+Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, uint64_t* nbytes);
 // numeric.cu: strconv.Atoi / ParseFloat(s, 64) of every row of column `col` into device values (+ nullable status)
 struct NumResult {
     uint64_t nbad = 0, nrare = 0;  // failing rows, rows the exact (rare) path converted

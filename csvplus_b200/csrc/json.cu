@@ -184,14 +184,15 @@ __global__ void json_value_bytes_kernel(const JsonCol* cols, int ncols, uint64_t
     *out = s;
 }
 
-Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbytes) {
+Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, uint64_t* nbytes) {
     const uint64_t n = (uint64_t)t.nrows;
     if (n == 0) {
         std::string s = std::string(first ? "[" : "") + (last ? "]" : "");
+        *nbytes = s.size();
+        if (*nbytes > room) return nullptr;
         Buf out = dev_alloc(c, 16);
         if (!s.empty()) CPB_CUDA(cudaMemcpyAsync(out->p, s.data(), s.size(), cudaMemcpyHostToDevice, c->stream));
         sync_stream(c);  // s is pageable stack memory
-        *nbytes = s.size();
         return out;
     }
     const int ncols = (int)t.cols.size();
@@ -237,6 +238,8 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbyte
     sync_stream(c);
     const uint64_t body = ht[0], value_bytes = ht[1];
     if (body >= 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToJSON output exceeds 4 GiB; write in smaller batches"};
+    *nbytes = body + (last ? 1 : 0);
+    if (*nbytes > room) return nullptr;
     Buf out = dev_alloc(c, body + 1 + 16);
     {
         KernelTimer kt(c, "json_write", value_bytes + n * 4 * (ncols + 1) + body);
@@ -249,7 +252,6 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t* nbyte
         CPB_CUDA(cudaGetLastError());
     }
     if (last) CPB_CUDA(cudaMemsetAsync(out->as<uint8_t>() + body, ']', 1, c->stream));
-    *nbytes = body + (last ? 1 : 0);
     return out;
 }
 

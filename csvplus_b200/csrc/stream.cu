@@ -199,13 +199,12 @@ struct Stream {
     std::shared_ptr<Table> next(bool* had_error, DataError* derr) {
         *had_error = false;
         bool trial = false;
-        if (done) return nullptr;
+        if (done || (!last_pushed && len == 0)) return nullptr;  // (nothing pushed yet: no slot either)
         CPB_CUDA(cudaStreamWaitEvent(c->stream, copied, 0));
         uint8_t* in = slot[cur]->as<uint8_t>();
         CPB_CUDA(cudaMemsetAsync(in + len, 0, std::min<uint64_t>(cap[cur] - len, 256), c->stream));
         uint64_t cut = len;
         if (!last_pushed) {
-            if (len == 0) return nullptr;
             stream_cut(c, in, len, o, cut_dev->as<uint64_t>());
             uint64_t* h = (uint64_t*)c->pinned_scratch(8);
             CPB_CUDA(cudaMemcpyAsync(h, cut_dev->p, 8, cudaMemcpyDeviceToHost, c->stream));
@@ -250,7 +249,14 @@ struct Stream {
                 line_base = (o.header_from_first_row ? 2 : 1) + records;
             }
         } else line_base += records;
-        if (*had_error) { done = true; return t; }
+        if (*had_error || last_pushed) {
+            // the input is parsed (the tables own their bytes): the slots go back to the pool now, stream-ordered after
+            // the parse, instead of staying allocated through the caller's plan until the stream is freed
+            done = true;
+            slot[0].reset(); slot[1].reset();
+            cap[0] = cap[1] = 0;
+            return t;
+        }
         // carry [cut, len) to the front of the other slot
         const int nx = cur ^ 1;
         const uint64_t tail = len - cut;
@@ -259,7 +265,6 @@ struct Stream {
         CPB_CUDA(cudaEventRecord(freed[cur], c->stream));
         CPB_CUDA(cudaEventRecord(freed[nx], c->stream));
         cur = nx; len = tail;
-        if (last_pushed && len == 0) done = true;
         return t;
     }
 };
@@ -273,8 +278,7 @@ Stream* stream_open(Ctx* c, const cpb_reader_opts& o, std::vector<std::pair<std:
         for (auto& e : s->freed) CPB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (auto& e : s->freed) CPB_CUDA(cudaEventRecord(e, c->stream));
         CPB_CUDA(cudaEventRecord(s->copied, s->copy));
-        s->cut_dev = dev_alloc(c, 16);
-        s->reserve(0, 0, 0);
+        s->cut_dev = dev_alloc(c, 16);  // the first slot is allocated by the first push, at that push's size
     } catch (...) {
         delete s;
         throw;

@@ -102,18 +102,18 @@ __global__ void __launch_bounds__(CW_WARPS * 32) csv_row_write_kernel(WriteCols 
     }
 }
 
-Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, uint64_t* nbytes,
-                 uint64_t* header_bytes) {
+Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, bool with_header,
+                 uint64_t room, uint64_t* nbytes) {
     if ((int)cols.size() > MAXW) throw ArgError{CPB_ERR_UNSUPPORTED, "more than 64 columns in ToCsv"};
     // header line (csvplus.go:387): the caller's column names through the same quoting rule
     std::string header;
-    for (size_t i = 0; i < names.size(); i++) {
+    for (size_t i = 0; with_header && i < names.size(); i++) {
         if (i) header += ',';
         std::vector<uint8_t> tmp(names[i].size() * 2 + 2);
         uint32_t k = field_write((const uint8_t*)names[i].data(), (uint32_t)names[i].size(), tmp.data());
         header.append((const char*)tmp.data(), k);
     }
-    header += '\n';
+    if (with_header) header += '\n';
     const uint64_t n = (uint64_t)t.nrows;
     WriteCols wc{};
     wc.n = (int)cols.size();
@@ -131,6 +131,8 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     sync_stream(c);
     const uint64_t body = *ht;
     if (body > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToCsv output exceeds 4 GiB; write in smaller batches"};
+    *nbytes = header.size() + body;
+    if (*nbytes > room) return nullptr;
     Buf out = dev_alloc(c, header.size() + body + 16);
     CPB_CUDA(cudaMemcpyAsync(out->p, header.data(), header.size(), cudaMemcpyHostToDevice, c->stream));
     if (n) {
@@ -140,8 +142,6 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
         csv_row_write_kernel<<<wblocks, CW_WARPS * 32, 0, c->stream>>>(wc, n, len->as<uint32_t>(), out->as<uint8_t>() + header.size());
         CPB_CUDA(cudaGetLastError());
     }
-    *nbytes = header.size() + body;
-    if (header_bytes) *header_bytes = header.size();
     return out;
 }
 

@@ -55,10 +55,32 @@ struct Strs {
     std::vector<std::string> keep; std::vector<cpb_str> v;
     explicit Strs(const std::vector<std::string>& s) : keep(s) { for (auto& x : keep) v.push_back(cpb_str{x.data(), x.size()}); if (v.empty()) v.push_back(cpb_str{nullptr, 0}); }
 };
+// the pinned host buffer a sink serialises its batches into.  write(out, into): into(buf, cap, &n, &err) is a
+// cpb_table_to_*_into call, which writes nothing when its n exceeds cap: the buffer then grows and the call is repeated.
+struct Pinned {
+    void* p = nullptr; uint64_t cap = 0;
+    ~Pinned() { if (p) cpb_host_free(ctx(), p); }
+    template <class Into> void write(std::ostream& out, const Into& into) {
+        for (;;) {
+            uint64_t n = 0; cpb_error e{};
+            const int st = into(p, cap, &n, &e);
+            if (st == CPB_ERR_ARG && n > cap) {
+                if (p) cpb_host_free(ctx(), p);
+                p = nullptr; cap = 0;
+                if (cpb_host_alloc(ctx(), n + n / 4 + 64, &p) != CPB_OK) throw Error(cpb_last_error(ctx()));
+                cap = n + n / 4 + 64;
+                continue;
+            }
+            check(st, e);
+            out.write((const char*)p, (std::streamsize)n);
+            return;
+        }
+    }
+};
 }  // namespace detail
 
-// bytes per push of a streamed input (cpb_stream_*): FromFile / FromString inputs larger than this are parsed in batches
-// of whole records, smaller ones in one cpb_parse_csv call
+// bytes per push of an input (cpb_stream_*): FromFile / FromString inputs larger than this are parsed in batches of whole
+// records, smaller ones are one push
 inline uint64_t& StreamBatchBytes() { static uint64_t v = 128ull << 20; return v; }
 
 // maps nbytes of device memory into the context's pool ahead of time (cpb_pool_reserve); optional
@@ -211,12 +233,10 @@ private:
 // ---------------------------------------------------------------- Reader (csvplus.go:922-1076)
 class Reader {
 public:
-    // fills the next piece of the input; false at its end
+    // fills the next piece of the input; true when it is the last one
     using Pieces = std::function<bool(std::string&)>;
-    // source: the whole input, parsed in one cpb_parse_csv call.  pieces: null, or a function that returns null when the
-    // input fits one batch (then `source` is parsed) and else the input's pieces (cpb_stream_*)
-    explicit Reader(std::function<std::string()> source, std::function<Pieces()> pieces = nullptr)
-        : source_(std::move(source)), pieces_(std::move(pieces)) {}
+    // pieces: a function that starts reading the input and returns its pieces
+    explicit Reader(std::function<Pieces()> pieces) : pieces_(std::move(pieces)) {}
     Reader& Delimiter(char32_t c) { delimiter_ = c; return *this; }
     Reader& CommentChar(char32_t c) { comment_ = c; return *this; }
     Reader& LazyQuotes() { lazy_ = true; return *this; }
@@ -240,65 +260,44 @@ public:
         header_.assign(spec.begin(), spec.end()); from_first_row_ = false; return *this;
     }
     // one batch of Reader.Iterate: its rows, the DataSourceError raised after them (last batch only) and whether the
-    // input is parsed in several batches.  fn returns false to stop reading the input.
-    using BatchFn = std::function<bool(Table, std::unique_ptr<DataSourceError>, bool streamed)>;
-    // Reader.Iterate lowered to cpb_parse_csv (an input that fits one batch) or to cpb_stream_* (a larger one)
+    // input was pushed in more than one piece.  fn returns false to stop reading the input.
+    using BatchFn = std::function<bool(Table, std::unique_ptr<DataSourceError>, bool several)>;
+    // Reader.Iterate lowered to cpb_stream_*: an input that fits one piece is one push, parsed as one batch
     void batches(const Predicate* pred, const BatchFn& fn) const {
-        Pieces next = pieces_ ? pieces_() : nullptr;
+        Pieces next = pieces_();
         cpb_reader_opts o{}; o.delimiter = delimiter_; o.comment = comment_; o.num_fields = num_fields_;
         o.lazy_quotes = lazy_; o.trim_leading_space = trim_; o.header_from_first_row = from_first_row_;
         std::vector<cpb_header_col> spec;
         for (auto& h : header_) spec.push_back(cpb_header_col{cpb_str{h.first.data(), h.first.size()}, h.second, 0});
         std::unique_ptr<detail::CPred> cp; if (pred) cp.reset(new detail::CPred(*pred));
-        cpb_table* t = nullptr; cpb_error e{};
-        if (!next) {
-            std::string data = source_();
-            int st = cpb_parse_csv(detail::ctx(), data.data(), data.size(), 0, &o, spec.data(), (int)spec.size(), cp ? &cp->p : nullptr, &t, &e);
-            if (st == CPB_ERR_DATA && t && e.has_line) { fn(Table(t), std::unique_ptr<DataSourceError>(new DataSourceError(e.line, e.msg)), false); return; }
-            detail::check(st, e);
-            fn(Table(t), nullptr, false);
-            return;
-        }
-        cpb_stream* sp = nullptr;
+        cpb_stream* sp = nullptr; cpb_error e{};
         detail::check(cpb_stream_open(detail::ctx(), &o, spec.data(), (int)spec.size(), cp ? &cp->p : nullptr, &sp, &e), e);
         std::unique_ptr<cpb_stream, void (*)(cpb_stream*)> st(sp, cpb_stream_free);
         // One cpb_stream_next per push parses every complete record pushed so far.  A batch is delivered after the next
         // piece has been pushed: that piece's host-to-device copy (the stream's copy stream) overlaps what fn does with
         // the batch on the context's stream, and it is parsed only after fn has returned.
         Table pending; bool have = false;
-        auto deliver = [&]() -> bool { if (!have) return true; have = false; return fn(pending, nullptr, true); };
-        enum { GO, DONE, STOP };
-        auto step = [&]() -> int {
-            cpb_table* bt = nullptr; int done = 0;
-            const int s = cpb_stream_next(st.get(), &bt, &done, &e);
-            if (s == CPB_ERR_DATA && bt && e.has_line) {
-                Table failed(bt);
-                if (deliver()) fn(failed, std::unique_ptr<DataSourceError>(new DataSourceError(e.line, e.msg)), true);
-                return STOP;
-            }
-            if (s != CPB_OK) detail::check(s, e);
-            if (bt) { pending = Table(bt); have = true; }
-            return done ? DONE : GO;
-        };
-        auto push = [&](const void* p, uint64_t n, int last) {
-            if (cpb_stream_push(st.get(), p, n, last) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
-        };
+        bool several = false;  // known from the first piece, so every batch, the first one included, reports it
+        auto deliver = [&]() -> bool { if (!have) return true; have = false; return fn(pending, nullptr, several); };
         std::string piece;  // untouched until the cpb_stream_next after its push has returned
-        int r = GO;
-        while (r == GO && next(piece)) {
-            push(piece.data(), piece.size(), 0);
+        for (bool first = true, last = false, done = false; !last && !done; first = false) {
+            last = next(piece);
+            if (first) several = !last;
+            if (cpb_stream_push(st.get(), piece.data(), piece.size(), last) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
             if (!deliver()) return;
-            if ((r = step()) == STOP) return;
-        }
-        if (r == GO) {
-            push(nullptr, 0, 1);
-            if (!deliver()) return;
-            if (step() == STOP) return;
+            cpb_table* bt = nullptr; int fin = 0;
+            const int s = cpb_stream_next(st.get(), &bt, &fin, &e);
+            if (s == CPB_ERR_DATA && bt && e.has_line) {
+                fn(Table(bt), std::unique_ptr<DataSourceError>(new DataSourceError(e.line, e.msg)), several);
+                return;
+            }
+            detail::check(s, e);
+            if (bt) { pending = Table(bt); have = true; }
+            done = fin != 0;
         }
         deliver();
     }
 private:
-    std::function<std::string()> source_;
     std::function<Pieces()> pieces_;
     uint32_t delimiter_ = ',', comment_ = 0; int num_fields_ = 0; bool lazy_ = false, trim_ = false, from_first_row_ = true;
     std::vector<std::pair<std::string, int>> header_;
@@ -306,14 +305,12 @@ private:
 Reader FromFile(const std::string& name);  // csvplus.go:950 (defined below)
 inline Reader FromString(std::string data) {
     auto d = std::make_shared<std::string>(std::move(data));
-    return Reader([d] { return *d; }, [d]() -> Reader::Pieces {
-        if (d->size() <= StreamBatchBytes()) return nullptr;
+    return Reader([d]() -> Reader::Pieces {
         auto pos = std::make_shared<size_t>(0);
         return [d, pos](std::string& piece) {
-            if (*pos >= d->size()) return false;
             piece.assign(*d, *pos, (size_t)StreamBatchBytes());
             *pos += piece.size();
-            return true;
+            return *pos >= d->size();
         };
     });
 }
@@ -356,37 +353,16 @@ public:
     void ToCsv(std::ostream& out, const std::vector<std::string>& columns) const {
         if (columns.empty()) throw std::logic_error("empty column list in ToCsv() function");
         detail::Strs c(columns);
-        bool header = false;
-        void* buf = nullptr; uint64_t cap = 0;  // pinned: the batches of a streamed input are serialised into it
-        try {
-            each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool streamed) {
-                cpb_error e{};
-                if (!streamed) {
-                    void* bytes = nullptr; uint64_t n = 0;
-                    detail::check(cpb_table_to_csv(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), &bytes, &n, &e), e);
-                    out.write((const char*)bytes, (std::streamsize)n); cpb_host_free(detail::ctx(), bytes);
-                } else {
-                    for (;;) {  // the header line once, before the first batch (csvplus.go:387)
-                        uint64_t n = 0;
-                        const int st = cpb_table_to_csv_into(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), !header, buf, cap, &n, &e);
-                        if (st == CPB_ERR_ARG && n > cap) {  // grow to the size the batch needs and repeat it
-                            if (buf) cpb_host_free(detail::ctx(), buf);
-                            buf = nullptr; cap = 0;
-                            if (cpb_host_alloc(detail::ctx(), n + n / 4 + 64, &buf) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
-                            cap = n + n / 4 + 64;
-                            continue;
-                        }
-                        detail::check(st, e);
-                        out.write((const char*)buf, (std::streamsize)n);
-                        break;
-                    }
-                }
-                header = true;
-                if (err) throw *err;
-                return true;
+        detail::Pinned buf;
+        bool header = true;  // the header line once, before the first batch (csvplus.go:387)
+        each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool) {
+            buf.write(out, [&](void* p, uint64_t cap, uint64_t* n, cpb_error* e) {
+                return cpb_table_to_csv_into(detail::ctx(), t.get(), c.v.data(), (int)columns.size(), header, p, cap, n, e);
             });
-        } catch (...) { if (buf) cpb_host_free(detail::ctx(), buf); throw; }
-        if (buf) cpb_host_free(detail::ctx(), buf);
+            header = false;
+            if (err) throw *err;
+            return true;
+        });
     }
     // ToCsvFile, csvplus.go:411-443: the file is removed on error
     void ToCsvFile(const std::string& name, const std::vector<std::string>& columns) const {
@@ -399,47 +375,26 @@ public:
         } catch (...) { std::remove(name.c_str()); throw; }
     }
     // ToJSON, csvplus.go:446-474: the GPU serialises the result in row-range batches (each < 4 GiB) into one reused
-    // pinned buffer.  On a source error nothing is written when the input was parsed in one batch; a streamed input keeps
-    // what its earlier batches wrote (a prefix of the array without ']'), as the reference's encoder has flushed it.
+    // pinned buffer.  On a source error nothing is written when the input was pushed in one piece; an input pushed in
+    // several keeps what its batches wrote (a prefix of the array without ']'), as the reference's encoder has flushed it.
     void ToJSON(std::ostream& out) const {
-        void* buf = nullptr; uint64_t cap = 0;
+        detail::Pinned buf;
         bool opened = false;
-        auto json = [&](const Table& t, bool first, bool last) {
+        each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool several) {
+            if (err && !several) throw *err;
             const int64_t n = t.size(), step = int64_t(1) << 24;
-            for (int64_t lo = 0;;) {
-                const int64_t hi = std::min(n, lo + step);
-                cpb_error e{}; uint64_t w = 0;
-                Table p = t.slice(lo, hi);
-                int st = cpb_table_to_json_into(detail::ctx(), p.get(), first && lo == 0, last && hi == n, buf, cap, &w, &e);
-                if (st == CPB_ERR_ARG && w > cap) {  // grow the buffer to the size the batch needs and repeat it
-                    if (buf) cpb_host_free(detail::ctx(), buf);
-                    buf = nullptr; cap = 0;
-                    if (cpb_host_alloc(detail::ctx(), w + w / 4, &buf) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
-                    cap = w + w / 4;
-                    continue;
-                }
-                detail::check(st, e);
-                out.write((const char*)buf, (std::streamsize)w);
-                lo = hi;
-                if (lo >= n) break;
+            for (int64_t lo = 0; lo < n; lo += step) {
+                Table p = t.slice(lo, std::min(n, lo + step));
+                const bool first = !opened;
+                buf.write(out, [&](void* dst, uint64_t cap, uint64_t* w, cpb_error* e) {
+                    return cpb_table_to_json_into(detail::ctx(), p.get(), first, 0, dst, cap, w, e);
+                });
+                opened = true;
             }
-        };
-        try {
-            each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool streamed) {
-                if (!streamed) {
-                    if (err) throw *err;
-                    json(t, true, true);
-                    opened = true;
-                    return true;
-                }
-                if (t.size()) { json(t, !opened, false); opened = true; }
-                if (err) throw *err;
-                return true;
-            });
-        } catch (...) { if (buf) cpb_host_free(detail::ctx(), buf); throw; }
-        if (buf) cpb_host_free(detail::ctx(), buf);
-        if (!opened) out << "[]";
-        else if (streamed_) out << ']';
+            if (err) throw *err;
+            return true;
+        });
+        out << (opened ? "]" : "[]");
     }
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }
@@ -464,15 +419,14 @@ private:
         if (cpb_table_concat(detail::ctx(), hs.data(), (int)hs.size(), &out) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
         return Table(out);
     }
-    // the operations over every batch of the source, in order: fn(rows, error after them, streamed) returns false to stop.
+    // the operations over every batch of the source, in order: fn(rows, error after them, several) returns false to stop;
+    // several: the input was pushed in more than one piece.
     // Top / Drop count rows across batches; once Top has pulled n + 1 rows the input is no longer read.
     using EachFn = std::function<bool(Table&, std::unique_ptr<DataSourceError>&, bool)>;
     void each(const EachFn& fn) const {
         size_t first = 0;
         std::vector<uint64_t> seen(ops_.size(), 0);
-        streamed_ = false;
-        auto apply = [&](Table t, std::unique_ptr<DataSourceError> err, bool streamed) -> bool {
-            streamed_ = streamed;
+        auto apply = [&](Table t, std::unique_ptr<DataSourceError> err, bool several) -> bool {
             bool stop = false;
             for (size_t i = first; i < ops_.size(); i++) {
                 const Op& o = ops_[i]; cpb_table* out = nullptr; cpb_error e{}; detail::Strs c(o.cols);
@@ -504,7 +458,7 @@ private:
                 t = Table(out);
             }
             const bool failed = err != nullptr;
-            return fn(t, err, streamed) && !stop && !failed;
+            return fn(t, err, several) && !stop && !failed;
         };
         if (reader_) {
             const Predicate* fused = (!ops_.empty() && ops_[0].kind == FILTER && ops_[0].pred.lowerable()) ? &ops_[0].pred : nullptr;
@@ -513,7 +467,6 @@ private:
         } else apply(*table_, nullptr, false);
     }
     std::shared_ptr<Reader> reader_; std::shared_ptr<Table> table_; std::vector<Op> ops_;
-    mutable bool streamed_ = false;  // the last each() parsed its input in several batches
 };
 
 inline DataSource Take(const Reader& r) { return DataSource(r); }                          // csvplus.go:252
@@ -525,28 +478,35 @@ inline DataSource Index::Find(const std::vector<std::string>& values) const {
     if (cpb_index_find(detail::ctx(), h_.get(), v.v.data(), (int)values.size(), &t) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
     return DataSource(Table(t));
 }
-// a file that fits one batch is read whole and parsed in one call; a larger one is read and parsed one batch at a time
+// the file in pieces of StreamBatchBytes(): a file that fits one piece is read whole and is one push.  A regular file's
+// pieces are read at their exact size, another file's (a pipe) in steps of 64 KiB: a piece is never sized above the
+// bytes it holds.
 inline Reader FromFile(const std::string& name) {
-    auto whole = [name] {
-        FILE* f = fopen(name.c_str(), "rb");
-        if (!f) throw DataSourceError(1, std::string("open: ") + strerror(errno));  // mapError, csvplus.go:1216-1220
-        std::string s; char buf[1 << 16]; size_t n;
-        while ((n = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, n);
-        fclose(f); return s;
-    };
-    auto pieces = [name]() -> Reader::Pieces {
-        struct stat sb;
-        if (stat(name.c_str(), &sb) != 0 || !S_ISREG(sb.st_mode) || (uint64_t)sb.st_size <= StreamBatchBytes()) return nullptr;
+    return Reader([name]() -> Reader::Pieces {
         std::shared_ptr<FILE> f(fopen(name.c_str(), "rb"), [](FILE* p) { if (p) fclose(p); });
-        if (!f) throw DataSourceError(1, std::string("open: ") + strerror(errno));
-        return [f](std::string& piece) {
-            piece.resize((size_t)StreamBatchBytes());
-            const size_t n = fread(&piece[0], 1, piece.size(), f.get());
-            piece.resize(n);
-            return n > 0;
+        if (!f) throw DataSourceError(1, std::string("open: ") + strerror(errno));  // mapError, csvplus.go:1216-1220
+        struct stat sb;
+        const bool regular = fstat(fileno(f.get()), &sb) == 0 && S_ISREG(sb.st_mode);
+        auto left = std::make_shared<uint64_t>(regular ? (uint64_t)sb.st_size : 0);
+        return [f, regular, left](std::string& piece) {
+            const uint64_t cap = StreamBatchBytes();
+            if (regular) {
+                piece.resize((size_t)std::min(*left, cap));
+                piece.resize(fread(&piece[0], 1, piece.size(), f.get()));
+                const bool short_read = piece.size() < std::min(*left, cap);
+                *left -= piece.size();
+                return short_read || *left == 0;
+            }
+            piece.clear();
+            char buf[1 << 16]; size_t n;
+            while (piece.size() < cap && (n = fread(buf, 1, (size_t)std::min<uint64_t>(sizeof buf, cap - piece.size()), f.get())) > 0)
+                piece.append(buf, n);
+            const int c = fgetc(f.get());
+            if (c == EOF) return true;
+            ungetc(c, f.get());
+            return false;
         };
-    };
-    return Reader(whole, pieces);
+    });
 }
 
 }  // namespace csvplus

@@ -79,6 +79,23 @@ int main() {
             } catch (const DataSourceError& e) { CHECK(std::string(e.what()) == "row 122: wrong number of fields"); }
             std::ifstream gone(out_name);
             CHECK(!gone.good());
+            // ToJSON with the error in the first batch of an input pushed in two pieces: the 5 rows before it are written
+            // without ']'; pushed in one piece, nothing is written
+            size_t at = 0;
+            for (int k = 0; k < 6; k++) at = people.find('\n', at) + 1;
+            const std::string bad = people.substr(0, at) + "1,2\n" + people.substr(at);
+            std::ostringstream top5;
+            Take(FromString(people)).Top(5).ToJSON(top5);
+            for (uint64_t batch : {(uint64_t)bad.size() / 2 + 1, (uint64_t)bad.size() + 1}) {
+                StreamBatchBytes() = batch;
+                std::ostringstream js_err;
+                try {
+                    Take(FromString(bad)).ToJSON(js_err);
+                    CHECK(false);
+                } catch (const DataSourceError& e) { CHECK(std::string(e.what()) == "row 7: wrong number of fields"); }
+                const std::string want = batch <= bad.size() ? top5.str().substr(0, top5.str().size() - 1) : "";
+                CHECK(js_err.str() == want);
+            }
             StreamBatchBytes() = saved;
             std::ostringstream whole_js;
             Take(FromString(orders).SelectColumns({"order_id", "cust_id", "qty"})).Join(idx, {"cust_id"}).Top(3).ToJSON(whole_js);

@@ -101,11 +101,23 @@ def _same_tables(a, b):
         assert np.array_equal(oa, ob) and np.array_equal(da, db), c
 
 
-def check_stream(monkeypatch, tmp_path, data, o, batch, kind="bytes", **spec):
-    """streamed == single shot == oracle: rows, column bytes, error text and line"""
+def _parse_whole(data, o, select=None, expect=None, assume=None, like=None):
+    """the input in one cpb_parse_csv call with the options, header spec and predicate of _plan"""
     import csvplus_b200 as cp
+    spec = [(n, -1) for n in select] if select else list((expect or assume or {}).items())
+    return cp.parse_csv(gpu_ctx(), data, delimiter=o.comma, comment=o.comment, num_fields=o.fields_per_record,
+                        lazy_quotes=o.lazy_quotes, trim_leading_space=o.trim_leading_space, header_from_first_row=not assume,
+                        spec=spec, pred=cp.Like(like) if like else None)
+
+
+def check_stream(monkeypatch, tmp_path, data, o, batch, kind="bytes", **spec):
+    """streamed == one piece == one cpb_parse_csv call == oracle: rows, column bytes, error text and line"""
+    import csvplus_b200 as cp
+    t0, e0 = _parse_whole(data, o, **spec)
     monkeypatch.setattr(cp.api, "STREAM_BATCH_BYTES", 1 << 40)
     t1, e1 = _plan(kind, data, tmp_path, o, **spec)._table()
+    assert (str(e0), getattr(e0, "Line", None)) == (str(e1), getattr(e1, "Line", None)), data
+    _same_tables(t0, t1)
     monkeypatch.setattr(cp.api, "STREAM_BATCH_BYTES", batch)
     t2, e2 = _plan(kind, data, tmp_path, o, **spec)._table()
     assert (str(e1), getattr(e1, "Line", None)) == (str(e2), getattr(e2, "Line", None)), (data, batch)
@@ -316,6 +328,19 @@ def test_streamed_json_on_error_keeps_the_prefix(monkeypatch):
     with pytest.raises(cp.DataSourceError):
         cp.Take(cp.FromBytes(data)).ToJSON(out)
     assert out.getvalue() == b""  # one batch: nothing written, as before
+    # the error inside the first batch of an input pushed in two pieces: the rows before it are still the written prefix
+    body = people_csv(60).split(b"\n")
+    body[10] = body[10] + b",extra"
+    early = b"\n".join(body)
+    monkeypatch.setattr(cp.api, "STREAM_BATCH_BYTES", len(early) // 2 + 1)
+    for kind in ("bytes", "reader"):
+        src = (lambda: cp.FromBytes(early)) if kind == "bytes" else (lambda: cp.FromReader(io.BytesIO(early)))
+        out = io.BytesIO()
+        with pytest.raises(cp.DataSourceError) as e:
+            cp.Take(src()).ToJSON(out)
+        assert e.value.Line == 11
+        t, _ = cp.Take(src())._table()
+        assert len(t) == 9 and out.getvalue() == t.to_json()[:-1], kind
 
 
 # ------------------------------------------------------------------ scale

@@ -5,11 +5,10 @@
      3.35 TB/s;
   2. end to end: FromFile(orders).SelectColumns(cust_id, prod_id, qty, ts).Join(custIdx, "cust_id").Join(prodIdx)
      .ToCsv(...) from the page cache into a writer that keeps a CRC of the bytes, streamed in batches of
-     STREAM_BATCH_BYTES against the single-shot public path on the same file in the same run (alternating, best of three):
+     STREAM_BATCH_BYTES against the same file pushed as one piece in the same run (alternating, best of three):
      input GB/s, rows/s, batches, host synchronisations, and the peak device memory of the context's pool during the run
-     (cpb_pool_used_high; it includes the two indices).  The two outputs are compared by length and CRC-32.  By default at 30 M rows (the
-     single-shot ToCsv output, ~1.8 GB, stays below the 2 GiB `Table.to_csv` can hand to Python in one bytes object) and at
-     125 M rows, where the single-shot public path fails (a ToCsv output above 4 GiB) and the streamed path runs alone.
+     (cpb_pool_used_high; it includes the two indices).  The two outputs are compared by length and CRC-32.  By default at 30 M rows and
+     at 125 M rows, where the one-piece path fails (a ToCsv batch output above 4 GiB) and the streamed path runs alone.
 The card's name and power limit are printed first."""
 import os
 import subprocess
@@ -137,7 +136,7 @@ def compare(rows):
             else:
                 res[streamed].append(r)
     for streamed in (True, False):
-        name = "streamed" if streamed else "single shot"
+        name = "streamed" if streamed else "one piece"
         if streamed in fail:
             print(f"  {name:11s} fails: {fail[streamed]}", flush=True)
             continue
@@ -146,7 +145,7 @@ def compare(rows):
               f"batches {nb}  host syncs {syncs}  peak device memory {peak / 2**30:.2f} GiB  output {out.n} bytes", flush=True)
     if res[True] and res[False]:
         a, b = res[True][0][1], res[False][0][1]
-        assert (a.n, a.crc) == (b.n, b.crc), "streamed and single-shot outputs differ"
+        assert (a.n, a.crc) == (b.n, b.crc), "streamed and one-piece outputs differ"
         print(f"  outputs identical: {a.n} bytes, crc32 {a.crc:08x}; batch {batch_mib} MiB", flush=True)
     os.remove(path)
     os.rmdir(tmp)
