@@ -398,10 +398,7 @@ int cpb_csv_stream_cut(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_de
     if ((reinterpret_cast<uintptr_t>(dev) & 15) != 0) throw ArgError{CPB_ERR_ARG, "device input must be 16-byte aligned"};
     Buf out = dev_alloc(c, 16);
     stream_cut(c, dev, nbytes, *opts, out->as<uint64_t>());
-    uint64_t* hp = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(hp, out->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    *cut = *hp;
+    *cut = read_back<uint64_t>(c, out->p);
     return CPB_OK;
     CPB_CATCH(c, nullptr)
 }
@@ -737,10 +734,35 @@ int cpb_except(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cp
     return join_common(h, probe, ix, cols, n, true, out, err);
 }
 
+// ------------------------------------------------------------------ ToCsv / ToJSON output
+// mode 0: into new pinned host memory, 1: into caller-owned (ideally pinned) host memory of cap bytes, 2: left on the
+// device.  A destination that is too small gets nothing: the call fails with CPB_ERR_ARG (too_small) and *nbytes = the
+// size needed (the serialiser then returns no buffer).
+static void deliver(Ctx* c, const Buf& out, uint64_t total, int mode, void** bytes, void* host_dst, uint64_t cap, const char* too_small) {
+    if (mode == 0) {
+        void* hp = nullptr;
+        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
+        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        *bytes = hp;
+    } else if (mode == 1) {
+        if (total > cap) throw ArgError{CPB_ERR_ARG, too_small};
+        if (total) {
+            KernelTimer kt(c, "d2h_output", total, 0);
+            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        }
+        sync_stream(c);
+    } else {
+        void* dp = nullptr;
+        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
+        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
+        *bytes = dp;
+    }
+}
+
 // ------------------------------------------------------------------ ToCsv
-// mode 0: into new pinned host memory, 1: into caller-owned (ideally pinned) host memory of cap bytes, with the header
-// line only when asked for (a csv.Writer writes it once, before the first batch: csvplus.go:387), 2: left on the device.
-// A destination that is too small gets nothing: the call fails with CPB_ERR_ARG and *nbytes = the size needed.
+// modes as deliver(); in mode 1 the header line is written only when asked for (a csv.Writer writes it once, before the
+// first batch: csvplus.go:387)
 static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, int mode, void** bytes,
                          void* host_dst, uint64_t cap, uint64_t* nbytes, cpb_error* err) {
     if (!h || !t || !nbytes || (mode != 1 && !bytes) || (mode == 1 && cap && !host_dst)) return CPB_ERR_ARG;
@@ -759,25 +781,7 @@ static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, in
     uint64_t total = 0;
     Buf out = table_to_csv(c, *t->t, idx, names, with_header != 0, mode == 1 ? cap : UINT64_MAX, &total);
     *nbytes = total;
-    if (mode == 0) {
-        void* hp = nullptr;
-        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
-        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        *bytes = hp;
-    } else if (mode == 1) {
-        if (total > cap) throw ArgError{CPB_ERR_ARG, "ToCsv destination too small"};
-        if (total) {
-            KernelTimer kt(c, "d2h_output", total, 0);
-            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        }
-        sync_stream(c);
-    } else {
-        void* dp = nullptr;
-        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
-        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
-        *bytes = dp;
-    }
+    deliver(c, out, total, mode, bytes, host_dst, cap, "ToCsv destination too small");
     return CPB_OK;
     CPB_CATCH(c, err)
 }
@@ -803,25 +807,7 @@ static int to_json_common(cpb_ctx* h, const cpb_table* t, int first, int last, i
     uint64_t total = 0;
     Buf out = table_to_json(c, *t->t, first != 0, last != 0, mode == 1 ? cap : UINT64_MAX, &total);
     *nbytes = total;
-    if (mode == 0) {
-        void* hp = nullptr;
-        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
-        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        *bytes = hp;
-    } else if (mode == 1) {
-        if (total > cap) throw ArgError{CPB_ERR_ARG, "ToJSON destination too small"};
-        if (total) {
-            KernelTimer kt(c, "d2h_output", total, 0);
-            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        }
-        sync_stream(c);
-    } else {
-        void* dp = nullptr;
-        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
-        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
-        *bytes = dp;
-    }
+    deliver(c, out, total, mode, bytes, host_dst, cap, "ToJSON destination too small");
     return CPB_OK;
     CPB_CATCH(c, err)
 }

@@ -152,11 +152,7 @@ void job_sizes(GatherJob& j) {  // the one host round trip
     Ctx* c = j.c;
     cudaSetDevice(c->device);
     const int M = 1 + 2 * j.ncols;
-    j.meta.resize((size_t)M * c->nranks);
-    uint64_t* h = (uint64_t*)c->pinned_scratch(j.meta.size() * 8);
-    CPB_CUDA(cudaMemcpyAsync(h, j.meta_all->p, j.meta.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    memcpy(j.meta.data(), h, j.meta.size() * 8);
+    j.meta = read_back<uint64_t>(c, j.meta_all->p, (size_t)M * c->nranks);
 }
 void job_data_collective(GatherJob& j) {  // inside ncclGroupStart/End
     Ctx* c = j.c;
@@ -206,7 +202,7 @@ void job_finish(GatherJob& j) {
         for (int q = 0; q < R; q++)
             rp.seg[q] = Seg{row_base[q], byte_base[(size_t)k * (R + 1) + q], j.meta[(size_t)q * M], j.meta[(size_t)q * M + 1 + 2 * k]};
         KernelTimer kt(c, "gather_rebase", (row_base[R] + 1) * 8);
-        gather_rebase_kernel<<<(uint32_t)((row_base[R] + 1 + 255) / 256), 256, 0, c->stream>>>(j.out->cols[k].offsets->as<uint32_t>(), rp);
+        gather_rebase_kernel<<<nblk(row_base[R] + 1, 256), 256, 0, c->stream>>>(j.out->cols[k].offsets->as<uint32_t>(), rp);
         CPB_CUDA(cudaGetLastError());
         moved += rp.total_bytes + rp.total_rows * 4;
     }

@@ -196,6 +196,23 @@ inline void sync_stream(Ctx* c) {
     CPB_CUDA(cudaStreamSynchronize(c->stream));
 }
 
+// device-to-host readback of one value / n values through the pinned scratch, with one (counted) synchronisation; the
+// values are returned, so nothing keeps pointing into the scratch the next readback reuses
+template <class T> T read_back(Ctx* c, const void* dev) {
+    T* h = static_cast<T*>(c->pinned_scratch(sizeof(T)));
+    CPB_CUDA(cudaMemcpyAsync(h, dev, sizeof(T), cudaMemcpyDeviceToHost, c->stream));
+    sync_stream(c);
+    return *h;
+}
+template <class T> std::vector<T> read_back(Ctx* c, const void* dev, size_t n) {
+    T* h = static_cast<T*>(c->pinned_scratch(n * sizeof(T)));
+    if (n) CPB_CUDA(cudaMemcpyAsync(h, dev, n * sizeof(T), cudaMemcpyDeviceToHost, c->stream));
+    sync_stream(c);
+    return std::vector<T>(h, h + n);
+}
+
+inline uint32_t nblk(uint64_t n, int threads) { return (uint32_t)((n + threads - 1) / threads); }  // grid size
+
 inline Ready record_ready(Ctx* c) {
     auto r = std::make_shared<ReadyEvent>();
     CPB_CUDA(cudaEventCreateWithFlags(&r->ev, cudaEventDisableTiming));
@@ -251,6 +268,12 @@ void stream_free(Stream* s);
 Ctx* stream_ctx(Stream* s);
 // gather.cu
 void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, uint64_t* total_dev);  // out[n] = total
+// compaction of 0/1 flags into the ascending list of the set positions, in two calls so that the caller allocates the
+// output in between: scan_flags scans the flags and reads the count back (one host synchronisation); compact_flags
+// writes out[j] = (j-th set position) + add and the sentinel out[count] = n + add, so out holds count + 1 entries
+struct FlagScan { const uint32_t* flags; uint64_t n; Buf pos; uint64_t count; };  // pos: uint32[n + 1] exclusive scan
+FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n);
+void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out);
 Column gather_column(Ctx* c, const Column& src, const uint32_t* row_ids, int64_t nout);
 std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout);
 std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred);
@@ -276,6 +299,8 @@ struct KeyDesc {  // key columns + the widths of the order-preserving image (sor
 };
 void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, KeyDesc& kd);
 uint32_t prefix_bytes(const Index& ix, int nk);  // image bytes covered by the first nk key columns
+// head[i] = 1 when the first pbytes image bytes of row i differ from those of row i - 1 (row 0 always)
+void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head);
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
 // join.cu
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols,

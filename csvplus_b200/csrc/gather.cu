@@ -112,6 +112,25 @@ void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, u
     scan_impl(c, in, nullptr, nullptr, out, n, total_dev);
 }
 
+// ------------------------------------------------------------------ compaction of flags (scan_flags / compact_flags)
+__global__ void compact_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* out, uint64_t n, uint32_t add) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && flags[i]) out[pos[i]] = (uint32_t)i + add;
+    if (i == 0) out[pos[n]] = (uint32_t)n + add;  // sentinel: the end of the last run when the flags mark run heads
+}
+FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n) {
+    FlagScan s{flags, n, dev_alloc(c, (n + 1) * 4), 0};
+    Buf tot = dev_alloc(c, 8);
+    exclusive_scan_u32(c, flags, s.pos->as<uint32_t>(), n, tot->as<uint64_t>());
+    s.count = read_back<uint64_t>(c, tot->p);
+    return s;
+}
+void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out) {
+    if (s.n == 0) return;
+    compact_kernel<<<nblk(s.n, 256), 256, 0, c->stream>>>(s.flags, s.pos->as<uint32_t>(), out, s.n, add);
+    CPB_CUDA(cudaGetLastError());
+}
+
 // ------------------------------------------------------------------ gather by row ids
 // One warp gathers 32 consecutive output values.  Their destination bytes are contiguous, so the lanes first
 // copy their (randomly placed) source strings into a per-warp shared-memory stage laid out like the
@@ -181,8 +200,6 @@ __global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32
     }
 }
 
-static inline uint32_t blocks_for(uint64_t n, int threads) { return (uint32_t)((n + threads - 1) / threads); }
-
 struct PendingGather { Column col; const Column* src; Buf total; };
 
 // gathers several columns with ONE host synchronisation (totals of all columns read back together)
@@ -196,10 +213,7 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
         uint32_t* o = out[k].offsets->as<uint32_t>();
         scan_impl(c, nullptr, srcs[k]->off(), ids, o, (uint64_t)nout, totals->as<uint64_t>() + k);
     }
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(srcs.size() * 8);
-    CPB_CUDA(cudaMemcpyAsync(ht, totals->p, srcs.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    std::vector<uint64_t> tot(ht, ht + srcs.size());
+    const std::vector<uint64_t> tot = read_back<uint64_t>(c, totals->p, srcs.size());
     for (size_t k = 0; k < srcs.size(); k++) {
         if (tot[k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, (int)k, 0, false, "a result column exceeds 4 GiB; process in smaller batches"};
         out[k].data = dev_alloc(c, tot[k] + 16);
@@ -537,18 +551,16 @@ static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& col
         uint64_t col_bytes = n * 4 * sc.nc;
         {
             KernelTimer kt(c, "slot_build", col_bytes + n * 4);
-            slot_lens_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(sc, perm, n, lens->as<uint32_t>(), stat->as<uint32_t>());
+            slot_lens_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(sc, perm, n, lens->as<uint32_t>(), stat->as<uint32_t>());
             CPB_CUDA(cudaGetLastError());
         }
-        uint32_t* hs = (uint32_t*)c->pinned_scratch(8);
-        CPB_CUDA(cudaMemcpyAsync(hs, stat->p, 8, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
+        const std::vector<uint32_t> hs = read_back<uint32_t>(c, stat->p, 2);
         if (hs[1] == 0 && hs[0] <= RS_MAXS) {
             rs.S = std::max<uint32_t>(16, (hs[0] + 15) & ~15u);
             rs.slots = dev_alloc_owned(ix.ctx, c, n * rs.S);
             rs.lens = lens;
             KernelTimer kt(c, "slot_build", n * rs.S * 2);
-            slot_fill_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(sc, perm, n, rs.S, rs.slots->as<uint8_t>());
+            slot_fill_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(sc, perm, n, rs.S, rs.slots->as<uint8_t>());
             CPB_CUDA(cudaGetLastError());
             rs.usable = true;
         }
@@ -604,9 +616,7 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
 #undef CPB_LS
         CPB_CUDA(cudaGetLastError());
     }
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(RS_MAXC * 8);
-    CPB_CUDA(cudaMemcpyAsync(ht, totals, nc * 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint64_t> ht = read_back<uint64_t>(c, totals, nc);
     uint64_t all = 0;
     for (int k = 0; k < nc; k++) {
         if (ht[k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, k, 0, false, "a result column exceeds 4 GiB; process in smaller batches"};
@@ -647,9 +657,22 @@ __global__ void filter_flags_kernel(FilterCols cols, PredProg prog, const uint8_
     }
     flags[i] = eval_pred(prog, eq) ? 1u : 0u;
 }
-__global__ void compact_ids_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* ids, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) ids[pos[i]] = (uint32_t)i;
+// flags[i] = 1 when pred holds for row i of t.  The predicate is compiled against t's columns first, so a bad one throws
+// whether or not t has rows; for an empty t nothing is enqueued and the result is null.
+static Buf predicate_flags(Ctx* c, const Table& t, const cpb_pred* pred) {
+    if (!pred) throw ArgError{CPB_ERR_ARG, "nil predicate"};
+    Compiled comp;
+    compile_pred(pred, [&](const std::string& key) { return t.find(key); }, comp);
+    const uint64_t n = (uint64_t)t.nrows;
+    if (n == 0) return nullptr;
+    FilterCols fc{};
+    for (int i = 0; i < comp.prog.nterms; i++) { fc.off[i] = t.cols[comp.prog.term_col[i]].off(); fc.data[i] = t.cols[comp.prog.term_col[i]].bytes(); }
+    Buf lits = dev_alloc(c, comp.lits.size() + 16);
+    if (!comp.lits.empty()) CPB_CUDA(cudaMemcpyAsync(lits->p, comp.lits.data(), comp.lits.size(), cudaMemcpyHostToDevice, c->stream));
+    Buf flags = dev_alloc(c, n * 4);
+    filter_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(fc, comp.prog, lits->as<uint8_t>(), flags->as<uint32_t>(), n);
+    CPB_CUDA(cudaGetLastError());
+    return flags;
 }
 
 // TakeWhile / DropWhile (csvplus.go:346-374) with a recognisable predicate: the index of the first row for which the
@@ -659,57 +682,35 @@ __global__ void first_false_kernel(const uint32_t* __restrict__ flags, uint64_t 
     if (i < n && flags[i] == 0) atomicMin(out, (unsigned long long)i);
 }
 int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred) {
-    if (!pred) throw ArgError{CPB_ERR_ARG, "nil predicate"};
-    Compiled comp;
-    compile_pred(pred, [&](const std::string& key) { return t.find(key); }, comp);
     const uint64_t n = (uint64_t)t.nrows;
-    if (n == 0) return 0;
-    FilterCols fc{};
-    for (int i = 0; i < comp.prog.nterms; i++) { fc.off[i] = t.cols[comp.prog.term_col[i]].off(); fc.data[i] = t.cols[comp.prog.term_col[i]].bytes(); }
-    Buf lits = dev_alloc(c, comp.lits.size() + 16);
-    if (!comp.lits.empty()) CPB_CUDA(cudaMemcpyAsync(lits->p, comp.lits.data(), comp.lits.size(), cudaMemcpyHostToDevice, c->stream));
-    Buf flags = dev_alloc(c, n * 4), out = dev_alloc(c, 8);
+    if (n == 0) { predicate_flags(c, t, pred); return 0; }  // (checks the predicate)
+    Buf out = dev_alloc(c, 8);
     CPB_CUDA(cudaMemsetAsync(out->p, 0xff, 8, c->stream));
     {
         KernelTimer kt(c, "filter_like", n * 12, 2);
-        filter_flags_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(fc, comp.prog, lits->as<uint8_t>(), flags->as<uint32_t>(), n);
-        first_false_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(flags->as<uint32_t>(), n, (unsigned long long*)out->p);
+        Buf flags = predicate_flags(c, t, pred);
+        first_false_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(flags->as<uint32_t>(), n, (unsigned long long*)out->p);
         CPB_CUDA(cudaGetLastError());
     }
-    uint64_t* h = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(h, out->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return *h == ~0ull ? (int64_t)n : (int64_t)*h;
+    const uint64_t first = read_back<uint64_t>(c, out->p);
+    return first == ~0ull ? (int64_t)n : (int64_t)first;
 }
 
 std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred) {
-    if (!pred) throw ArgError{CPB_ERR_ARG, "nil predicate"};
-    Compiled comp;
-    compile_pred(pred, [&](const std::string& key) { return t.find(key); }, comp);
     const uint64_t n = (uint64_t)t.nrows;
-    if (n == 0) return gather_rows(c, t, nullptr, 0);
-    FilterCols fc{};
-    for (int i = 0; i < comp.prog.nterms; i++) { fc.off[i] = t.cols[comp.prog.term_col[i]].off(); fc.data[i] = t.cols[comp.prog.term_col[i]].bytes(); }
-    Buf lits = dev_alloc(c, comp.lits.size() + 16);
-    if (!comp.lits.empty()) CPB_CUDA(cudaMemcpyAsync(lits->p, comp.lits.data(), comp.lits.size(), cudaMemcpyHostToDevice, c->stream));
-    Buf flags = dev_alloc(c, n * 4), pos = dev_alloc(c, (n + 1) * 4), total = dev_alloc(c, 8);
+    if (n == 0) { predicate_flags(c, t, pred); return gather_rows(c, t, nullptr, 0); }  // (checks the predicate)
+    Buf flags;
     {
         KernelTimer kt(c, "filter_like", n * 12);
-        filter_flags_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(fc, comp.prog, lits->as<uint8_t>(), flags->as<uint32_t>(), n);
-        CPB_CUDA(cudaGetLastError());
+        flags = predicate_flags(c, t, pred);
     }
-    exclusive_scan_u32(c, flags->as<uint32_t>(), pos->as<uint32_t>(), n, total->as<uint64_t>());
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(ht, total->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    const uint64_t m = *ht;
-    Buf ids = dev_alloc(c, (m + 1) * 4);
+    const FlagScan s = scan_flags(c, flags->as<uint32_t>(), n);
+    Buf ids = dev_alloc(c, (s.count + 1) * 4);
     {
-        KernelTimer kt(c, "compact_ids", n * 8 + m * 4);
-        compact_ids_kernel<<<blocks_for(n, 256), 256, 0, c->stream>>>(flags->as<uint32_t>(), pos->as<uint32_t>(), ids->as<uint32_t>(), n);
-        CPB_CUDA(cudaGetLastError());
+        KernelTimer kt(c, "compact_ids", n * 8 + s.count * 4);
+        compact_flags(c, s, 0, ids->as<uint32_t>());
     }
-    return gather_rows(c, t, ids->as<uint32_t>(), (int64_t)m);
+    return gather_rows(c, t, ids->as<uint32_t>(), (int64_t)s.count);
 }
 
 // ------------------------------------------------------------------ concat
@@ -751,7 +752,7 @@ std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& pa
             uint32_t b0 = ext[2 * (p * K + k)], b1 = ext[2 * (p * K + k) + 1];
             uint64_t pr = (uint64_t)parts[p]->nrows;
             KernelTimer kt(c, "concat", (uint64_t)(b1 - b0) * 2 + pr * 8);
-            rebase_offsets_kernel<<<blocks_for(pr + 1, 256), 256, 0, c->stream>>>(parts[p]->cols[k].off(), col.offsets->as<uint32_t>() + row, pr, (uint32_t)byte);
+            rebase_offsets_kernel<<<nblk(pr + 1, 256), 256, 0, c->stream>>>(parts[p]->cols[k].off(), col.offsets->as<uint32_t>() + row, pr, (uint32_t)byte);
             CPB_CUDA(cudaGetLastError());
             if (b1 > b0) CPB_CUDA(cudaMemcpyAsync(col.data->as<uint8_t>() + byte, parts[p]->cols[k].bytes() + b0, b1 - b0, cudaMemcpyDeviceToDevice, c->stream));
             row += pr; byte += b1 - b0;

@@ -123,20 +123,18 @@ extern "C" int cpb_gen_csv(cpb_ctx* h, int kind, uint64_t seed, uint64_t row_lo,
     const uint64_t rows = row_hi - row_lo;
     Buf len = dev_alloc(c, (rows + 1) * 4), total = dev_alloc(c, 8);
     if (rows) {
-        gen_len_kernel<<<(uint32_t)((rows + 255) / 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>());
+        gen_len_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), rows, total->as<uint64_t>());
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(ht, total->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    if (*ht > 0xffffffffull) throw ArgError{CPB_ERR_ARG, "generate at most 4 GiB per call (split the row range)"};
-    *nbytes = *ht + gp.header_len;
+    const uint64_t body = read_back<uint64_t>(c, total->p);
+    if (body > 0xffffffffull) throw ArgError{CPB_ERR_ARG, "generate at most 4 GiB per call (split the row range)"};
+    *nbytes = body + gp.header_len;
     if (dst) {
         if (*nbytes > cap) throw ArgError{CPB_ERR_ARG, "generator destination too small"};
         if (gp.header_len) CPB_CUDA(cudaMemcpyAsync(dst, headers[kind], gp.header_len, cudaMemcpyHostToDevice, c->stream));
         if (rows) {
-            gen_write_kernel<<<(uint32_t)((rows + 255) / 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>(), (uint8_t*)dst);
+            gen_write_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>(), (uint8_t*)dst);
             CPB_CUDA(cudaGetLastError());
         }
         sync_stream(c);

@@ -18,7 +18,6 @@
 
 namespace cpb {
 
-static inline uint32_t nblk(uint64_t n, int t) { return (uint32_t)((n + t - 1) / t); }
 constexpr uint32_t EMPTY = 0xffffffffu;
 
 __device__ __forceinline__ uint64_t mix64(uint64_t h) {
@@ -31,27 +30,6 @@ __device__ __forceinline__ uint64_t hash_prefix(const uint64_t* img, uint64_t n,
     for (uint32_t w = 0; w < full; w++) h = mix64(h ^ img[(uint64_t)w * n + r]);
     if (rem) h = mix64(h ^ (img[(uint64_t)full * n + r] & (~0ull << (8 * (8 - rem)))));
     return h;
-}
-__device__ __forceinline__ bool prefix_equal2(const uint64_t* a, uint64_t na, uint64_t ra, const uint64_t* b, uint64_t nb, uint64_t rb,
-                                              uint32_t pbytes) {
-    uint32_t full = pbytes >> 3, rem = pbytes & 7;
-    for (uint32_t w = 0; w < full; w++) if (a[(uint64_t)w * na + ra] != b[(uint64_t)w * nb + rb]) return false;
-    if (rem) {
-        uint64_t m = ~0ull << (8 * (8 - rem));
-        if ((a[(uint64_t)full * na + ra] & m) != (b[(uint64_t)full * nb + rb] & m)) return false;
-    }
-    return true;
-}
-
-__global__ void head_flags2_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, uint32_t* head) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    head[i] = (i == 0 || !prefix_equal2(image, n, i, image, n, i - 1, pbytes)) ? 1u : 0u;
-}
-__global__ void compact_heads_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* out, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) out[pos[i]] = (uint32_t)i;
-    if (i == 0) out[pos[n]] = (uint32_t)n;  // sentinel: heads[nheads] = nrows
 }
 __global__ void hash_insert_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, const uint32_t* __restrict__ heads,
                                    uint64_t nheads, uint32_t* slots, uint64_t mask) {
@@ -95,7 +73,7 @@ __global__ void __launch_bounds__(256) join_probe_kernel(const uint64_t* __restr
             uint32_t j = slots[s];
             if (j == EMPTY) break;
             uint32_t r = heads[j];
-            if (prefix_equal2(pimg, np, i, iimg, ni, r, pbytes)) { l = r; c = heads[j + 1] - r; break; }
+            if (prefix_equal(pimg, np, i, iimg, ni, r, pbytes)) { l = r; c = heads[j + 1] - r; break; }
             s = (s + 1) & mask;
         }
         lo[i] = l; cnt[i] = c; matches += c;
@@ -248,17 +226,6 @@ __global__ void zero_flag_kernel(const uint32_t* __restrict__ cnt, uint32_t* fla
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) flag[i] = cnt[i] == 0 ? 1u : 0u;
 }
-__global__ void compact_ids2_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* ids, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) ids[pos[i]] = (uint32_t)i;
-}
-
-static uint64_t read_u64(Ctx* c, const void* dev) {
-    uint64_t* h = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(h, dev, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return *h;
-}
 
 __global__ void iota_heads_kernel(uint32_t* heads, uint64_t n) {  // heads[i] = i for i in [0, n]
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -284,17 +251,16 @@ static HashTable& ensure_hash(Ctx* c, Index& ix, int nk, bool by_src, uint32_t* 
         iota_heads_kernel<<<nblk(n + 1, 256), 256, 0, c->stream>>>(ht.heads->as<uint32_t>(), n);
         CPB_CUDA(cudaGetLastError());
     } else {
-        Buf head = dev_alloc(c, (n + 1) * 4), pos = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8);
+        Buf head = dev_alloc(c, (n + 1) * 4);
         {
             KernelTimer kt(c, "hash_heads", (uint64_t)ix.image_words * n * 8 + n * 4);
-            head_flags2_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(image->as<uint64_t>(), n, ht.pbytes, head->as<uint32_t>());
-            CPB_CUDA(cudaGetLastError());
+            head_flags(c, image->as<uint64_t>(), n, ht.pbytes, head->as<uint32_t>());
         }
-        exclusive_scan_u32(c, head->as<uint32_t>(), pos->as<uint32_t>(), n, tot->as<uint64_t>());
-        ht.nheads = read_u64(c, tot->p);
+        const FlagScan s = scan_flags(c, head->as<uint32_t>(), n);  // (its temporaries: this context's pool)
+        ht.nheads = s.count;
         // what stays in the index comes from the index owner's pool: the probing context may be shut down first
         ht.heads = dev_alloc_owned(ix.ctx, c, (ht.nheads + 1) * 4);
-        compact_heads_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), pos->as<uint32_t>(), ht.heads->as<uint32_t>(), n);
+        compact_flags(c, s, 0, ht.heads->as<uint32_t>());  // heads[nheads] = nrows: the end of the last run
     }
     uint64_t want = std::max<uint64_t>(16, ht.nheads * 2);
     ht.nslots = 1; while (ht.nslots < want) ht.nslots <<= 1;
@@ -431,22 +397,17 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         HashTable& ht = ensure_hash(c, ix, nk, by_src);
         probe_dispatch(c, probe, pidx, ix, ht, iimage, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
     }
-    Buf tot = flags;
     if (anti) {
-        Buf flag = dev_alloc(c, np * 4), pos = dev_alloc(c, (np + 1) * 4);
+        Buf flag = dev_alloc(c, np * 4);
         zero_flag_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(cnt->as<uint32_t>(), flag->as<uint32_t>(), np);
-        exclusive_scan_u32(c, flag->as<uint32_t>(), pos->as<uint32_t>(), np, tot->as<uint64_t>());
-        uint64_t m = read_u64(c, tot->p);
-        Buf ids = dev_alloc(c, (m + 1) * 4);
-        compact_ids2_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(flag->as<uint32_t>(), pos->as<uint32_t>(), ids->as<uint32_t>(), np);
-        CPB_CUDA(cudaGetLastError());
-        auto r = gather_rows(c, probe, ids->as<uint32_t>(), (int64_t)m);
+        const FlagScan s = scan_flags(c, flag->as<uint32_t>(), np);
+        Buf ids = dev_alloc(c, (s.count + 1) * 4);
+        compact_flags(c, s, 0, ids->as<uint32_t>());
+        auto r = gather_rows(c, probe, ids->as<uint32_t>(), (int64_t)s.count);
         r->first_line = probe.first_line;
         return r;
     }
-    uint32_t* hf = (uint32_t*)c->pinned_scratch(32);
-    CPB_CUDA(cudaMemcpyAsync(hf, flags->p, 32, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint32_t> hf = read_back<uint32_t>(c, flags->p, 8);
     const uint64_t m = (uint64_t)hf[4] | ((uint64_t)hf[5] << 32);  // counted by the probe kernel (0 when ni == 0)
     // every probe row matched exactly one index row (the usual foreign-key join): the probe-side columns of the
     // result ARE the probe columns, in order — share their buffers instead of copying them; no scan of the counts
@@ -461,7 +422,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         return out;
     }
     Buf pos = dev_alloc(c, (np + 1) * 4);
-    exclusive_scan_u32(c, cnt->as<uint32_t>(), pos->as<uint32_t>(), np, tot->as<uint64_t>());
+    exclusive_scan_u32(c, cnt->as<uint32_t>(), pos->as<uint32_t>(), np, flags->as<uint64_t>());
     Buf pid = dev_alloc(c, m * 4), iid = dev_alloc(c, m * 4);
     {
         KernelTimer kt(c, "join_pairs", np * 12 + m * 8);
@@ -493,12 +454,8 @@ bool index_has_duplicates(Ctx* c, Index& ix) {
     Buf flags = dev_alloc(c, 64);
     CPB_CUDA(cudaMemsetAsync(flags->p, 0, 64, c->stream));
     HashTable& ht = ensure_hash(c, ix, nk, true, flags->as<uint32_t>() + 8);
-    if (ht.slots16) {  // the 16-byte-slot insert saw every key it met twice: no self probe needed
-        uint32_t* hf = (uint32_t*)c->pinned_scratch(64);
-        CPB_CUDA(cudaMemcpyAsync(hf, flags->p, 64, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        return hf[8] != 0;
-    }
+    if (ht.slots16)  // the 16-byte-slot insert saw every key it met twice: no self probe needed
+        return read_back<uint32_t>(c, flags->as<uint32_t>() + 8) != 0;
     Buf lo = dev_alloc(c, n * 4), cnt = dev_alloc(c, (n + 1) * 4);
     probe_dispatch(c, *ix.src, ix.key_col_idx, ix, ht, ix.uimage, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags->as<uint32_t>() + 2);
     {
@@ -506,10 +463,7 @@ bool index_has_duplicates(Ctx* c, Index& ix) {
         self_check_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(lo->as<uint32_t>(), cnt->as<uint32_t>(), n, flags->as<uint32_t>() + 8);
         CPB_CUDA(cudaGetLastError());
     }
-    uint32_t* hf = (uint32_t*)c->pinned_scratch(64);
-    CPB_CUDA(cudaMemcpyAsync(hf, flags->p, 64, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return hf[8] != 0;
+    return read_back<uint32_t>(c, flags->as<uint32_t>() + 8) != 0;
 }
 
 // ------------------------------------------------------------------ Index.Find: [lower, upper) of a key prefix
@@ -561,9 +515,7 @@ void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64
         find_range_kernel<<<1, 1, 0, c->stream>>>(ix.image->as<uint64_t>(), n, dv->as<uint64_t>(), (uint32_t)b, (unsigned long long*)out->p);
         CPB_CUDA(cudaGetLastError());
     }
-    uint64_t* h = (uint64_t*)c->pinned_scratch(16);
-    CPB_CUDA(cudaMemcpyAsync(h, out->p, 16, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint64_t> h = read_back<uint64_t>(c, out->p, 2);
     *lo = (int64_t)h[0]; *hi = (int64_t)h[1];
 }
 

@@ -227,15 +227,13 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, 
     Buf len = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 16);
     {
         KernelTimer kt(c, "json_row_len", n * 4 * (ncols + 1));
-        json_row_len_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, c->stream>>>(dcols, ncols, row_const, n, len->as<uint32_t>());
+        json_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dcols, ncols, row_const, n, len->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
     json_value_bytes_kernel<<<1, 1, 0, c->stream>>>(dcols, ncols, n, tot->as<unsigned long long>() + 1);
     CPB_CUDA(cudaGetLastError());
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(16);
-    CPB_CUDA(cudaMemcpyAsync(ht, tot->p, 16, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint64_t> ht = read_back<uint64_t>(c, tot->p, 2);
     const uint64_t body = ht[0], value_bytes = ht[1];
     if (body >= 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToJSON output exceeds 4 GiB; write in smaller batches"};
     *nbytes = body + (last ? 1 : 0);

@@ -100,10 +100,7 @@ uint32_t quote_parity(Ctx* c, const uint8_t* in, uint64_t n) {
         quote_parity_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(in, n, out->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
-    uint32_t* h = (uint32_t*)c->pinned_scratch(4);
-    CPB_CUDA(cudaMemcpyAsync(h, out->p, 4, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return *h & 1u;
+    return read_back<uint32_t>(c, out->p) & 1u;
 }
 
 std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, const cpb_reader_opts& o_arg,
@@ -352,28 +349,34 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
     P.lits = lits->as<uint8_t>();
     P.lits_len = (uint32_t)comp.lits.size();
 
+    // the result of either path: the table of the slot buffers, and the error err_key names (ordinal << 16 | kind << 8 |
+    // slot of the first failing record, ~0 = none)
+    auto finish = [&](int64_t nrows, uint64_t first_line, uint64_t err_key, const std::vector<Buf>& offs, const std::vector<Buf>& datas) {
+        auto t = std::make_shared<Table>();
+        t->ctx = c; t->nrows = nrows; t->first_line = first_line; t->record_fields = first_nfields;
+        if (err_key != ~0ull) {
+            uint64_t ordinal = err_key >> 16;
+            int kind = (int)((err_key >> 8) & 0xff), slot = (int)(err_key & 0xff);
+            if (kind == CPB_E_COLUMN_INDEX) {
+                int ci = 0;
+                for (size_t i = 0; i < cols.size(); i++) if (col_slot[i] == slot) { ci = (int)i; break; }
+                fail(kind, ci, line_base + ordinal,
+                     "column not found: " + go_quote(cols[ci].first) + " (" + std::to_string(cols[ci].second) + ")");  // csvplus.go:1128
+            } else fail(kind, -1, line_base + ordinal, kind_text(kind));
+        }
+        for (size_t i = 0; i < cols.size(); i++) {
+            Column col; col.name = cols[i].first; col.offsets = offs[col_slot[i]]; col.data = datas[col_slot[i]];
+            t->cols.push_back(col);
+            t->src_field.push_back(cols[i].second);
+        }
+        return t;
+    };
     auto run_general = [&]() -> std::shared_ptr<Table> {
         GenResult gr;
         P.subs = subs_dev; P.trim = 0; P.comment = 0;
         general_parse(c, P, o, &sub, data_start, &gr);
         if (ba) *ba->records = gr.nrec;
-        auto t = std::make_shared<Table>();
-        t->ctx = c; t->nrows = (int64_t)gr.rows; t->first_line = line_base; t->record_fields = first_nfields;
-        if (gr.err_key != ~0ull) {
-            uint64_t ordinal = gr.err_key >> 16;
-            int kind = (int)((gr.err_key >> 8) & 0xff), slot = (int)(gr.err_key & 0xff);
-            if (kind == CPB_E_COLUMN_INDEX) {
-                int ci = 0;
-                for (size_t i = 0; i < cols.size(); i++) if (col_slot[i] == slot) { ci = (int)i; break; }
-                fail(kind, ci, line_base + ordinal, "column not found: " + go_quote(cols[ci].first) + " (" + std::to_string(cols[ci].second) + ")");
-            } else fail(kind, -1, line_base + ordinal, kind_text(kind));
-        }
-        for (size_t i = 0; i < cols.size(); i++) {
-            Column col; col.name = cols[i].first; col.offsets = gr.offs[col_slot[i]]; col.data = gr.datas[col_slot[i]];
-            t->cols.push_back(col);
-            t->src_field.push_back(cols[i].second);
-        }
-        return t;
+        return finish((int64_t)gr.rows, line_base, gr.err_key, gr.offs, gr.datas);
     };
     if (general) return run_general();
 
@@ -436,10 +439,7 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
             case 8: launch_scan<8, true>(c, P, algo); break;
             default: launch_scan<16, false>(c, P, algo); break;
         }
-        ParseResult* hr = (ParseResult*)c->pinned_scratch(sizeof(ParseResult));
-        CPB_CUDA(cudaMemcpyAsync(hr, P.result, sizeof(ParseResult), cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        res = *hr;
+        res = read_back<ParseResult>(c, P.result);
         if (optimistic) {  // did the shortcut hold?
             const int ekind = res.err_key == ~0ull ? 0 : (int)((res.err_key >> 8) & 0xff);
             const bool lazy_matters = o.lazy_quotes && (ekind == CPB_E_BARE_QUOTE || ekind == CPB_E_QUOTE);
@@ -473,28 +473,8 @@ std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, 
         c->stats["csv_scan"].bytes += s_out;
     }
 
-    auto t = std::make_shared<Table>();
-    t->ctx = c;
-    t->nrows = (int64_t)res.totals[1];
-    t->first_line = line_base + (res.first_row_ordinal == ~0ull ? 0 : res.first_row_ordinal);
-    if (res.err_key != ~0ull) {
-        uint64_t ordinal = res.err_key >> 16;
-        int kind = (int)((res.err_key >> 8) & 0xff), slot = (int)(res.err_key & 0xff);
-        t->nrows = (int64_t)res.err_rows;
-        if (kind == CPB_E_COLUMN_INDEX) {
-            int ci = 0;
-            for (size_t i = 0; i < cols.size(); i++) if (col_slot[i] == slot) { ci = (int)i; break; }
-            fail(kind, ci, line_base + ordinal,
-                 "column not found: " + go_quote(cols[ci].first) + " (" + std::to_string(cols[ci].second) + ")");  // csvplus.go:1128
-        } else fail(kind, -1, line_base + ordinal, kind_text(kind));
-    }
-    for (size_t i = 0; i < cols.size(); i++) {
-        Column col; col.name = cols[i].first; col.offsets = offs[col_slot[i]]; col.data = datas[col_slot[i]];
-        t->cols.push_back(col);
-        t->src_field.push_back(cols[i].second);
-    }
-    t->record_fields = first_nfields;
-    return t;
+    return finish((int64_t)(res.err_key != ~0ull ? res.err_rows : res.totals[1]),
+                  line_base + (res.first_row_ordinal == ~0ull ? 0 : res.first_row_ordinal), res.err_key, offs, datas);
 }
 
 }  // namespace cpb

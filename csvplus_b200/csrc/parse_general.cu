@@ -192,36 +192,39 @@ __global__ void g_sentinel(ParseParams P, const uint32_t* __restrict__ offs, uin
     if (k < P.nsel) P.out_off[k][rows] = offs[(uint64_t)k * (nrec + 1) + nrec_eff];
 }
 
-static inline uint32_t nblk(uint64_t n, int t) { return (uint32_t)((n + t - 1) / t); }
-
 // Returns the raw pieces of the general parse; parse.cu turns them into a Table and error (shared logic).
 
-static void gen_subs(GenOpts& g, const Substitution* sub) {
+// the transition table T of g's trim option; without a comment byte (has_comment false) the comment class is ordinary data
+static void gen_transitions(GenOpts& g, bool has_comment) {
+    for (int cl = 0; cl < NCLASS; cl++) {
+        uint32_t v = 0;
+        for (int s = 0; s < 8; s++) v |= (uint32_t)gen_delta(s, (cl == C_C && !has_comment) ? C_O : cl, g.trim) << (3 * s);
+        g.T[cl] = v;
+    }
+}
+
+// the machine of the (single-byte, after subst.cu) reader options and the substitution's stand-in bytes
+static GenOpts gen_opts(const cpb_reader_opts& o, const Substitution* sub) {
+    GenOpts g{};
+    g.delim = (uint8_t)o.delimiter; g.comment = (uint8_t)o.comment; g.lazy = o.lazy_quotes; g.trim = o.trim_leading_space;
     if (sub && sub->table) {
         g.subs = sub->table->as<SubTable>();
         memcpy(g.sp_bits, sub->host_table.space_bits, sizeof g.sp_bits);
         for (int i = 0; i < 8; i++) if (g.sp_bits[i]) g.has_sp = 1;
     }
+    gen_transitions(g, g.comment != 0);
+    return g;
 }
 
 void general_header(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o, const Substitution* sub, HeaderOut* dev_out) {
-    GenOpts g{};
-    g.delim = (uint8_t)o.delimiter; g.comment = (uint8_t)o.comment; g.lazy = o.lazy_quotes; g.trim = o.trim_leading_space;
-    gen_subs(g, sub);
+    const GenOpts g = gen_opts(o, sub);
     KernelTimer kt(c, "csv_header_general", 0);
     g_header_kernel<<<1, 1, 0, c->stream>>>(in, n, g, dev_out);
     CPB_CUDA(cudaGetLastError());
 }
 
 void general_parse(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substitution* sub, uint64_t data_start, GenResult* out) {
-    GenOpts g{};
-    g.delim = (uint8_t)o.delimiter; g.comment = (uint8_t)o.comment; g.lazy = o.lazy_quotes; g.trim = o.trim_leading_space;
-    gen_subs(g, sub);
-    for (int cl = 0; cl < NCLASS; cl++) {
-        uint32_t v = 0;
-        for (int s = 0; s < 8; s++) v |= (uint32_t)gen_delta(s, (cl == C_C && !g.comment) ? C_O : cl, g.trim) << (3 * s);
-        g.T[cl] = v;
-    }
+    const GenOpts g = gen_opts(o, sub);
     const uint64_t n = P.n;
     const uint64_t nchunks = (n + GCHUNK - 1) / GCHUNK, nblocks = (nchunks + GBLOCK - 1) / GBLOCK;
     Buf vec = dev_alloc(c, nchunks * 4), bvec = dev_alloc(c, nblocks * 4), bstate = dev_alloc(c, nblocks + 1), cstate = dev_alloc(c, nchunks);
@@ -236,10 +239,7 @@ void general_parse(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substi
         CPB_CUDA(cudaGetLastError());
     }
     exclusive_scan_u32(c, counts->as<uint32_t>(), counts->as<uint32_t>(), nchunks, tot->as<uint64_t>());
-    uint64_t* hp = (uint64_t*)c->pinned_scratch(64);
-    CPB_CUDA(cudaMemcpyAsync(hp, tot->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    const uint64_t nstarts = hp[0];
+    const uint64_t nstarts = read_back<uint64_t>(c, tot->p);
     if (nstarts > 0xfffffff0ull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "more than 2^32 records in one batch"};
     Buf starts = dev_alloc(c, (nstarts + 1) * 8);
     g_starts<true><<<nblk(nchunks, 128), 128, 0, c->stream>>>(P.in, n, g, cstate->as<uint8_t>(), nullptr, counts->as<uint32_t>(),
@@ -266,18 +266,13 @@ void general_parse(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substi
         g_rec_count<<<nblk(nrec, 128), 128, 0, c->stream>>>(P, g, (const unsigned long long*)starts->p, nrec, first, flag->as<uint32_t>(), lens->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
-    ParseResult* hr = (ParseResult*)c->pinned_scratch(sizeof(ParseResult));
-    CPB_CUDA(cudaMemcpyAsync(hr, res->p, sizeof(ParseResult), cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    out->err_key = hr->err_key;
+    out->err_key = read_back<ParseResult>(c, res->p).err_key;
     const uint64_t nrec_eff = out->err_key == ~0ull ? nrec : (uint64_t)(out->err_key >> 16);  // rows before the first failing record
     out->nrec_eff = nrec_eff;
     exclusive_scan_u32(c, flag->as<uint32_t>(), rowpos->as<uint32_t>(), nrec_eff, tots->as<uint64_t>());
     for (int k = 0; k < nsel; k++)
         exclusive_scan_u32(c, lens->as<uint32_t>() + (uint64_t)k * nrec, offs->as<uint32_t>() + (uint64_t)k * (nrec + 1), nrec_eff, tots->as<uint64_t>() + 1 + k);
-    uint64_t* ht = (uint64_t*)c->pinned_scratch((nsel + 1) * 8);
-    CPB_CUDA(cudaMemcpyAsync(ht, tots->p, (nsel + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint64_t> ht = read_back<uint64_t>(c, tots->p, nsel + 1);
     out->rows = ht[0];
     for (int k = 0; k < nsel; k++) {
         if (ht[1 + k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, k, 0, false, "a column of this batch exceeds 4 GiB; parse the input in smaller batches"};
@@ -351,11 +346,7 @@ void general_cut(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o
     g.delim = o.delimiter < 0x80 ? (uint8_t)o.delimiter : (uint8_t)'"';  // '"' classifies first: a multi-byte delimiter is a token
     g.comment = o.comment < 0x80 ? (uint8_t)o.comment : 0;
     g.lazy = o.lazy_quotes; g.trim = o.trim_leading_space;
-    for (int cl = 0; cl < NCLASS; cl++) {
-        uint32_t v = 0;
-        for (int s = 0; s < 8; s++) v |= (uint32_t)gen_delta(s, (cl == C_C && !o.comment) ? C_O : cl, g.trim) << (3 * s);
-        g.T[cl] = v;
-    }
+    gen_transitions(g, o.comment != 0);
     CutTokens tk{};
     auto add = [&](uint32_t r, int cls) {
         if (r < 0x80 || tk.n >= MAX_SUB_SEQ) return;

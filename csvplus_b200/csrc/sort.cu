@@ -16,9 +16,6 @@
 
 namespace cpb {
 
-static inline uint32_t nblk(uint64_t n, int t) { return (uint32_t)((n + t - 1) / t); }
-
-
 // ------------------------------------------------------------------ key widths
 __global__ void max_len_kernel(const uint32_t* __restrict__ off, uint64_t n, uint32_t* out) {
     uint32_t m = 0;
@@ -158,9 +155,7 @@ static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t
         CPB_CUDA(cudaGetLastError());
     }
     *traffic += n * 8 * words;
-    uint32_t* hh = (uint32_t*)c->pinned_scratch((size_t)words * 8 * 256 * 4);
-    CPB_CUDA(cudaMemcpyAsync(hh, hist->p, (size_t)words * 8 * 256 * 4, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<uint32_t> hh = read_back<uint32_t>(c, hist->p, (size_t)words * 8 * 256);
     std::vector<uint8_t> skip((size_t)words * 8, 0);
     for (uint32_t w = 0; w < words; w++)
         for (int b = 0; b < 8; b++)
@@ -191,20 +186,14 @@ static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t
 }
 
 // ------------------------------------------------------------------ adjacent compare (unique check, groups)
-// flags[i] = 1 when row i starts a new key (first `pbytes` bytes of the image differ from row i-1)
-__device__ __forceinline__ bool image_prefix_equal(const uint64_t* image, uint64_t n, uint64_t a, uint64_t b, uint32_t pbytes) {
-    uint32_t full = pbytes >> 3, rem = pbytes & 7;
-    for (uint32_t w = 0; w < full; w++) if (image[(uint64_t)w * n + a] != image[(uint64_t)w * n + b]) return false;
-    if (rem) {
-        uint64_t m = ~0ull << (8 * (8 - rem));
-        if ((image[(uint64_t)full * n + a] & m) != (image[(uint64_t)full * n + b] & m)) return false;
-    }
-    return true;
-}
 __global__ void head_flags_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, uint32_t* head) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    head[i] = (i == 0 || !image_prefix_equal(image, n, i, i - 1, pbytes)) ? 1u : 0u;
+    head[i] = (i == 0 || !prefix_equal(image, n, i, image, n, i - 1, pbytes)) ? 1u : 0u;
+}
+void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head) {
+    head_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(image, n, pbytes, head);
+    CPB_CUDA(cudaGetLastError());
 }
 __global__ void first_dup_kernel(const uint32_t* __restrict__ head, uint64_t n, unsigned long long* first) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -218,10 +207,6 @@ __global__ void group_flags_kernel(const uint32_t* __restrict__ head, uint64_t n
     gs[i] = (h && !nh) ? 1u : 0u;
     ge[i] = (!h && nh) ? 1u : 0u;
 }
-__global__ void compact_pos_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* out, uint64_t n, uint32_t add) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) out[pos[i]] = (uint32_t)i + add;
-}
 __global__ void singleton_flags_kernel(const uint32_t* __restrict__ head, uint64_t n, uint32_t* keep) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -233,13 +218,6 @@ __global__ void set_flags_kernel(const int64_t* __restrict__ rows, uint64_t m, u
     if (i < m && rows[i] >= 0 && (uint64_t)rows[i] < n) keep[rows[i]] = 1u;
 }
 __global__ void clear_one_kernel(uint32_t* keep, uint64_t i) { keep[i] = 0; }
-
-static uint64_t read_u64(Ctx* c, const void* dev) {
-    uint64_t* h = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(h, dev, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return *h;
-}
 
 void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, KeyDesc& kd) {
     kd.nkeys = (int)kidx.size();
@@ -276,27 +254,46 @@ Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const
     return img;
 }
 
-static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic);
+// per key column the longest value of rows [0, n) of t: the column widths of the key image
+static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n) {
+    Buf wd = dev_alloc(c, key_cols.size() * 4);
+    CPB_CUDA(cudaMemsetAsync(wd->p, 0, key_cols.size() * 4, c->stream));
+    for (size_t k = 0; k < key_cols.size() && n; k++)
+        max_len_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(t.cols[key_cols[k]].off(), n, wd->as<uint32_t>() + k);
+    CPB_CUDA(cudaGetLastError());
+    return read_back<uint32_t>(c, wd->p, key_cols.size());
+}
+
+// rows ids[0..m) of a key image of n_src rows, as an image of m rows
+static Buf gather_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n_src, const uint32_t* ids, uint64_t m) {
+    Buf out = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)words * m) * 8);
+    for (uint32_t w = 0; w < words && m; w++)
+        gather_u64_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(image + (uint64_t)w * n_src, ids, out->as<uint64_t>() + (uint64_t)w * m, m);
+    CPB_CUDA(cudaGetLastError());
+    return out;
+}
+
+// while in scope, what c allocates stays inside an index: it comes from the pool of the index's owner (dev_alloc)
+struct OwnerPool {
+    Ctx* c; Ctx* prev;
+    OwnerPool(Ctx* ctx, Ctx* owner) : c(ctx), prev(ctx->alloc_for) { c->alloc_for = owner; }
+    ~OwnerPool() { c->alloc_for = prev; }
+    OwnerPool(const OwnerPool&) = delete; OwnerPool& operator=(const OwnerPool&) = delete;
+};
+
 static void ensure_sorted_locked(Ctx* c, Index& ix) {
     if (ix.sorted) return;
     const uint64_t n = (uint64_t)ix.nrows;
-    Ctx* prev = c->alloc_for;
-    c->alloc_for = ix.ctx;  // what stays inside the index comes from its owner's pool
-    try {
-        uint64_t traffic = 0;
-        Buf perm = sort_by_image(c, ix.uimage->as<uint64_t>(), ix.image_words, n, &traffic);
-        Buf simg = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)ix.image_words * n) * 8);
-        {
-            KernelTimer kt(c, "image_gather", (uint64_t)ix.image_words * n * 20, (int)ix.image_words);
-            for (uint32_t w = 0; w < ix.image_words; w++)
-                gather_u64_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(ix.uimage->as<uint64_t>() + (uint64_t)w * n, perm->as<uint32_t>(),
-                                                                       simg->as<uint64_t>() + (uint64_t)w * n, n);
-            CPB_CUDA(cudaGetLastError());
-        }
-        sync_stream(c);  // complete before another context (stream) can see it
-        ix.perm = perm; ix.image = simg; ix.sorted = true;
-    } catch (...) { c->alloc_for = prev; throw; }
-    c->alloc_for = prev;
+    OwnerPool scope(c, ix.ctx);
+    uint64_t traffic = 0;
+    Buf perm = sort_by_image(c, ix.uimage->as<uint64_t>(), ix.image_words, n, &traffic);
+    Buf simg;
+    {
+        KernelTimer kt(c, "image_gather", (uint64_t)ix.image_words * n * 20, (int)ix.image_words);
+        simg = gather_image(c, ix.uimage->as<uint64_t>(), ix.image_words, n, perm->as<uint32_t>(), n);
+    }
+    sync_stream(c);  // complete before another context (stream) can see it
+    ix.perm = perm; ix.image = simg; ix.sorted = true;
 }
 void ensure_sorted(Ctx* c, Index& ix) {
     std::lock_guard<std::mutex> lk(ix.mu);
@@ -307,14 +304,10 @@ std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix) {
     std::lock_guard<std::mutex> lk(ix.mu);
     if (ix.table) return ix.table;
     ensure_sorted_locked(c, ix);
-    Ctx* prev = c->alloc_for;
-    c->alloc_for = ix.ctx;  // the sorted rows stay inside the index: they come from its owner's pool
-    try {
-        ix.table = gather_rows(c, *ix.src, ix.perm->as<uint32_t>(), ix.nrows);
-        ix.table->first_line = 0;  // iterating an Index reports 0-based rows (csvplus.go:243)
-        sync_stream(c);  // complete before another context (stream) can see it
-    } catch (...) { c->alloc_for = prev; throw; }
-    c->alloc_for = prev;
+    OwnerPool scope(c, ix.ctx);
+    ix.table = gather_rows(c, *ix.src, ix.perm->as<uint32_t>(), ix.nrows);
+    ix.table->first_line = 0;  // iterating an Index reports 0-based rows (csvplus.go:243)
+    sync_stream(c);  // complete before another context (stream) can see it
     return ix.table;
 }
 
@@ -346,18 +339,10 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
     }
     if (n > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "an index holds at most 2^32-2 rows"};
     // 1. key widths
-    Buf wd = dev_alloc(c, keys.size() * 4);
-    CPB_CUDA(cudaMemsetAsync(wd->p, 0, keys.size() * 4, c->stream));
     {
         KernelTimer kt(c, "key_width", n * 4 * keys.size(), (int)keys.size());
-        for (size_t k = 0; k < keys.size(); k++)
-            max_len_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(t.cols[ix->key_col_idx[k]].off(), n, wd->as<uint32_t>() + k);
-        CPB_CUDA(cudaGetLastError());
+        ix->key_width = key_widths(c, t, ix->key_col_idx, n);
     }
-    uint32_t* hw = (uint32_t*)c->pinned_scratch(keys.size() * 4);
-    CPB_CUDA(cudaMemcpyAsync(hw, wd->p, keys.size() * 4, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    ix->key_width.assign(hw, hw + keys.size());
     // 2. image of the unsorted rows
     uint32_t words = 0;
     Buf img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &words);
@@ -377,38 +362,30 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
     Buf perm = sort_by_image(c, img->as<uint64_t>(), words, n, &traffic);
     // 4. the sorted key image; the sorted rows themselves stay virtual (src + perm) until something needs them
     ix->src = tp; ix->perm = perm; ix->nrows = (int64_t)n;
-    Buf simg = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)words * n) * 8);
     {
         KernelTimer kt(c, "image_gather", (uint64_t)words * n * 20, (int)words);
-        for (uint32_t w = 0; w < words; w++)
-            gather_u64_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(img->as<uint64_t>() + (uint64_t)w * n, perm->as<uint32_t>(),
-                                                                   simg->as<uint64_t>() + (uint64_t)w * n, n);
-        CPB_CUDA(cudaGetLastError());
+        ix->image = gather_image(c, img->as<uint64_t>(), words, n, perm->as<uint32_t>(), n);
     }
-    ix->image = simg;
+    const uint64_t* simg = ix->image->as<uint64_t>();
     // 5. uniqueness (createUniqueIndex, csvplus.go:740-756)
     if (unique && n >= 2) {
         Buf head = dev_alloc(c, n * 4), first = dev_alloc(c, 8);
         CPB_CUDA(cudaMemsetAsync(first->p, 0xff, 8, c->stream));
         {
             KernelTimer kt(c, "unique_check", (uint64_t)words * n * 8, 2);
-            head_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(simg->as<uint64_t>(), n, words * 8, head->as<uint32_t>());
+            head_flags(c, simg, n, words * 8, head->as<uint32_t>());
             first_dup_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, (unsigned long long*)first->p);
             CPB_CUDA(cudaGetLastError());
         }
-        uint64_t fd = read_u64(c, first->p);
+        const uint64_t fd = read_back<uint64_t>(c, first->p);
         if (fd != ~0ull) {
             // "duplicate value while creating unique index: " + rows[i].SelectExisting(columns...).String()  (:751, :90-104)
             std::vector<std::pair<std::string, std::string>> kv;
             for (size_t k = 0; k < keys.size(); k++) {
                 const Column& col = sorted_table(c, *ix)->cols[ix->key_col_idx[k]];
-                uint32_t oo[2];
-                CPB_CUDA(cudaMemcpyAsync(oo, col.off() + fd, 8, cudaMemcpyDeviceToHost, c->stream));
-                sync_stream(c);
-                std::string v(oo[1] - oo[0], '\0');
-                if (!v.empty()) CPB_CUDA(cudaMemcpyAsync(&v[0], col.bytes() + oo[0], v.size(), cudaMemcpyDeviceToHost, c->stream));
-                sync_stream(c);
-                kv.emplace_back(keys[k], v);
+                const std::vector<uint32_t> oo = read_back<uint32_t>(c, col.off() + fd, 2);
+                const std::vector<char> v = read_back<char>(c, col.bytes() + oo[0], oo[1] - oo[0]);
+                kv.emplace_back(keys[k], std::string(v.begin(), v.end()));
             }
             std::sort(kv.begin(), kv.end());
             std::string s = "{ ";
@@ -424,16 +401,6 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
 }
 
 // ------------------------------------------------------------------ ResolveDuplicates support
-static Buf compact_flags(Ctx* c, const uint32_t* flags, uint64_t n, uint32_t add, uint64_t* count) {
-    Buf pos = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8);
-    exclusive_scan_u32(c, flags, pos->as<uint32_t>(), n, tot->as<uint64_t>());
-    *count = read_u64(c, tot->p);
-    Buf out = dev_alloc(c, (*count + 1) * 4);
-    if (n) compact_pos_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(flags, pos->as<uint32_t>(), out->as<uint32_t>(), n, add);
-    CPB_CUDA(cudaGetLastError());
-    return out;
-}
-
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi) {
     lo.clear(); hi.clear();
     const uint64_t n = (uint64_t)ix.nrows;
@@ -441,13 +408,20 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
     Buf head = dev_alloc(c, n * 4), gs = dev_alloc(c, n * 4), ge = dev_alloc(c, n * 4);
     {
         KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 12, 2);
-        head_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
+        head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
         group_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>(), ge->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
+    auto compact = [&](const Buf& flags, uint32_t add, uint64_t* count) {
+        const FlagScan s = scan_flags(c, flags->as<uint32_t>(), n);
+        Buf out = dev_alloc(c, (s.count + 1) * 4);
+        compact_flags(c, s, add, out->as<uint32_t>());
+        *count = s.count;
+        return out;
+    };
     uint64_t ng = 0, ne = 0;
-    Buf los = compact_flags(c, gs->as<uint32_t>(), n, 0, &ng);
-    Buf his = compact_flags(c, ge->as<uint32_t>(), n, 1, &ne);
+    Buf los = compact(gs, 0, &ng);
+    Buf his = compact(ge, 1, &ne);
     if (ng != ne) throw ArgError{CPB_ERR_CUDA, "internal: group start/end mismatch"};
     std::vector<uint32_t> a(ng), b(ng);
     if (ng) {
@@ -492,32 +466,27 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
             }
     }
     Buf head = dev_alloc(c, n * 4), flag = dev_alloc(c, n * 4);
-    head_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
+    head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
     singleton_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, flag->as<uint32_t>());
     Buf kd = dev_alloc(c, keep.size() * 8);
     CPB_CUDA(cudaMemcpyAsync(kd->p, keep.data(), keep.size() * 8, cudaMemcpyHostToDevice, c->stream));
     set_flags_kernel<<<nblk(keep.size(), 256), 256, 0, c->stream>>>(kd->as<int64_t>(), keep.size(), flag->as<uint32_t>(), n);
     if (bug_compatible) {
         // SURVEY §Q1: when a group exists and the last sorted row is a singleton it is never copied (:851-864)
-        uint32_t hl[2];
-        CPB_CUDA(cudaMemcpyAsync(&hl[0], head->as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        if (hl[0] != 0) clear_one_kernel<<<1, 1, 0, c->stream>>>(flag->as<uint32_t>(), n - 1);
+        if (read_back<uint32_t>(c, head->as<uint32_t>() + (n - 1)) != 0) clear_one_kernel<<<1, 1, 0, c->stream>>>(flag->as<uint32_t>(), n - 1);
     }
     CPB_CUDA(cudaGetLastError());
     // compaction of the kept positions (the scanned positions are needed again to patch replacement ids in)
-    Buf pos = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8);
-    exclusive_scan_u32(c, flag->as<uint32_t>(), pos->as<uint32_t>(), n, tot->as<uint64_t>());
-    const uint64_t m = read_u64(c, tot->p);
+    const FlagScan kept = scan_flags(c, flag->as<uint32_t>(), n);
+    const uint64_t m = kept.count;
     Buf ids = dev_alloc(c, (m + 1) * 4);
-    compact_pos_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(flag->as<uint32_t>(), pos->as<uint32_t>(), ids->as<uint32_t>(), n, 0);
-    CPB_CUDA(cudaGetLastError());
+    compact_flags(c, kept, 0, ids->as<uint32_t>());
     std::shared_ptr<Table> nt;
     if (!rpos.empty()) {
         Buf dp = dev_alloc(c, rpos.size() * 8), dr = dev_alloc(c, rid.size() * 4);
         CPB_CUDA(cudaMemcpyAsync(dp->p, rpos.data(), rpos.size() * 8, cudaMemcpyHostToDevice, c->stream));
         CPB_CUDA(cudaMemcpyAsync(dr->p, rid.data(), rid.size() * 4, cudaMemcpyHostToDevice, c->stream));
-        patch_ids_kernel<<<nblk(rpos.size(), 256), 256, 0, c->stream>>>(pos->as<uint32_t>(), dp->as<int64_t>(), dr->as<uint32_t>(), rpos.size(), ids->as<uint32_t>());
+        patch_ids_kernel<<<nblk(rpos.size(), 256), 256, 0, c->stream>>>(kept.pos->as<uint32_t>(), dp->as<int64_t>(), dr->as<uint32_t>(), rpos.size(), ids->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
         // rows [0, n) = the index, rows [n, n + repl) = the replacement rows in the index's column order
         Table rsel; rsel.ctx = c; rsel.nrows = repl->nrows;
@@ -529,14 +498,7 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
         nt->first_line = 0;
         ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m; ix.unique = false;
         for (size_t k = 0; k < ix.key_cols.size(); k++) ix.key_col_idx[k] = nt->find(ix.key_cols[k]);
-        Buf wd = dev_alloc(c, ix.key_cols.size() * 4);
-        CPB_CUDA(cudaMemsetAsync(wd->p, 0, ix.key_cols.size() * 4, c->stream));
-        for (size_t k = 0; k < ix.key_cols.size() && m; k++)
-            max_len_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(nt->cols[ix.key_col_idx[k]].off(), m, wd->as<uint32_t>() + k);
-        uint32_t* hw = (uint32_t*)c->pinned_scratch(ix.key_cols.size() * 4);
-        CPB_CUDA(cudaMemcpyAsync(hw, wd->p, ix.key_cols.size() * 4, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        ix.key_width.assign(hw, hw + ix.key_cols.size());
+        ix.key_width = key_widths(c, *nt, ix.key_col_idx, m);
         uint32_t words = 0;
         ix.image = pack_with_widths(c, *nt, ix.key_col_idx, ix.key_width, &words);
         ix.image_words = words;
@@ -544,11 +506,7 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
         return;
     }
     nt = gather_rows(c, *ix.table, ids->as<uint32_t>(), (int64_t)m);
-    Buf simg = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)ix.image_words * m) * 8);
-    for (uint32_t w = 0; w < ix.image_words && m; w++)
-        gather_u64_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(ix.image->as<uint64_t>() + (uint64_t)w * n, ids->as<uint32_t>(),
-                                                               simg->as<uint64_t>() + (uint64_t)w * m, m);
-    CPB_CUDA(cudaGetLastError());
+    Buf simg = gather_image(c, ix.image->as<uint64_t>(), ix.image_words, n, ids->as<uint32_t>(), m);
     nt->first_line = 0;
     ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m;
     ix.image = simg; ix.hash.clear(); ix.row_slots.clear();

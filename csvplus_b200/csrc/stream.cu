@@ -206,10 +206,7 @@ struct Stream {
         uint64_t cut = len;
         if (!last_pushed) {
             stream_cut(c, in, len, o, cut_dev->as<uint64_t>());
-            uint64_t* h = (uint64_t*)c->pinned_scratch(8);
-            CPB_CUDA(cudaMemcpyAsync(h, cut_dev->p, 8, cudaMemcpyDeviceToHost, c->stream));
-            sync_stream(c);
-            cut = *h;
+            cut = read_back<uint64_t>(c, cut_dev->p);
             if (cut == 0) {
                 // No line end outside quotes.  Either one record is longer than what was pushed so far, or (default
                 // options) a bare quote flipped the quote parity for the rest of the input, and the reference would stop

@@ -109,9 +109,7 @@ Substitution substitute_runes(Ctx* c, const uint8_t* in, uint64_t n, const cpb_r
         hist256_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(in, n, (unsigned long long*)hist->p);
         CPB_CUDA(cudaGetLastError());
     }
-    unsigned long long* hh = (unsigned long long*)c->pinned_scratch(256 * 8);
-    CPB_CUDA(cudaMemcpyAsync(hh, hist->p, 256 * 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
+    const std::vector<unsigned long long> hh = read_back<unsigned long long>(c, hist->p, 256);
     std::vector<int> unused;
     auto reserved = [&](int b) {
         return b == 0 || b == '"' || b == '\n' || b == '\r' || b == ' ' || b == '\t' || b == '\v' || b == '\f' || (uint32_t)b == o.delimiter ||
@@ -160,10 +158,7 @@ Substitution substitute_runes(Ctx* c, const uint8_t* in, uint64_t n, const cpb_r
         CPB_CUDA(cudaGetLastError());
     }
     exclusive_scan_u32(c, counts->as<uint32_t>(), counts->as<uint32_t>(), nchunks, tot->as<uint64_t>());
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(ht, tot->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    r.nbytes = *ht;
+    r.nbytes = read_back<uint64_t>(c, tot->p);
     r.buffer = dev_alloc(c, ((r.nbytes + 15) & ~15ull) + 256);
     CPB_CUDA(cudaMemsetAsync(r.buffer->as<uint8_t>() + (r.nbytes & ~15ull), 0, ((r.nbytes + 15) & ~15ull) + 256 - (r.nbytes & ~15ull), c->stream));
     {

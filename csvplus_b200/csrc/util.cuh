@@ -1,5 +1,5 @@
 // util.cuh — device-side helpers (sm_90a): mbarrier + bulk-async (TMA 1-D) staging, gpu-scope
-// acquire/release for the decoupled look-back chains, warp scans.
+// acquire/release for the decoupled look-back chains, warp scans, key-image compare.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -83,6 +83,19 @@ __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
     return v;
+}
+
+// ---- key images (sort.cu): word w of row r of an image of n rows is img[w * n + r], first byte most significant
+// the first pbytes bytes of row ra of image a equal those of row rb of image b
+__device__ __forceinline__ bool prefix_equal(const uint64_t* a, uint64_t na, uint64_t ra, const uint64_t* b, uint64_t nb, uint64_t rb,
+                                             uint32_t pbytes) {
+    uint32_t full = pbytes >> 3, rem = pbytes & 7;
+    for (uint32_t w = 0; w < full; w++) if (a[(uint64_t)w * na + ra] != b[(uint64_t)w * nb + rb]) return false;
+    if (rem) {
+        uint64_t m = ~0ull << (8 * (8 - rem));
+        if ((a[(uint64_t)full * na + ra] & m) != (b[(uint64_t)full * nb + rb] & m)) return false;
+    }
+    return true;
 }
 
 // ---- SWAR byte classification

@@ -122,14 +122,11 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     uint64_t in_bytes = 0;
     if (n) {
         KernelTimer kt(c, "csv_row_len", n * 4 * (wc.n + 1));
-        csv_row_len_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, c->stream>>>(wc, n, len->as<uint32_t>());
+        csv_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(wc, n, len->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
-    uint64_t* ht = (uint64_t*)c->pinned_scratch(8);
-    CPB_CUDA(cudaMemcpyAsync(ht, tot->p, 8, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    const uint64_t body = *ht;
+    const uint64_t body = read_back<uint64_t>(c, tot->p);
     if (body > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToCsv output exceeds 4 GiB; write in smaller batches"};
     *nbytes = header.size() + body;
     if (*nbytes > room) return nullptr;
