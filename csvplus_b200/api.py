@@ -27,6 +27,8 @@ Row = dict  # map[string]string, csvplus.go:59 (values are str; bytes survive vi
 # rows per cpb_table_to_json_into call when DataSource.ToJSON writes a device table: one call produces < 4 GiB, and
 # about 2.4 GB for joined rows of ~150 B.  A batch that is still too large is split in halves.
 JSON_BATCH_ROWS = 1 << 24
+# rows per cpb_index_gob_into call of Index.WriteTo (one call produces < 4 GiB; a batch that is still too large is halved)
+GOB_BATCH_ROWS = 1 << 24
 # bytes per host push of an input (FromFile / FromReader / host FromBytes, cpb_stream_*): one batch is parsed per push, so
 # every column of a batch stays far below the 4 GiB a column of one table may hold.  An input of at most this size is one
 # push.  128 MiB: on an H100 the streamed orders join of DESIGN §3.7 ran as fast as at 64 MiB with half the host
@@ -772,6 +774,91 @@ class Index:
                                                  rt.h if rt is not None else None, int(bug_compatible), C.byref(e))
         if st:
             _raise(st, e, self.ctx)
+
+    def WriteTo(self, fileName: str):  # csvplus.go:655-680: the file is removed on error
+        """the index as the reference's encoding/gob file (its key columns, then its rows in stored order), encoded on the
+        GPU and written in row-range batches through one pinned buffer.  A path that cannot be created raises the OS
+        error and leaves no file; any later error removes the file."""
+        f = open(fileName, "wb")
+        try:
+            with f:
+                self._write_gob(f)
+        except BaseException:
+            os.remove(fileName)
+            raise
+
+    def _write_gob(self, out: io.IOBase):
+        # one pinned buffer, sized up front so that the prefix and every batch are serialised in one call each: the prefix
+        # holds the key column names and about 100 bytes more, a batch at most the rows' total (and less than 4 GiB)
+        bound = 256 + sum(len(_enc(c)) + 10 for c in self.columns)
+        hold: list = [HostBuffer(self.ctx, bound)]
+        try:
+            plen, total = C.c_uint64(), C.c_uint64()
+            _write_into(out, hold, self.ctx, lambda buf: self._gob_begin(buf, plen, total))
+            rows_bytes = total.value - plen.value
+            if rows_bytes > hold[0].nbytes:
+                hold[0].free()
+                hold[:] = [HostBuffer(self.ctx, min(rows_bytes, 1 << 32) + 64)]
+            n, lo, step = len(self), 0, GOB_BATCH_ROWS
+            while lo < n:
+                hi = min(n, lo + step)
+                try:
+                    _write_into(out, hold, self.ctx, lambda buf: self._gob_into(buf, lo, hi))
+                except CsvPlusError as e:
+                    if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
+                        raise
+                    step = (hi - lo) // 2
+                    continue
+                lo = hi
+        finally:
+            for b in hold:
+                b.free()
+
+    def _gob_begin(self, buf: "HostBuffer | None", plen, total) -> int:
+        e = _abi.Error()
+        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
+        st = self.ctx.lib.cpb_index_gob_begin(self.ctx.h, self.h, C.c_void_p(ptr), cap, C.byref(plen), C.byref(total), C.byref(e))
+        if st == 2 and plen.value > cap:  # CPB_ERR_ARG: destination too small
+            return plen.value
+        if st:
+            _raise(st, e, self.ctx)
+        return plen.value
+
+    def _gob_into(self, buf: "HostBuffer | None", lo: int, hi: int) -> int:
+        n = C.c_uint64(); e = _abi.Error()
+        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
+        st = self.ctx.lib.cpb_index_gob_into(self.ctx.h, self.h, lo, hi, C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
+        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
+            return n.value
+        if st:
+            _raise(st, e, self.ctx)
+        return n.value
+
+
+def LoadIndex(fileName: str, ctx: Context | None = None) -> Index:  # csvplus.go:683-705
+    """an index from a file Index.WriteTo (or the reference) wrote, decoded on the GPU: its rows in file order, its key
+    columns from the file.  A missing file raises the OS error; an empty file raises CsvPlusError("EOF"), a cut one
+    CsvPlusError("unexpected EOF"), any other file that is not an index CsvPlusError with a description."""
+    ctx = ctx or Context.default()
+    with open(fileName, "rb") as f:
+        size = os.fstat(f.fileno()).st_size
+        buf = HostBuffer(ctx, max(size, 1))  # pinned: the rows are copied to the device from here
+        try:
+            got = f.readinto(memoryview(buf.array())[:size]) if size else 0
+            if got != size:
+                raise OSError(f"read {fileName}: short read")
+            h = C.c_void_p(); e = _abi.Error()
+            st = ctx.lib.cpb_index_load_gob(ctx.h, C.c_void_p(buf.ptr), size, C.byref(h), C.byref(e))
+            if st:
+                _raise(st, e, ctx)
+        finally:
+            buf.free()
+    cols = []
+    for k in range(ctx.lib.cpb_index_num_keys(h)):
+        s = _abi.Str()
+        ctx.lib.cpb_index_key_col(h, k, C.byref(s))
+        cols.append(_dec(C.string_at(s.ptr, s.len)))
+    return Index(ctx, h, cols)
 
 
 # ------------------------------------------------------------------ Reader (csvplus.go:922-1146)

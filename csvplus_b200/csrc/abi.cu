@@ -710,6 +710,52 @@ void cpb_index_free(cpb_index* ix) {
     delete ix;
 }
 void cpb_free(void* p) { free(p); }
+int cpb_index_key_col(const cpb_index* ix, int k, cpb_str* out) {
+    if (!ix || !out || k < 0 || k >= (int)ix->ix->key_cols.size()) return CPB_ERR_ARG;
+    out->ptr = ix->ix->key_cols[k].data(); out->len = ix->ix->key_cols[k].size();
+    return CPB_OK;
+}
+
+// ------------------------------------------------------------------ index files (gob.cu)
+static void deliver(Ctx* c, const Buf& out, uint64_t total, int mode, void** bytes, void* host_dst, uint64_t cap, const char* too_small);
+int cpb_index_gob_begin(cpb_ctx* h, const cpb_index* ix, void* prefix, uint64_t cap, uint64_t* prefix_len, uint64_t* total_len,
+                        cpb_error* err) {
+    if (!h || !ix || !prefix_len || !total_len || (cap && !prefix)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    const std::string p = gob_prefix(c, *ix->ix, total_len);
+    *prefix_len = p.size();
+    if (p.size() > cap) throw ArgError{CPB_ERR_ARG, "index file prefix destination too small"};
+    memcpy(prefix, p.data(), p.size());
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_index_gob_into(cpb_ctx* h, const cpb_index* ix, int64_t lo, int64_t hi, void* host_dst, uint64_t cap, uint64_t* nbytes,
+                       cpb_error* err) {
+    if (!h || !ix || !nbytes || (cap && !host_dst)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    if (lo < 0 || hi < lo || hi > ix->ix->nrows) throw ArgError{CPB_ERR_ARG, "bad row range"};
+    uint64_t total = 0;
+    Buf out = gob_rows(c, *ix->ix, (uint64_t)lo, (uint64_t)hi, cap, &total);
+    *nbytes = total;
+    deliver(c, out, total, 1, nullptr, host_dst, cap, "index file destination too small");
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_index_load_gob(cpb_ctx* h, const void* bytes, uint64_t nbytes, cpb_index** out, cpb_error* err) {
+    if (!h || !out || (nbytes && !bytes)) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    *out = nullptr;
+    CPB_TRY(c, err)
+    std::vector<std::string> keys;
+    *out = new cpb_index{gob_load(c, (const uint8_t*)bytes, nbytes, &keys)};
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
 
 static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, bool anti,
                        cpb_table** out, cpb_error* err) {

@@ -140,6 +140,9 @@ struct Index {
     std::map<std::vector<int>, RowSlots> row_slots_src;  // row slots in source order (filled sequentially, no permutation)
     const Table& schema() const { return table ? *table : *src; }  // column names / count only
     bool unique = false;               // built by UniqueIndexOn and verified: every full key occurs once
+    // false when the stored rows are not in key order (ResolveDuplicates with replacement rows, LoadIndex of such a file):
+    // Join / Except then search the rows exactly as the reference's binary search does instead of probing a hash table
+    bool in_order = true;
     std::vector<std::string> key_cols; // index.impl.columns
     std::vector<int> key_col_idx;      // positions in table->cols
     std::vector<uint32_t> key_width;   // per key column: max value length (bytes) in this index
@@ -309,6 +312,14 @@ void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi);
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep, bool bug_compatible, const Table* repl = nullptr);
+// the index takes the rows of nt in their stored order: key columns, widths and key image are rebuilt from them, in_order
+// is set from the image (sort.cu)
+void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt);
+// gob.cu: Index.WriteTo / LoadIndex.  gob_prefix: the file's bytes before the first row, *total = the file's size;
+// gob_rows: rows [lo, hi) of the stored rows (room as table_to_csv); gob_load: an index from a whole file's bytes
+std::string gob_prefix(Ctx* c, Index& ix, uint64_t* total);
+Buf gob_rows(Ctx* c, Index& ix, uint64_t lo, uint64_t hi, uint64_t room, uint64_t* nbytes);
+std::shared_ptr<Index> gob_load(Ctx* c, const uint8_t* bytes, uint64_t nbytes, std::vector<std::string>* key_cols);
 // write.cu: ToCsv of columns cols under the header line of names (when with_header).  room: the most bytes the caller can
 // take; when *nbytes exceeds it, null is returned after the length pass, before any output is allocated or written.
 Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, bool with_header,

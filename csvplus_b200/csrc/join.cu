@@ -334,6 +334,49 @@ static void probe_dispatch(Ctx* c, const Table& probe, const std::vector<int>& p
     CPB_CUDA(cudaGetLastError());
 }
 
+// the first pbytes of row r of image a (na rows) against those of row i of image b (nb rows): <0, 0, >0
+__device__ __forceinline__ int prefix_cmp(const uint64_t* a, uint64_t na, uint64_t r, const uint64_t* b, uint64_t nb, uint64_t i, uint32_t pbytes) {
+    const uint32_t full = pbytes >> 3, rem = pbytes & 7;
+    for (uint32_t w = 0; w < full; w++) {
+        const uint64_t x = a[(uint64_t)w * na + r], y = b[(uint64_t)w * nb + i];
+        if (x != y) return x < y ? -1 : 1;
+    }
+    if (rem) {
+        const uint64_t m = ~0ull << (8 * (8 - rem));
+        const uint64_t x = a[(uint64_t)full * na + r] & m, y = b[(uint64_t)full * nb + i] & m;
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return 0;
+}
+// An index whose rows are not in key order: per probe row what the reference computes, on any order of rows.
+// first = sort.Search(n, row >= v) (indexImpl.first, csvplus.go:893-897), then Join takes every row from there while
+// row <= v (:557); Except keeps the probe row when that run is empty (has, :899-905: the row at first equals v).
+__global__ void __launch_bounds__(256) join_search_kernel(const uint64_t* __restrict__ pimg, uint64_t np, const uint64_t* __restrict__ iimg,
+                                                          uint64_t ni, uint32_t pbytes, uint32_t* lo, uint32_t* cnt, uint32_t* not_one) {
+    unsigned long long matches = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t a = 0, b = ni;
+        while (a < b) { const uint64_t h = a + (b - a) / 2; if (prefix_cmp(iimg, ni, h, pimg, np, i, pbytes) < 0) a = h + 1; else b = h; }
+        uint64_t e = a;
+        while (e < ni && prefix_cmp(iimg, ni, e, pimg, np, i, pbytes) <= 0) e++;
+        const uint32_t c = (uint32_t)(e - a);
+        lo[i] = (uint32_t)a; cnt[i] = c; matches += c;
+        if (c != 1) *not_one = 1u;  // benign race: every writer stores 1
+    }
+    add_matches(not_one, matches);
+}
+static void search_probe(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, int nk, uint32_t* lo, uint32_t* cnt,
+                         uint32_t* not_one) {
+    const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
+    std::vector<uint32_t> widths(ix.key_width.begin(), ix.key_width.begin() + nk);
+    uint32_t pwords = 0;
+    Buf pimg = pack_with_widths(c, probe, pidx, widths, &pwords);
+    KernelTimer kt(c, "join_search", np * ((uint64_t)pwords * 8 + 8));
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
+    join_search_kernel<<<grid, 256, 0, c->stream>>>(pimg->as<uint64_t>(), np, ix.image->as<uint64_t>(), ni, prefix_bytes(ix, nk), lo, cnt, not_one);
+    CPB_CUDA(cudaGetLastError());
+}
+
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti,
                                    DataError* derr, bool* failed) {
     *failed = false;
@@ -393,6 +436,8 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     const Buf& iimage = by_src ? ix.uimage : ix.image;
     if (ni == 0) {
         CPB_CUDA(cudaMemsetAsync(cnt->p, 0, (np + 1) * 4, c->stream));
+    } else if (!ix.in_order) {
+        search_probe(c, probe, pidx, ix, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
     } else {
         HashTable& ht = ensure_hash(c, ix, nk, by_src);
         probe_dispatch(c, probe, pidx, ix, ht, iimage, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
@@ -483,12 +528,13 @@ __global__ void find_range_kernel(const uint64_t* __restrict__ image, uint64_t n
         }
         return 0;
     };
-    uint64_t i = 0, j = n;  // lower bound: first row >= val
-    while (i < j) { uint64_t h = i + (j - i) / 2; if (cmp(h) < 0) i = h + 1; else j = h; }
-    out[0] = i;
-    j = n;                  // upper bound: first row > val
+    // in the reference's order (:882-888), which decides the result when the rows are not in key order (in_order):
+    uint64_t i = 0, j = n;  // upper = sort.Search(n, row > val)
     while (i < j) { uint64_t h = i + (j - i) / 2; if (cmp(h) <= 0) i = h + 1; else j = h; }
     out[1] = i;
+    j = i; i = 0;           // lower = sort.Search(upper, row >= val)
+    while (i < j) { uint64_t h = i + (j - i) / 2; if (cmp(h) < 0) i = h + 1; else j = h; }
+    out[0] = i;
 }
 
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi) {

@@ -441,6 +441,39 @@ __global__ void patch_ids_kernel(const uint32_t* __restrict__ pos, const int64_t
     if (i < m) ids[pos[at[i]]] = with[i];
 }
 
+// *out = 1 when some row's key image is below the previous row's
+__global__ void order_check_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t words, uint32_t* out) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0 || i >= n) return;
+    for (uint32_t w = 0; w < words; w++) {
+        const uint64_t a = image[(uint64_t)w * n + i - 1], b = image[(uint64_t)w * n + i];
+        if (a != b) { if (a > b) *out = 1u; return; }  // benign race: every writer stores 1
+    }
+}
+
+void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt) {
+    const uint64_t m = (uint64_t)nt->nrows;
+    nt->first_line = 0;
+    ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.uimage = nullptr; ix.sorted = true; ix.nrows = (int64_t)m; ix.unique = false;
+    for (size_t k = 0; k < ix.key_cols.size(); k++) ix.key_col_idx[k] = nt->find(ix.key_cols[k]);
+    ix.key_width = key_widths(c, *nt, ix.key_col_idx, m);
+    uint32_t words = 0;
+    ix.image = pack_with_widths(c, *nt, ix.key_col_idx, ix.key_width, &words);
+    ix.image_words = words;
+    ix.hash.clear(); ix.row_slots.clear(); ix.hash_src.clear(); ix.row_slots_src.clear();
+    ix.in_order = true;
+    if (m >= 2 && words) {
+        Buf flag = dev_alloc(c, 8);
+        CPB_CUDA(cudaMemsetAsync(flag->p, 0, 8, c->stream));
+        {
+            KernelTimer kt(c, "order_check", m * words * 8);
+            order_check_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(ix.image->as<uint64_t>(), m, words, flag->as<uint32_t>());
+            CPB_CUDA(cudaGetLastError());
+        }
+        ix.in_order = read_back<uint32_t>(c, flag->p) == 0;
+    }
+}
+
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, bool bug_compatible, const Table* repl) {
     const uint64_t n = (uint64_t)ix.nrows;
     if (n < 2 || keep_in.empty()) return;  // no duplicate group: the reference returns early (:820-822)
@@ -495,14 +528,7 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
         nt = gather_rows(c, *both, ids->as<uint32_t>(), (int64_t)m);
         sync_stream(c);  // rpos / rid are pageable host vectors
         // keys may have changed (even their widths): the image is rebuilt from the new rows, their order is kept
-        nt->first_line = 0;
-        ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m; ix.unique = false;
-        for (size_t k = 0; k < ix.key_cols.size(); k++) ix.key_col_idx[k] = nt->find(ix.key_cols[k]);
-        ix.key_width = key_widths(c, *nt, ix.key_col_idx, m);
-        uint32_t words = 0;
-        ix.image = pack_with_widths(c, *nt, ix.key_col_idx, ix.key_width, &words);
-        ix.image_words = words;
-        ix.hash.clear(); ix.row_slots.clear();
+        index_adopt_rows(c, ix, nt);
         return;
     }
     nt = gather_rows(c, *ix.table, ids->as<uint32_t>(), (int64_t)m);

@@ -60,6 +60,13 @@ struct Strs {
 struct Pinned {
     void* p = nullptr; uint64_t cap = 0;
     ~Pinned() { if (p) cpb_host_free(ctx(), p); }
+    void reserve(uint64_t n) {  // at least n bytes (the contents are not kept)
+        if (n <= cap) return;
+        if (p) cpb_host_free(ctx(), p);
+        p = nullptr; cap = 0;
+        if (cpb_host_alloc(ctx(), n, &p) != CPB_OK) throw Error(cpb_last_error(ctx()));
+        cap = n;
+    }
     template <class Into> void write(std::ostream& out, const Into& into) {
         for (;;) {
             uint64_t n = 0; cpb_error e{};
@@ -225,6 +232,46 @@ public:
         }
         cpb_free(lo); cpb_free(hi);
         if (cpb_index_dedup_apply(detail::ctx(), h_.get(), ng, keep.data(), bug_compatible) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+    }
+    // WriteTo, csvplus.go:655-680: the reference's encoding/gob index file, encoded on the GPU and written in row-range
+    // batches through one pinned buffer.  A path that cannot be created throws and leaves no file; any later error
+    // removes the file.
+    void WriteTo(const std::string& name) const {
+        std::ofstream f(name, std::ios::binary | std::ios::trunc);
+        if (!f) throw Error("open " + name + ": " + strerror(errno));
+        try {
+            // one pinned buffer sized up front: the prefix (the key column names and about 100 bytes more) and then every
+            // batch (at most the rows' total, and less than 4 GiB) are serialised in one call each
+            detail::Pinned buf;
+            uint64_t bound = 256, total = 0, plen = 0;
+            for (auto& c : columns_) bound += c.size() + 10;
+            buf.reserve(bound);
+            buf.write(f, [&](void* p, uint64_t cap, uint64_t* n, cpb_error* e) {
+                const int st = cpb_index_gob_begin(detail::ctx(), h_.get(), p, cap, n, &total, e);
+                plen = *n;
+                return st;
+            });
+            buf.reserve(std::min<uint64_t>(total - plen, uint64_t(1) << 32) + 64);
+            const int64_t n = size();
+            for (int64_t lo = 0, step = int64_t(1) << 24; lo < n;) {
+                const int64_t hi = std::min(n, lo + step);
+                bool too_large = false;  // CPB_E_TOO_LARGE: the batch is 4 GiB or more
+                try {
+                    buf.write(f, [&](void* dst, uint64_t cap, uint64_t* w, cpb_error* e) {
+                        const int st = cpb_index_gob_into(detail::ctx(), h_.get(), lo, hi, dst, cap, w, e);
+                        too_large = st == CPB_ERR_DATA && e->kind == CPB_E_TOO_LARGE;
+                        return st;
+                    });
+                } catch (const Error&) {
+                    if (!too_large || hi - lo < 2) throw;
+                    step = (hi - lo) / 2;  // halve the batch
+                    continue;
+                }
+                lo = hi;
+            }
+            f.close();
+            if (!f) throw Error("write " + name + " failed");
+        } catch (...) { f.close(); std::remove(name.c_str()); throw; }
     }
 private:
     std::shared_ptr<cpb_index> h_; std::vector<std::string> columns_;
@@ -478,6 +525,24 @@ inline DataSource Index::Find(const std::vector<std::string>& values) const {
     if (cpb_index_find(detail::ctx(), h_.get(), v.v.data(), (int)values.size(), &t) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
     return DataSource(Table(t));
 }
+// LoadIndex, csvplus.go:683-705: the index in a file WriteTo (or the reference) wrote, decoded on the GPU; its rows in
+// file order.  A missing file throws the OS error, an empty one Error("EOF"), a cut one Error("unexpected EOF").
+inline Index LoadIndex(const std::string& name) {
+    std::shared_ptr<FILE> f(fopen(name.c_str(), "rb"), [](FILE* p) { if (p) fclose(p); });
+    if (!f) throw Error("open " + name + ": " + strerror(errno));
+    struct stat sb;
+    if (fstat(fileno(f.get()), &sb) != 0) throw Error("stat " + name + ": " + strerror(errno));
+    detail::Pinned buf;  // the rows are copied to the device from pinned memory
+    const uint64_t size = (uint64_t)sb.st_size;
+    buf.reserve(size ? size : 1);
+    if (size && fread(buf.p, 1, (size_t)size, f.get()) != size) throw Error("read " + name + ": short read");
+    cpb_index* ix = nullptr; cpb_error e{};
+    detail::check(cpb_index_load_gob(detail::ctx(), buf.p, size, &ix, &e), e);
+    std::vector<std::string> cols;
+    for (int k = 0; k < cpb_index_num_keys(ix); k++) { cpb_str s; cpb_index_key_col(ix, k, &s); cols.emplace_back(s.ptr, s.len); }
+    return Index(ix, cols);
+}
+
 // the file in pieces of StreamBatchBytes(): a file that fits one piece is read whole and is one push.  A regular file's
 // pieces are read at their exact size, another file's (a pipe) in steps of 64 KiB: a piece is never sized above the
 // bytes it holds.

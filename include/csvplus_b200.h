@@ -68,7 +68,8 @@ typedef enum cpb_err_kind {
     CPB_E_CUDA = 14,
     CPB_E_UNSUPPORTED = 15,
     CPB_E_NUM_SYNTAX = 16,      /* csvplus.go:176/:198  cannot convert %q to integer|float: invalid syntax */
-    CPB_E_NUM_RANGE = 17        /* csvplus.go:176/:198  ...: value out of range */
+    CPB_E_NUM_RANGE = 17,       /* csvplus.go:176/:198  ...: value out of range */
+    CPB_E_GOB = 18              /* LoadIndex (csvplus.go:683-705): the file is not an index gob stream ("EOF", "unexpected EOF", ...) */
 } cpb_err_kind;
 
 typedef struct cpb_error {
@@ -236,6 +237,29 @@ int cpb_index_dedup_apply2(cpb_ctx* ctx, cpb_index* ix, int64_t ngroups, const i
                            int bug_compatible, cpb_error* err);
 void cpb_free(void* p); /* releases arrays returned by cpb_index_dup_groups / cpb_table_to_csv */
 void cpb_index_free(cpb_index* ix);
+/* key column k of the index (index.impl.columns[k]); valid while the index lives */
+int cpb_index_key_col(const cpb_index* ix, int k, cpb_str* out);
+
+/* ------------------------------------------------------------------ index files (encoding/gob)
+ * Index.WriteTo (csvplus.go:655-680): the gob stream of `columns []string` then `rows []Row`, the rows in the index's
+ * stored order, the pairs of a row in bytewise column-name order.  The file = the prefix, then the rows in row-range
+ * batches.
+ *   begin : *prefix_len = the bytes before the first row (type definitions, the columns value, the rows message header),
+ *           written to prefix when they fit cap (else CPB_ERR_ARG, nothing written); *total_len = the whole file.  A rows
+ *           message that encoding/gob's decoder would refuse (8 GiB or more) fails here: CPB_ERR_DATA / CPB_E_TOO_LARGE.
+ *   into  : rows [row_lo, row_hi) into caller-owned (pinned) host memory; cap too small: CPB_ERR_ARG with *nbytes = the
+ *           size needed, nothing written.  One call produces less than 4 GiB (else CPB_ERR_DATA / CPB_E_TOO_LARGE).
+ * LoadIndex (csvplus.go:683-705): an index from the bytes of a whole file.  Type ids and definition order are free, and
+ * so is the pair order of every row; the rows are decoded on the GPU.  The index holds the rows in file order (Find /
+ * Join / Except search them as the reference does, sorted or not) and is not marked unique.  A stream that is not an
+ * index file fails with CPB_ERR_DATA / CPB_E_GOB: msg "EOF" (no message where one is due), "unexpected EOF" (a cut
+ * message) or a description; so do rows whose column sets differ.  Limits: at most 256 columns per row, each column
+ * of the loaded rows below 4 GiB (CPB_E_TOO_LARGE). */
+int cpb_index_gob_begin(cpb_ctx* ctx, const cpb_index* ix, void* prefix, uint64_t cap, uint64_t* prefix_len, uint64_t* total_len,
+                        cpb_error* err);
+int cpb_index_gob_into(cpb_ctx* ctx, const cpb_index* ix, int64_t row_lo, int64_t row_hi, void* host_dst, uint64_t cap,
+                       uint64_t* nbytes, cpb_error* err);
+int cpb_index_load_gob(cpb_ctx* ctx, const void* bytes, uint64_t nbytes, cpb_index** out, cpb_error* err);
 
 /* ------------------------------------------------------------------ join
  * DataSource.Join (csvplus.go:545-583): inner join of probe rows against the index on probe_cols
