@@ -581,6 +581,49 @@ class Table:
             _raise(st, e, self.ctx)
         return values, status, None
 
+    def with_column(self, name: str, value, fmt: str | None = None, prec: int = -1) -> "Table":
+        """the reference's Map(func(row) Row { row[name] = value; return row }) on the GPU: a new table with column `name`
+        set, replaced in place when it exists, else appended; every other column shares this table's buffers.  value is a
+        str (the same bytes in every row), an int64 CUDA tensor (strconv.FormatInt(v, 10)), a float64 CUDA tensor
+        (strconv.FormatFloat(x, fmt, prec, 64); fmt defaults to 'g', prec -1 gives the shortest digits that read back as x)
+        or a FormatFloat marker.  A tensor holds one value per row; it may be freed as soon as the call returns."""
+        if isinstance(value, FormatFloat):
+            if fmt is not None:
+                raise TypeError("with_column: the format of a FormatFloat value is given in FormatFloat")
+            value, fmt, prec = value.values, value.fmt, value.prec
+        b = _enc(name); h = C.c_void_p(); e = _abi.Error(); lib = self.ctx.lib
+        if isinstance(value, (str, bytes)):
+            if fmt is not None:
+                raise TypeError("with_column: fmt applies to float64 tensors only")
+            v = _enc(value)
+            st = lib.cpb_table_set_literal(self.ctx.h, self.h, _abi.Str(b, len(b)), _abi.Str(v, len(v)), C.byref(h), C.byref(e))
+        else:
+            import torch
+            values = _device_tensor(self, value, (torch.int64, torch.float64), "with_column")
+            if values.dtype == torch.float64:
+                fmt = "g" if fmt is None else fmt
+                _check_format(fmt, prec)
+                st = lib.cpb_table_set_float64(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), fmt.encode(), prec,
+                                               C.byref(h), C.byref(e))
+            else:
+                if fmt is not None:
+                    raise TypeError("with_column: fmt applies to float64 tensors only")
+                st = lib.cpb_table_set_int64(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), C.byref(h), C.byref(e))
+        if st:
+            _raise(st, e, self.ctx)
+        return Table(self.ctx, h)
+
+    def filter_mask(self, mask) -> "Table":
+        """the rows where the bool CUDA tensor mask (one value per row) is true, in order: the reference's
+        Filter(func(row) bool) with the predicate computed on the GPU"""
+        import torch
+        keep = _device_tensor(self, mask, (torch.bool,), "filter_mask")
+        h = C.c_void_p(); e = _abi.Error()
+        st = self.ctx.lib.cpb_table_filter_flags(self.ctx.h, self.h, C.c_void_p(keep.data_ptr()), C.byref(h), C.byref(e))
+        if st:
+            _raise(st, e, self.ctx)
+        return Table(self.ctx, h)
+
     @staticmethod
     def concat(parts: list["Table"]) -> "Table":
         ctx = parts[0].ctx
@@ -589,6 +632,56 @@ class Table:
         if st:
             _raise(st, None, ctx)
         return Table(ctx, h)
+
+
+FORMAT_VERBS = "eEfgG"
+
+
+def _check_format(fmt, prec):
+    if not isinstance(fmt, str) or len(fmt) != 1 or fmt not in FORMAT_VERBS:
+        raise ValueError(f"FormatFloat: unsupported format {fmt!r} (want one of e E f g G)")
+    if isinstance(prec, bool) or not isinstance(prec, int) or not -1 <= prec <= 64:
+        raise ValueError(f"FormatFloat: precision {prec!r} outside -1..64")
+
+
+class FormatFloat:
+    """strconv.FormatFloat(x, fmt, prec, 64) of every value of a float64 CUDA tensor: a value for Table.with_column and
+    MapTensors.  fmt is one of e E f g G; prec runs from -1 (the shortest digits that read back as x) to 64."""
+
+    def __init__(self, values, fmt: str = "g", prec: int = -1):
+        _check_format(fmt, prec)
+        self.values, self.fmt, self.prec = values, fmt, prec
+
+
+def _device_tensor(t: Table, x, dtypes: tuple, what: str):
+    """x as a contiguous 1-D CUDA tensor of one of dtypes with one value per row of t, on t's device, ready to be read on
+    the ctx stream: the ctx stream waits for torch's current stream (where x was produced), and x's memory is not reused
+    before the ctx stream's work is done, so the caller may free x at once"""
+    import torch
+    if not isinstance(x, torch.Tensor) or x.dtype not in dtypes:
+        got = x.dtype if isinstance(x, torch.Tensor) else type(x).__name__
+        raise TypeError(f"{what}: want a CUDA tensor of {' or '.join(str(d) for d in dtypes)}, got {got}")
+    dev = torch.device("cuda", t.ctx.device)
+    if x.device != dev:
+        raise ValueError(f"{what}: the tensor is on {x.device}, the table on {dev}")
+    if x.dim() != 1 or x.numel() != len(t):
+        raise ValueError(f"{what}: want one value per row ({len(t)}), got shape {tuple(x.shape)}")
+    x = x.contiguous()
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(dev))
+    s = torch.cuda.ExternalStream(t.ctx.stream, device=dev)
+    s.wait_event(ev)
+    x.record_stream(s)
+    return x
+
+
+def _tensor_kinds(inputs: dict, what: str) -> dict:
+    kinds = {}
+    for name, kind in inputs.items():
+        if kind not in ("int", "float64"):
+            raise ValueError(f"{what}: unknown type {kind!r} for column {name!r} (want 'int' or 'float64')")
+        kinds[name] = kind == "float64"
+    return kinds
 
 
 def parse_csv(ctx: Context, data, *, on_device=False, nbytes=None, delimiter=",", comment="", num_fields=0, lazy_quotes=False,
@@ -1139,6 +1232,20 @@ class DataSource:
     def TakeWhile(self, pred): return self._with(("takewhile", pred))
     def DropWhile(self, pred): return self._with(("dropwhile", pred))
 
+    def MapTensors(self, inputs: dict, fn):
+        """a device Map (an extension beyond the reference API, like ToTensors): inputs = {column: "int" | "float64"} are
+        converted per batch as ToTensors converts them, fn(dict of CUDA tensors) returns {name: value} and each name is set
+        as Table.with_column sets it (an int64 / float64 tensor with one value per row, a FormatFloat, a str).  fn is called
+        once per non-empty batch and must be row-wise.  A conversion error (the lowest failing row, ties to the earlier
+        input) ends the plan there like a source error: the rows before it flow on and the sink raises CsvPlusError with
+        .row = the row's ordinal among the rows that reached the step."""
+        return self._with(("maptensors", _tensor_kinds(inputs, "MapTensors"), fn))
+
+    def FilterTensors(self, inputs: dict, fn):
+        """a device Filter: as MapTensors, fn returns a bool CUDA tensor with one value per row; the rows where it is true
+        are kept"""
+        return self._with(("filtertensors", _tensor_kinds(inputs, "FilterTensors"), fn))
+
     def DropColumns(self, *columns):
         if len(columns) == 0:
             raise ValueError("no columns specified in DropColumns()")
@@ -1204,7 +1311,7 @@ class DataSource:
         stop = False
         for i, op in enumerate(ops):
             kind = op[0]
-            device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop")
+            device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop", "maptensors", "filtertensors")
                          or (kind in ("filter", "takewhile", "dropwhile") and isinstance(op[1], Predicate) and op[1].lowerable()))
             if device_ok:
                 if state[0] == "rows":
@@ -1230,6 +1337,12 @@ class DataSource:
                         if cut < len(t):
                             err = None; stop = True
                         t = t.slice(0, cut)
+                    elif kind in ("maptensors", "filtertensors"):
+                        seen = carry.get(i, 0)
+                        carry[i] = seen + len(t)
+                        t, step_err = _tensor_step(t, op, seen)
+                        if step_err is not None:  # the rows before it flow on; the sink raises it as a source error
+                            err = step_err; stop = True
                     elif kind == "dropwhile":  # :361-374
                         if carry.get(i, True):
                             k = t.first_false(op[1])
@@ -1418,6 +1531,33 @@ class DataSource:
         if t is None:
             t = Table.from_rows(self._ctx(), [], list(columns))
         return t.index_on(*columns, unique=unique)
+
+
+def _tensor_step(t: Table, op, seen: int):
+    """MapTensors / FilterTensors over one batch -> (table, CsvPlusError of the first failing conversion or None)"""
+    kind, kinds, fn = op
+    vals, first = {}, None
+    for name, is_float in kinds.items():
+        values, _, e = t._convert(name, is_float)
+        vals[name] = values
+        if e is not None and (first is None or e.row < first.row):
+            first = e
+    err = None
+    if first is not None:
+        err = CsvPlusError(str(first), first.status, first.kind)
+        err.row = seen + first.row
+        t = t.slice(0, first.row)
+        vals = {name: v[: first.row] for name, v in vals.items()}
+    if len(t):
+        res = fn(vals)
+        if kind == "maptensors":
+            if not isinstance(res, dict):
+                raise TypeError(f"MapTensors: fn must return a dict of column values, got {type(res).__name__}")
+            for name, value in res.items():
+                t = t.with_column(name, value)
+        else:
+            t = t.filter_mask(res)
+    return t, err
 
 
 def _concat(tables: list) -> "Table | None":

@@ -902,6 +902,45 @@ int cpb_table_column_as_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, 
     return column_as_common(h, t, column, true, values, status, nbad, err);
 }
 
+// ------------------------------------------------------------------ computed columns
+int cpb_table_set_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, const int64_t* dev_values, cpb_table** out, cpb_error* err) {
+    if (!h || !t || !out) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    *out = wrap(table_set_values(c, *t->t, to_string(column), dev_values, false, 'f', 0));
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_table_set_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, const double* dev_values, char fmt, int prec, cpb_table** out,
+                          cpb_error* err) {
+    if (!h || !t || !out) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    *out = wrap(table_set_values(c, *t->t, to_string(column), dev_values, true, fmt, prec));
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_table_set_literal(cpb_ctx* h, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err) {
+    if (!h || !t || !out) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    *out = wrap(table_set_literal(c, *t->t, to_string(column), to_string(value)));
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+int cpb_table_filter_flags(cpb_ctx* h, const cpb_table* t, const uint8_t* dev_keep, cpb_table** out, cpb_error* err) {
+    if (!h || !t || !out) return CPB_ERR_ARG;
+    Ctx* c = &h->c; DeviceGuard g(c);
+    clear_error(err);
+    CPB_TRY(c, err)
+    *out = wrap(table_filter_mask(c, *t->t, dev_keep));
+    return CPB_OK;
+    CPB_CATCH(c, err)
+}
+
 // ------------------------------------------------------------------ stats
 int cpb_stats_enable(cpb_ctx* h, int on) { DeviceGuard g(&h->c); h->c.stats_on = on != 0; return CPB_OK; }
 int cpb_stats_reset(cpb_ctx* h) {

@@ -335,6 +335,12 @@ struct NumResult {
     std::string first_value;
 };
 NumResult column_as_number(Ctx* c, const Table& t, int col, bool is_float, void* values, uint8_t* status);
+// format.cu: computed columns.  t with column `name` set (replaced in place, else appended; the other columns share t's
+// buffers) to strconv.FormatInt(v, 10) / FormatFloat(x, fmt, prec, 64) of the n device values, or to one literal value
+std::shared_ptr<Table> table_set_values(Ctx* c, const Table& t, const std::string& name, const void* values, bool is_float, char fmt, int prec);
+std::shared_ptr<Table> table_set_literal(Ctx* c, const Table& t, const std::string& name, const std::string& value);
+// the rows of t whose keep byte is nonzero, in order
+std::shared_ptr<Table> table_filter_mask(Ctx* c, const Table& t, const uint8_t* keep);
 
 }  // namespace cpb
 

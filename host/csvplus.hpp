@@ -190,7 +190,34 @@ public:
     uint64_t ValuesAsFloat64(const std::string& column, double* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
         return convert(column, true, dev_values, dev_status, strict);
     }
+    // Map(func(row) Row { row[column] = value; return row }) on the GPU: a table with `column` set (replaced in place, else
+    // appended; every other column shares this table's buffers).  dev_values[size()] is device memory read on the ctx
+    // stream: strconv.FormatInt(v, 10), strconv.FormatFloat(x, fmt, prec, 64) (fmt e E f g G, prec -1..64), or one
+    // literal value in every row.  A column of 4 GiB or more throws.
+    Table WithColumn(const std::string& column, const int64_t* dev_values) const {
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) { return cpb_table_set_int64(detail::ctx(), h_.get(), c, dev_values, out, e); });
+    }
+    Table WithColumn(const std::string& column, const double* dev_values, char fmt = 'g', int prec = -1) const {
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
+            return cpb_table_set_float64(detail::ctx(), h_.get(), c, dev_values, fmt, prec, out, e);
+        });
+    }
+    Table WithColumn(const std::string& column, const std::string& value) const {
+        const cpb_str v{value.data(), value.size()};
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) { return cpb_table_set_literal(detail::ctx(), h_.get(), c, v, out, e); });
+    }
+    // the rows whose dev_keep[row] byte (device memory, size() bytes) is nonzero, in order
+    Table FilterMask(const uint8_t* dev_keep) const {
+        cpb_table* out = nullptr; cpb_error e{};
+        detail::check(cpb_table_filter_flags(detail::ctx(), h_.get(), dev_keep, &out, &e), e);
+        return Table(out);
+    }
 private:
+    template <class F> Table set(const std::string& column, F call) const {
+        cpb_table* out = nullptr; cpb_error e{};
+        detail::check(call(cpb_str{column.data(), column.size()}, &out, &e), e);
+        return Table(out);
+    }
     uint64_t convert(const std::string& column, bool is_float, void* values, uint8_t* status, bool strict) const {
         cpb_error e{}; uint64_t nbad = 0;
         const cpb_str c{column.data(), column.size()};

@@ -314,6 +314,25 @@ int cpb_table_column_as_int64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, 
 int cpb_table_column_as_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, double* values, uint8_t* status,
                                 uint64_t* nbad, cpb_error* err);
 
+/* ------------------------------------------------------------------ computed columns
+ * The reference's Map(func(row) Row { row[column] = value; return row }) over every row: *out = t with `column` set,
+ * replaced in place when t has it, else appended.  Every other column shares t's buffers (row-range views too); t is
+ * not modified.  dev_values[nrows] is device memory, read on the ctx stream (the caller orders its producer before
+ * the call); it may be released once the call returns.
+ *   set_int64  : strconv.FormatInt(v, 10).
+ *   set_float64: strconv.FormatFloat(x, fmt, prec, 64), byte for byte; fmt one of e E f g G, prec -1..64 (-1: the
+ *                shortest digits that read back as x).  Another fmt or prec: CPB_ERR_ARG, nothing computed.
+ *   set_literal: value in every row.
+ * One column stays below 4 GiB: a column of 4 GiB or more fails with CPB_ERR_DATA / CPB_E_TOO_LARGE (checked on the
+ * exact 64-bit total, before any offset is written).  Host synchronisations: none for an empty table; for set_float64
+ * one, or two when some row needs the exact big-integer path (its kernel, format_rare, then shows in cpb_stats_get).
+ * filter_flags: the rows whose dev_keep[row] byte is nonzero, in order (dev_keep[nrows] read on the ctx stream). */
+int cpb_table_set_int64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const int64_t* dev_values, cpb_table** out, cpb_error* err);
+int cpb_table_set_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const double* dev_values, char fmt, int prec,
+                          cpb_table** out, cpb_error* err);
+int cpb_table_set_literal(cpb_ctx* ctx, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err);
+int cpb_table_filter_flags(cpb_ctx* ctx, const cpb_table* t, const uint8_t* dev_keep, cpb_table** out, cpb_error* err);
+
 /* ------------------------------------------------------------------ multi-GPU (SURVEY §8e)
  * The probe stream shards by row range with no data-path collective; the one exchange step is the all-gather of the
  * build-side columns (each rank parses 1/N of the build file) so that every rank can build the full Index
