@@ -120,6 +120,15 @@ struct RowSlots {
     Buf slots;        // uint8[nrows][S]
     Buf lens;         // uint32[nrows]: length of column c in bits 8c..8c+7
 };
+// Row-carrying hash table of a unique index whose full-key image is <= 12 bytes and whose other columns (at most 4) take
+// <= 16 bytes in every row: one 32-byte slot (one DRAM sector) per entry holds the key, the lengths of those columns
+// and their bytes (RowSlot, rowhash.cuh), so a full-key Join finds key, lengths and payload with ONE random access.
+// Built by UniqueIndexOn (the insert is the duplicate check) and complete when the index is returned: read-only after.
+struct RowHash {
+    uint64_t nslots = 0;    // load factor 1/2
+    Buf slots;              // RowSlot[nslots]; null = the index has no row-carrying table
+    std::vector<int> cols;  // payload: every non-key column of the source, in schema order
+};
 struct Index {
     Ctx* ctx = nullptr;
     // The sorted rows exist in two forms.  A join needs neither the sorted columns nor their offsets: it probes the
@@ -133,8 +142,10 @@ struct Index {
     // A UNIQUE index whose duplicate check passed is not even sorted until something needs the order (iteration, Find,
     // SubIndex, a prefix join, dedup): a full-key join only needs "key -> row", which the hash table built over the rows
     // in SOURCE order gives (and that build doubles as the duplicate check: every key must find itself).  `uimage` is the
-    // key image in source order; `sorted` tells whether perm / image (sorted order) exist yet (ensure_sorted()).
+    // key image in source order; `sorted` tells whether perm / image (sorted order) exist yet (ensure_sorted()).  An index
+    // with a row-carrying table has no uimage: the sort packs the image when it first needs it.
     Buf uimage;
+    RowHash rowhash;
     bool sorted = true;
     std::map<int, HashTable> hash_src;                   // probe tables over the source order (payload = source row)
     std::map<std::vector<int>, RowSlots> row_slots_src;  // row slots in source order (filled sequentially, no permutation)
@@ -286,6 +297,11 @@ Column materialize(Ctx* c, const Column& col, int64_t nrows);  // view -> own co
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout,
                                          bool by_src = false);
 std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& parts);
+// full-key join against ix.rowhash: payload columns `cols` (source column numbers, a non-empty subset of ix.rowhash.cols)
+// for every probe row, empty where the row finds no key; *matches = probe rows that found their key.  One random access
+// and one host synchronisation.
+std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, const std::vector<int>& pidx, const std::vector<int>& cols,
+                                      uint64_t* matches);
 // sort.cu
 std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::vector<std::string>& keys, bool unique,
                                    DataError* derr, bool* failed);
@@ -310,6 +326,8 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
                                    bool anti, DataError* derr, bool* failed);
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi);
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
+// fills ix.rowhash (nslots, cols set by the caller) from ix.src; true when some key was inserted twice
+bool rowhash_build(Ctx* c, Index& ix);
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi);
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep, bool bug_compatible, const Table* repl = nullptr);
 // the index takes the rows of nt in their stored order: key columns, widths and key image are rebuilt from them, in_order

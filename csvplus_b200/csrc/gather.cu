@@ -8,6 +8,7 @@
 
 #include "core.hpp"
 #include "pred.cuh"
+#include "rowhash.cuh"
 #include "util.cuh"
 
 namespace cpb {
@@ -313,13 +314,81 @@ __global__ void __launch_bounds__(256) slot_fill_kernel(SlotCols sc, const uint3
     for (uint32_t x = threadIdx.x; x < rows * wps; x += 256) g[x] = sw[(x / wps) * (wps + RS_PAD / 4) + x % wps];
 }
 
-// exclusive scans of the NC length fields of lens[ids[i]] in one pass (same chained look-back as scan_u32_kernel;
-// warp c resolves column c)
+// Row-carrying hash table: probe row i looks its key up with one 32-byte slot read; the lengths of the output columns
+// (8 bits each, as row slots pack them) go to lens[i], their bytes back to back to scratch[i] (zero on a miss), both
+// written sequentially, and the hits are counted into *matches.  (Probing inside the length scan, 8 rows per thread,
+// needs ~170 registers: one CTA per SM, and the kernel ran latency-bound at 3.6x this one + the scan.)
+__global__ void __launch_bounds__(256) rowhash_probe_kernel(KeyDesc kd, uint64_t np, const RowSlot* __restrict__ slots, uint64_t nslots,
+                                                            int npay, uint32_t sel, uint32_t* lens, uint4* scratch, unsigned long long* matches) {
+    unsigned long long hits = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
+        unsigned long long k0; uint32_t k1;
+        uint64_t s = rh_start(kd, i, nslots, k0, k1);
+        uint4 h = rh_header(slots, s), v = __ldg(&slots[s].pay);  // one sector, both halves
+        const uint64_t s0 = s;
+        const bool found = rh_walk(slots, nslots, k0, k1, s, h);
+        if (found && s != s0) v = __ldg(&slots[s].pay);
+        unsigned long long a = 0, b = 0;
+        uint32_t p = 0;
+        if (found) {
+            const unsigned long long pa = ((unsigned long long)v.y << 32) | v.x, pb = ((unsigned long long)v.w << 32) | v.z;
+            uint32_t pos = 0, opos = 0;
+            int oc = 0;
+#pragma unroll
+            for (int j = 0; j < RH_MAXC; j++) {
+                if (j >= npay) break;
+                const uint32_t l = (h.w >> (5 * j)) & 31u;
+                if (sel >> j & 1u) {
+                    unsigned long long x, y;
+                    take16(pa, pb, pos, l, x, y);
+                    or_at16(a, b, opos, x, y);
+                    p |= l << (8 * oc);
+                    opos += l; oc++;
+                }
+                pos += l;
+            }
+            hits++;
+        }
+        lens[i] = p;
+        scratch[i] = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+    }
+    hits = warp_sum_u64(hits);
+    if ((threadIdx.x & 31) == 0 && hits) atomicAdd(matches, hits);
+}
+
+// exclusive scans of the NC length fields (8 bits each) of row i's packed lengths in one pass (same chained look-back
+// as scan_u32_kernel; warp c resolves column c).  Src::load(base, n, p) gives the packed lengths of rows
+// [base, base + LS_ITEMS) (0 past n).
 constexpr int LS_ITEMS = 8;
 constexpr int LS_TILE = SCAN_THREADS * LS_ITEMS;
-template <int NC>
-__global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const uint32_t* __restrict__ lens, const uint32_t* __restrict__ ids, uint64_t n,
-                                                                 SlotOut out, unsigned long long* state, uint32_t* ticket,
+struct LensById {  // row slots: lens[ids[i]]
+    const uint32_t* __restrict__ lens;
+    const uint32_t* __restrict__ ids;
+    __device__ __forceinline__ void load(uint64_t base, uint64_t n, uint32_t (&p)[LS_ITEMS]) const {
+        if (base + LS_ITEMS <= n) {
+            const uint4 a = *reinterpret_cast<const uint4*>(ids + base), b = *reinterpret_cast<const uint4*>(ids + base + 4);
+            p[0] = lens[a.x]; p[1] = lens[a.y]; p[2] = lens[a.z]; p[3] = lens[a.w];
+            p[4] = lens[b.x]; p[5] = lens[b.y]; p[6] = lens[b.z]; p[7] = lens[b.w];
+        } else {
+#pragma unroll
+            for (int i = 0; i < LS_ITEMS; i++) p[i] = base + i < n ? lens[ids[base + i]] : 0u;
+        }
+    }
+};
+struct LensSeq {  // row-carrying hash table: lens[i], written by rowhash_probe_kernel
+    const uint32_t* __restrict__ lens;
+    __device__ __forceinline__ void load(uint64_t base, uint64_t n, uint32_t (&p)[LS_ITEMS]) const {
+        if (base + LS_ITEMS <= n) {
+            const uint4 a = *reinterpret_cast<const uint4*>(lens + base), b = *reinterpret_cast<const uint4*>(lens + base + 4);
+            p[0] = a.x; p[1] = a.y; p[2] = a.z; p[3] = a.w; p[4] = b.x; p[5] = b.y; p[6] = b.z; p[7] = b.w;
+        } else {
+#pragma unroll
+            for (int i = 0; i < LS_ITEMS; i++) p[i] = base + i < n ? lens[base + i] : 0u;
+        }
+    }
+};
+template <int NC, class Src>
+__global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const Src src, uint64_t n, SlotOut out, unsigned long long* state, uint32_t* ticket,
                                                                  unsigned long long* totals) {
     __shared__ uint32_t s_tile;
     __shared__ uint32_t s_warp[NC][SCAN_THREADS / 32];
@@ -333,14 +402,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const uint32_t*
         if (tile >= ntiles) break;
         const uint64_t base = tile * LS_TILE + (uint64_t)tid * LS_ITEMS;
         uint32_t p[LS_ITEMS];
-        if (base + LS_ITEMS <= n) {
-            const uint4 a = *reinterpret_cast<const uint4*>(ids + base), b = *reinterpret_cast<const uint4*>(ids + base + 4);
-            p[0] = lens[a.x]; p[1] = lens[a.y]; p[2] = lens[a.z]; p[3] = lens[a.w];
-            p[4] = lens[b.x]; p[5] = lens[b.y]; p[6] = lens[b.z]; p[7] = lens[b.w];
-        } else {
-#pragma unroll
-            for (int i = 0; i < LS_ITEMS; i++) p[i] = base + i < n ? lens[ids[base + i]] : 0u;
-        }
+        src.load(base, n, p);
         uint32_t sum[NC], inc[NC];
 #pragma unroll
         for (int c = 0; c < NC; c++) {
@@ -378,7 +440,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const uint32_t*
             }
             if (lane == 0) {
                 s_prefix[c] = excl;
-                if (tile == ntiles - 1) { totals[c] = excl + tot; out.off[c][n] = (uint32_t)(excl + tot); }
+                if (tile == ntiles - 1) totals[c] = excl + tot;
             }
         }
         __syncthreads();
@@ -398,6 +460,8 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const uint32_t*
 #pragma unroll
                 for (int i = 0; i < LS_ITEMS; i++) { if (base + i < n) o[base + i] = run; run += (p[i] >> (8 * c)) & 255u; }
             }
+            if (base < n && n <= base + LS_ITEMS) o[n] = run;  // (the thread holding the last row: the total; a column index
+                                                                // taken from the warp number would put `out` on the stack)
         }
         __syncthreads();
     }
@@ -439,7 +503,7 @@ __device__ __forceinline__ void or_value(uint8_t* stage, uint32_t q, const uint8
 // out like the destination (all columns of the group, one 16-byte aligned region each), and the warp writes every
 // column's region in ONE pass of aligned 16-byte stores, the partial first / last vector of a column with a few
 // aligned narrower stores.  No lane loops over the bytes of a value.  A column whose region does not fit the stage
-// any more is copied straight to its destination.
+// any more is copied straight to its destination.  Row i's slot is slots[ids[i]], or slots[i] when ids is null.
 constexpr uint32_t SC_STRIDE_PAD = 12;  // slot stride S + 12 bytes: an odd number of words, and room for or_value's over-read
 template <int NC, int SV>  // SV: 16-byte vectors held per prefetched slot (S <= 16 SV)
 __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
@@ -460,7 +524,7 @@ __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t*
 #pragma unroll
         for (int c = 0; c < NC; c++) { nd[c] = 0; nlen[c] = 0; }
         if (i < n) {
-            const uint4* sp = reinterpret_cast<const uint4*>(slots + (uint64_t)ids[i] * S);
+            const uint4* sp = reinterpret_cast<const uint4*>(slots + (ids ? (uint64_t)ids[i] : i) * S);
 #pragma unroll
             for (int j = 0; j < SV; j++) if (j < (int)(S / 16)) v[j] = __ldg(sp + j);
 #pragma unroll
@@ -569,6 +633,58 @@ static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& col
     return smap.emplace(cols, std::move(rs)).first->second;
 }
 
+// Columns `names` of n rows from slots of S bytes: the offsets scanned from the packed lengths `src` gives
+// (scan_lens_kernel), ONE host synchronisation for the column totals and *counter (the 64-bit count at counter_dev,
+// when given), then the bytes copied by slot_copy_kernel from slot ids[i] (slot i when ids is null).
+template <class Src>
+static std::vector<Column> slot_gather(Ctx* c, const std::vector<std::string>& names, uint64_t n, const Src& src, const char* scan_name,
+                                       uint64_t scan_bytes, const uint8_t* slots, uint32_t S, const uint32_t* ids,
+                                       const unsigned long long* counter_dev, uint64_t* counter) {
+    const int nc = (int)names.size();
+    SlotOut so{};
+    std::vector<Column> out(nc);
+    for (int k = 0; k < nc; k++) {
+        out[k].name = names[k];
+        out[k].offsets = dev_alloc(c, (n + 1) * 4);
+        so.off[k] = out[k].offsets->as<uint32_t>();
+    }
+    const uint64_t ntiles = (n + LS_TILE - 1) / LS_TILE;
+    Buf st = dev_alloc(c, ntiles * nc * 8 + 64 + RS_MAXC * 8);
+    CPB_CUDA(cudaMemsetAsync(st->p, 0, ntiles * nc * 8 + 64 + RS_MAXC * 8, c->stream));
+    uint32_t* ticket = st->as<uint32_t>();
+    unsigned long long* totals = st->as<unsigned long long>() + 1;  // [RS_MAXC]: *counter_dev
+    unsigned long long* state = st->as<unsigned long long>() + 8 + RS_MAXC;
+    {
+        KernelTimer kt(c, scan_name, scan_bytes);
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 8);
+#define CPB_LS(NC) scan_lens_kernel<NC, Src><<<grid, SCAN_THREADS, 0, c->stream>>>(src, n, so, state, ticket, totals)
+        switch (nc) { case 1: CPB_LS(1); break; case 2: CPB_LS(2); break; case 3: CPB_LS(3); break; default: CPB_LS(4); break; }
+#undef CPB_LS
+        CPB_CUDA(cudaGetLastError());
+    }
+    if (counter_dev) CPB_CUDA(cudaMemcpyAsync(totals + RS_MAXC, counter_dev, 8, cudaMemcpyDeviceToDevice, c->stream));
+    const std::vector<uint64_t> ht = read_back<uint64_t>(c, totals, RS_MAXC + 1);
+    if (counter) *counter = ht[RS_MAXC];
+    uint64_t all = 0;
+    for (int k = 0; k < nc; k++) {
+        if (ht[k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, k, 0, false, "a result column exceeds 4 GiB; process in smaller batches"};
+        out[k].data = dev_alloc(c, ht[k] + 16);
+        so.data[k] = out[k].data->as<uint8_t>();
+        all += ht[k];
+    }
+    {
+        KernelTimer kt(c, "slot_copy", 2 * all + n * (4 + 4 * (uint64_t)nc));
+        const uint32_t gblocks = (uint32_t)std::min<uint64_t>((n + GW_WARPS * 32 - 1) / (GW_WARPS * 32), (uint64_t)c->sm_count * 16);
+#define CPB_SC2(NC, SV) slot_copy_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(slots, S, ids, so, n)
+#define CPB_SC(NC) (S <= 16 ? CPB_SC2(NC, 1) : S <= 32 ? CPB_SC2(NC, 2) : CPB_SC2(NC, 4))
+        switch (nc) { case 1: CPB_SC(1); break; case 2: CPB_SC(2); break; case 3: CPB_SC(3); break; default: CPB_SC(4); break; }
+#undef CPB_SC
+#undef CPB_SC2
+        CPB_CUDA(cudaGetLastError());
+    }
+    return out;
+}
+
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, bool by_src) {
     if (cols.empty()) {  // nothing to gather (a join whose index columns are all key columns): no slots, no sorted rows
         auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = ix.schema().first_line;
@@ -592,49 +708,40 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
     RowSlots& rs = ensure_row_slots(c, ix, cols, by_src);
     if (!rs.usable) return plain();
     const Table& t = ix.schema();
-
-    const int nc = (int)cols.size();
+    std::vector<std::string> names;
+    for (int ci : cols) names.push_back(t.cols[ci].name);
     auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = t.first_line;
-    SlotOut so{};
-    std::vector<Column> out(nc);
-    for (int k = 0; k < nc; k++) {
-        out[k].name = t.cols[cols[k]].name;
-        out[k].offsets = dev_alloc(c, ((size_t)nout + 1) * 4);
-        so.off[k] = out[k].offsets->as<uint32_t>();
+    const uint64_t n = (uint64_t)nout;
+    r->cols = slot_gather(c, names, n, LensById{rs.lens->as<uint32_t>(), ids}, "slot_scan_lens", n * (8 + 4 * (uint64_t)cols.size()),
+                          rs.slots->as<uint8_t>(), rs.S, ids, nullptr, nullptr);
+    return r;
+}
+
+std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, const std::vector<int>& pidx, const std::vector<int>& cols,
+                                      uint64_t* matches) {
+    const RowHash& rh = ix.rowhash;
+    const Table& t = ix.schema();
+    const uint64_t np = (uint64_t)probe.nrows;
+    KeyDesc kd{};
+    describe_keys(c, probe, pidx, ix.key_width, kd);
+    std::vector<std::string> names;
+    uint32_t sel = 0;
+    for (int ci : cols) {  // cols is a subset of the payload in payload order (both in schema order)
+        names.push_back(t.cols[ci].name);
+        sel |= 1u << (int)(std::find(rh.cols.begin(), rh.cols.end(), ci) - rh.cols.begin());
     }
-    const uint64_t n = (uint64_t)nout, ntiles = (n + LS_TILE - 1) / LS_TILE;
-    Buf st = dev_alloc(c, ntiles * nc * 8 + 64 + RS_MAXC * 8);
-    CPB_CUDA(cudaMemsetAsync(st->p, 0, ntiles * nc * 8 + 64 + RS_MAXC * 8, c->stream));
-    uint32_t* ticket = st->as<uint32_t>();
-    unsigned long long* totals = st->as<unsigned long long>() + 1;
-    unsigned long long* state = st->as<unsigned long long>() + 8 + RS_MAXC;
+    Buf lens = dev_alloc(c, np * 4), scratch = dev_alloc(c, np * RH_PAY), cnt = dev_alloc(c, 8);
+    CPB_CUDA(cudaMemsetAsync(cnt->p, 0, 8, c->stream));
     {
-        KernelTimer kt(c, "slot_scan_lens", n * (8 + 4 * (uint64_t)nc));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 8);
-#define CPB_LS(NC) scan_lens_kernel<NC><<<grid, SCAN_THREADS, 0, c->stream>>>(rs.lens->as<uint32_t>(), ids, n, so, state, ticket, totals)
-        switch (nc) { case 1: CPB_LS(1); break; case 2: CPB_LS(2); break; case 3: CPB_LS(3); break; default: CPB_LS(4); break; }
-#undef CPB_LS
+        KernelTimer kt(c, "rowhash_probe", np * ((uint64_t)kd.words * 8 + 4 * (uint64_t)kd.nkeys + sizeof(RowSlot) + RH_PAY + 4));
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
+        rowhash_probe_kernel<<<grid, 256, 0, c->stream>>>(kd, np, rh.slots->as<RowSlot>(), rh.nslots, (int)rh.cols.size(), sel,
+                                                          lens->as<uint32_t>(), scratch->as<uint4>(), cnt->as<unsigned long long>());
         CPB_CUDA(cudaGetLastError());
     }
-    const std::vector<uint64_t> ht = read_back<uint64_t>(c, totals, nc);
-    uint64_t all = 0;
-    for (int k = 0; k < nc; k++) {
-        if (ht[k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, k, 0, false, "a result column exceeds 4 GiB; process in smaller batches"};
-        out[k].data = dev_alloc(c, ht[k] + 16);
-        so.data[k] = out[k].data->as<uint8_t>();
-        all += ht[k];
-    }
-    {
-        KernelTimer kt(c, "slot_copy", 2 * all + n * (4 + 4 * (uint64_t)nc));
-        const uint32_t gblocks = (uint32_t)std::min<uint64_t>((n + GW_WARPS * 32 - 1) / (GW_WARPS * 32), (uint64_t)c->sm_count * 16);
-#define CPB_SC2(NC, SV) slot_copy_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(rs.slots->as<uint8_t>(), rs.S, ids, so, n)
-#define CPB_SC(NC) (rs.S <= 16 ? CPB_SC2(NC, 1) : rs.S <= 32 ? CPB_SC2(NC, 2) : CPB_SC2(NC, 4))
-        switch (nc) { case 1: CPB_SC(1); break; case 2: CPB_SC(2); break; case 3: CPB_SC(3); break; default: CPB_SC(4); break; }
-#undef CPB_SC
-#undef CPB_SC2
-        CPB_CUDA(cudaGetLastError());
-    }
-    for (int k = 0; k < nc; k++) r->cols.push_back(out[k]);
+    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = (int64_t)np; r->first_line = t.first_line;
+    r->cols = slot_gather(c, names, np, LensSeq{lens->as<uint32_t>()}, "rowhash_scan_lens", np * (4 + 4 * (uint64_t)cols.size()),
+                          scratch->as<uint8_t>(), RH_PAY, nullptr, cnt->as<unsigned long long>(), matches);
     return r;
 }
 

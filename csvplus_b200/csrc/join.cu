@@ -14,16 +14,13 @@
 #include <algorithm>
 
 #include "core.hpp"
+#include "rowhash.cuh"
 #include "util.cuh"
 
 namespace cpb {
 
 constexpr uint32_t EMPTY = 0xffffffffu;
 
-__device__ __forceinline__ uint64_t mix64(uint64_t h) {
-    h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33;
-    return h;
-}
 __device__ __forceinline__ uint64_t hash_prefix(const uint64_t* img, uint64_t n, uint64_t r, uint32_t pbytes) {
     uint32_t full = pbytes >> 3, rem = pbytes & 7;
     uint64_t h = 0x9E3779B97F4A7C15ull;
@@ -88,11 +85,6 @@ __global__ void __launch_bounds__(256) join_probe_kernel(const uint64_t* __restr
 // key is packed in registers straight from the probe column (no materialised probe image).
 struct __align__(32) Slot32 { unsigned long long k[3]; unsigned long long payload; };  // payload = lo | cnt << 32; 0 = empty
 
-__device__ __forceinline__ uint64_t hash3(unsigned long long a, unsigned long long b, unsigned long long c) {
-    return mix64(mix64(mix64(0x9E3779B97F4A7C15ull ^ a) ^ b) ^ c);
-}
-__device__ __forceinline__ uint64_t slot_of(uint64_t h, uint64_t nslots) { return __umul64hi(h, nslots); }
-
 __global__ void hash32_insert_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, const uint32_t* __restrict__ heads,
                                      uint64_t nheads, Slot32* slots, uint64_t nslots) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -109,43 +101,6 @@ __global__ void hash32_insert_kernel(const uint64_t* __restrict__ image, uint64_
     }
 }
 
-__device__ __forceinline__ unsigned long long bswap64(unsigned long long x) {
-    return ((unsigned long long)__byte_perm((uint32_t)x, 0, 0x0123) << 32) | __byte_perm((uint32_t)(x >> 32), 0, 0x0123);
-}
-// the first min(len,16) bytes of a string, little-endian in (a, b), the rest zero: aligned 8-byte loads only (the
-// probe rows of a warp are ~one sector apart, a byte loop costs one L1 request per byte)
-__device__ __forceinline__ void load16(const uint8_t* p, uint32_t len, unsigned long long& a, unsigned long long& b) {
-    a = b = 0;
-    if (len == 0) return;
-    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(p) & 7u), sh = mis * 8;
-    const unsigned long long* wp = reinterpret_cast<const unsigned long long*>(p - mis);
-    const uint32_t need = mis + (len < 16u ? len : 16u);
-    const unsigned long long w0 = __ldg(wp), w1 = need > 8 ? __ldg(wp + 1) : 0ull, w2 = need > 16 ? __ldg(wp + 2) : 0ull;
-    a = sh ? (w0 >> sh) | (w1 << (64 - sh)) : w0;
-    b = sh ? (w1 >> sh) | (w2 << (64 - sh)) : w1;
-    if (len < 8) { a &= (1ull << (8 * len)) - 1; b = 0; }
-    else if (len < 16) b &= (1ull << (8 * (len - 8))) - 1;
-}
-// packs the probe key exactly like key_pack_kernel (sort.cu), but into three registers
-__device__ __forceinline__ void pack3(const KeyDesc& kd, uint64_t r, unsigned long long& w0, unsigned long long& w1, unsigned long long& w2) {
-    unsigned long long cur = 0; int cnt = 0, word = 0;
-    w0 = w1 = w2 = 0;
-    auto flush = [&](unsigned long long v) { if (word == 0) w0 = v; else if (word == 1) w1 = v; else w2 = v; word++; };
-    auto push = [&](uint32_t b) { cur = (cur << 8) | b; if (++cnt == 8) { flush(cur); cnt = 0; cur = 0; } };
-    for (int k = 0; k < kd.nkeys; k++) {
-        const uint32_t s = kd.off[k][r], len = kd.off[k][r + 1] - s, wd = kd.width[k];
-        const uint8_t* p = kd.data[k] + s;
-        unsigned long long a, b;
-        load16(p, len < wd ? len : wd, a, b);
-        uint32_t i = 0;
-        if (cnt == 0 && wd >= 8) { flush(bswap64(a)); i = 8; if (wd >= 16) { flush(bswap64(b)); i = 16; } }
-        for (; i < wd; i++)
-            push(i < 8 ? (uint32_t)(a >> (8 * i)) & 255u : i < 16 ? (uint32_t)(b >> (8 * (i - 8))) & 255u : (i < len ? p[i] : 0u));
-        const uint32_t lf = len > wd ? 0xffffffffu : len;
-        for (int i2 = (int)kd.lenbytes[k] - 1; i2 >= 0; i2--) push((lf >> (8 * i2)) & 0xffu);
-    }
-    if (cnt) flush(cur << (8 * (8 - cnt)));
-}
 __global__ void __launch_bounds__(256) join_probe32_kernel(KeyDesc kd, uint64_t np, const Slot32* __restrict__ slots, uint64_t nslots,
                                                            uint32_t* lo, uint32_t* cnt, uint32_t* not_one) {
     unsigned long long matches = 0;
@@ -169,14 +124,9 @@ __global__ void __launch_bounds__(256) join_probe32_kernel(KeyDesc kd, uint64_t 
 // 16-byte slots for key prefixes <= 12 bytes whose runs all have length 1 (unique keys): four slots per 64-byte
 // DRAM granule at load factor 1/2, so a probe costs about one granule (a 32-byte slot at 2/3 costs about two).
 struct __align__(16) Slot16 { unsigned long long k0; uint32_t k1; uint32_t row1; };  // row1 = sorted row + 1; 0 = empty
-// (a slot is claimed and filled by ONE 128-bit compare-and-swap — SASS ATOMG.E.CAS.128 — so a slot is never seen half
-// written and an insert that meets its own key knows it: `dup`, when given, is set if any key is inserted twice.  That
-// is the whole duplicate check of UniqueIndexOn for keys <= 12 bytes: the second inserter of a key walks the same probe
-// sequence as the first and reaches its slot.)
-__device__ __forceinline__ void cas128(void* addr, unsigned long long vl, unsigned long long vh, unsigned long long& ol, unsigned long long& oh) {
-    asm volatile("{\n.reg .b128 c, v, o;\nmov.b128 c, {%3, %4};\nmov.b128 v, {%5, %6};\natom.global.cas.b128 o, [%2], c, v;\nmov.b128 {%0, %1}, o;\n}"
-                 : "=l"(ol), "=l"(oh) : "l"(addr), "l"(0ull), "l"(0ull), "l"(vl), "l"(vh) : "memory");
-}
+// (claimed by cas128: `dup`, when given, is set if any key is inserted twice.  That is the whole duplicate check of
+// UniqueIndexOn for keys <= 12 bytes: the second inserter of a key walks the same probe sequence as the first and
+// reaches its slot.)
 __global__ void hash16_insert_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, const uint32_t* __restrict__ heads,
                                      uint64_t nheads, Slot16* slots, uint64_t nslots, uint32_t* dup) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -377,6 +327,83 @@ static void search_probe(Ctx* c, const Table& probe, const std::vector<int>& pid
     CPB_CUDA(cudaGetLastError());
 }
 
+// ------------------------------------------------------------------ row-carrying hash table (Index::rowhash)
+// Per source row: the key packed straight from the key columns, the payload columns' lengths and bytes gathered in
+// registers, the header claimed with one cas128, then the payload stored.  `dup` is set when a key meets itself, as in
+// hash16_insert: that is the whole duplicate check of UniqueIndexOn for such an index.
+struct PayCols { int nc; const uint32_t* off[RH_MAXC]; const uint8_t* data[RH_MAXC]; };
+__global__ void __launch_bounds__(256) rowhash_insert_kernel(KeyDesc kd, PayCols pc, uint64_t n, RowSlot* slots, uint64_t nslots, uint32_t* dup) {
+    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    unsigned long long w0, w1, w2;
+    pack3(kd, r, w0, w1, w2);
+    unsigned long long pa = 0, pb = 0;
+    uint32_t hdr = RH_OCCUPIED, pos = 0;
+#pragma unroll
+    for (int j = 0; j < RH_MAXC; j++) {
+        if (j >= pc.nc) break;
+        const uint32_t s = pc.off[j][r], l = pc.off[j][r + 1] - s;
+        unsigned long long a, b;
+        load16(pc.data[j] + s, l, a, b);
+        or_at16(pa, pb, pos, a, b);
+        hdr |= l << (5 * j);
+        pos += l;
+    }
+    const unsigned long long lo = w0, hi = (w1 >> 32) | ((unsigned long long)hdr << 32);
+    uint64_t s = slot_of(hash3(w0, w1, 0ull), nslots);
+    for (;;) {
+        unsigned long long ol, oh;
+        cas128(&slots[s], lo, hi, ol, oh);
+        if ((ol | oh) == 0ull) {
+            slots[s].pay = make_uint4((uint32_t)pa, (uint32_t)(pa >> 32), (uint32_t)pb, (uint32_t)(pb >> 32));
+            return;
+        }
+        if (ol == lo && (uint32_t)oh == (uint32_t)hi) { *dup = 1u; return; }  // benign race: every writer stores 1
+        if (++s == nslots) s = 0;
+    }
+}
+bool rowhash_build(Ctx* c, Index& ix) {
+    RowHash& rh = ix.rowhash;
+    const uint64_t n = (uint64_t)ix.nrows;
+    const Table& t = *ix.src;
+    KeyDesc kd{};
+    describe_keys(c, t, ix.key_col_idx, ix.key_width, kd);
+    PayCols pc{};
+    pc.nc = (int)rh.cols.size();
+    for (int j = 0; j < pc.nc; j++) { pc.off[j] = t.cols[rh.cols[j]].off(); pc.data[j] = t.cols[rh.cols[j]].bytes(); }
+    rh.slots = dev_alloc(c, rh.nslots * sizeof(RowSlot));
+    Buf dup = dev_alloc(c, 8);
+    CPB_CUDA(cudaMemsetAsync(dup->p, 0, 8, c->stream));
+    CPB_CUDA(cudaMemsetAsync(rh.slots->p, 0, rh.nslots * sizeof(RowSlot), c->stream));
+    {
+        KernelTimer kt(c, "rowhash_build", n * ((uint64_t)kd.words * 8 + RH_PAY + 4 * (uint64_t)(kd.nkeys + pc.nc)) + rh.nslots * sizeof(RowSlot));
+        rowhash_insert_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(kd, pc, n, rh.slots->as<RowSlot>(), rh.nslots, dup->as<uint32_t>());
+        CPB_CUDA(cudaGetLastError());
+    }
+    return read_back<uint32_t>(c, dup->p) != 0;
+}
+// flag[i] = whether probe row i finds its key (want 1) / finds nothing (want 0): the slot headers only
+__global__ void __launch_bounds__(256) rowhash_flags_kernel(KeyDesc kd, uint64_t np, const RowSlot* __restrict__ slots, uint64_t nslots,
+                                                            uint32_t want, uint32_t* flag) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
+        unsigned long long k0; uint32_t k1;
+        uint64_t s = rh_start(kd, i, nslots, k0, k1);
+        uint4 h = rh_header(slots, s);
+        flag[i] = rh_walk(slots, nslots, k0, k1, s, h) == (want != 0) ? 1u : 0u;
+    }
+}
+static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, const Index& ix, bool want) {
+    const uint64_t np = (uint64_t)probe.nrows;
+    KeyDesc kd{};
+    describe_keys(c, probe, pidx, ix.key_width, kd);
+    Buf flag = dev_alloc(c, np * 4);
+    KernelTimer kt(c, "rowhash_flags", np * ((uint64_t)kd.words * 8 + 4 * (uint64_t)kd.nkeys + 16 + 4));
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
+    rowhash_flags_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ix.rowhash.slots->as<RowSlot>(), ix.rowhash.nslots, want ? 1u : 0u, flag->as<uint32_t>());
+    CPB_CUDA(cudaGetLastError());
+    return flag;
+}
+
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti,
                                    DataError* derr, bool* failed) {
     *failed = false;
@@ -427,6 +454,44 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         return gather_rows(c, e, nullptr, 0);
     };
     if (np == 0) return empty_result();
+    // the probe rows whose flag is set (Except's result)
+    auto flagged_rows = [&](const Table& t, const FlagScan& s) {
+        Buf ids = dev_alloc(c, (s.count + 1) * 4);
+        compact_flags(c, s, 0, ids->as<uint32_t>());
+        auto r = gather_rows(c, t, ids->as<uint32_t>(), (int64_t)s.count);
+        r->first_line = probe.first_line;
+        return r;
+    };
+    if (ix.rowhash.slots && nk == (int)ix.key_cols.size()) {
+        // a unique index with a row-carrying table joined on its full key: one random access per probe row
+        if (anti) {
+            Buf miss = rowhash_flags(c, probe, pidx, ix, false);
+            return flagged_rows(probe, scan_flags(c, miss->as<uint32_t>(), np));
+        }
+        Buf hit;
+        FlagScan hits{};  // hits.pos stays null until the hit rows are needed
+        std::shared_ptr<Table> gi;
+        uint64_t m = 0;
+        if (gather_idx.empty()) {  // no index column to fetch: only the matches
+            hit = rowhash_flags(c, probe, pidx, ix, true);
+            hits = scan_flags(c, hit->as<uint32_t>(), np);
+            m = hits.count;
+            gi = std::make_shared<Table>(); gi->ctx = c; gi->nrows = (int64_t)np;
+        } else {
+            gi = rowhash_gather(c, ix, probe, pidx, gather_idx, &m);
+        }
+        if (m == 0) return empty_result();
+        out->nrows = (int64_t)np;
+        put_index_cols(*gi, [&](int k) { return probe.cols[pidx[k]]; });
+        for (auto* p : pcols) out->cols.push_back(*p);
+        if (m == np) return out;  // every probe row matched: the probe columns are shared as they are
+        // probe rows that found nothing: the full-length result (empty index values there) compacted to the rows that did
+        if (!hits.pos) {
+            hit = rowhash_flags(c, probe, pidx, ix, true);
+            hits = scan_flags(c, hit->as<uint32_t>(), np);
+        }
+        return flagged_rows(*out, hits);
+    }
     Buf lo = dev_alloc(c, np * 4), cnt = dev_alloc(c, (np + 1) * 4), flags = dev_alloc(c, 32);
     CPB_CUDA(cudaMemsetAsync(flags->p, 0, 32, c->stream));
     uint32_t* not_one = flags->as<uint32_t>() + 2;  // [0..1] = scan total
@@ -445,12 +510,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     if (anti) {
         Buf flag = dev_alloc(c, np * 4);
         zero_flag_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(cnt->as<uint32_t>(), flag->as<uint32_t>(), np);
-        const FlagScan s = scan_flags(c, flag->as<uint32_t>(), np);
-        Buf ids = dev_alloc(c, (s.count + 1) * 4);
-        compact_flags(c, s, 0, ids->as<uint32_t>());
-        auto r = gather_rows(c, probe, ids->as<uint32_t>(), (int64_t)s.count);
-        r->first_line = probe.first_line;
-        return r;
+        return flagged_rows(probe, scan_flags(c, flag->as<uint32_t>(), np));
     }
     const std::vector<uint32_t> hf = read_back<uint32_t>(c, flags->p, 8);
     const uint64_t m = (uint64_t)hf[4] | ((uint64_t)hf[5] << 32);  // counted by the probe kernel (0 when ni == 0)

@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "core.hpp"
+#include "rowhash.cuh"
 #include "util.cuh"
 
 namespace cpb {
@@ -254,14 +255,40 @@ Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const
     return img;
 }
 
-// per key column the longest value of rows [0, n) of t: the column widths of the key image
-static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n) {
-    Buf wd = dev_alloc(c, key_cols.size() * 4);
-    CPB_CUDA(cudaMemsetAsync(wd->p, 0, key_cols.size() * 4, c->stream));
-    for (size_t k = 0; k < key_cols.size() && n; k++)
+// the longest row of up to 4 columns taken together (the bytes of all their values in one row)
+struct RowCols { int nc; const uint32_t* off[4]; };
+__global__ void max_row_bytes_kernel(RowCols rc, uint64_t n, uint32_t* out) {
+    uint32_t m = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t t = 0;
+#pragma unroll
+        for (int c = 0; c < 4; c++) if (c < rc.nc) t += rc.off[c][i + 1] - rc.off[c][i];
+        m = max(m, t);
+    }
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
+}
+
+// per key column the longest value of rows [0, n) of t: the column widths of the key image.  With `row_cols` (at most
+// 4 columns), *row_max = their longest row, from the same readback.
+static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n,
+                                        const std::vector<int>* row_cols = nullptr, uint32_t* row_max = nullptr) {
+    const size_t nk = key_cols.size();
+    Buf wd = dev_alloc(c, (nk + 1) * 4);
+    CPB_CUDA(cudaMemsetAsync(wd->p, 0, (nk + 1) * 4, c->stream));
+    for (size_t k = 0; k < nk && n; k++)
         max_len_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(t.cols[key_cols[k]].off(), n, wd->as<uint32_t>() + k);
+    if (row_cols && !row_cols->empty() && n) {
+        RowCols rc{};
+        rc.nc = (int)row_cols->size();
+        for (int j = 0; j < rc.nc; j++) rc.off[j] = t.cols[(*row_cols)[j]].off();
+        max_row_bytes_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(rc, n, wd->as<uint32_t>() + nk);
+    }
     CPB_CUDA(cudaGetLastError());
-    return read_back<uint32_t>(c, wd->p, key_cols.size());
+    std::vector<uint32_t> w = read_back<uint32_t>(c, wd->p, nk + 1);
+    if (row_max) *row_max = w[nk];
+    w.pop_back();
+    return w;
 }
 
 // rows ids[0..m) of a key image of n_src rows, as an image of m rows
@@ -285,12 +312,14 @@ static void ensure_sorted_locked(Ctx* c, Index& ix) {
     if (ix.sorted) return;
     const uint64_t n = (uint64_t)ix.nrows;
     OwnerPool scope(c, ix.ctx);
+    uint32_t words = ix.image_words;
+    const Buf uimg = ix.uimage ? ix.uimage : pack_with_widths(c, *ix.src, ix.key_col_idx, ix.key_width, &words);  // (row-carrying table)
     uint64_t traffic = 0;
-    Buf perm = sort_by_image(c, ix.uimage->as<uint64_t>(), ix.image_words, n, &traffic);
+    Buf perm = sort_by_image(c, uimg->as<uint64_t>(), ix.image_words, n, &traffic);
     Buf simg;
     {
         KernelTimer kt(c, "image_gather", (uint64_t)ix.image_words * n * 20, (int)ix.image_words);
-        simg = gather_image(c, ix.uimage->as<uint64_t>(), ix.image_words, n, perm->as<uint32_t>(), n);
+        simg = gather_image(c, uimg->as<uint64_t>(), ix.image_words, n, perm->as<uint32_t>(), n);
     }
     sync_stream(c);  // complete before another context (stream) can see it
     ix.perm = perm; ix.image = simg; ix.sorted = true;
@@ -338,25 +367,42 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
         return ix;
     }
     if (n > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "an index holds at most 2^32-2 rows"};
-    // 1. key widths
+    static const bool eager = getenv("CPB_EAGER_SORT") != nullptr;
+    const bool lazy = unique && n >= 2 && !eager;
+    // 1. key widths; for a UniqueIndexOn with at most 4 other columns also their longest row: whether the row-carrying
+    //    hash table can hold the index
+    std::vector<int> pay;  // the non-key columns, in schema order
+    for (int q = 0; q < (int)t.cols.size(); q++)
+        if (std::find(ix->key_col_idx.begin(), ix->key_col_idx.end(), q) == ix->key_col_idx.end()) pay.push_back(q);
+    uint32_t pay_max = ~0u;
     {
         KernelTimer kt(c, "key_width", n * 4 * keys.size(), (int)keys.size());
-        ix->key_width = key_widths(c, t, ix->key_col_idx, n);
+        ix->key_width = key_widths(c, t, ix->key_col_idx, n, lazy && (int)pay.size() <= RH_MAXC ? &pay : nullptr, &pay_max);
     }
-    // 2. image of the unsorted rows
-    uint32_t words = 0;
-    Buf img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &words);
+    const uint32_t kbytes = prefix_bytes(*ix, (int)keys.size()), words = (kbytes + 7) / 8;
     ix->image_words = words;
     if ((uint64_t)words * 8 > 4096) throw ArgError{CPB_ERR_UNSUPPORTED, "index keys longer than 4 KiB are not supported"};
-    // 3a. UniqueIndexOn: the duplicate check does not need the order — a probe table over the rows as they are, in which
-    //     every key must find itself.  When it passes (the usual case) the sort is left for whoever needs the order.
-    static const bool eager = getenv("CPB_EAGER_SORT") != nullptr;
-    if (unique && n >= 2 && !eager) {
-        ix->src = tp; ix->nrows = (int64_t)n; ix->uimage = img; ix->sorted = false; ix->unique = true;
-        if (!index_has_duplicates(c, *ix)) return ix;
+    // 2. UniqueIndexOn: the duplicate check does not need the order — a probe table over the rows as they are, in which
+    //    every key must find itself.  When it passes (the usual case) the sort is left for whoever needs the order.
+    Buf img;  // image of the unsorted rows
+    if (lazy) {
+        ix->src = tp; ix->nrows = (int64_t)n; ix->sorted = false; ix->unique = true;
+        if (kbytes <= 12 && (int)pay.size() <= RH_MAXC && pay_max <= RH_PAY) {
+            // key, lengths and payload fit one 32-byte slot: the row-carrying table is the index's probe structure (and
+            // its insert the duplicate check); no key image until something needs the order
+            ix->rowhash.cols = pay;
+            ix->rowhash.nslots = n * 2 + 16;
+            if (!rowhash_build(c, *ix)) return ix;
+            ix->rowhash = RowHash{};
+        } else {
+            img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &ix->image_words);
+            ix->uimage = img;
+            if (!index_has_duplicates(c, *ix)) return ix;
+        }
         // a duplicate exists: sort, so that the error names the key the reference would name (the lowest in sort order)
         ix->unique = false; ix->sorted = true; ix->uimage = nullptr; ix->hash_src.clear(); ix->row_slots_src.clear();
     }
+    if (!img) img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &ix->image_words);
     // 3. stable LSD radix sort -> permutation
     uint64_t traffic = 0;
     Buf perm = sort_by_image(c, img->as<uint64_t>(), words, n, &traffic);
@@ -460,7 +506,7 @@ void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt) {
     uint32_t words = 0;
     ix.image = pack_with_widths(c, *nt, ix.key_col_idx, ix.key_width, &words);
     ix.image_words = words;
-    ix.hash.clear(); ix.row_slots.clear(); ix.hash_src.clear(); ix.row_slots_src.clear();
+    ix.hash.clear(); ix.row_slots.clear(); ix.hash_src.clear(); ix.row_slots_src.clear(); ix.rowhash = RowHash{};
     ix.in_order = true;
     if (m >= 2 && words) {
         Buf flag = dev_alloc(c, 8);
@@ -535,7 +581,7 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
     Buf simg = gather_image(c, ix.image->as<uint64_t>(), ix.image_words, n, ids->as<uint32_t>(), m);
     nt->first_line = 0;
     ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m;
-    ix.image = simg; ix.hash.clear(); ix.row_slots.clear();
+    ix.image = simg; ix.hash.clear(); ix.row_slots.clear(); ix.rowhash = RowHash{};
 }
 
 }  // namespace cpb
