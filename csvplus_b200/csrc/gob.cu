@@ -21,9 +21,9 @@
 // The rows of the index are taken in its stored order (sorted_table).  A message of 8 GiB or more (encoding/gob's tooBig
 // on 64-bit), or a rows slice above 8 GiB of Go maps, is refused before anything is written, as gob's encoder refuses it.
 //
-// Encode: gob_row_len (bytes per row) -> exclusive_scan_u32 -> gob_write (one warp per 32 rows through a shared stage
-// laid out like the destination, as json_write).  The prefix (type definitions, columns, rows header) is built here on
-// the host; the rows are written in row-range batches (each < 4 GiB) by cpb_index_gob_into.
+// Encode: gob_row_len (bytes per row) -> exclusive_scan_u32 -> gob_write (warp_write_rows of rowwrite.cuh) over a
+// keyed-column table whose names are uint(len name) name.  The prefix (type definitions, columns, rows header) is built
+// here on the host; the rows are written in row-range batches (each < 4 GiB) by cpb_index_gob_into.
 //
 // Decode: the host parses the type definitions (any ids, any order), the columns value, the rows message header and the
 // first row (k and the column set).  The rows body is uploaded once.  A row has no marker and its start depends on every
@@ -45,9 +45,9 @@
 // gob_sum_kernel gives every column's exact total (a column holds less than 4 GiB), the offsets are scanned per column,
 // and gob_copy gathers the bytes.
 #include <algorithm>
-#include <numeric>
 
 #include "core.hpp"
+#include "rowwrite.cuh"
 #include "util.cuh"
 
 namespace cpb {
@@ -122,14 +122,9 @@ static std::string map_def(const std::string& name, int64_t id, int64_t key, int
 }
 
 // ------------------------------------------------------------------ encode kernels
-struct GobCol {
-    const uint32_t* off; const uint8_t* data;
-    uint32_t key, key_len;  // the column's pre-encoded name in the key blob: uint(len name) name
-};
-
 // len[r] = bytes of row r, saturated at 0xFFFFFFFF (then *sum is >= 4 GiB too); *sum += the exact 64-bit total.  The
 // 32-bit scan of the lengths is run only when that total is below 4 GiB, so no partial sum of it can wrap.
-__global__ void gob_row_len_kernel(const GobCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len,
+__global__ void gob_row_len_kernel(const KeyedCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len,
                                    unsigned long long* sum) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint64_t total = 0;
@@ -154,102 +149,41 @@ __global__ void gob_sum_kernel(const uint32_t* __restrict__ v, uint64_t n, uint6
     if ((threadIdx.x & 31) == 0 && s) atomicAdd(out + blockIdx.y, (unsigned long long)s);
 }
 
-// One warp writes 32 consecutive rows into a per-warp shared stage laid out like the destination, then stores it with
-// aligned 16-byte vectors (json_write_kernel's scheme); a group longer than the stage is written directly.
+// the keyed-column table is copied to shared memory when it fits (meta_smem)
 constexpr int GB_WARPS = 8;
 constexpr int GB_STAGE = 4096;
 constexpr uint32_t GB_STAGE_BYTES = GB_WARPS * (GB_STAGE + 16);
 constexpr uint32_t GB_META_SMEM = 16384;
-__global__ void __launch_bounds__(GB_WARPS * 32) gob_write_kernel(const GobCol* gcols, const uint8_t* gkeys, int ncols, uint32_t meta_bytes,
+__global__ void __launch_bounds__(GB_WARPS * 32) gob_write_kernel(const KeyedCol* cols, const uint8_t* keys, int ncols, uint32_t meta_bytes,
                                                                   int meta_smem, uint64_t n, const uint32_t* __restrict__ pos, uint8_t* out) {
     extern __shared__ __align__(16) uint8_t smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint8_t* stage = smem + warp * (GB_STAGE + 16);
-    const GobCol* cols = gcols;
-    const uint8_t* keys = gkeys;
-    if (meta_smem) {  // descriptors then key blob, contiguous in global memory as in shared
-        uint8_t* sm = smem + GB_STAGE_BYTES;
-        const uint8_t* gm = reinterpret_cast<const uint8_t*>(gcols);
-        for (uint32_t i = threadIdx.x; i < meta_bytes; i += blockDim.x) sm[i] = gm[i];
-        __syncthreads();
-        cols = reinterpret_cast<const GobCol*>(sm);
-        keys = sm + (gkeys - gm);
-    }
-    const uint64_t nwarps = (uint64_t)gridDim.x * GB_WARPS;
-    for (uint64_t g = (uint64_t)blockIdx.x * GB_WARPS + warp; g * 32 < n; g += nwarps) {
-        const uint64_t r = g * 32 + lane;
-        const bool valid = r < n;
-        const uint32_t d = valid ? pos[r] : 0u;
-        const uint64_t lastr = g * 32 + 31 < n ? g * 32 + 31 : n - 1;
-        const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
-        const uint32_t dend = pos[lastr + 1];
-        const uint32_t sh = (uint32_t)((reinterpret_cast<uintptr_t>(out) + d0) & 15u), total = dend - d0;
-        const bool staged = (uint64_t)sh + total <= GB_STAGE;
-        if (valid) {
-            uint8_t* q = staged ? stage + sh + (d - d0) : out + d;
-            q += gob_put_uint(q, (uint64_t)ncols);
-            for (int k = 0; k < ncols; k++) {
-                const GobCol c = cols[k];
-                for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
-                q += c.key_len;
-                const uint32_t s = c.off[r], l = c.off[r + 1] - s;
-                q += gob_put_uint(q, l);
-                const uint8_t* p = c.data + s;
-                for (uint32_t j = 0; j < l; j++) q[j] = p[j];
-                q += l;
-            }
+    stage_keyed_cols(smem + GB_STAGE_BYTES, meta_smem, meta_bytes, cols, keys);
+    warp_write_rows<GB_WARPS, GB_STAGE>(smem, n, pos, out, [&](uint64_t r, uint8_t* q) {
+        q += gob_put_uint(q, (uint64_t)ncols);
+        for (int k = 0; k < ncols; k++) {
+            const KeyedCol c = cols[k];
+            for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
+            q += c.key_len;
+            const uint32_t s = c.off[r], l = c.off[r + 1] - s;
+            q += gob_put_uint(q, l);
+            const uint8_t* p = c.data + s;
+            for (uint32_t j = 0; j < l; j++) q[j] = p[j];
+            q += l;
         }
-        if (staged) {
-            __syncwarp();
-            uint8_t* gb = out + d0 - sh;
-            for (uint32_t x = lane * 16; x < sh + total; x += 32 * 16) {
-                if (x >= sh && x + 16 <= sh + total) *reinterpret_cast<uint4*>(gb + x) = *reinterpret_cast<const uint4*>(stage + x);
-                else for (uint32_t y = x; y < x + 16; y++) if (y >= sh && y < sh + total) gb[y] = stage[y];
-            }
-            __syncwarp();
-        }
-    }
+    });
 }
 
-__global__ void gob_value_bytes_kernel(const GobCol* cols, int ncols, uint64_t n, unsigned long long* out) {
-    unsigned long long s = 0;
-    for (int k = 0; k < ncols; k++) s += cols[k].off[n] - cols[k].off[0];
-    *out = s;
-}
-
-// the column descriptors and pre-encoded names of rows [lo, hi) of the index's stored rows, names in bytewise order,
-// uploaded as one blob: GobCol[ncols] then the names
+// the keyed columns of rows [lo, hi) of the index's stored rows
 struct GobMeta {
-    std::shared_ptr<Table> t;
-    Buf md; uint32_t meta_bytes = 0, keys_at = 0; int ncols = 0;
-    uint64_t row_const = 0;  // uint(k) + every pre-encoded name
+    std::shared_ptr<Table> t;  // the stored rows, kept alive while the kernels read them
+    KeyedCols kc;
+    uint64_t row_const = 0;    // uint(k) + every pre-encoded name
 };
 static GobMeta gob_meta(Ctx* c, Index& ix, uint64_t lo) {
     GobMeta m;
     m.t = sorted_table(c, ix);
-    const Table& t = *m.t;
-    m.ncols = (int)t.cols.size();
-    std::vector<int> order(m.ncols);
-    std::iota(order.begin(), order.end(), 0);
-    std::sort(order.begin(), order.end(), [&](int a, int b) { return t.cols[a].name < t.cols[b].name; });  // bytewise
-    std::vector<GobCol> hc(m.ncols);
-    std::string keys;
-    m.row_const = gob_uint_len((uint64_t)m.ncols);
-    for (int k = 0; k < m.ncols; k++) {
-        const Column& col = t.cols[order[k]];
-        const uint32_t at = (uint32_t)keys.size();
-        put_str(keys, col.name);
-        hc[k] = GobCol{col.off() + lo, col.bytes(), at, (uint32_t)(keys.size() - at)};
-        m.row_const += hc[k].key_len;
-    }
-    m.keys_at = (uint32_t)(m.ncols * sizeof(GobCol));
-    m.meta_bytes = m.keys_at + (uint32_t)keys.size();
-    std::vector<uint8_t> meta(m.meta_bytes + 1);
-    if (m.ncols) memcpy(meta.data(), hc.data(), m.keys_at);
-    if (!keys.empty()) memcpy(meta.data() + m.keys_at, keys.data(), keys.size());
-    m.md = dev_alloc(c, m.meta_bytes + 16);
-    if (m.meta_bytes) CPB_CUDA(cudaMemcpyAsync(m.md->p, meta.data(), m.meta_bytes, cudaMemcpyHostToDevice, c->stream));
-    sync_stream(c);  // meta is pageable host memory
+    m.kc = keyed_cols(c, *m.t, lo, [](std::string& keys, const std::string& name, int) { put_str(keys, name); });
+    m.row_const = gob_uint_len((uint64_t)m.kc.ncols) + (m.kc.meta_bytes - m.kc.keys_at);
     return m;
 }
 
@@ -258,15 +192,13 @@ static void gob_lengths(Ctx* c, const GobMeta& m, uint64_t n, Buf& len, uint64_t
     len = dev_alloc(c, (n + 1) * 4);
     Buf tot = dev_alloc(c, 16);
     CPB_CUDA(cudaMemsetAsync(tot->p, 0, 16, c->stream));
-    const GobCol* dcols = m.md->as<GobCol>();
     if (n) {
-        KernelTimer kt(c, "gob_row_len", n * 4 * (m.ncols + 1));
-        gob_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dcols, m.ncols, m.row_const, n, len->as<uint32_t>(),
+        KernelTimer kt(c, "gob_row_len", n * 4 * (m.kc.ncols + 1));
+        gob_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(m.kc.md->as<KeyedCol>(), m.kc.ncols, m.row_const, n, len->as<uint32_t>(),
                                                                  tot->as<unsigned long long>());
         CPB_CUDA(cudaGetLastError());
     }
-    gob_value_bytes_kernel<<<1, 1, 0, c->stream>>>(dcols, m.ncols, n, tot->as<unsigned long long>() + 1);
-    CPB_CUDA(cudaGetLastError());
+    keyed_value_bytes(c, m.kc, n, tot->as<unsigned long long>() + 1);
     const std::vector<uint64_t> h = read_back<uint64_t>(c, tot->p, 2);
     out[0] = h[0]; out[1] = h[1];
 }
@@ -310,13 +242,14 @@ Buf gob_rows(Ctx* c, Index& ix, uint64_t lo, uint64_t hi, uint64_t room, uint64_
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());  // every partial sum < 4 GiB
     Buf out = dev_alloc(c, t[0] + 16);
     if (n) {
-        KernelTimer kt(c, "gob_write", t[1] + n * 4 * (m.ncols + 1) + t[0]);
-        const bool meta_smem = m.meta_bytes <= GB_META_SMEM;
-        const uint32_t smem = GB_STAGE_BYTES + (meta_smem ? m.meta_bytes : 0);
+        const KeyedCols& kc = m.kc;
+        KernelTimer kt(c, "gob_write", t[1] + n * 4 * (kc.ncols + 1) + t[0]);
+        const bool meta_smem = kc.meta_bytes <= GB_META_SMEM;
+        const uint32_t smem = GB_STAGE_BYTES + (meta_smem ? kc.meta_bytes : 0);
         CPB_CUDA(cudaFuncSetAttribute(gob_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GB_STAGE_BYTES + GB_META_SMEM));
         const uint32_t blocks = (uint32_t)std::min<uint64_t>((n + GB_WARPS * 32 - 1) / (GB_WARPS * 32), (uint64_t)c->sm_count * 8);
-        gob_write_kernel<<<blocks, GB_WARPS * 32, smem, c->stream>>>(m.md->as<GobCol>(), m.md->as<uint8_t>() + m.keys_at, m.ncols, m.meta_bytes,
-                                                                     meta_smem, n, len->as<uint32_t>(), out->as<uint8_t>());
+        gob_write_kernel<<<blocks, GB_WARPS * 32, smem, c->stream>>>(kc.md->as<KeyedCol>(), kc.md->as<uint8_t>() + kc.keys_at, kc.ncols,
+                                                                     kc.meta_bytes, meta_smem, n, len->as<uint32_t>(), out->as<uint8_t>());
         CPB_CUDA(cudaGetLastError());
     }
     return out;

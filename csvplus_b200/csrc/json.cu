@@ -15,20 +15,15 @@
 //
 // One call serialises one table or one row-range batch of a larger result: first_batch puts '[' before its first row
 // (else ','), last_batch appends ']'.  An empty batch writes only those brackets, so first = last = 1 gives "[]".
-// Kernels: json_row_len (bytes per row) -> exclusive_scan_u32 -> json_write (one warp per 32 rows through a shared
-// stage, as csv_row_write_kernel).  Column descriptors live in a device array, so there is no column limit.
+// Kernels: json_row_len (bytes per row) -> exclusive_scan_u32 -> json_write (warp_write_rows of rowwrite.cuh).  The
+// columns are a keyed-column table (rowwrite.cuh) whose names are the key prefixes, so there is no column limit.
 #include <algorithm>
 #include <numeric>
 
 #include "core.hpp"
-#include "util.cuh"
+#include "rowwrite.cuh"
 
 namespace cpb {
-
-struct JsonCol {
-    const uint32_t* off; const uint8_t* data;
-    uint32_t key, key_len;  // the column's prefix in the key blob: [","] enc(name) ':' '"'
-};
 
 // true when no byte of p[0..n) needs attention (< 0x20, '"', '\', >= 0x80): such a value is written as '"' p '"'.
 // Reads the aligned 8-byte words covering the value; the word holding the last byte lies inside its allocation.
@@ -102,7 +97,7 @@ __host__ __device__ inline uint64_t json_escape(const uint8_t* p, uint64_t n, ui
 }
 
 // len[r] = output bytes of row r, saturated at 0xFFFFFFFF (the host then reports CPB_E_TOO_LARGE)
-__global__ void json_row_len_kernel(const JsonCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len) {
+__global__ void json_row_len_kernel(const KeyedCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     uint64_t total = row_const;
@@ -115,73 +110,79 @@ __global__ void json_row_len_kernel(const JsonCol* __restrict__ cols, int ncols,
     len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
 }
 
-// One warp serialises 32 consecutive rows into a per-warp shared stage laid out like the destination, then stores it
-// with aligned 16-byte vectors (see csv_row_write_kernel).  A JSON row repeats every key, so it is several times longer
-// than the CSV line of the same row (about 120-150 B for a joined orders x customers row): the stage holds 32 rows of
-// up to 190 B, where ToCsv's 4 KB would send most such groups down the direct path.  Longer groups are written directly.
-// The column descriptors and key prefixes are copied to shared memory when they fit (meta_smem), else read from global.
+// A JSON row repeats every key, so it is several times longer than the CSV line of the same row (about 120-150 B for a
+// joined orders x customers row): the stage holds 32 rows of up to 190 B, where ToCsv's 4 KB would send most such
+// groups down the direct path.  The keyed-column table is copied to shared memory when it fits (meta_smem).
 constexpr int JW_WARPS = 8;
 constexpr int JW_STAGE = 6144;
 constexpr uint32_t JW_STAGE_BYTES = JW_WARPS * (JW_STAGE + 16);
 constexpr uint32_t JW_META_SMEM = 16384;
-__global__ void __launch_bounds__(JW_WARPS * 32) json_write_kernel(const JsonCol* gcols, const uint8_t* gkeys, int ncols, uint32_t meta_bytes,
+__global__ void __launch_bounds__(JW_WARPS * 32) json_write_kernel(const KeyedCol* cols, const uint8_t* keys, int ncols, uint32_t meta_bytes,
                                                                    int meta_smem, uint8_t first_byte, uint64_t n,
                                                                    const uint32_t* __restrict__ pos, uint8_t* out) {
     extern __shared__ __align__(16) uint8_t smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint8_t* stage = smem + warp * (JW_STAGE + 16);
-    const JsonCol* cols = gcols;
-    const uint8_t* keys = gkeys;
-    if (meta_smem) {  // descriptors then key blob, contiguous in global memory as in shared
-        uint8_t* sm = smem + JW_STAGE_BYTES;
-        const uint8_t* gm = reinterpret_cast<const uint8_t*>(gcols);
-        for (uint32_t i = threadIdx.x; i < meta_bytes; i += blockDim.x) sm[i] = gm[i];
-        __syncthreads();
-        cols = reinterpret_cast<const JsonCol*>(sm);
-        keys = sm + (gkeys - gm);
-    }
-    const uint64_t nwarps = (uint64_t)gridDim.x * JW_WARPS;
-    for (uint64_t g = (uint64_t)blockIdx.x * JW_WARPS + warp; g * 32 < n; g += nwarps) {
-        const uint64_t r = g * 32 + lane;
-        const bool valid = r < n;
-        const uint32_t d = valid ? pos[r] : 0u;
-        const uint64_t lastr = g * 32 + 31 < n ? g * 32 + 31 : n - 1;
-        const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
-        const uint32_t dend = pos[lastr + 1];
-        const uint32_t sh = (uint32_t)((reinterpret_cast<uintptr_t>(out) + d0) & 15u), total = dend - d0;
-        const bool staged = (uint64_t)sh + total <= JW_STAGE;
-        if (valid) {
-            uint8_t* q = staged ? stage + sh + (d - d0) : out + d;
-            *q++ = r == 0 ? first_byte : ',';
-            *q++ = '{';
-            for (int k = 0; k < ncols; k++) {
-                const JsonCol c = cols[k];
-                for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
-                q += c.key_len;
-                const uint32_t s = c.off[r], l = c.off[r + 1] - s;
-                const uint8_t* p = c.data + s;
-                if (json_plain(p, l)) { for (uint32_t j = 0; j < l; j++) q[j] = p[j]; q += l; }
-                else q += json_escape(p, l, q);
-                *q++ = '"';
-            }
-            q[0] = '}'; q[1] = '\n';
+    stage_keyed_cols(smem + JW_STAGE_BYTES, meta_smem, meta_bytes, cols, keys);
+    warp_write_rows<JW_WARPS, JW_STAGE>(smem, n, pos, out, [&](uint64_t r, uint8_t* q) {
+        *q++ = r == 0 ? first_byte : ',';
+        *q++ = '{';
+        for (int k = 0; k < ncols; k++) {
+            const KeyedCol c = cols[k];
+            for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
+            q += c.key_len;
+            const uint32_t s = c.off[r], l = c.off[r + 1] - s;
+            const uint8_t* p = c.data + s;
+            if (json_plain(p, l)) { for (uint32_t j = 0; j < l; j++) q[j] = p[j]; q += l; }
+            else q += json_escape(p, l, q);
+            *q++ = '"';
         }
-        if (staged) {
-            __syncwarp();
-            uint8_t* gb = out + d0 - sh;
-            for (uint32_t x = lane * 16; x < sh + total; x += 32 * 16) {
-                if (x >= sh && x + 16 <= sh + total) *reinterpret_cast<uint4*>(gb + x) = *reinterpret_cast<const uint4*>(stage + x);
-                else for (uint32_t y = x; y < x + 16; y++) if (y >= sh && y < sh + total) gb[y] = stage[y];
-            }
-            __syncwarp();
-        }
-    }
+        q[0] = '}'; q[1] = '\n';
+    });
 }
 
-__global__ void json_value_bytes_kernel(const JsonCol* cols, int ncols, uint64_t n, unsigned long long* out) {
+// ---- the keyed-column table of rowwrite.cuh (ToJSON and Index.WriteTo)
+__global__ void keyed_value_bytes_kernel(const KeyedCol* cols, int ncols, uint64_t n, unsigned long long* out) {
     unsigned long long s = 0;
     for (int k = 0; k < ncols; k++) s += cols[k].off[n] - cols[k].off[0];
     *out = s;
+}
+
+void keyed_value_bytes(Ctx* c, const KeyedCols& kc, uint64_t n, unsigned long long* out) {
+    keyed_value_bytes_kernel<<<1, 1, 0, c->stream>>>(kc.md->as<KeyedCol>(), kc.ncols, n, out);
+    CPB_CUDA(cudaGetLastError());
+}
+
+KeyedCols keyed_cols(Ctx* c, const Table& t, uint64_t lo, void (*enc)(std::string& keys, const std::string& name, int k)) {
+    KeyedCols kc;
+    kc.ncols = (int)t.cols.size();
+    std::vector<int> order(kc.ncols);
+    std::iota(order.begin(), order.end(), 0);
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return t.cols[a].name < t.cols[b].name; });  // bytewise
+    std::vector<KeyedCol> hc(kc.ncols);
+    std::string keys;
+    for (int k = 0; k < kc.ncols; k++) {
+        const Column& col = t.cols[order[k]];
+        const uint32_t at = (uint32_t)keys.size();
+        enc(keys, col.name, k);
+        hc[k] = KeyedCol{col.off() + lo, col.bytes(), at, (uint32_t)(keys.size() - at)};
+    }
+    kc.keys_at = (uint32_t)(kc.ncols * sizeof(KeyedCol));
+    kc.meta_bytes = kc.keys_at + (uint32_t)keys.size();
+    std::string meta(reinterpret_cast<const char*>(hc.data()), kc.keys_at);
+    meta += keys;
+    kc.md = dev_alloc(c, kc.meta_bytes);
+    // (pageable source: the call returns once the bytes are staged, so meta may go away)
+    if (kc.meta_bytes) CPB_CUDA(cudaMemcpyAsync(kc.md->p, meta.data(), kc.meta_bytes, cudaMemcpyHostToDevice, c->stream));
+    return kc;
+}
+
+// a column's key prefix: [","] '"' enc(name) '"' ':' '"'
+static void json_key(std::string& keys, const std::string& name, int k) {
+    std::vector<uint8_t> e(name.size() * 6 + 2);
+    const uint64_t m = json_escape((const uint8_t*)name.data(), name.size(), e.data());
+    if (k) keys += ',';
+    keys += '"';
+    keys.append((const char*)e.data(), m);
+    keys += "\":\"";
 }
 
 Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, uint64_t* nbytes) {
@@ -195,34 +196,11 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, 
         sync_stream(c);  // s is pageable stack memory
         return out;
     }
-    const int ncols = (int)t.cols.size();
-    std::vector<int> order(ncols);
-    std::iota(order.begin(), order.end(), 0);
-    std::sort(order.begin(), order.end(), [&](int a, int b) { return t.cols[a].name < t.cols[b].name; });  // bytewise
-    // metadata blob: JsonCol[ncols] then the key prefixes
-    std::vector<JsonCol> hc(ncols);
-    std::vector<uint8_t> keys;
-    uint64_t row_const = 4;  // '['/',' '{' '}' '\n'
-    for (int k = 0; k < ncols; k++) {
-        const Column& col = t.cols[order[k]];
-        std::vector<uint8_t> e(col.name.size() * 6 + 2);
-        const uint64_t m = json_escape((const uint8_t*)col.name.data(), col.name.size(), e.data());
-        const uint32_t at = (uint32_t)keys.size();
-        if (k) keys.push_back(',');
-        keys.push_back('"');
-        keys.insert(keys.end(), e.begin(), e.begin() + m);
-        keys.push_back('"'); keys.push_back(':'); keys.push_back('"');
-        hc[k] = JsonCol{col.off(), col.bytes(), at, (uint32_t)(keys.size() - at)};
-        row_const += hc[k].key_len + 1;  // + the closing quote of the value
-    }
-    const uint32_t keys_at = (uint32_t)(ncols * sizeof(JsonCol)), meta_bytes = keys_at + (uint32_t)keys.size();
-    std::vector<uint8_t> meta(meta_bytes);
-    if (ncols) memcpy(meta.data(), hc.data(), keys_at);
-    if (!keys.empty()) memcpy(meta.data() + keys_at, keys.data(), keys.size());
-    Buf md = dev_alloc(c, meta_bytes);
-    if (meta_bytes) CPB_CUDA(cudaMemcpyAsync(md->p, meta.data(), meta_bytes, cudaMemcpyHostToDevice, c->stream));
-    const JsonCol* dcols = md->as<JsonCol>();
-    const uint8_t* dkeys = md->as<uint8_t>() + keys_at;
+    const KeyedCols kc = keyed_cols(c, t, 0, json_key);
+    const int ncols = kc.ncols;
+    // '['/',' '{' '}' '\n', the key prefixes and the closing quote of every value
+    const uint64_t row_const = 4 + (kc.meta_bytes - kc.keys_at) + ncols;
+    const KeyedCol* dcols = kc.md->as<KeyedCol>();
 
     Buf len = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 16);
     {
@@ -230,8 +208,7 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, 
         json_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dcols, ncols, row_const, n, len->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
-    json_value_bytes_kernel<<<1, 1, 0, c->stream>>>(dcols, ncols, n, tot->as<unsigned long long>() + 1);
-    CPB_CUDA(cudaGetLastError());
+    keyed_value_bytes(c, kc, n, tot->as<unsigned long long>() + 1);
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
     const std::vector<uint64_t> ht = read_back<uint64_t>(c, tot->p, 2);
     const uint64_t body = ht[0], value_bytes = ht[1];
@@ -241,12 +218,13 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, 
     Buf out = dev_alloc(c, body + 1 + 16);
     {
         KernelTimer kt(c, "json_write", value_bytes + n * 4 * (ncols + 1) + body);
-        const bool meta_smem = meta_bytes <= JW_META_SMEM;
-        const uint32_t smem = JW_STAGE_BYTES + (meta_smem ? meta_bytes : 0);
+        const bool meta_smem = kc.meta_bytes <= JW_META_SMEM;
+        const uint32_t smem = JW_STAGE_BYTES + (meta_smem ? kc.meta_bytes : 0);
         CPB_CUDA(cudaFuncSetAttribute(json_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, JW_STAGE_BYTES + JW_META_SMEM));
         const uint32_t blocks = (uint32_t)std::min<uint64_t>((n + JW_WARPS * 32 - 1) / (JW_WARPS * 32), (uint64_t)c->sm_count * 8);
-        json_write_kernel<<<blocks, JW_WARPS * 32, smem, c->stream>>>(dcols, dkeys, ncols, meta_bytes, meta_smem, first ? '[' : ',', n,
-                                                                      len->as<uint32_t>(), out->as<uint8_t>());
+        json_write_kernel<<<blocks, JW_WARPS * 32, smem, c->stream>>>(dcols, kc.md->as<uint8_t>() + kc.keys_at, ncols, kc.meta_bytes,
+                                                                      meta_smem, first ? '[' : ',', n, len->as<uint32_t>(),
+                                                                      out->as<uint8_t>());
         CPB_CUDA(cudaGetLastError());
     }
     if (last) CPB_CUDA(cudaMemsetAsync(out->as<uint8_t>() + body, ']', 1, c->stream));

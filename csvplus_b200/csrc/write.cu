@@ -2,11 +2,11 @@
 // encoding/csv.Writer (comma ',', UseCRLF=false; SURVEY App. B): header line, then one line per row
 // with the named columns in caller order.  A field is quoted iff it is non-empty and (it is `\.` or
 // contains , " \r \n or its first rune is unicode.IsSpace); inside quotes " is doubled.
-// Two kernels: per-row output length -> exclusive scan -> per-row serialisation.
+// Two kernels: per-row output length -> exclusive scan -> serialisation through warp_write_rows (rowwrite.cuh).
 #include <algorithm>
 
 #include "core.hpp"
-#include "util.cuh"
+#include "rowwrite.cuh"
 
 namespace cpb {
 
@@ -60,46 +60,18 @@ __global__ void csv_row_len_kernel(WriteCols wc, uint64_t n, uint32_t* len) {
     }
     len[r] = total;
 }
-// One warp serialises 32 consecutive rows.  Their output bytes are contiguous, so every lane writes its line into a
-// per-warp shared-memory stage laid out like the destination and the warp stores the stage with aligned 16-byte
-// vectors (a thread-per-row kernel storing bytes straight to HBM touches ~20 sectors per store instruction).
-// Groups longer than the stage (very long rows) are written directly.
 constexpr int CW_WARPS = 8;
 constexpr int CW_STAGE = 4096;
 __global__ void __launch_bounds__(CW_WARPS * 32) csv_row_write_kernel(WriteCols wc, uint64_t n, const uint32_t* __restrict__ pos, uint8_t* out) {
     __shared__ __align__(16) uint8_t stage_all[CW_WARPS][CW_STAGE + 16];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint8_t* stage = stage_all[warp];
-    const uint64_t nwarps = (uint64_t)gridDim.x * CW_WARPS;
-    for (uint64_t g = (uint64_t)blockIdx.x * CW_WARPS + warp; g * 32 < n; g += nwarps) {
-        const uint64_t r = g * 32 + lane;
-        const bool valid = r < n;
-        const uint32_t d = valid ? pos[r] : 0u;
-        const uint64_t lastr = g * 32 + 31 < n ? g * 32 + 31 : n - 1;
-        const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
-        const uint32_t dend = pos[lastr + 1];  // pos has n+1 entries
-        // the absolute destination is out + d; alignment is that of the pointer, not of the offset alone
-        const uint32_t sh = (uint32_t)((reinterpret_cast<uintptr_t>(out) + d0) & 15u), total = dend - d0;
-        const bool staged = sh + total <= CW_STAGE;
-        if (valid) {
-            uint8_t* q = staged ? stage + sh + (d - d0) : out + d;
-            for (int k = 0; k < wc.n; k++) {
-                if (k) *q++ = ',';
-                const uint32_t s = wc.off[k][r], l = wc.off[k][r + 1] - s;
-                q += field_write(wc.data[k] + s, l, q);
-            }
-            *q = '\n';
+    warp_write_rows<CW_WARPS, CW_STAGE>(&stage_all[0][0], n, pos, out, [&](uint64_t r, uint8_t* q) {
+        for (int k = 0; k < wc.n; k++) {
+            if (k) *q++ = ',';
+            const uint32_t s = wc.off[k][r], l = wc.off[k][r + 1] - s;
+            q += field_write(wc.data[k] + s, l, q);
         }
-        if (staged) {
-            __syncwarp();
-            uint8_t* gb = out + d0 - sh;
-            for (uint32_t x = lane * 16; x < sh + total; x += 32 * 16) {
-                if (x >= sh && x + 16 <= sh + total) *reinterpret_cast<uint4*>(gb + x) = *reinterpret_cast<const uint4*>(stage + x);
-                else for (uint32_t y = x; y < x + 16; y++) if (y >= sh && y < sh + total) gb[y] = stage[y];
-            }
-            __syncwarp();
-        }
-    }
+        *q = '\n';
+    });
 }
 
 Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, bool with_header,
@@ -119,7 +91,6 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     wc.n = (int)cols.size();
     for (int k = 0; k < wc.n && n; k++) { wc.off[k] = t.cols[cols[k]].off(); wc.data[k] = t.cols[cols[k]].bytes(); }
     Buf len = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8);
-    uint64_t in_bytes = 0;
     if (n) {
         KernelTimer kt(c, "csv_row_len", n * 4 * (wc.n + 1));
         csv_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(wc, n, len->as<uint32_t>());
@@ -133,7 +104,6 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     Buf out = dev_alloc(c, header.size() + body + 16);
     CPB_CUDA(cudaMemcpyAsync(out->p, header.data(), header.size(), cudaMemcpyHostToDevice, c->stream));
     if (n) {
-        (void)in_bytes;
         KernelTimer kt(c, "csv_write", 2 * body + n * 4 * (wc.n + 1));
         const uint32_t wblocks = (uint32_t)std::min<uint64_t>((n + CW_WARPS * 32 - 1) / (CW_WARPS * 32), (uint64_t)c->sm_count * 16);
         csv_row_write_kernel<<<wblocks, CW_WARPS * 32, 0, c->stream>>>(wc, n, len->as<uint32_t>(), out->as<uint8_t>() + header.size());
