@@ -123,9 +123,13 @@ struct RowSlots {
 // Row-carrying hash table of a unique index whose full-key image is <= 12 bytes and whose other columns (at most 4) take
 // <= 16 bytes in every row: one 32-byte slot (one DRAM sector) per entry holds the key, the lengths of those columns
 // and their bytes (RowSlot, rowhash.cuh), so a full-key Join finds key, lengths and payload with ONE random access.
-// Built by UniqueIndexOn (the insert is the duplicate check) and complete when the index is returned: read-only after.
+// Built by UniqueIndexOn (the build is the duplicate check) and complete when the index is returned: read-only after.
+// Layout: nslots / region regions of `region` consecutive slots.  A key's probe sequence starts at slot_of(hash, nslots)
+// and wraps from the last slot of that slot's region to the region's first, never into the next region; so each region
+// is built on its own in shared memory, and a region can hold at most region - 1 keys.
 struct RowHash {
-    uint64_t nslots = 0;    // load factor 1/2
+    uint64_t nslots = 0;    // a multiple of region, at least 2 * rows + 16 (load factor about 1/2)
+    uint32_t region = 0;    // slots per region: a power of two, RH_REGION (rowhash.cuh) unless the table is smaller
     Buf slots;              // RowSlot[nslots]; null = the index has no row-carrying table
     std::vector<int> cols;  // payload: every non-key column of the source, in schema order
 };
@@ -326,8 +330,10 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
                                    bool anti, DataError* derr, bool* failed);
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi);
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
-// fills ix.rowhash (nslots, cols set by the caller) from ix.src; true when some key was inserted twice
-bool rowhash_build(Ctx* c, Index& ix);
+// fills ix.rowhash (cols set by the caller) from ix.src.  built: the table is complete; duplicate: some key occurs twice;
+// overflow: some region received more keys than it can hold (no duplicate was seen, but the table is unusable)
+enum class RhBuild { built, duplicate, overflow };
+RhBuild rowhash_build(Ctx* c, Index& ix);
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi);
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep, bool bug_compatible, const Table* repl = nullptr);
 // the index takes the rows of nt in their stored order: key columns, widths and key image are rebuilt from them, in_order

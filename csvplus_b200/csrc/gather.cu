@@ -319,14 +319,15 @@ __global__ void __launch_bounds__(256) slot_fill_kernel(SlotCols sc, const uint3
 // written sequentially, and the hits are counted into *matches.  (Probing inside the length scan, 8 rows per thread,
 // needs ~170 registers: one CTA per SM, and the kernel ran latency-bound at 3.6x this one + the scan.)
 __global__ void __launch_bounds__(256) rowhash_probe_kernel(KeyDesc kd, uint64_t np, const RowSlot* __restrict__ slots, uint64_t nslots,
-                                                            int npay, uint32_t sel, uint32_t* lens, uint4* scratch, unsigned long long* matches) {
+                                                            uint64_t rmask, int npay, uint32_t sel, uint32_t* lens, uint4* scratch,
+                                                            unsigned long long* matches) {
     unsigned long long hits = 0;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
         unsigned long long k0; uint32_t k1;
         uint64_t s = rh_start(kd, i, nslots, k0, k1);
         uint4 h = rh_header(slots, s), v = __ldg(&slots[s].pay);  // one sector, both halves
         const uint64_t s0 = s;
-        const bool found = rh_walk(slots, nslots, k0, k1, s, h);
+        const bool found = rh_walk(slots, rmask, k0, k1, s, h);
         if (found && s != s0) v = __ldg(&slots[s].pay);
         unsigned long long a = 0, b = 0;
         uint32_t p = 0;
@@ -735,7 +736,7 @@ std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, con
     {
         KernelTimer kt(c, "rowhash_probe", np * ((uint64_t)kd.words * 8 + 4 * (uint64_t)kd.nkeys + sizeof(RowSlot) + RH_PAY + 4));
         const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-        rowhash_probe_kernel<<<grid, 256, 0, c->stream>>>(kd, np, rh.slots->as<RowSlot>(), rh.nslots, (int)rh.cols.size(), sel,
+        rowhash_probe_kernel<<<grid, 256, 0, c->stream>>>(kd, np, rh.slots->as<RowSlot>(), rh.nslots, rh.region - 1ull, (int)rh.cols.size(), sel,
                                                           lens->as<uint32_t>(), scratch->as<uint4>(), cnt->as<unsigned long long>());
         CPB_CUDA(cudaGetLastError());
     }

@@ -328,11 +328,19 @@ static void search_probe(Ctx* c, const Table& probe, const std::vector<int>& pid
 }
 
 // ------------------------------------------------------------------ row-carrying hash table (Index::rowhash)
-// Per source row: the key packed straight from the key columns, the payload columns' lengths and bytes gathered in
-// registers, the header claimed with one cas128, then the payload stored.  `dup` is set when a key meets itself, as in
-// hash16_insert: that is the whole duplicate check of UniqueIndexOn for such an index.
+// Built region by region in two passes, so that no insert is a random read-modify-write of DRAM:
+//  1. rowhash_scatter, one thread per source row: the key packed straight from the key columns, the payload columns'
+//     lengths and bytes gathered in registers, and the row's slot image {k0, k1, hdr, payload} appended to its region's
+//     part of the table itself (fill[g] counts region g's rows).  A region's appends are consecutive sectors, so the
+//     writes of a warp's rows merge in L2 and reach DRAM as whole sectors.
+//  2. rowhash_region, one CTA per region: the region's staged images read, inserted into the region built in shared
+//     memory with one 128-bit CAS per claim, and the whole region, empty slots included, written back over them.  So
+//     the table needs no zeroing.  A key that meets itself sets flags[0]: that is the whole duplicate check of
+//     UniqueIndexOn for such an index (equal keys hash to one region).  A region given more than region - 1 rows is
+//     not built and sets flags[1] (its images past `region` were dropped by the scatter).
 struct PayCols { int nc; const uint32_t* off[RH_MAXC]; const uint8_t* data[RH_MAXC]; };
-__global__ void __launch_bounds__(256) rowhash_insert_kernel(KeyDesc kd, PayCols pc, uint64_t n, RowSlot* slots, uint64_t nslots, uint32_t* dup) {
+__global__ void __launch_bounds__(256) rowhash_scatter_kernel(KeyDesc kd, PayCols pc, uint64_t n, RowSlot* slots, uint64_t nslots,
+                                                              uint32_t rshift, uint32_t* fill) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     unsigned long long w0, w1, w2;
@@ -349,20 +357,54 @@ __global__ void __launch_bounds__(256) rowhash_insert_kernel(KeyDesc kd, PayCols
         hdr |= l << (5 * j);
         pos += l;
     }
-    const unsigned long long lo = w0, hi = (w1 >> 32) | ((unsigned long long)hdr << 32);
-    uint64_t s = slot_of(hash3(w0, w1, 0ull), nslots);
-    for (;;) {
-        unsigned long long ol, oh;
-        cas128(&slots[s], lo, hi, ol, oh);
-        if ((ol | oh) == 0ull) {
-            slots[s].pay = make_uint4((uint32_t)pa, (uint32_t)(pa >> 32), (uint32_t)pb, (uint32_t)(pb >> 32));
-            return;
+    const uint64_t g = slot_of(hash3(w0, w1, 0ull), nslots) >> rshift;
+    const uint32_t p = atomicAdd(&fill[g], 1u);
+    if (p >> rshift) return;  // the region overflows: rowhash_region reports it
+    uint4* d = reinterpret_cast<uint4*>(&slots[(g << rshift) + p]);
+    d[0] = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)(w1 >> 32), hdr);
+    d[1] = make_uint4((uint32_t)pa, (uint32_t)(pa >> 32), (uint32_t)pb, (uint32_t)(pb >> 32));
+}
+constexpr int RH_THREADS = 256, RH_UNROLL = 2;  // staged images in flight per thread
+__global__ void __launch_bounds__(RH_THREADS) rowhash_region_kernel(RowSlot* slots, uint64_t nslots, uint64_t nregions, uint32_t rshift,
+                                                                    const uint32_t* __restrict__ fill, uint32_t* flags) {
+    extern __shared__ uint4 sm[];  // the region: 2 x uint4 per slot
+    const uint32_t rs = 1u << rshift, rmask = rs - 1;
+    for (uint64_t g = blockIdx.x; g < nregions; g += gridDim.x) {
+        const uint32_t cnt = fill[g];
+        if (cnt >= rs) {  // at most rs - 1 keys: a probe for a missing key must meet an empty slot
+            if (threadIdx.x == 0) flags[1] = 1u;
+            continue;
         }
-        if (ol == lo && (uint32_t)oh == (uint32_t)hi) { *dup = 1u; return; }  // benign race: every writer stores 1
-        if (++s == nslots) s = 0;
+        for (uint32_t i = threadIdx.x; i < 2 * rs; i += RH_THREADS) sm[i] = make_uint4(0, 0, 0, 0);
+        __syncthreads();
+        uint4* reg = reinterpret_cast<uint4*>(slots + (g << rshift));
+        for (uint32_t i0 = 0; i0 < cnt; i0 += RH_THREADS * RH_UNROLL) {
+            uint4 hd[RH_UNROLL], pay[RH_UNROLL];
+#pragma unroll
+            for (int u = 0; u < RH_UNROLL; u++) {
+                const uint32_t i = i0 + u * RH_THREADS + threadIdx.x;
+                if (i < cnt) { hd[u] = __ldcs(reg + 2 * i); pay[u] = __ldcs(reg + 2 * i + 1); }
+            }
+#pragma unroll
+            for (int u = 0; u < RH_UNROLL; u++) {
+                if (i0 + u * RH_THREADS + threadIdx.x >= cnt) break;
+                const unsigned long long lo = ((unsigned long long)hd[u].y << 32) | hd[u].x, hi = ((unsigned long long)hd[u].w << 32) | hd[u].z;
+                uint32_t s = (uint32_t)slot_of(hash3(lo, (unsigned long long)hd[u].z << 32, 0ull), nslots) & rmask;
+                for (;;) {
+                    unsigned long long ol, oh;
+                    cas128_shared(&sm[2 * s], lo, hi, ol, oh);
+                    if ((ol | oh) == 0ull) { sm[2 * s + 1] = pay[u]; break; }
+                    if (ol == lo && (uint32_t)oh == (uint32_t)hi) { flags[0] = 1u; break; }  // benign race: every writer stores 1
+                    s = (s + 1) & rmask;
+                }
+            }
+        }
+        __syncthreads();  // every staged image is read: the region is written over them
+        for (uint32_t i = threadIdx.x; i < 2 * rs; i += RH_THREADS) __stcs(reg + i, sm[i]);
+        __syncthreads();
     }
 }
-bool rowhash_build(Ctx* c, Index& ix) {
+RhBuild rowhash_build(Ctx* c, Index& ix) {
     RowHash& rh = ix.rowhash;
     const uint64_t n = (uint64_t)ix.nrows;
     const Table& t = *ix.src;
@@ -371,25 +413,45 @@ bool rowhash_build(Ctx* c, Index& ix) {
     PayCols pc{};
     pc.nc = (int)rh.cols.size();
     for (int j = 0; j < pc.nc; j++) { pc.off[j] = t.cols[rh.cols[j]].off(); pc.data[j] = t.cols[rh.cols[j]].bytes(); }
+    // at least 2n + 16 slots (load factor about 1/2) in whole regions; a table smaller than RH_REGION is one region
+    const uint64_t want = n * 2 + 16;
+    uint32_t rshift = 0;
+    while ((1ull << rshift) < want && (1u << rshift) < RH_REGION) rshift++;
+    rh.region = 1u << rshift;
+    const uint64_t nregions = (want + rh.region - 1) >> rshift;
+    rh.nslots = nregions << rshift;
     rh.slots = dev_alloc(c, rh.nslots * sizeof(RowSlot));
-    Buf dup = dev_alloc(c, 8);
-    CPB_CUDA(cudaMemsetAsync(dup->p, 0, 8, c->stream));
-    CPB_CUDA(cudaMemsetAsync(rh.slots->p, 0, rh.nslots * sizeof(RowSlot), c->stream));
+    Buf fill = dev_alloc(c, nregions * 4), flags = dev_alloc(c, 8);
+    CPB_CUDA(cudaMemsetAsync(fill->p, 0, nregions * 4, c->stream));
+    CPB_CUDA(cudaMemsetAsync(flags->p, 0, 8, c->stream));
     {
-        KernelTimer kt(c, "rowhash_build", n * ((uint64_t)kd.words * 8 + RH_PAY + 4 * (uint64_t)(kd.nkeys + pc.nc)) + rh.nslots * sizeof(RowSlot));
-        rowhash_insert_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(kd, pc, n, rh.slots->as<RowSlot>(), rh.nslots, dup->as<uint32_t>());
+        KernelTimer kt(c, "rowhash_scatter", n * ((uint64_t)kd.words * 8 + RH_PAY + 4 * (uint64_t)(kd.nkeys + pc.nc) + sizeof(RowSlot)));
+        rowhash_scatter_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(kd, pc, n, rh.slots->as<RowSlot>(), rh.nslots, rshift, fill->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
-    return read_back<uint32_t>(c, dup->p) != 0;
+    {
+        KernelTimer kt(c, "rowhash_build", n * sizeof(RowSlot) + rh.nslots * sizeof(RowSlot));
+        const size_t smem = (size_t)rh.region * sizeof(RowSlot);
+        // (per device, and cheap: set on every launch rather than cached per process)
+        CPB_CUDA(cudaFuncSetAttribute(rowhash_region_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = 0;
+        CPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rowhash_region_kernel, RH_THREADS, smem));
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(nregions, (uint64_t)c->sm_count * std::max(per_sm, 1));
+        rowhash_region_kernel<<<grid, RH_THREADS, smem, c->stream>>>(rh.slots->as<RowSlot>(), rh.nslots, nregions, rshift, fill->as<uint32_t>(),
+                                                                     flags->as<uint32_t>());
+        CPB_CUDA(cudaGetLastError());
+    }
+    const uint64_t f = read_back<uint64_t>(c, flags->p);
+    return (uint32_t)f ? RhBuild::duplicate : (f >> 32) ? RhBuild::overflow : RhBuild::built;
 }
 // flag[i] = whether probe row i finds its key (want 1) / finds nothing (want 0): the slot headers only
 __global__ void __launch_bounds__(256) rowhash_flags_kernel(KeyDesc kd, uint64_t np, const RowSlot* __restrict__ slots, uint64_t nslots,
-                                                            uint32_t want, uint32_t* flag) {
+                                                            uint64_t rmask, uint32_t want, uint32_t* flag) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
         unsigned long long k0; uint32_t k1;
         uint64_t s = rh_start(kd, i, nslots, k0, k1);
         uint4 h = rh_header(slots, s);
-        flag[i] = rh_walk(slots, nslots, k0, k1, s, h) == (want != 0) ? 1u : 0u;
+        flag[i] = rh_walk(slots, rmask, k0, k1, s, h) == (want != 0) ? 1u : 0u;
     }
 }
 static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, const Index& ix, bool want) {
@@ -399,7 +461,8 @@ static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pid
     Buf flag = dev_alloc(c, np * 4);
     KernelTimer kt(c, "rowhash_flags", np * ((uint64_t)kd.words * 8 + 4 * (uint64_t)kd.nkeys + 16 + 4));
     const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-    rowhash_flags_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ix.rowhash.slots->as<RowSlot>(), ix.rowhash.nslots, want ? 1u : 0u, flag->as<uint32_t>());
+    rowhash_flags_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ix.rowhash.slots->as<RowSlot>(), ix.rowhash.nslots, ix.rowhash.region - 1ull,
+                                                       want ? 1u : 0u, flag->as<uint32_t>());
     CPB_CUDA(cudaGetLastError());
     return flag;
 }

@@ -1,6 +1,6 @@
 // rowhash.cuh — device-side key hashing shared by the probe tables (join.cu) and the row-carrying hash table's fused
-// probe / length scan (gather.cu): the probe key packed in registers, its hash, the 128-bit slot claim, and the
-// 32-byte row-carrying slot.
+// probe / length scan (gather.cu): the probe key packed in registers, its hash, the 128-bit slot claims (global and
+// shared memory), and the 32-byte row-carrying slot with its region-wrapped probe sequence.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -62,15 +62,25 @@ __device__ __forceinline__ void cas128(void* addr, unsigned long long vl, unsign
     asm volatile("{\n.reg .b128 c, v, o;\nmov.b128 c, {%3, %4};\nmov.b128 v, {%5, %6};\natom.global.cas.b128 o, [%2], c, v;\nmov.b128 {%0, %1}, o;\n}"
                  : "=l"(ol), "=l"(oh) : "l"(addr), "l"(0ull), "l"(0ull), "l"(vl), "l"(vh) : "memory");
 }
+// the same claim on a shared-memory slot (SASS ATOMS.CAS.128)
+__device__ __forceinline__ void cas128_shared(void* addr, unsigned long long vl, unsigned long long vh, unsigned long long& ol, unsigned long long& oh) {
+    const uint32_t a = (uint32_t)__cvta_generic_to_shared(addr);
+    asm volatile("{\n.reg .b128 c, v, o;\nmov.b128 c, {%3, %4};\nmov.b128 v, {%5, %6};\natom.shared.cas.b128 o, [%2], c, v;\nmov.b128 {%0, %1}, o;\n}"
+                 : "=l"(ol), "=l"(oh) : "r"(a), "l"(0ull), "l"(0ull), "l"(vl), "l"(vh) : "memory");
+}
 
 // ------------------------------------------------------------------ row-carrying slot (Index::rowhash)
-// One 32-byte slot = one DRAM sector: a 16-byte header {12 key bytes, hdr} claimed by cas128, then the payload columns'
-// values back to back.  hdr = RH_OCCUPIED | length of payload column j in bits 5j..5j+4 (a value is at most 16 bytes):
-// the occupied bit keeps the header of an empty key (an all-zero image) from reading as an empty slot.
+// One 32-byte slot = one DRAM sector: a 16-byte header {12 key bytes, hdr}, then the payload columns' values back to
+// back.  hdr = RH_OCCUPIED | length of payload column j in bits 5j..5j+4 (a value is at most 16 bytes): the occupied
+// bit keeps the header of an empty key (an all-zero image) from reading as an empty slot.
 struct __align__(32) RowSlot { unsigned long long k0; uint32_t k1; uint32_t hdr; uint4 pay; };
 constexpr uint32_t RH_OCCUPIED = 0x80000000u;
 constexpr int RH_MAXC = 4;         // payload columns
 constexpr uint32_t RH_PAY = 16;    // payload bytes
+// The table is cut into regions of RowHash::region slots (a power of two, RH_REGION for all but small tables): a key's
+// probe sequence starts at slot_of(hash, nslots) and wraps from its region's last slot to the region's first, so each
+// region is built on its own in shared memory (join.cu: rowhash_build).
+constexpr uint32_t RH_REGION = 1024;
 
 // the packed key of probe row r (12 bytes: k0, k1) and the first slot of its probe sequence
 __device__ __forceinline__ uint64_t rh_start(const KeyDesc& kd, uint64_t r, uint64_t nslots, unsigned long long& k0, uint32_t& k1) {
@@ -80,12 +90,15 @@ __device__ __forceinline__ uint64_t rh_start(const KeyDesc& kd, uint64_t r, uint
     return slot_of(hash3(w0, w1, 0ull), nslots);
 }
 __device__ __forceinline__ uint4 rh_header(const RowSlot* slots, uint64_t s) { return __ldg(reinterpret_cast<const uint4*>(&slots[s])); }
-// linear probing from slot s, whose header h is loaded: true when the key is found, s and h then are its slot's
-__device__ __forceinline__ bool rh_walk(const RowSlot* slots, uint64_t nslots, unsigned long long k0, uint32_t k1, uint64_t& s, uint4& h) {
+// the slot after s in s's region (rmask = region - 1)
+__device__ __forceinline__ uint64_t rh_next(uint64_t s, uint64_t rmask) { return (s & ~rmask) | ((s + 1) & rmask); }
+// linear probing from slot s, whose header h is loaded, inside s's region: true when the key is found, s and h then are
+// its slot's
+__device__ __forceinline__ bool rh_walk(const RowSlot* slots, uint64_t rmask, unsigned long long k0, uint32_t k1, uint64_t& s, uint4& h) {
     for (;;) {
         if (h.w == 0u) return false;
         if (h.x == (uint32_t)k0 && h.y == (uint32_t)(k0 >> 32) && h.z == k1) return true;
-        if (++s == nslots) s = 0;
+        s = rh_next(s, rmask);
         h = rh_header(slots, s);
     }
 }

@@ -387,14 +387,19 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
     Buf img;  // image of the unsorted rows
     if (lazy) {
         ix->src = tp; ix->nrows = (int64_t)n; ix->sorted = false; ix->unique = true;
+        bool dup_seen = false;
         if (kbytes <= 12 && (int)pay.size() <= RH_MAXC && pay_max <= RH_PAY) {
             // key, lengths and payload fit one 32-byte slot: the row-carrying table is the index's probe structure (and
-            // its insert the duplicate check); no key image until something needs the order
+            // its build the duplicate check); no key image until something needs the order
             ix->rowhash.cols = pay;
-            ix->rowhash.nslots = n * 2 + 16;
-            if (!rowhash_build(c, *ix)) return ix;
+            const RhBuild rb = rowhash_build(c, *ix);
+            if (rb == RhBuild::built) return ix;
             ix->rowhash = RowHash{};
-        } else {
+            dup_seen = rb == RhBuild::duplicate;
+        }
+        // no row-carrying table, or one of its regions overflowed (keys crafted to collide): a probe table over the key
+        // image in source order and the row slots, exact for any input
+        if (!dup_seen) {
             img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &ix->image_words);
             ix->uimage = img;
             if (!index_has_duplicates(c, *ix)) return ix;
