@@ -86,9 +86,6 @@ struct Table {
     }
 };
 
-// csvplus Index (csvplus.go:610-614, :785-788): rows sorted on `key_cols`.  `table` holds the
-// rows physically in sorted order.  `image` is the order-preserving fixed-width key image
-// (sort.cu) of the sorted rows; `hash*` is the probe table over distinct full keys / key prefixes.
 // "Built on some context's stream": what several contexts may use (the lazily built structures of an index) carries the
 // event recorded after its last kernel; a user makes its own stream wait for it — no host synchronisation.
 struct ReadyEvent {
@@ -97,20 +94,25 @@ struct ReadyEvent {
 };
 using Ready = std::shared_ptr<ReadyEvent>;
 
-struct HashTable {
+// The order of the index rows that probe tables and row slots refer to: sorted (ix.image, ix.perm / ix.table) or as
+// given (ix.derived.uimage, ix.src: a lazily sorted unique index)
+enum class RowOrder { sorted, source };
+
+// Probe table over the runs of equal prefixes of the first nk key columns (join.cu); run j = rows [heads[j], heads[j+1]).
+// smem / global: uint32 slots holding j (0xFFFFFFFF = empty, linear probing), the key compared with the key image at
+// heads[j]; smem when slots + heads fit 200 KB of shared memory.  unique16: 16-byte slots {12 key bytes, row + 1}, every
+// run one row.  run32: 32-byte slots {24 key bytes, first row | run length << 32}.
+struct ProbeTable {
+    enum class Kind { smem, global, unique16, run32 };
+    Kind kind = Kind::smem;
     Ready ready;
-    int nkeys = 0;           // number of leading key columns hashed
-    uint32_t pbytes = 0;     // image bytes those columns cover
-    uint64_t nslots = 0;     // power of two
-    uint64_t nheads = 0;     // distinct key prefixes
-    Buf slots;               // uint32 head ordinal or 0xFFFFFFFF (open addressing, linear probing)
-    Buf heads;               // uint32[nheads+1]: sorted position of each distinct prefix; heads[nheads] = nrows
-    uint64_t nslots32 = 0;   // embedded-key table (prefix <= 24 bytes, table too large for shared memory)
-    Buf slots32;             // 32-byte slots: 3 key words + (first row | run length << 32)
-    uint64_t nslots16 = 0;   // unique keys with prefix <= 12 bytes: 16-byte slots (12 key bytes + row + 1)
-    Buf slots16;
+    uint32_t pbytes = 0;     // image bytes of the prefix
+    uint64_t nslots = 0;     // slots of `kind`
+    Buf slots;
+    uint64_t nheads = 0;     // runs
+    Buf heads;               // uint32[nheads+1]; heads[nheads] = nrows
 };
-// Row slots (gather.cu): the output columns of the sorted rows re-laid as one fixed-size slot per row (their
+// Row slots (gather.cu): the output columns of the index rows re-laid as one fixed-size slot per row (their
 // bytes back to back) + one packed word of lengths per row, so that a join fetches an index row with ONE random
 // access instead of two per column.  Built lazily per set of output columns when every value is short.
 struct RowSlots {
@@ -133,6 +135,7 @@ struct RowHash {
     Buf slots;              // RowSlot[nslots]; null = the index has no row-carrying table
     std::vector<int> cols;  // payload: every non-key column of the source, in schema order
 };
+// csvplus Index (csvplus.go:610-614, :785-788): rows sorted on `key_cols`.
 struct Index {
     Ctx* ctx = nullptr;
     // The sorted rows exist in two forms.  A join needs neither the sorted columns nor their offsets: it probes the
@@ -144,15 +147,9 @@ struct Index {
     int64_t nrows = 0;
     std::shared_ptr<Table> table;      // sorted rows (lazily materialised, under `mu`)
     // A UNIQUE index whose duplicate check passed is not even sorted until something needs the order (iteration, Find,
-    // SubIndex, a prefix join, dedup): a full-key join only needs "key -> row", which the hash table built over the rows
-    // in SOURCE order gives (and that build doubles as the duplicate check: every key must find itself).  `uimage` is the
-    // key image in source order; `sorted` tells whether perm / image (sorted order) exist yet (ensure_sorted()).  An index
-    // with a row-carrying table has no uimage: the sort packs the image when it first needs it.
-    Buf uimage;
-    RowHash rowhash;
+    // SubIndex, a prefix join, dedup): a full-key join only needs "key -> row".  `sorted` tells whether perm / image
+    // exist yet (ensure_sorted()).
     bool sorted = true;
-    std::map<int, HashTable> hash_src;                   // probe tables over the source order (payload = source row)
-    std::map<std::vector<int>, RowSlots> row_slots_src;  // row slots in source order (filled sequentially, no permutation)
     const Table& schema() const { return table ? *table : *src; }  // column names / count only
     bool unique = false;               // built by UniqueIndexOn and verified: every full key occurs once
     // false when the stored rows are not in key order (ResolveDuplicates with replacement rows, LoadIndex of such a file):
@@ -162,9 +159,17 @@ struct Index {
     std::vector<int> key_col_idx;      // positions in table->cols
     std::vector<uint32_t> key_width;   // per key column: max value length (bytes) in this index
     uint32_t image_words = 0;          // uint64 words per row of the key image
-    Buf image;                         // uint64[image_words][nrows] (word-major / SoA)
-    std::map<int, HashTable> hash;     // by number of leading key columns (built lazily, under `mu`)
-    std::map<std::vector<int>, RowSlots> row_slots;  // by output column set (built lazily, under `mu`)
+    Buf image;                         // uint64[image_words][nrows] (word-major / SoA): key image of the sorted rows
+    // Built from the stored rows and dropped together by whatever replaces them (reset_derived()).  uimage: the key
+    // image in source order of a unique index without a row-carrying table; the full-key probe table over it is the
+    // duplicate check (every key must find itself) and serves full-key joins (join_order(), join.cu).
+    struct Derived {
+        Buf uimage;
+        RowHash rowhash;
+        std::map<std::pair<RowOrder, int>, ProbeTable> probe;                // by (order, leading key columns)
+        std::map<std::pair<RowOrder, std::vector<int>>, RowSlots> row_slots;  // by (order, output columns)
+    } derived;                         // (the maps are filled lazily, under `mu`)
+    void reset_derived() { derived = Derived{}; }
     std::mutex mu;                     // several contexts may probe one index concurrently
 };
 
@@ -297,11 +302,11 @@ std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_i
 std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred);
 int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred);
 Column materialize(Ctx* c, const Column& col, int64_t nrows);  // view -> own compact buffers
-// rows `ids` of the index's sorted table restricted to columns `cols` (row-slot path when it pays, else gather_rows)
+// rows `ids` (positions in `order`) of the index restricted to columns `cols` (row-slot path when it pays, else gather_rows)
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout,
-                                         bool by_src = false);
+                                         RowOrder order);
 std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& parts);
-// full-key join against ix.rowhash: payload columns `cols` (source column numbers, a non-empty subset of ix.rowhash.cols)
+// full-key join against ix.derived.rowhash: payload columns `cols` (source column numbers, a non-empty subset of its cols)
 // for every probe row, empty where the row finds no key; *matches = probe rows that found their key.  One random access
 // and one host synchronisation.
 std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, const std::vector<int>& pidx, const std::vector<int>& cols,
@@ -320,6 +325,8 @@ struct KeyDesc {  // key columns + the widths of the order-preserving image (sor
     uint32_t lenbytes[MAXKEYS];  // bytes of the big-endian length field
     uint32_t words;              // image words per row
 };
+// bytes of the big-endian length field after a key column of `width` value bytes in the key image
+inline uint32_t len_field_bytes(uint32_t width) { return width < 255 ? 1 : (width < 65535 ? 2 : 4); }
 void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, KeyDesc& kd);
 uint32_t prefix_bytes(const Index& ix, int nk);  // image bytes covered by the first nk key columns
 // head[i] = 1 when the first pbytes image bytes of row i differ from those of row i - 1 (row 0 always)
@@ -330,7 +337,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
                                    bool anti, DataError* derr, bool* failed);
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi);
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
-// fills ix.rowhash (cols set by the caller) from ix.src.  built: the table is complete; duplicate: some key occurs twice;
+// fills ix.derived.rowhash (cols set by the caller) from ix.src.  built: the table is complete; duplicate: some key occurs twice;
 // overflow: some region received more keys than it can hold (no duplicate was seen, but the table is unusable)
 enum class RhBuild { built, duplicate, overflow };
 RhBuild rowhash_build(Ctx* c, Index& ix);

@@ -596,14 +596,15 @@ __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t*
     }
 }
 
-static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& cols, bool by_src) {
+static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& cols, RowOrder order) {
     std::lock_guard<std::mutex> lk(ix.mu);
-    auto& smap = by_src ? ix.row_slots_src : ix.row_slots;
-    auto it = smap.find(cols);
+    auto& smap = ix.derived.row_slots;
+    auto it = smap.find({order, cols});
     if (it != smap.end()) { wait_ready(c, it->second.ready); return it->second; }
     RowSlots rs;
-    // by_src: slot r = source row r (filled sequentially); else sorted order: the sorted rows if they exist, else the source
-    // rows through the permutation
+    // source order: slot r = source row r (filled sequentially); sorted order: the sorted rows if they exist, else the
+    // source rows through the permutation
+    const bool by_src = order == RowOrder::source;
     const Table& t = by_src ? *ix.src : (ix.table ? *ix.table : *ix.src);
     const uint32_t* perm = (by_src || ix.table) ? nullptr : ix.perm->as<uint32_t>();
     const uint64_t n = (uint64_t)ix.nrows;
@@ -631,7 +632,7 @@ static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& col
         }
     }
     rs.ready = record_ready(c);  // another context (stream) that finds it in the map waits for this event, not the host
-    return smap.emplace(cols, std::move(rs)).first->second;
+    return smap.emplace(std::make_pair(order, cols), std::move(rs)).first->second;
 }
 
 // Columns `names` of n rows from slots of S bytes: the offsets scanned from the packed lengths `src` gives
@@ -686,27 +687,26 @@ static std::vector<Column> slot_gather(Ctx* c, const std::vector<std::string>& n
     return out;
 }
 
-std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, bool by_src) {
+std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, RowOrder order) {
     if (cols.empty()) {  // nothing to gather (a join whose index columns are all key columns): no slots, no sorted rows
         auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = ix.schema().first_line;
         return r;
     }
     auto plain = [&]() {  // per-column gather: from the source rows (ids = source rows), or from the physically sorted rows
-        std::shared_ptr<Table> keep = by_src ? ix.src : sorted_table(c, ix);
+        std::shared_ptr<Table> keep = order == RowOrder::source ? ix.src : sorted_table(c, ix);
         const Table& st = *keep;
         Table sub; sub.ctx = c; sub.nrows = st.nrows; sub.first_line = st.first_line;
         for (int ci : cols) sub.cols.push_back(st.cols[ci]);
         return gather_rows(c, sub, ids, nout);
     };
-    static const bool disabled = getenv("CPB_NO_ROWSLOTS") != nullptr;
-    bool use = !disabled && ids != nullptr && nout > 0 && !cols.empty() && cols.size() <= (size_t)RS_MAXC;
+    bool use = ids != nullptr && nout > 0 && cols.size() <= (size_t)RS_MAXC;
     if (use) {
         bool built;
-        { std::lock_guard<std::mutex> lk(ix.mu); built = (by_src ? ix.row_slots_src : ix.row_slots).count(cols) != 0; }
+        { std::lock_guard<std::mutex> lk(ix.mu); built = ix.derived.row_slots.count({order, cols}) != 0; }
         if (!built && nout < ix.nrows) use = false;  // laying the slots out costs about one gather of the whole index
     }
     if (!use) return plain();
-    RowSlots& rs = ensure_row_slots(c, ix, cols, by_src);
+    RowSlots& rs = ensure_row_slots(c, ix, cols, order);
     if (!rs.usable) return plain();
     const Table& t = ix.schema();
     std::vector<std::string> names;
@@ -720,7 +720,7 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
 
 std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, const std::vector<int>& pidx, const std::vector<int>& cols,
                                       uint64_t* matches) {
-    const RowHash& rh = ix.rowhash;
+    const RowHash& rh = ix.derived.rowhash;
     const Table& t = ix.schema();
     const uint64_t np = (uint64_t)probe.nrows;
     KeyDesc kd{};

@@ -182,19 +182,40 @@ __global__ void iota_heads_kernel(uint32_t* heads, uint64_t n) {  // heads[i] = 
     if (i <= n) heads[i] = (uint32_t)i;
 }
 
-// by_src: the table is built over the rows in SOURCE order (a lazily sorted unique index: payload = source row, key
-// image = ix.uimage); otherwise over the sorted order (payload = sorted position, key image = ix.image).
-static HashTable& ensure_hash(Ctx* c, Index& ix, int nk, bool by_src, uint32_t* dup_flag = nullptr) {
+// The order a join on the first nk key columns uses: a lazily sorted unique index joined on its full key is probed
+// over the rows as they were given (no sort needed); everything else over the sorted rows.
+static RowOrder join_order(const Index& ix, int nk) {
+    return ix.unique && ix.derived.uimage && nk == (int)ix.key_cols.size() ? RowOrder::source : RowOrder::sorted;
+}
+static const Buf& key_image(const Index& ix, RowOrder order) { return order == RowOrder::source ? ix.derived.uimage : ix.image; }
+
+// ordinal slots for nheads runs: a power of two, load factor at most 1/2
+static uint64_t ordinal_slots(uint64_t nheads) {
+    const uint64_t want = std::max<uint64_t>(16, nheads * 2);
+    uint64_t s = 1;
+    while (s < want) s <<= 1;
+    return s;
+}
+static ProbeTable::Kind probe_kind(uint64_t nheads, uint32_t pbytes, uint64_t nrows) {
+    if ((ordinal_slots(nheads) + nheads + 1) * 4 <= 200 * 1024) return ProbeTable::Kind::smem;
+    if (pbytes <= 12 && nheads == nrows) return ProbeTable::Kind::unique16;
+    if (pbytes <= 24) return ProbeTable::Kind::run32;
+    return ProbeTable::Kind::global;
+}
+
+// The probe table over the first nk key columns of the rows in `order` (payload = position in that order).  dup_flag,
+// when given, is set by a unique16 insert that meets a key twice.
+static ProbeTable& ensure_hash(Ctx* c, Index& ix, RowOrder order, int nk, uint32_t* dup_flag = nullptr) {
     std::lock_guard<std::mutex> lk(ix.mu);
-    auto& hmap = by_src ? ix.hash_src : ix.hash;
-    const Buf& image = by_src ? ix.uimage : ix.image;
-    auto it = hmap.find(nk);
-    if (it != hmap.end()) { wait_ready(c, it->second.ready); return it->second; }
-    HashTable ht;
-    ht.nkeys = nk; ht.pbytes = prefix_bytes(ix, nk);
+    auto& tables = ix.derived.probe;
+    const Buf& image = key_image(ix, order);
+    auto it = tables.find({order, nk});
+    if (it != tables.end()) { wait_ready(c, it->second.ready); return it->second; }
+    ProbeTable ht;
+    ht.pbytes = prefix_bytes(ix, nk);
     const uint64_t n = (uint64_t)ix.nrows;
     if (ix.unique && nk == (int)ix.key_cols.size()) {
-        // a verified unique index probed on its full key: every sorted row is its own run — no adjacent compare, no scan,
+        // a verified unique index probed on its full key: every row is its own run — no adjacent compare, no scan,
         // no host round trip for the number of distinct keys
         ht.nheads = n;
         ht.heads = dev_alloc_owned(ix.ctx, c, (n + 1) * 4);
@@ -212,74 +233,60 @@ static HashTable& ensure_hash(Ctx* c, Index& ix, int nk, bool by_src, uint32_t* 
         ht.heads = dev_alloc_owned(ix.ctx, c, (ht.nheads + 1) * 4);
         compact_flags(c, s, 0, ht.heads->as<uint32_t>());  // heads[nheads] = nrows: the end of the last run
     }
-    uint64_t want = std::max<uint64_t>(16, ht.nheads * 2);
-    ht.nslots = 1; while (ht.nslots < want) ht.nslots <<= 1;
-    // one of three probe tables: ordinal slots (+ heads + key image; shared-memory sized or wide keys), or the
-    // embedded-key 16 / 32 byte slots
-    const bool large = (ht.nslots + ht.nheads + 1) * 4 > 200 * 1024;
-    if (!(large && ht.pbytes <= 24)) {
-        ht.slots = dev_alloc_owned(ix.ctx, c, ht.nslots * 4);
-        CPB_CUDA(cudaMemsetAsync(ht.slots->p, 0xff, ht.nslots * 4, c->stream));
-        KernelTimer kt(c, "hash_build", ht.nheads * (ht.pbytes + 8));
-        hash_insert_kernel<<<nblk(ht.nheads, 256), 256, 0, c->stream>>>(image->as<uint64_t>(), n, ht.pbytes, ht.heads->as<uint32_t>(), ht.nheads,
-                                                                        ht.slots->as<uint32_t>(), ht.nslots - 1);
-        CPB_CUDA(cudaGetLastError());
-    }
-    const bool too_large_for_smem = (ht.nslots + ht.nheads + 1) * 4 > 200 * 1024;
-    if (ht.pbytes <= 12 && ht.nheads == n && too_large_for_smem) {  // unique short keys: 16-byte slots
-        ht.nslots16 = ht.nheads * 2 + 16;
-        ht.slots16 = dev_alloc_owned(ix.ctx, c, ht.nslots16 * sizeof(Slot16));
-        CPB_CUDA(cudaMemsetAsync(ht.slots16->p, 0, ht.nslots16 * sizeof(Slot16), c->stream));
-        KernelTimer kt(c, "hash_build", ht.nheads * (ht.pbytes + 8) + ht.nslots16 * 16);
-        hash16_insert_kernel<<<nblk(ht.nheads, 256), 256, 0, c->stream>>>(image->as<uint64_t>(), n, ht.pbytes, ht.heads->as<uint32_t>(), ht.nheads,
-                                                                          ht.slots16->as<Slot16>(), ht.nslots16, dup_flag);
-        CPB_CUDA(cudaGetLastError());
-    } else if (ht.pbytes <= 24 && too_large_for_smem) {  // key fits a sector
-        ht.nslots32 = ht.nheads + ht.nheads / 2 + 16;
-        ht.slots32 = dev_alloc_owned(ix.ctx, c, ht.nslots32 * sizeof(Slot32));
-        CPB_CUDA(cudaMemsetAsync(ht.slots32->p, 0, ht.nslots32 * sizeof(Slot32), c->stream));
-        KernelTimer kt(c, "hash_build", ht.nheads * (ht.pbytes + 8) + ht.nslots32 * 32);
-        hash32_insert_kernel<<<nblk(ht.nheads, 256), 256, 0, c->stream>>>(image->as<uint64_t>(), n, ht.pbytes, ht.heads->as<uint32_t>(), ht.nheads,
-                                                                          ht.slots32->as<Slot32>(), ht.nslots32);
+    ht.kind = probe_kind(ht.nheads, ht.pbytes, n);
+    const bool ordinal = ht.kind == ProbeTable::Kind::smem || ht.kind == ProbeTable::Kind::global, u16 = ht.kind == ProbeTable::Kind::unique16;
+    const size_t slot = ordinal ? 4 : u16 ? sizeof(Slot16) : sizeof(Slot32);
+    ht.nslots = ordinal ? ordinal_slots(ht.nheads) : u16 ? ht.nheads * 2 + 16 : ht.nheads + ht.nheads / 2 + 16;
+    ht.slots = dev_alloc_owned(ix.ctx, c, ht.nslots * slot);
+    CPB_CUDA(cudaMemsetAsync(ht.slots->p, ordinal ? 0xff : 0, ht.nslots * slot, c->stream));  // all slots empty
+    {
+        KernelTimer kt(c, "hash_build", ht.nheads * (ht.pbytes + 8) + (ordinal ? 0 : ht.nslots * slot));
+        const uint64_t* img = image->as<uint64_t>();
+        const uint32_t* heads = ht.heads->as<uint32_t>();
+        const uint32_t grid = nblk(ht.nheads, 256);
+        if (ordinal) hash_insert_kernel<<<grid, 256, 0, c->stream>>>(img, n, ht.pbytes, heads, ht.nheads, ht.slots->as<uint32_t>(), ht.nslots - 1);
+        else if (u16) hash16_insert_kernel<<<grid, 256, 0, c->stream>>>(img, n, ht.pbytes, heads, ht.nheads, ht.slots->as<Slot16>(), ht.nslots, dup_flag);
+        else hash32_insert_kernel<<<grid, 256, 0, c->stream>>>(img, n, ht.pbytes, heads, ht.nheads, ht.slots->as<Slot32>(), ht.nslots);
         CPB_CUDA(cudaGetLastError());
     }
     ht.ready = record_ready(c);  // another context (stream) that finds it in the map waits for this event, not the host
-    return hmap.emplace(nk, std::move(ht)).first->second;
+    return tables.emplace(std::make_pair(order, nk), std::move(ht)).first->second;
 }
 
-// per probe row the matching run [lo, lo+cnt) of index rows, through whichever probe table the index has for nk columns
-static void probe_dispatch(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, HashTable& ht, const Buf& iimage, int nk,
+// per probe row the matching run [lo, lo+cnt) of the index rows in `order`, through the probe table ht over nk columns
+static void probe_dispatch(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, const ProbeTable& ht, RowOrder order, int nk,
                            uint32_t* lo, uint32_t* cnt, uint32_t* not_one) {
     const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
     std::vector<uint32_t> widths(ix.key_width.begin(), ix.key_width.begin() + nk);
-    uint32_t pwords = 0;
-    Buf pimg;
-    if (!ht.slots32 && !ht.slots16) pimg = pack_with_widths(c, probe, pidx, widths, &pwords);
-    else pwords = (ht.pbytes + 7) / 8;
-    // algorithmic bytes (SURVEY §8d): probe keys once + build table once
-    uint64_t algo = np * ((uint64_t)pwords * 8 + 8) + ht.nslots * 4 + ht.nheads * ((uint64_t)ht.pbytes + 4);
-    size_t smem = (ht.nslots + ht.nheads + 1) * 4;
+    // the ordinal tables compare a packed probe image with the index's key image; the others pack the probe key in registers
+    const bool ordinal = ht.kind == ProbeTable::Kind::smem || ht.kind == ProbeTable::Kind::global;
+    uint32_t pwords = (ht.pbytes + 7) / 8;
+    KeyDesc kd{};
+    const Buf pimg = ordinal ? pack_with_widths(c, probe, pidx, widths, &pwords) : nullptr;
+    if (!ordinal) describe_keys(c, probe, pidx, widths, kd);
+    const uint64_t* pi = ordinal ? pimg->as<uint64_t>() : nullptr;
+    const uint64_t* ii = ordinal ? key_image(ix, order)->as<uint64_t>() : nullptr;
+    // algorithmic bytes (SURVEY §8d): probe keys once + build table once (counted as the ordinal table for every kind)
+    const uint64_t algo = np * ((uint64_t)pwords * 8 + 8) + ordinal_slots(ht.nheads) * 4 + ht.nheads * ((uint64_t)ht.pbytes + 4);
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
     KernelTimer kt(c, "join_probe", algo);
-    if (ht.slots16) {
-        KeyDesc kd{};
-        describe_keys(c, probe, pidx, widths, kd);
-        uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-        join_probe16_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ht.slots16->as<Slot16>(), ht.nslots16, lo, cnt, not_one);
-    } else if (ht.slots32) {
-        KeyDesc kd{};
-        describe_keys(c, probe, pidx, widths, kd);
-        uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-        join_probe32_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ht.slots32->as<Slot32>(), ht.nslots32, lo, cnt, not_one);
-    } else if (smem <= 200 * 1024) {
+    switch (ht.kind) {
+    case ProbeTable::Kind::smem:
         // (per device, and cheap: set on every launch rather than cached per process)
         CPB_CUDA(cudaFuncSetAttribute(join_probe_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count);
-        join_probe_kernel<true><<<grid, 256, smem, c->stream>>>(pimg->as<uint64_t>(), np, iimage->as<uint64_t>(), ni, ht.pbytes,
-                                                                ht.slots->as<uint32_t>(), ht.nslots, ht.heads->as<uint32_t>(), ht.nheads, lo, cnt, not_one);
-    } else {
-        uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-        join_probe_kernel<false><<<grid, 256, 0, c->stream>>>(pimg->as<uint64_t>(), np, iimage->as<uint64_t>(), ni, ht.pbytes,
-                                                              ht.slots->as<uint32_t>(), ht.nslots, ht.heads->as<uint32_t>(), ht.nheads, lo, cnt, not_one);
+        join_probe_kernel<true><<<(uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count), 256, (ht.nslots + ht.nheads + 1) * 4, c->stream>>>(
+            pi, np, ii, ni, ht.pbytes, ht.slots->as<uint32_t>(), ht.nslots, ht.heads->as<uint32_t>(), ht.nheads, lo, cnt, not_one);
+        break;
+    case ProbeTable::Kind::global:
+        join_probe_kernel<false><<<grid, 256, 0, c->stream>>>(pi, np, ii, ni, ht.pbytes, ht.slots->as<uint32_t>(), ht.nslots, ht.heads->as<uint32_t>(),
+                                                              ht.nheads, lo, cnt, not_one);
+        break;
+    case ProbeTable::Kind::unique16:
+        join_probe16_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ht.slots->as<Slot16>(), ht.nslots, lo, cnt, not_one);
+        break;
+    case ProbeTable::Kind::run32:
+        join_probe32_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ht.slots->as<Slot32>(), ht.nslots, lo, cnt, not_one);
+        break;
     }
     CPB_CUDA(cudaGetLastError());
 }
@@ -327,7 +334,7 @@ static void search_probe(Ctx* c, const Table& probe, const std::vector<int>& pid
     CPB_CUDA(cudaGetLastError());
 }
 
-// ------------------------------------------------------------------ row-carrying hash table (Index::rowhash)
+// ------------------------------------------------------------------ row-carrying hash table (Index::derived.rowhash)
 // Built region by region in two passes, so that no insert is a random read-modify-write of DRAM:
 //  1. rowhash_scatter, one thread per source row: the key packed straight from the key columns, the payload columns'
 //     lengths and bytes gathered in registers, and the row's slot image {k0, k1, hdr, payload} appended to its region's
@@ -405,7 +412,7 @@ __global__ void __launch_bounds__(RH_THREADS) rowhash_region_kernel(RowSlot* slo
     }
 }
 RhBuild rowhash_build(Ctx* c, Index& ix) {
-    RowHash& rh = ix.rowhash;
+    RowHash& rh = ix.derived.rowhash;
     const uint64_t n = (uint64_t)ix.nrows;
     const Table& t = *ix.src;
     KeyDesc kd{};
@@ -461,8 +468,8 @@ static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pid
     Buf flag = dev_alloc(c, np * 4);
     KernelTimer kt(c, "rowhash_flags", np * ((uint64_t)kd.words * 8 + 4 * (uint64_t)kd.nkeys + 16 + 4));
     const uint32_t grid = (uint32_t)std::min<uint64_t>(nblk(np, 256), (uint64_t)c->sm_count * 16);
-    rowhash_flags_kernel<<<grid, 256, 0, c->stream>>>(kd, np, ix.rowhash.slots->as<RowSlot>(), ix.rowhash.nslots, ix.rowhash.region - 1ull,
-                                                       want ? 1u : 0u, flag->as<uint32_t>());
+    const RowHash& rh = ix.derived.rowhash;
+    rowhash_flags_kernel<<<grid, 256, 0, c->stream>>>(kd, np, rh.slots->as<RowSlot>(), rh.nslots, rh.region - 1ull, want ? 1u : 0u, flag->as<uint32_t>());
     CPB_CUDA(cudaGetLastError());
     return flag;
 }
@@ -525,7 +532,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         r->first_line = probe.first_line;
         return r;
     };
-    if (ix.rowhash.slots && nk == (int)ix.key_cols.size()) {
+    if (ix.derived.rowhash.slots && nk == (int)ix.key_cols.size()) {
         // a unique index with a row-carrying table joined on its full key: one random access per probe row
         if (anti) {
             Buf miss = rowhash_flags(c, probe, pidx, ix, false);
@@ -558,17 +565,15 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     Buf lo = dev_alloc(c, np * 4), cnt = dev_alloc(c, (np + 1) * 4), flags = dev_alloc(c, 32);
     CPB_CUDA(cudaMemsetAsync(flags->p, 0, 32, c->stream));
     uint32_t* not_one = flags->as<uint32_t>() + 2;  // [0..1] = scan total
-    // a lazily sorted unique index joined on its full key: probe table and row slots over the source order
-    const bool by_src = ix.unique && ix.uimage && nk == (int)ix.key_cols.size();
-    if (ni != 0 && !by_src) ensure_sorted(c, ix);
-    const Buf& iimage = by_src ? ix.uimage : ix.image;
+    const RowOrder order = join_order(ix, nk);
+    if (ni != 0 && order == RowOrder::sorted) ensure_sorted(c, ix);
     if (ni == 0) {
         CPB_CUDA(cudaMemsetAsync(cnt->p, 0, (np + 1) * 4, c->stream));
     } else if (!ix.in_order) {
         search_probe(c, probe, pidx, ix, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
     } else {
-        HashTable& ht = ensure_hash(c, ix, nk, by_src);
-        probe_dispatch(c, probe, pidx, ix, ht, iimage, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
+        const ProbeTable& ht = ensure_hash(c, ix, order, nk);
+        probe_dispatch(c, probe, pidx, ix, ht, order, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
     }
     if (anti) {
         Buf flag = dev_alloc(c, np * 4);
@@ -583,7 +588,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     if (m > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "join result exceeds 2^32-2 rows; probe in smaller batches"};
     if (m == 0) return empty_result();
     if (probe_identity) {
-        auto gi = gather_index_rows(c, ix, gather_idx, lo->as<uint32_t>(), (int64_t)m, by_src);  // lo[i] is the single matching index row
+        auto gi = gather_index_rows(c, ix, gather_idx, lo->as<uint32_t>(), (int64_t)m, order);  // lo[i] is the single matching index row
         out->nrows = (int64_t)m;
         put_index_cols(*gi, [&](int k) { return probe.cols[pidx[k]]; });
         for (auto* p : pcols) out->cols.push_back(*p);
@@ -600,7 +605,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     }
     Table pt; pt.ctx = c; pt.nrows = (int64_t)np;
     for (auto* p : pcols) pt.cols.push_back(*p);
-    auto gi = gather_index_rows(c, ix, gather_idx, iid->as<uint32_t>(), (int64_t)m, by_src);
+    auto gi = gather_index_rows(c, ix, gather_idx, iid->as<uint32_t>(), (int64_t)m, order);
     auto gp = gather_rows(c, pt, pid->as<uint32_t>(), (int64_t)m);
     out->nrows = (int64_t)m;
     put_index_cols(*gi, [&](int k) { return gp->cols[pidx[k]]; });
@@ -621,11 +626,11 @@ bool index_has_duplicates(Ctx* c, Index& ix) {
     const int nk = (int)ix.key_cols.size();
     Buf flags = dev_alloc(c, 64);
     CPB_CUDA(cudaMemsetAsync(flags->p, 0, 64, c->stream));
-    HashTable& ht = ensure_hash(c, ix, nk, true, flags->as<uint32_t>() + 8);
-    if (ht.slots16)  // the 16-byte-slot insert saw every key it met twice: no self probe needed
+    const ProbeTable& ht = ensure_hash(c, ix, RowOrder::source, nk, flags->as<uint32_t>() + 8);
+    if (ht.kind == ProbeTable::Kind::unique16)  // the insert saw every key it met twice: no self probe needed
         return read_back<uint32_t>(c, flags->as<uint32_t>() + 8) != 0;
     Buf lo = dev_alloc(c, n * 4), cnt = dev_alloc(c, (n + 1) * 4);
-    probe_dispatch(c, *ix.src, ix.key_col_idx, ix, ht, ix.uimage, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags->as<uint32_t>() + 2);
+    probe_dispatch(c, *ix.src, ix.key_col_idx, ix, ht, RowOrder::source, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags->as<uint32_t>() + 2);
     {
         KernelTimer kt(c, "unique_check", n * 8);
         self_check_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(lo->as<uint32_t>(), cnt->as<uint32_t>(), n, flags->as<uint32_t>() + 8);
@@ -635,28 +640,15 @@ bool index_has_duplicates(Ctx* c, Index& ix) {
 }
 
 // ------------------------------------------------------------------ Index.Find: [lower, upper) of a key prefix
+// val: the key image of one row (the lookup values)
 __global__ void find_range_kernel(const uint64_t* __restrict__ image, uint64_t n, const uint64_t* __restrict__ val, uint32_t pbytes,
                                   unsigned long long* out) {
-    // compare row r's first pbytes with val: <0, 0, >0
-    auto cmp = [&](uint64_t r) {
-        uint32_t full = pbytes >> 3, rem = pbytes & 7;
-        for (uint32_t w = 0; w < full; w++) {
-            uint64_t a = image[(uint64_t)w * n + r], b = val[w];
-            if (a != b) return a < b ? -1 : 1;
-        }
-        if (rem) {
-            uint64_t m = ~0ull << (8 * (8 - rem));
-            uint64_t a = image[(uint64_t)full * n + r] & m, b = val[full] & m;
-            if (a != b) return a < b ? -1 : 1;
-        }
-        return 0;
-    };
     // in the reference's order (:882-888), which decides the result when the rows are not in key order (in_order):
     uint64_t i = 0, j = n;  // upper = sort.Search(n, row > val)
-    while (i < j) { uint64_t h = i + (j - i) / 2; if (cmp(h) <= 0) i = h + 1; else j = h; }
+    while (i < j) { uint64_t h = i + (j - i) / 2; if (prefix_cmp(image, n, h, val, 1, 0, pbytes) <= 0) i = h + 1; else j = h; }
     out[1] = i;
     j = i; i = 0;           // lower = sort.Search(upper, row >= val)
-    while (i < j) { uint64_t h = i + (j - i) / 2; if (cmp(h) < 0) i = h + 1; else j = h; }
+    while (i < j) { uint64_t h = i + (j - i) / 2; if (prefix_cmp(image, n, h, val, 1, 0, pbytes) < 0) i = h + 1; else j = h; }
     out[0] = i;
 }
 
@@ -665,23 +657,22 @@ void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64
     *lo = 0; *hi = 0;
     if (n == 0) return;
     ensure_sorted(c, ix);
-    // pack the lookup values on the host with the index's widths (a handful of bytes)
-    std::vector<uint8_t> img((size_t)ix.image_words * 8 + 8, 0);
-    size_t b = 0;
-    for (size_t k = 0; k < values.size(); k++) {
-        uint32_t w = ix.key_width[k], lb = w < 255 ? 1 : (w < 65535 ? 2 : 4);
-        for (uint32_t i = 0; i < w; i++) img[b++] = i < values[k].size() ? (uint8_t)values[k][i] : 0;
-        uint32_t lf = values[k].size() > w ? 0xffffffffu : (uint32_t)values[k].size();
-        for (int i = (int)lb - 1; i >= 0; i--) img[b++] = (lf >> (8 * i)) & 0xff;
-    }
-    std::vector<uint64_t> words(ix.image_words + 1, 0);
-    for (size_t w = 0; w < words.size() && w * 8 < img.size(); w++)
-        for (int i = 0; i < 8 && w * 8 + i < img.size(); i++) words[w] |= (uint64_t)img[w * 8 + i] << (8 * (7 - i));
-    Buf dv = dev_alloc(c, words.size() * 8), out = dev_alloc(c, 16);
-    CPB_CUDA(cudaMemcpyAsync(dv->p, words.data(), words.size() * 8, cudaMemcpyHostToDevice, c->stream));
+    // the lookup values as a one-row table: value k is column k, a view at row k of one offsets / bytes pair
+    std::vector<uint32_t> off(1, 0);
+    std::string bytes;
+    std::vector<int> kidx;
+    for (const std::string& v : values) { bytes += v; off.push_back((uint32_t)bytes.size()); kidx.push_back((int)kidx.size()); }
+    Buf doff = dev_alloc(c, off.size() * 4), dbytes = dev_alloc(c, bytes.size()), out = dev_alloc(c, 16);
+    CPB_CUDA(cudaMemcpyAsync(doff->p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    if (!bytes.empty()) CPB_CUDA(cudaMemcpyAsync(dbytes->p, bytes.data(), bytes.size(), cudaMemcpyHostToDevice, c->stream));
+    Table t; t.ctx = c; t.nrows = 1;
+    for (int k : kidx) t.cols.push_back(Column{"", doff, dbytes, k});
+    uint32_t words = 0;
+    const Buf val = pack_with_widths(c, t, kidx, std::vector<uint32_t>(ix.key_width.begin(), ix.key_width.begin() + kidx.size()), &words);
     {
         KernelTimer kt(c, "index_find", 0);
-        find_range_kernel<<<1, 1, 0, c->stream>>>(ix.image->as<uint64_t>(), n, dv->as<uint64_t>(), (uint32_t)b, (unsigned long long*)out->p);
+        find_range_kernel<<<1, 1, 0, c->stream>>>(ix.image->as<uint64_t>(), n, val->as<uint64_t>(), prefix_bytes(ix, (int)kidx.size()),
+                                                  (unsigned long long*)out->p);
         CPB_CUDA(cudaGetLastError());
     }
     const std::vector<uint64_t> h = read_back<uint64_t>(c, out->p, 2);

@@ -69,7 +69,7 @@ __device__ __forceinline__ void cas128_shared(void* addr, unsigned long long vl,
                  : "=l"(ol), "=l"(oh) : "r"(a), "l"(0ull), "l"(0ull), "l"(vl), "l"(vh) : "memory");
 }
 
-// ------------------------------------------------------------------ row-carrying slot (Index::rowhash)
+// ------------------------------------------------------------------ row-carrying slot (Index::derived.rowhash)
 // One 32-byte slot = one DRAM sector: a 16-byte header {12 key bytes, hdr}, then the payload columns' values back to
 // back.  hdr = RH_OCCUPIED | length of payload column j in bits 5j..5j+4 (a value is at most 16 bytes): the occupied
 // bit keeps the header of an empty key (an all-zero image) from reading as an empty slot.

@@ -226,7 +226,7 @@ void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const s
     for (int k = 0; k < kd.nkeys; k++) {
         kd.off[k] = t.cols[kidx[k]].off(); kd.data[k] = t.cols[kidx[k]].bytes();
         kd.width[k] = width[k];
-        kd.lenbytes[k] = width[k] < 255 ? 1 : (width[k] < 65535 ? 2 : 4);
+        kd.lenbytes[k] = len_field_bytes(width[k]);
         bytes += kd.width[k] + kd.lenbytes[k];
     }
     kd.words = (bytes + 7) / 8;
@@ -236,7 +236,7 @@ void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const s
 // bytes of the image covered by the first nk key columns
 uint32_t prefix_bytes(const Index& ix, int nk) {
     uint32_t b = 0;
-    for (int k = 0; k < nk; k++) b += ix.key_width[k] + (ix.key_width[k] < 255 ? 1 : (ix.key_width[k] < 65535 ? 2 : 4));
+    for (int k = 0; k < nk; k++) b += ix.key_width[k] + len_field_bytes(ix.key_width[k]);
     return b;
 }
 
@@ -313,7 +313,7 @@ static void ensure_sorted_locked(Ctx* c, Index& ix) {
     const uint64_t n = (uint64_t)ix.nrows;
     OwnerPool scope(c, ix.ctx);
     uint32_t words = ix.image_words;
-    const Buf uimg = ix.uimage ? ix.uimage : pack_with_widths(c, *ix.src, ix.key_col_idx, ix.key_width, &words);  // (row-carrying table)
+    const Buf uimg = ix.derived.uimage ? ix.derived.uimage : pack_with_widths(c, *ix.src, ix.key_col_idx, ix.key_width, &words);  // (row-carrying table)
     uint64_t traffic = 0;
     Buf perm = sort_by_image(c, uimg->as<uint64_t>(), ix.image_words, n, &traffic);
     Buf simg;
@@ -367,8 +367,7 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
         return ix;
     }
     if (n > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "an index holds at most 2^32-2 rows"};
-    static const bool eager = getenv("CPB_EAGER_SORT") != nullptr;
-    const bool lazy = unique && n >= 2 && !eager;
+    const bool lazy = unique && n >= 2;
     // 1. key widths; for a UniqueIndexOn with at most 4 other columns also their longest row: whether the row-carrying
     //    hash table can hold the index
     std::vector<int> pay;  // the non-key columns, in schema order
@@ -391,21 +390,21 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
         if (kbytes <= 12 && (int)pay.size() <= RH_MAXC && pay_max <= RH_PAY) {
             // key, lengths and payload fit one 32-byte slot: the row-carrying table is the index's probe structure (and
             // its build the duplicate check); no key image until something needs the order
-            ix->rowhash.cols = pay;
+            ix->derived.rowhash.cols = pay;
             const RhBuild rb = rowhash_build(c, *ix);
             if (rb == RhBuild::built) return ix;
-            ix->rowhash = RowHash{};
+            ix->derived.rowhash = RowHash{};
             dup_seen = rb == RhBuild::duplicate;
         }
         // no row-carrying table, or one of its regions overflowed (keys crafted to collide): a probe table over the key
         // image in source order and the row slots, exact for any input
         if (!dup_seen) {
             img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &ix->image_words);
-            ix->uimage = img;
+            ix->derived.uimage = img;
             if (!index_has_duplicates(c, *ix)) return ix;
         }
         // a duplicate exists: sort, so that the error names the key the reference would name (the lowest in sort order)
-        ix->unique = false; ix->sorted = true; ix->uimage = nullptr; ix->hash_src.clear(); ix->row_slots_src.clear();
+        ix->reset_derived(); ix->unique = false; ix->sorted = true;
     }
     if (!img) img = pack_with_widths(c, t, ix->key_col_idx, ix->key_width, &ix->image_words);
     // 3. stable LSD radix sort -> permutation
@@ -505,13 +504,13 @@ __global__ void order_check_kernel(const uint64_t* __restrict__ image, uint64_t 
 void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt) {
     const uint64_t m = (uint64_t)nt->nrows;
     nt->first_line = 0;
-    ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.uimage = nullptr; ix.sorted = true; ix.nrows = (int64_t)m; ix.unique = false;
+    ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.sorted = true; ix.nrows = (int64_t)m; ix.unique = false;
+    ix.reset_derived();
     for (size_t k = 0; k < ix.key_cols.size(); k++) ix.key_col_idx[k] = nt->find(ix.key_cols[k]);
     ix.key_width = key_widths(c, *nt, ix.key_col_idx, m);
     uint32_t words = 0;
     ix.image = pack_with_widths(c, *nt, ix.key_col_idx, ix.key_width, &words);
     ix.image_words = words;
-    ix.hash.clear(); ix.row_slots.clear(); ix.hash_src.clear(); ix.row_slots_src.clear(); ix.rowhash = RowHash{};
     ix.in_order = true;
     if (m >= 2 && words) {
         Buf flag = dev_alloc(c, 8);
@@ -585,8 +584,8 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
     nt = gather_rows(c, *ix.table, ids->as<uint32_t>(), (int64_t)m);
     Buf simg = gather_image(c, ix.image->as<uint64_t>(), ix.image_words, n, ids->as<uint32_t>(), m);
     nt->first_line = 0;
-    ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m;
-    ix.image = simg; ix.hash.clear(); ix.row_slots.clear(); ix.rowhash = RowHash{};
+    ix.table = nt; ix.src = nullptr; ix.perm = nullptr; ix.nrows = (int64_t)m; ix.image = simg;
+    ix.reset_derived();
 }
 
 }  // namespace cpb
