@@ -8,6 +8,12 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CPB_LIB", os.path.join(HERE, "libcsvplus_b200.so"))  # CPB_LIB: A/B builds of the same ABI
 
+# the header's limits (tests check that these equal its #defines)
+MAX_PARSE_COLS = 16  # CPB_MAX_PARSE_COLS
+PRED_MAX_TERMS = 32  # CPB_PRED_MAX_TERMS
+PRED_MAX_OPS = 64    # CPB_PRED_MAX_OPS
+PRED_MAX_DEPTH = 48  # CPB_PRED_MAX_DEPTH
+
 
 class Str(C.Structure):
     _fields_ = [("ptr", C.c_char_p), ("len", C.c_uint64)]

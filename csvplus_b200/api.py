@@ -289,7 +289,30 @@ class Predicate:
         return not self.kids[0](row)
 
     def lowerable(self) -> bool:
-        return all(isinstance(k, Predicate) and k.lowerable() for k in self.kids)
+        """True when the device compiles the tree: every node is a Predicate and the tree stays within the header's
+        CPB_PRED_MAX_* limits.  Terms are counted as if every Like key named a column (a missing one compiles to a constant
+        false), so a tree over missing columns may be declined where the device would have taken it.  A declined tree
+        is evaluated on host rows, as an opaque function is."""
+        terms = ops = 0
+
+        def walk(p, depth) -> bool:
+            nonlocal terms, ops
+            if not isinstance(p, Predicate) or depth > _abi.PRED_MAX_DEPTH:
+                return False
+            if p.op == 0:  # one term per pair, ANDed together
+                terms += len(p.match); ops += 2 * len(p.match) - 1
+                return True
+            if not p.kids:  # All() / Any(): a constant
+                ops += 1
+                return True
+            ops += 1 if p.op == 3 else len(p.kids) - 1
+            return all(walk(k, depth + 1) for k in p.kids)
+
+        return walk(self, 0) and terms <= _abi.PRED_MAX_TERMS and ops <= _abi.PRED_MAX_OPS
+
+    def columns(self) -> set:
+        """the distinct column names the tree's Like terms compare"""
+        return set(self.match).union(*(k.columns() for k in self.kids))
 
     def _c(self, keep: list) -> _abi.Pred:
         p = _abi.Pred()
@@ -1286,8 +1309,11 @@ class DataSource:
         carry: dict = {}
         if isinstance(s, Reader):
             pred = None
-            if ops and ops[0][0] == "filter" and isinstance(ops[0][1], Predicate) and ops[0][1].lowerable():
-                pred = ops.pop(0)[1]  # fused into the parse kernel
+            # fused into the parse kernel, which extracts the predicate's columns beside every group of output columns
+            # (CPB_MAX_PARSE_COLS at a time); a predicate over more columns filters the parsed table instead
+            if (ops and ops[0][0] == "filter" and isinstance(ops[0][1], Predicate) and ops[0][1].lowerable()
+                    and len(ops[0][1].columns()) < _abi.MAX_PARSE_COLS):
+                pred = ops.pop(0)[1]
             src = s._batches(pred)
             try:
                 for t, err, several in src:

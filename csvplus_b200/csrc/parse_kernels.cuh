@@ -429,6 +429,7 @@ struct SlowSink {
     bool emit;
     int next_slot = 0, cur = -1;
     uint32_t len = 0, present = 0, alive = 0, eq = 0;
+    uint32_t alive_before = 0;  // count: alive before the last put1, restored by unput (a retracted '\r' must not kill a term)
     uint32_t ulen[MAXSEL];
     uint8_t* dst[MAXSEL];
     uint32_t maxlen[MAXSEL];  // emit: value lengths known from pass 1 (a retracted '\r' must never be stored)
@@ -447,6 +448,7 @@ struct SlowSink {
     __device__ void put1(int c) {
         if (emit) { if (dst[cur] && len < maxlen[cur]) dst[cur][len] = (uint8_t)c; }
         else {
+            alive_before = alive;
             uint32_t m = alive;
             while (m) {
                 int t = __ffs(m) - 1; m &= m - 1;
@@ -455,7 +457,7 @@ struct SlowSink {
         }
         len++;
     }
-    __device__ void unput() { if (cur >= 0) len--; }
+    __device__ void unput() { if (cur >= 0) { len--; alive = alive_before; } }
     __device__ void end_field() {
         if (cur < 0) return;
         ulen[cur] = len; present |= 1u << cur;

@@ -9,8 +9,8 @@
 
 namespace cpb {
 
-constexpr int MAXTERMS = 32;
-constexpr int MAXOPS = 64;
+constexpr int MAXTERMS = CPB_PRED_MAX_TERMS;
+constexpr int MAXOPS = CPB_PRED_MAX_OPS;
 enum { OP_TERM = 0, OP_AND = 1, OP_OR = 2, OP_NOT = 3, OP_FALSE = 4, OP_TRUE = 5 };
 
 struct PredProg {
@@ -56,7 +56,7 @@ inline void compile_pred(const cpb_pred* p, const std::function<int(const std::s
         if (out.prog.nops >= MAXOPS) throw ArgError{CPB_ERR_UNSUPPORTED, "predicate too large"};
         out.prog.op[out.prog.nops] = op; out.prog.arg[out.prog.nops] = arg; out.prog.nops++;
     };
-    if (depth > 48) throw ArgError{CPB_ERR_UNSUPPORTED, "predicate too deep"};
+    if (depth > CPB_PRED_MAX_DEPTH) throw ArgError{CPB_ERR_UNSUPPORTED, "predicate too deep"};
     switch (p->op) {
         case CPB_PRED_LIKE: {
             if (p->n <= 0) throw ArgError{CPB_ERR_ARG, "empty match row in Like() predicate"};  // csvplus.go:1280-1282

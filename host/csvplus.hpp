@@ -106,7 +106,21 @@ struct Predicate {
             default: return fn(r);
         }
     }
-    bool lowerable() const { if (op < 0) return false; for (auto& k : kids) if (!k.lowerable()) return false; return true; }
+    // the device compiles the tree: no opaque function in it, within the CPB_PRED_MAX_* limits (every Like pair counted
+    // as a term); a declined tree runs on host rows
+    bool lowerable() const { int terms = 0, ops = 0; return fits(0, terms, ops) && terms <= CPB_PRED_MAX_TERMS && ops <= CPB_PRED_MAX_OPS; }
+    bool fits(int depth, int& terms, int& ops) const {
+        if (op < 0 || depth > CPB_PRED_MAX_DEPTH) return false;
+        if (op == CPB_PRED_LIKE) { terms += (int)match.size(); ops += 2 * (int)match.size() - 1; return true; }
+        ops += kids.empty() || op == CPB_PRED_NOT ? 1 : (int)kids.size() - 1;
+        for (auto& k : kids) if (!k.fits(depth + 1, terms, ops)) return false;
+        return true;
+    }
+    // the distinct columns the Like terms compare
+    void columns(std::vector<std::string>& out) const {
+        for (auto& kv : match) if (std::find(out.begin(), out.end(), kv.first) == out.end()) out.push_back(kv.first);
+        for (auto& k : kids) k.columns(out);
+    }
 };
 inline Predicate Like(const Row& match) {
     if (match.empty()) throw std::logic_error("empty match row in Like() predicate");
@@ -535,7 +549,11 @@ private:
             return fn(t, err, several) && !stop && !failed;
         };
         if (reader_) {
-            const Predicate* fused = (!ops_.empty() && ops_[0].kind == FILTER && ops_[0].pred.lowerable()) ? &ops_[0].pred : nullptr;
+            // a predicate over CPB_MAX_PARSE_COLS or more columns filters the parsed table instead of the parse
+            std::vector<std::string> pcols;
+            if (!ops_.empty() && ops_[0].kind == FILTER) ops_[0].pred.columns(pcols);
+            const Predicate* fused = (!ops_.empty() && ops_[0].kind == FILTER && ops_[0].pred.lowerable() && (int)pcols.size() < CPB_MAX_PARSE_COLS)
+                                         ? &ops_[0].pred : nullptr;
             if (fused) first = 1;
             reader_->batches(fused, apply);
         } else apply(*table_, nullptr, false);

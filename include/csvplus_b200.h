@@ -29,6 +29,10 @@ extern "C" {
 
 #define CPB_ABI_VERSION 1
 #define CPB_MAX_PARSE_COLS 16 /* columns extracted by one fused parse call (output + predicate columns) */
+/* the largest cpb_pred tree the device compiles; a larger one fails with CPB_ERR_UNSUPPORTED */
+#define CPB_PRED_MAX_TERMS 32 /* Like (column, literal) pairs whose column exists */
+#define CPB_PRED_MAX_OPS 64   /* postfix operations: one per Like pair, per AND / OR / NOT joining them, per empty All / Any */
+#define CPB_PRED_MAX_DEPTH 48 /* All / Any / Not nodes above the deepest node */
 
 typedef struct cpb_ctx cpb_ctx;
 typedef struct cpb_table cpb_table; /* columnar batch of rows: Arrow-style string columns in HBM */
