@@ -102,6 +102,12 @@ KernelTimer::~KernelTimer() {
     }
 }
 
+// a data error of the reference: CPB_ERR_DATA, with the error in *err
+static int data_error(cpb_error* err, const DataError& d) {
+    fill_error(err, d.kind, d.column_index, d.line, d.has_line, d.msg);
+    return CPB_ERR_DATA;
+}
+
 int translate_exception(Ctx* c, cpb_error* err) {
     try { throw; }
     catch (const CudaFail& f) {
@@ -112,9 +118,8 @@ int translate_exception(Ctx* c, cpb_error* err) {
         cudaGetLastError();
         return CPB_ERR_CUDA;
     } catch (const DataError& d) {
-        fill_error(err, d.kind, d.column_index, d.line, d.has_line, d.msg);
         if (c) c->last_error = d.msg;
-        return CPB_ERR_DATA;
+        return data_error(err, d);
     } catch (const ArgError& a) {
         if (c) c->last_error = a.msg;
         fill_error(err, a.status == CPB_ERR_UNSUPPORTED ? CPB_E_UNSUPPORTED : CPB_E_NONE, -1, 0, false, a.msg);
@@ -328,11 +333,9 @@ int cpb_parse_csv(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device,
     auto sp = header_spec(spec, nspec);
     Buf staged;
     const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    bool had_error = false; DataError de{};
-    auto t = parse_csv(c, dev, nbytes, *opts, sp, filter, &had_error, &de);
-    *out = wrap(t);
-    if (had_error) { fill_error(err, de.kind, de.column_index, de.line, de.has_line, de.msg); return CPB_ERR_DATA; }
-    return CPB_OK;
+    const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, opts->header_from_first_row ? 2 : 1);
+    *out = wrap(p.table);
+    return p.error ? data_error(err, *p.error) : CPB_OK;
     CPB_CATCH(c, err)
 }
 
@@ -362,12 +365,11 @@ int cpb_stream_next(cpb_stream* st, cpb_table** out, int* done, cpb_error* err) 
     clear_error(err);
     *out = nullptr; *done = 0;
     CPB_TRY(c, err)
-    bool had_error = false, fin = false; DataError de{};
-    auto t = stream_next(st->s, &had_error, &de, &fin);
+    bool fin = false;
+    const Parsed p = stream_next(st->s, &fin);
     *done = fin ? 1 : 0;
-    if (t) *out = wrap(t);
-    if (had_error) { fill_error(err, de.kind, de.column_index, de.line, de.has_line, de.msg); return CPB_ERR_DATA; }
-    return CPB_OK;
+    if (p.table) *out = wrap(p.table);
+    return p.error ? data_error(err, *p.error) : CPB_OK;
     CPB_CATCH(c, err)
 }
 void cpb_stream_free(cpb_stream* st) {
@@ -414,20 +416,17 @@ int cpb_parse_csv_shard(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_d
     for (int i = 0; i < nspec; i++) sp.emplace_back(to_string(spec[i].name), spec[i].index);
     Buf staged;
     const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    uint64_t recs = 0;
-    ShardArgs sh{own_bytes, shard_index, is_last != 0, initial_parity, &recs};
-    bool had_error = false; DataError de{};
-    auto t = parse_csv(c, dev, nbytes, *opts, sp, filter, &had_error, &de, &sh);
-    if (records) *records = recs;
-    *out = wrap(t);
-    if (had_error) {
-        // the line is LOCAL: (0-based) ordinal of the failing record among this shard's records; the host adds the records
-        // of the shards before it and the reader's base (csvplus.go:1102-1137)
-        const uint64_t base = opts->header_from_first_row ? 2 : 1;
-        fill_error(err, de.kind, de.column_index, de.line >= base ? de.line - base : 0, de.has_line, de.msg);
-        return CPB_ERR_DATA;
-    }
-    return CPB_OK;
+    const uint64_t base = opts->header_from_first_row ? 2 : 1;
+    const ShardArgs sh{own_bytes, shard_index, is_last != 0, initial_parity};
+    const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, base, &sh);
+    if (records) *records = p.records;
+    *out = wrap(p.table);
+    if (!p.error) return CPB_OK;
+    // the line is LOCAL: (0-based) ordinal of the failing record among this shard's records; the host adds the records
+    // of the shards before it and the reader's base (csvplus.go:1102-1137)
+    DataError local = *p.error;
+    local.line = local.line >= base ? local.line - base : 0;
+    return data_error(err, local);
     CPB_CATCH(c, err)
 }
 
@@ -628,10 +627,7 @@ int cpb_index_build(cpb_ctx* h, const cpb_table* t, const cpb_str* key_cols, int
     for (int i = 0; i < nkeys; i++)
         for (int j = i + 1; j < nkeys; j++)
             if (keys[i] == keys[j]) throw ArgError{CPB_ERR_ARG, "duplicate column name(s) in CreateIndex()"};  // :714-716
-    DataError de{}; bool failed = false;
-    auto ix = build_index(c, t->t, keys, unique != 0, &de, &failed);
-    if (failed) { fill_error(err, de.kind, de.column_index, de.line, de.has_line, de.msg); return CPB_ERR_DATA; }
-    *out = new cpb_index{ix};
+    *out = new cpb_index{build_index(c, t->t, keys, unique != 0)};
     return CPB_OK;
     CPB_CATCH(c, err)
 }
@@ -667,10 +663,7 @@ int cpb_index_sub(cpb_ctx* h, const cpb_index* ix, const cpb_str* values, int n,
     auto view = std::make_shared<Table>(); view->ctx = c; view->nrows = hi - lo;
     for (auto col : sorted_table(c, *ix->ix)->cols) { col.row0 += lo; view->cols.push_back(col); }
     std::vector<std::string> keys(ix->ix->key_cols.begin() + n, ix->ix->key_cols.end());
-    DataError de{}; bool failed = false;
-    auto sub = build_index(c, view, keys, false, &de, &failed);
-    if (failed) throw de;
-    *out = new cpb_index{sub};
+    *out = new cpb_index{build_index(c, view, keys, false)};
     return CPB_OK;
     CPB_CATCH(c, nullptr)
 }
@@ -766,10 +759,7 @@ static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, 
     std::vector<std::string> names = n ? str_list(cols, n) : ix->ix->key_cols;  // natural join, csvplus.go:546-547
     if (names.size() > ix->ix->key_cols.size())
         throw ArgError{CPB_ERR_ARG, anti ? "too many source columns in Except()" : "too many source columns in Join()"};  // :548-549, :591-592
-    DataError de{}; bool failed = false;
-    auto t = join_tables(c, *probe->t, *ix->ix, names, anti, &de, &failed);
-    if (failed) { fill_error(err, de.kind, de.column_index, de.line, de.has_line, de.msg); return CPB_ERR_DATA; }
-    *out = wrap(t);
+    *out = wrap(join_tables(c, *probe->t, *ix->ix, names, anti));
     return CPB_OK;
     CPB_CATCH(c, err)
 }

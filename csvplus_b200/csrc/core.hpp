@@ -11,6 +11,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -270,23 +271,26 @@ struct ShardArgs {  // byte-range shard of one file (cpb_parse_csv_shard)
     int index;           // 0 = the shard holding the start of the file
     bool is_last;        // the buffer ends where the file ends
     uint32_t pin0;       // parity of the quote bytes of the file before this buffer
-    uint64_t* records;   // out: records owned by this shard (before filtering)
 };
-struct BatchArgs {       // one batch of a streamed input (cpb_stream): it starts at a record boundary of the input
-    uint64_t line_base;  // DataSourceError.Line of the batch's first data record
-    uint64_t* records;   // out: data records of the batch (before filtering)
-    bool* no_record;     // out: the batch holds no record at all (only blank or comment lines)
+// One parse: the rows before the first data error (all of them when there is none) and that error, as the reference
+// delivers them; the record counts are what a shard or a batch of a stream adds to the records before it.
+struct Parsed {
+    std::shared_ptr<Table> table;
+    std::optional<DataError> error;
+    uint64_t records = 0;    // data records of the input (before filtering)
+    bool no_record = false;  // the input holds no record at all (only blank or comment lines)
 };
-std::shared_ptr<Table> parse_csv(Ctx* c, const uint8_t* dev_bytes, uint64_t n, const cpb_reader_opts& o,
-                                 const std::vector<std::pair<std::string, int>>& spec, const cpb_pred* filter,
-                                 bool* had_error, DataError* derr, const ShardArgs* sh = nullptr, const BatchArgs* ba = nullptr);
+// line_base: DataSourceError.Line of the input's first data record (2 after a header row, 1 without; a later batch of a
+// stream continues the count)
+Parsed parse_csv(Ctx* c, const uint8_t* dev_bytes, uint64_t n, const cpb_reader_opts& o, const std::vector<std::pair<std::string, int>>& spec,
+                 const cpb_pred* filter, uint64_t line_base, const ShardArgs* sh = nullptr);
 uint32_t quote_parity(Ctx* c, const uint8_t* dev_bytes, uint64_t n);
 // stream.cu: batches of whole records (cpb_stream_*)
 struct Stream;
 void stream_cut(Ctx* c, const uint8_t* in, uint64_t n, const cpb_reader_opts& o, uint64_t* cut_dev);  // enqueued, 8 bytes
 Stream* stream_open(Ctx* c, const cpb_reader_opts& o, std::vector<std::pair<std::string, int>> spec, const cpb_pred* filter);
 void stream_push(Stream* s, const void* bytes, uint64_t n, bool is_last);
-std::shared_ptr<Table> stream_next(Stream* s, bool* had_error, DataError* derr, bool* done);
+Parsed stream_next(Stream* s, bool* done);  // table null: no complete record yet
 void stream_free(Stream* s);
 Ctx* stream_ctx(Stream* s);
 // gather.cu
@@ -311,9 +315,8 @@ std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& pa
 // and one host synchronisation.
 std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, const std::vector<int>& pidx, const std::vector<int>& cols,
                                       uint64_t* matches);
-// sort.cu
-std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::vector<std::string>& keys, bool unique,
-                                   DataError* derr, bool* failed);
+// sort.cu.  A missing key column (of a non-empty table) or a duplicate key of a unique index throws DataError.
+std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::vector<std::string>& keys, bool unique);
 std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix);  // materialises ix.table on first use
 void ensure_sorted(Ctx* c, Index& ix);                    // sorts a lazily-sorted unique index on first need of the order
 constexpr int MAXKEYS = 16;
@@ -332,9 +335,8 @@ uint32_t prefix_bytes(const Index& ix, int nk);  // image bytes covered by the f
 // head[i] = 1 when the first pbytes image bytes of row i differ from those of row i - 1 (row 0 always)
 void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head);
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
-// join.cu
-std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols,
-                                   bool anti, DataError* derr, bool* failed);
+// join.cu.  A join column missing from a non-empty probe table throws DataError.
+std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti);
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi);
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
 // fills ix.derived.rowhash (cols set by the caller) from ix.src.  built: the table is complete; duplicate: some key occurs twice;

@@ -474,19 +474,14 @@ static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pid
     return flag;
 }
 
-std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti,
-                                   DataError* derr, bool* failed) {
-    *failed = false;
+std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti) {
     const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
     const int nk = (int)cols.size();
     std::vector<int> pidx;
     for (int k = 0; k < nk; k++) {
         int ci = probe.find(cols[k]);
-        if (ci < 0 && np > 0) {  // row.SelectValues(columns...) fails on the first probe row (csvplus.go:556, :145)
-            *failed = true;
-            *derr = DataError{CPB_E_MISSING_COLUMN, k, probe.first_line, true, "missing column " + go_quote(cols[k])};
-            return nullptr;
-        }
+        if (ci < 0 && np > 0)  // row.SelectValues(columns...) fails on the first probe row (csvplus.go:556, :145)
+            throw DataError{CPB_E_MISSING_COLUMN, k, probe.first_line, true, "missing column " + go_quote(cols[k])};
         pidx.push_back(ci);
     }
     // output schema: mergeRows(indexRow, probeRow) — probe wins name collisions (csvplus.go:571-583)

@@ -340,10 +340,8 @@ std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix) {
     return ix.table;
 }
 
-std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std::vector<std::string>& keys, bool unique, DataError* derr,
-                                   bool* failed) {
+std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std::vector<std::string>& keys, bool unique) {
     const Table& t = *tp;
-    *failed = false;
     if ((int)keys.size() > MAXKEYS) throw ArgError{CPB_ERR_UNSUPPORTED, "more than 16 index key columns"};
     auto ix = std::make_shared<Index>();
     ix->ctx = c; ix->key_cols = keys;
@@ -352,11 +350,8 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
         int ci = t.find(keys[k]);
         if (ci < 0) {
             if (n == 0) { ci = -1; }
-            else {  // csvplus.go:723-727, raised for the first row pulled
-                *failed = true;
-                *derr = DataError{CPB_E_MISSING_INDEX_COLUMN, (int)k, t.first_line, true, "missing column " + go_quote(keys[k]) + " while creating an index"};
-                return nullptr;
-            }
+            else  // csvplus.go:723-727, raised for the first row pulled
+                throw DataError{CPB_E_MISSING_INDEX_COLUMN, (int)k, t.first_line, true, "missing column " + go_quote(keys[k]) + " while creating an index"};
         }
         ix->key_col_idx.push_back(ci);
     }
@@ -441,9 +436,7 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
             std::string s = "{ ";
             for (size_t i = 0; i < kv.size(); i++) { if (i) s += ", "; s += "\"" + kv[i].first + "\" : \"" + kv[i].second + "\""; }
             s += " }";
-            *failed = true;
-            *derr = DataError{CPB_E_DUPLICATE_KEY, -1, 0, false, "duplicate value while creating unique index: " + s};
-            return nullptr;
+            throw DataError{CPB_E_DUPLICATE_KEY, -1, 0, false, "duplicate value while creating unique index: " + s};
         }
     }
     ix->unique = unique;

@@ -195,11 +195,10 @@ struct Stream {
         max_push = std::max(max_push, n);
     }
 
-    // -> the next batch's table (null: no complete record yet); had_error / derr as parse_csv
-    std::shared_ptr<Table> next(bool* had_error, DataError* derr) {
-        *had_error = false;
+    // -> the next batch (table null: no complete record yet)
+    Parsed next() {
         bool trial = false;
-        if (done || (!last_pushed && len == 0)) return nullptr;  // (nothing pushed yet: no slot either)
+        if (done || (!last_pushed && len == 0)) return {};  // (nothing pushed yet: no slot either)
         CPB_CUDA(cudaStreamWaitEvent(c->stream, copied, 0));
         uint8_t* in = slot[cur]->as<uint8_t>();
         CPB_CUDA(cudaMemsetAsync(in + len, 0, std::min<uint64_t>(cap[cur] - len, 256), c->stream));
@@ -212,7 +211,7 @@ struct Stream {
                 // options) a bare quote flipped the quote parity for the rest of the input, and the reference would stop
                 // at that record.  As the tail grows (at 4, 8, 16, ... times the largest push), it is parsed as if it
                 // ended the input: an error that the missing rest cannot have caused ends the stream there.
-                if (len < std::max(trial_at, 4 * max_push)) return nullptr;
+                if (len < std::max(trial_at, 4 * max_push)) return {};
                 trial_at = 2 * len;
                 cut = len;
                 trial = true;
@@ -222,37 +221,35 @@ struct Stream {
         // afterwards with the resolved (name, field) pairs, no header row and the first record's field count
         cpb_reader_opts bo = o;
         if (resolved) bo.header_from_first_row = 0;
-        uint64_t records = 0;
-        bool no_record = false;
-        BatchArgs ba{resolved ? line_base : (o.header_from_first_row ? 2u : 1u), &records, &no_record};
-        auto t = parse_csv(c, in, cut, bo, spec, filter, had_error, derr, nullptr, &ba);
+        const uint64_t base = resolved ? line_base : (o.header_from_first_row ? 2u : 1u);
+        Parsed p = parse_csv(c, in, cut, bo, spec, filter, base);
         if (trial) {
             // a bare quote is an error wherever the record ends; another error only if a later record starts after it
-            const bool sure = *had_error && derr->has_line &&
-                              (derr->kind == CPB_E_BARE_QUOTE || derr->line + 1 < ba.line_base + records);
-            if (!sure) { *had_error = false; return nullptr; }
+            const bool sure = p.error && p.error->has_line && (p.error->kind == CPB_E_BARE_QUOTE || p.error->line + 1 < base + p.records);
+            if (!sure) return {};
         }
         if (!resolved) {
-            if (no_record && !last_pushed) {
-                *had_error = false;  // only blank / comment lines so far: they hold no record, drop them
-                t = nullptr;
-            } else if (!*had_error) {
+            if (p.no_record && !last_pushed) {
+                p.error.reset();  // only blank / comment lines so far: they hold no record, drop them
+                p.table = nullptr;
+            } else if (!p.error) {
                 resolved = true;
+                const Table& t = *p.table;
                 if (o.header_from_first_row) {
                     spec.clear();
-                    for (size_t i = 0; i < t->cols.size(); i++) spec.emplace_back(t->cols[i].name, t->src_field[i]);
+                    for (size_t i = 0; i < t.cols.size(); i++) spec.emplace_back(t.cols[i].name, t.src_field[i]);
                 }
-                if (o.num_fields == 0) o.num_fields = t->record_fields;
-                line_base = (o.header_from_first_row ? 2 : 1) + records;
+                if (o.num_fields == 0) o.num_fields = t.record_fields;
+                line_base = (o.header_from_first_row ? 2 : 1) + p.records;
             }
-        } else line_base += records;
-        if (*had_error || last_pushed) {
+        } else line_base += p.records;
+        if (p.error || last_pushed) {
             // the input is parsed (the tables own their bytes): the slots go back to the pool now, stream-ordered after
             // the parse, instead of staying allocated through the caller's plan until the stream is freed
             done = true;
             slot[0].reset(); slot[1].reset();
             cap[0] = cap[1] = 0;
-            return t;
+            return p;
         }
         // carry [cut, len) to the front of the other slot
         const int nx = cur ^ 1;
@@ -262,7 +259,7 @@ struct Stream {
         CPB_CUDA(cudaEventRecord(freed[cur], c->stream));
         CPB_CUDA(cudaEventRecord(freed[nx], c->stream));
         cur = nx; len = tail;
-        return t;
+        return p;
     }
 };
 
@@ -283,10 +280,10 @@ Stream* stream_open(Ctx* c, const cpb_reader_opts& o, std::vector<std::pair<std:
     return s;
 }
 void stream_push(Stream* s, const void* bytes, uint64_t n, bool is_last) { s->push(bytes, n, is_last); }
-std::shared_ptr<Table> stream_next(Stream* s, bool* had_error, DataError* derr, bool* done) {
-    auto t = s->next(had_error, derr);
+Parsed stream_next(Stream* s, bool* done) {
+    Parsed p = s->next();
     *done = s->done;
-    return t;
+    return p;
 }
 void stream_free(Stream* s) { delete s; }
 Ctx* stream_ctx(Stream* s) { return s->c; }
