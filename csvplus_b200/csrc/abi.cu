@@ -659,11 +659,19 @@ int cpb_index_sub(cpb_ctx* h, const cpb_index* ix, const cpb_str* values, int n,
     if (n >= (int)ix->ix->key_cols.size()) throw ArgError{CPB_ERR_ARG, "too many values in SubIndex()"};  // csvplus.go:633-635
     int64_t lo = 0, hi = ix->ix->nrows;
     if (n > 0) find_range(c, *ix->ix, str_list(values, n), &lo, &hi);
-    // rows are already sorted on the remaining key columns inside the range: rebuild the index image on the slice
+    // the slice in the parent's stored order, not re-sorted (csvplus.go:637-640): on a parent in key order it is already
+    // sorted on the remaining key columns; on one out of key order it keeps that order, and the searches follow it
     auto view = std::make_shared<Table>(); view->ctx = c; view->nrows = hi - lo;
     for (auto col : sorted_table(c, *ix->ix)->cols) { col.row0 += lo; view->cols.push_back(col); }
     std::vector<std::string> keys(ix->ix->key_cols.begin() + n, ix->ix->key_cols.end());
-    *out = new cpb_index{build_index(c, view, keys, false)};
+    if (hi == lo) {  // (an empty index also from a parent whose table lacks the key columns)
+        *out = new cpb_index{build_index(c, view, keys, false)};
+        return CPB_OK;
+    }
+    auto sub = std::make_shared<Index>();
+    sub->ctx = c; sub->key_cols = keys; sub->key_col_idx.assign(keys.size(), -1);
+    index_adopt_rows(c, *sub, view);
+    *out = new cpb_index{sub};
     return CPB_OK;
     CPB_CATCH(c, nullptr)
 }

@@ -291,20 +291,6 @@ static void probe_dispatch(Ctx* c, const Table& probe, const std::vector<int>& p
     CPB_CUDA(cudaGetLastError());
 }
 
-// the first pbytes of row r of image a (na rows) against those of row i of image b (nb rows): <0, 0, >0
-__device__ __forceinline__ int prefix_cmp(const uint64_t* a, uint64_t na, uint64_t r, const uint64_t* b, uint64_t nb, uint64_t i, uint32_t pbytes) {
-    const uint32_t full = pbytes >> 3, rem = pbytes & 7;
-    for (uint32_t w = 0; w < full; w++) {
-        const uint64_t x = a[(uint64_t)w * na + r], y = b[(uint64_t)w * nb + i];
-        if (x != y) return x < y ? -1 : 1;
-    }
-    if (rem) {
-        const uint64_t m = ~0ull << (8 * (8 - rem));
-        const uint64_t x = a[(uint64_t)full * na + r] & m, y = b[(uint64_t)full * nb + i] & m;
-        if (x != y) return x < y ? -1 : 1;
-    }
-    return 0;
-}
 // An index whose rows are not in key order: per probe row what the reference computes, on any order of rows.
 // first = sort.Search(n, row >= v) (indexImpl.first, csvplus.go:893-897), then Join takes every row from there while
 // row <= v (:557); Except keeps the probe row when that run is empty (has, :899-905: the row at first equals v).
@@ -489,13 +475,14 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     // An index column that is one of the nk joined key columns is not gathered: a match means equal key images, and
     // equal images mean equal bytes (value zero-padded to the index's width, then its length), so the index value IS
     // the probe value.  icol_key[j] = k takes output column j from probe key column pidx[k]; -1 gathers it from the
-    // index (gather_idx: those index columns, in order).
+    // index (gather_idx: those index columns, in order).  Rows out of key order are searched as the reference does
+    // (join_search_kernel): a run there can hold rows whose keys are below the probe's, so every index column is gathered.
     std::vector<int> icol_key, gather_idx;
     const Table& ischema = ix.schema();  // names only: the sorted columns may not be materialised
     if (!anti) for (size_t q = 0; q < ischema.cols.size(); q++) {
         if (probe.find(ischema.cols[q].name) >= 0) continue;
         int key = -1;
-        for (int k = 0; k < nk && key < 0; k++) if (ix.key_col_idx[k] == (int)q) key = k;
+        for (int k = 0; k < nk && key < 0 && ix.in_order; k++) if (ix.key_col_idx[k] == (int)q) key = k;
         icols.push_back(&ischema.cols[q]);
         icol_key.push_back(key);
         if (key < 0) gather_idx.push_back((int)q);

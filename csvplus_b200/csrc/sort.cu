@@ -444,17 +444,34 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
 }
 
 // ------------------------------------------------------------------ ResolveDuplicates support
+// indexImpl.dedup's walk (csvplus.go:814-859) over rows in any order, one thread: a group starts at the first adjacent
+// equal pair (i - 1, i) with i >= lower (pairs: those i, ascending) and ends at upper = lower + sort.Search(n - lower,
+// row > key) (:831), which on rows out of key order can take in rows with other keys; the next search starts at
+// upper + 1.  Groups [lo, hi) come out ascending and disjoint.
+__global__ void dup_walk_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, const uint32_t* __restrict__ pairs,
+                                uint64_t npairs, uint32_t* lo, uint32_t* hi, unsigned long long* ngroups) {
+    uint64_t g = 0, lower = 1, p = 0;
+    for (;;) {
+        uint64_t a = p, b = npairs;
+        while (a < b) { const uint64_t h = a + (b - a) / 2; if (pairs[h] < lower) a = h + 1; else b = h; }
+        if (a == npairs) break;
+        p = a; lower = pairs[a];
+        uint64_t i = lower, j = n;  // (the midpoints of sort.Search over [0, n - lower), offset by lower)
+        while (i < j) { const uint64_t h = i + (j - i) / 2; if (prefix_cmp(image, n, h, image, n, lower, pbytes) <= 0) i = h + 1; else j = h; }
+        lo[g] = (uint32_t)(lower - 1); hi[g] = (uint32_t)i; g++;
+        lower = i + 1;
+    }
+    *ngroups = g;
+}
+__global__ void not_flags_kernel(const uint32_t* __restrict__ head, uint64_t n, uint32_t* out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = head[i] ? 0u : 1u;
+}
+
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi) {
     lo.clear(); hi.clear();
     const uint64_t n = (uint64_t)ix.nrows;
     if (n < 2 || ix.unique) return;  // (a verified unique index has no duplicate group)
-    Buf head = dev_alloc(c, n * 4), gs = dev_alloc(c, n * 4), ge = dev_alloc(c, n * 4);
-    {
-        KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 12, 2);
-        head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
-        group_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>(), ge->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
     auto compact = [&](const Buf& flags, uint32_t add, uint64_t* count) {
         const FlagScan s = scan_flags(c, flags->as<uint32_t>(), n);
         Buf out = dev_alloc(c, (s.count + 1) * 4);
@@ -462,10 +479,40 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
         *count = s.count;
         return out;
     };
+    Buf head = dev_alloc(c, n * 4), gs = dev_alloc(c, n * 4);
     uint64_t ng = 0, ne = 0;
-    Buf los = compact(gs, 0, &ng);
-    Buf his = compact(ge, 1, &ne);
-    if (ng != ne) throw ArgError{CPB_ERR_CUDA, "internal: group start/end mismatch"};
+    Buf los, his;
+    if (ix.in_order) {  // a group is a run of equal keys: its first row is a head followed by a non-head, and so on
+        Buf ge = dev_alloc(c, n * 4);
+        {
+            KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 12, 2);
+            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
+            group_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>(), ge->as<uint32_t>());
+            CPB_CUDA(cudaGetLastError());
+        }
+        los = compact(gs, 0, &ng);
+        his = compact(ge, 1, &ne);
+        if (ng != ne) throw ArgError{CPB_ERR_CUDA, "internal: group start/end mismatch"};
+    } else {
+        {
+            KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 8, 2);
+            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
+            not_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>());
+            CPB_CUDA(cudaGetLastError());
+        }
+        uint64_t npairs = 0;
+        Buf pairs = compact(gs, 0, &npairs);
+        if (npairs == 0) return;
+        los = dev_alloc(c, npairs * 4); his = dev_alloc(c, npairs * 4);
+        Buf cnt = dev_alloc(c, 8);
+        {
+            KernelTimer kt(c, "dedup_walk", 0);
+            dup_walk_kernel<<<1, 1, 0, c->stream>>>(ix.image->as<uint64_t>(), n, ix.image_words * 8, pairs->as<uint32_t>(), npairs,
+                                                    los->as<uint32_t>(), his->as<uint32_t>(), (unsigned long long*)cnt->p);
+            CPB_CUDA(cudaGetLastError());
+        }
+        ng = read_back<uint64_t>(c, cnt->p);
+    }
     std::vector<uint32_t> a(ng), b(ng);
     if (ng) {
         CPB_CUDA(cudaMemcpyAsync(a.data(), los->p, ng * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -476,9 +523,19 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
 }
 
 // indexImpl.dedup (csvplus.go:810-867) with the resolver's choices already made on the host.
-// keep[g] >= 0: sorted position of the row kept for group g; -1: the group is dropped (the resolver returned an "empty"
+// keep[g] >= 0: stored position of the row kept for group g; -1: the group is dropped (the resolver returned an "empty"
 // row, :845); <= -2: the resolver returned a row that is not one of the group's rows — row (-2 - keep[g]) of `repl`
 // takes the place of the group (:846 stores whatever row came back; the index is NOT re-sorted, exactly like the reference).
+// The rows kept: every row outside the groups, the chosen row of each group, in stored order — except that the walk
+// never copies the last row when no group covers it (SURVEY §Q1, bug_compatible).
+// keep[i] = 1 for the rows outside the groups [lo, hi) (ascending, disjoint)
+__global__ void uncovered_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ hi, uint64_t ng, uint64_t n, uint32_t* keep) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint64_t a = 0, b = ng;  // groups starting at or before i
+    while (a < b) { const uint64_t h = a + (b - a) / 2; if (lo[h] <= i) a = h + 1; else b = h; }
+    keep[i] = (a == 0 || i >= hi[a - 1]) ? 1u : 0u;
+}
 __global__ void patch_ids_kernel(const uint32_t* __restrict__ pos, const int64_t* __restrict__ at, const uint32_t* __restrict__ with, uint64_t m, uint32_t* ids) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < m) ids[pos[at[i]]] = with[i];
@@ -526,12 +583,12 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
     std::vector<int64_t> rpos; std::vector<uint32_t> rid;
     bool any_repl = false;
     for (auto k : keep) if (k <= -2) any_repl = true;
+    std::vector<int64_t> lo, hi;
+    if (any_repl || !ix.in_order) index_dup_groups(c, ix, lo, hi);
     if (any_repl) {
         if (!repl) throw ArgError{CPB_ERR_ARG, "replacement rows referenced but no replacement table given"};
         if (repl->cols.size() != ix.table->cols.size()) throw ArgError{CPB_ERR_UNSUPPORTED, "a replacement row must have the columns of the index rows"};
         for (auto& col : ix.table->cols) if (repl->find(col.name) < 0) throw ArgError{CPB_ERR_UNSUPPORTED, "a replacement row must have the columns of the index rows"};
-        std::vector<int64_t> lo, hi;
-        index_dup_groups(c, ix, lo, hi);
         if (lo.size() != keep.size()) throw ArgError{CPB_ERR_ARG, "keep[] does not match the duplicate groups of the index"};
         for (size_t g = 0; g < keep.size(); g++)
             if (keep[g] <= -2) {
@@ -541,16 +598,30 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
                 keep[g] = lo[g];
             }
     }
-    Buf head = dev_alloc(c, n * 4), flag = dev_alloc(c, n * 4);
-    head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
-    singleton_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, flag->as<uint32_t>());
+    // flag = the rows outside the groups.  In key order the groups are the runs of equal keys, so those are the rows
+    // that are heads of runs of one; out of key order they come from the groups the walk found.
+    Buf flag = dev_alloc(c, n * 4);
+    bool last_outside = false;
+    if (ix.in_order) {
+        Buf head = dev_alloc(c, n * 4);
+        head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
+        singleton_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, flag->as<uint32_t>());
+        if (bug_compatible) last_outside = read_back<uint32_t>(c, head->as<uint32_t>() + (n - 1)) != 0;
+    } else {
+        std::vector<uint32_t> lh(lo.begin(), lo.end()), hh(hi.begin(), hi.end());
+        Buf dlo = dev_alloc(c, (lh.size() + 1) * 4), dhi = dev_alloc(c, (hh.size() + 1) * 4);
+        if (!lh.empty()) {
+            CPB_CUDA(cudaMemcpyAsync(dlo->p, lh.data(), lh.size() * 4, cudaMemcpyHostToDevice, c->stream));
+            CPB_CUDA(cudaMemcpyAsync(dhi->p, hh.data(), hh.size() * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        uncovered_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dlo->as<uint32_t>(), dhi->as<uint32_t>(), lh.size(), n, flag->as<uint32_t>());
+        last_outside = hi.empty() || (uint64_t)hi.back() < n;
+        sync_stream(c);  // lh / hh are pageable host vectors
+    }
     Buf kd = dev_alloc(c, keep.size() * 8);
     CPB_CUDA(cudaMemcpyAsync(kd->p, keep.data(), keep.size() * 8, cudaMemcpyHostToDevice, c->stream));
     set_flags_kernel<<<nblk(keep.size(), 256), 256, 0, c->stream>>>(kd->as<int64_t>(), keep.size(), flag->as<uint32_t>(), n);
-    if (bug_compatible) {
-        // SURVEY §Q1: when a group exists and the last sorted row is a singleton it is never copied (:851-864)
-        if (read_back<uint32_t>(c, head->as<uint32_t>() + (n - 1)) != 0) clear_one_kernel<<<1, 1, 0, c->stream>>>(flag->as<uint32_t>(), n - 1);
-    }
+    if (bug_compatible && last_outside) clear_one_kernel<<<1, 1, 0, c->stream>>>(flag->as<uint32_t>(), n - 1);
     CPB_CUDA(cudaGetLastError());
     // compaction of the kept positions (the scanned positions are needed again to patch replacement ids in)
     const FlagScan kept = scan_flags(c, flag->as<uint32_t>(), n);

@@ -98,6 +98,20 @@ __device__ __forceinline__ bool prefix_equal(const uint64_t* a, uint64_t na, uin
     return true;
 }
 
+// the first pbytes of row r of image a (na rows) against those of row i of image b (nb rows): <0, 0, >0
+__device__ __forceinline__ int prefix_cmp(const uint64_t* a, uint64_t na, uint64_t r, const uint64_t* b, uint64_t nb, uint64_t i, uint32_t pbytes) {
+    const uint32_t full = pbytes >> 3, rem = pbytes & 7;
+    for (uint32_t w = 0; w < full; w++) {
+        const uint64_t x = a[(uint64_t)w * na + r], y = b[(uint64_t)w * nb + i];
+        if (x != y) return x < y ? -1 : 1;
+    }
+    if (rem) {
+        const uint64_t m = ~0ull << (8 * (8 - rem));
+        const uint64_t x = a[(uint64_t)full * na + r] & m, y = b[(uint64_t)full * nb + i] & m;
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return 0;
+}
 // ---- SWAR byte classification
 // exact per-byte equality flags: bit 7 of every byte of the result is set iff that byte of w == c
 __device__ __forceinline__ uint32_t eq_flags(uint32_t w, uint32_t c4) {

@@ -300,3 +300,15 @@ def take_rows(rows: list[dict]) -> Rows:
     b, l, n = _pack(names)
     oa = (C.c_void_p * n)(*[o.ctypes.data for o in offs]); da = (C.c_void_p * n)(*[d.ctypes.data for d in datas])
     return Rows(lib().orc_result_from_columns(n, b, l, oa, da, len(rows)))
+
+
+def take_columns(columns: dict) -> Rows:
+    """take_rows from columns: {name: (offsets int[n+1], bytes uint8[])}, every column of the same n rows."""
+    names = list(columns)
+    offs = [np.ascontiguousarray(columns[nm][0], dtype=np.int64) for nm in names]
+    datas = [np.ascontiguousarray(columns[nm][1], dtype=np.uint8) for nm in names]
+    datas = [d if d.size else np.zeros(1, np.uint8) for d in datas]
+    nrows = len(offs[0]) - 1 if offs else 0
+    b, l, n = _pack(names)
+    oa = (C.c_void_p * max(1, n))(*[o.ctypes.data for o in offs]); da = (C.c_void_p * max(1, n))(*[d.ctypes.data for d in datas])
+    return Rows(lib().orc_result_from_columns(n, b, l, oa, da, nrows))

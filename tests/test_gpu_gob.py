@@ -11,6 +11,7 @@ import zlib
 import pytest
 
 from tests import gob_oracle as g
+from tests.index_ref import find as ref_find, join as ref_join
 from tests.helpers import gpu_ctx, people_csv
 
 pytestmark = pytest.mark.gpu
@@ -160,50 +161,6 @@ def test_rows_message_above_4_gib(tmp_path, monkeypatch):
 
 
 # ------------------------------------------------------------------ LoadIndex
-def _cmp(row, cols, values, eq):  # indexImpl.cmp
-    for j, v in enumerate(values):
-        a = row[cols[j]]
-        if a > v:
-            return True
-        if a < v:
-            return False
-    return eq
-
-
-def _search(n, f):  # sort.Search
-    i, j = 0, n
-    while i < j:
-        h = (i + j) // 2
-        if not f(h):
-            i = h + 1
-        else:
-            j = h
-    return i
-
-
-def ref_find(rows, cols, values):
-    if not values:
-        return rows
-    upper = _search(len(rows), lambda i: _cmp(rows[i], cols, values, False))
-    lower = _search(upper, lambda i: _cmp(rows[i], cols, values, True))
-    return rows[lower:upper]
-
-
-def ref_join(rows, cols, probe, pcols, anti=False):
-    out = []
-    for p in probe:
-        values = [p[c] for c in pcols]
-        i = _search(len(rows), lambda h: _cmp(rows[h], cols, values, True))
-        if anti:
-            if not (i < len(rows) and not _cmp(rows[i], cols, values, False)):
-                out.append(p)
-            continue
-        while i < len(rows) and not _cmp(rows[i], cols, values, False):
-            out.append({**rows[i], **p})
-            i += 1
-    return out
-
-
 def _s(rows):
     return [{k.decode(): v.decode() for k, v in r.items()} for r in rows]
 
