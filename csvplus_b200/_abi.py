@@ -13,6 +13,11 @@ MAX_PARSE_COLS = 16  # CPB_MAX_PARSE_COLS
 PRED_MAX_TERMS = 32  # CPB_PRED_MAX_TERMS
 PRED_MAX_OPS = 64    # CPB_PRED_MAX_OPS
 PRED_MAX_DEPTH = 48  # CPB_PRED_MAX_DEPTH
+# the cpb_status and cpb_err_kind values the host layer tells apart (tests check them against the header's enums)
+CPB_ERR_DATA = 1
+CPB_ERR_ARG = 2
+CPB_E_MISSING_COLUMN = 10
+CPB_E_TOO_LARGE = 13
 
 
 class Str(C.Structure):

@@ -12,6 +12,7 @@ and whatever follows them is uploaded again with TakeRows semantics (cpb_table_f
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import io
 import os
@@ -111,13 +112,17 @@ def _strs(items: Iterable) -> tuple:
 
 def _raise(st: int, err: _abi.Error, ctx=None):
     msg = err.msg.decode("utf-8", "replace") if err is not None else ""
-    if st == 1:  # CPB_ERR_DATA
+    if st == _abi.CPB_ERR_DATA:
         if err.has_line:
-            raise DataSourceError(err.line, msg, err.kind)
+            raise _data_error(err)
         raise CsvPlusError(msg, st, err.kind)
     if not msg and ctx is not None:
         msg = _abi.load().cpb_last_error(ctx.h).decode("utf-8", "replace")
     raise CsvPlusError(msg or f"csvplus_b200 call failed with status {st}", st, err.kind if err is not None else 0)
+
+
+def _data_error(e: _abi.Error) -> DataSourceError:
+    return DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
 
 
 class Context:
@@ -152,13 +157,36 @@ class Context:
         """cpb_pool_reserve: map `nbytes` of device memory into this context's pool ahead of time (False: not available)"""
         return self.lib.cpb_pool_reserve(self.h, int(nbytes)) == 0
 
+    def _call(self, name: str, *args, err: "_abi.Error | None" = None, accept: tuple = (), h=None) -> int:
+        """lib.<name>(h, *args[, err]) -> its status.  h is the handle passed first, this context's by default; an entry
+        whose last parameter is a cpb_error* is given err (a fresh one by default).  A non-zero status that is not in
+        accept raises (_raise)."""
+        fn = getattr(self.lib, name)
+        if fn.argtypes[-1] is C.POINTER(_abi.Error):
+            err = _abi.Error() if err is None else err
+            args += (C.byref(err),)
+        st = fn(self.h if h is None else h, *args)
+        if st and st not in accept:
+            _raise(st, err, self)
+        return st
+
+    def _new_table(self, name: str, *args) -> "Table":
+        """an entry whose out-parameter, after args, is a new table handle"""
+        h = C.c_void_p()
+        self._call(name, *args, C.byref(h))
+        return Table(self, h)
+
+    def _new_index(self, name: str, *args, columns: list) -> "Index":
+        """an entry whose out-parameter, after args, is a new index handle; columns: the index's key columns"""
+        h = C.c_void_p()
+        self._call(name, *args, C.byref(h))
+        return Index(self, h, columns)
+
     def pool_used_high(self, reset: bool = False) -> int:
         """cpb_pool_used_high: the most device memory this context's pool has had allocated at once since the last reset
         (reset=True starts a new window at the current use)"""
         out = C.c_uint64()
-        st = self.lib.cpb_pool_used_high(self.h, int(reset), C.byref(out))
-        if st:
-            _raise(st, None, self)
+        self._call("cpb_pool_used_high", int(reset), C.byref(out))
         return out.value
 
     @property
@@ -196,27 +224,23 @@ class Context:
         """synthetic CSV of SURVEY §8(d) generated on the GPU (bench / tests only)"""
         k = {"people": 0, "customers": 0, "orders": 1, "products": 2}[kind]
         lo, hi = rows
-        sizes, total = [], 0
-        r = lo
+
+        def gen(r0, r1, dst, cap) -> int:
+            nb = C.c_uint64()
+            self._call("cpb_gen_csv", k, seed, r0, r1, n_cust, n_prod, int(header and r0 == lo), int(permute), dst, cap, C.byref(nb))
+            return nb.value
+        sizes, r = [], lo
         while True:
             e = min(hi, r + chunk_rows)
-            nb = C.c_uint64()
-            st = self.lib.cpb_gen_csv(self.h, k, seed, r, e, n_cust, n_prod, int(header and r == lo), int(permute), None, 0, C.byref(nb))
-            if st:
-                _raise(st, None, self)
-            sizes.append((r, e, nb.value)); total += nb.value
+            sizes.append((r, e, gen(r, e, None, 0)))
             r = e
             if r >= hi:
                 break
+        total = sum(nb for _, _, nb in sizes)
         buf = self.device_alloc(total)
         off = 0
         for (r0, r1, nb) in sizes:
-            got = C.c_uint64()
-            st = self.lib.cpb_gen_csv(self.h, k, seed, r0, r1, n_cust, n_prod, int(header and r0 == lo), int(permute),
-                                      C.c_void_p(buf.ptr + off), nb, C.byref(got))
-            if st:
-                _raise(st, None, self)
-            off += got.value
+            off += gen(r0, r1, C.c_void_p(buf.ptr + off), nb)
         buf.nbytes = total
         return buf
 
@@ -225,9 +249,7 @@ class HostBuffer:
     def __init__(self, ctx: Context, n: int):
         self.ctx, self.nbytes = ctx, n
         p = C.c_void_p()
-        st = ctx.lib.cpb_host_alloc(ctx.h, n, C.byref(p))
-        if st:
-            _raise(st, None, ctx)
+        ctx._call("cpb_host_alloc", n, C.byref(p))
         self.ptr = p.value
 
     def array(self) -> np.ndarray:
@@ -245,20 +267,24 @@ class HostBuffer:
 
 
 class DeviceBuffer:
-    def __init__(self, ctx: Context, n: int):
+    def __init__(self, ctx: Context, n: int, ptr: int | None = None):
+        """n bytes of new device memory (cpb_device_alloc), or the n bytes at ptr that the library allocated"""
         self.ctx, self.nbytes = ctx, n
-        p = C.c_void_p()
-        st = ctx.lib.cpb_device_alloc(ctx.h, n, C.byref(p))
-        if st:
-            _raise(st, None, ctx)
-        self.ptr = p.value
+        if ptr is None:
+            p = C.c_void_p()
+            ctx._call("cpb_device_alloc", n, C.byref(p))
+            ptr = p.value
+        self.ptr = ptr
+
+    @classmethod
+    def adopt(cls, ctx: Context, ptr: int, nbytes: int) -> "DeviceBuffer":
+        """device memory a call returned (cpb_table_to_csv_device, ...): released with the buffer, like its own"""
+        return cls(ctx, nbytes, ptr)
 
     def to_host(self, n: int | None = None, offset: int = 0) -> np.ndarray:
         n = self.nbytes - offset if n is None else n
         out = np.empty(n, np.uint8)
-        st = self.ctx.lib.cpb_memcpy_d2h(self.ctx.h, out.ctypes.data, C.c_void_p(self.ptr + offset), n)
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_memcpy_d2h", out.ctypes.data, C.c_void_p(self.ptr + offset), n)
         return out
 
     def free(self):
@@ -378,14 +404,10 @@ class Table:
         hi = len(self) if hi is None else hi
         idx = self.columns.index(name)
         nb = C.c_uint64()
-        st = self.ctx.lib.cpb_table_col_bytes(self.ctx.h, self.h, idx, lo, hi, C.byref(nb))
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_table_col_bytes", self.h, idx, lo, hi, C.byref(nb))
         off = np.empty(hi - lo + 1, np.int64)
         data = np.empty(max(1, nb.value), np.uint8)
-        st = self.ctx.lib.cpb_table_fetch_column(self.ctx.h, self.h, idx, lo, hi, off.ctypes.data, data.ctypes.data, data.size)
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_table_fetch_column", self.h, idx, lo, hi, off.ctypes.data, data.ctypes.data, data.size)
         return off, data[: nb.value]
 
     def values(self, name: str, lo: int = 0, hi: int | None = None) -> list[bytes]:
@@ -428,11 +450,7 @@ class Table:
             datas.append(np.frombuffer(b"".join(vals) + b"\0", np.uint8).copy()); offs.append(off)
         oa = (C.c_void_p * max(1, len(cols)))(*[o.ctypes.data for o in offs])
         da = (C.c_void_p * max(1, len(cols)))(*[d.ctypes.data for d in datas])
-        h = C.c_void_p()
-        st = ctx.lib.cpb_table_from_host(ctx.h, len(cols), na, oa, da, len(rows), C.byref(h))
-        if st:
-            _raise(st, None, ctx)
-        return Table(ctx, h)
+        return ctx._new_table("cpb_table_from_host", len(cols), na, oa, da, len(rows))
 
     @staticmethod
     def from_device_columns(ctx: Context, names: list[str], columns: list[tuple], nrows: int) -> "Table":
@@ -441,127 +459,79 @@ class Table:
         na, keep = _strs(names)
         oa = (C.c_void_p * max(1, len(names)))(*[c[0] for c in columns])
         da = (C.c_void_p * max(1, len(names)))(*[c[1] or 0 for c in columns])
-        h = C.c_void_p()
-        st = ctx.lib.cpb_table_from_device(ctx.h, len(names), na, oa, da, nrows, C.byref(h))
-        if st:
-            _raise(st, None, ctx)
-        return Table(ctx, h)
+        return ctx._new_table("cpb_table_from_device", len(names), na, oa, da, nrows)
 
     # thin wrappers of the table-level ABI
     def select(self, *cols) -> "Table":
-        a, keep = _strs(cols); h = C.c_void_p(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_select(self.ctx.h, self.h, a, len(cols), C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        return Table(self.ctx, h)
+        a, keep = _strs(cols)
+        return self.ctx._new_table("cpb_table_select", self.h, a, len(cols))
 
     def drop(self, *cols) -> "Table":
-        a, keep = _strs(cols); h = C.c_void_p()
-        st = self.ctx.lib.cpb_table_drop(self.ctx.h, self.h, a, len(cols), C.byref(h))
-        if st:
-            _raise(st, None, self.ctx)
-        return Table(self.ctx, h)
+        a, keep = _strs(cols)
+        return self.ctx._new_table("cpb_table_drop", self.h, a, len(cols))
 
     def filter(self, pred: Predicate) -> "Table":
-        keep = []; p = pred._c(keep); h = C.c_void_p()
-        st = self.ctx.lib.cpb_table_filter(self.ctx.h, self.h, C.byref(p), C.byref(h))
-        if st:
-            _raise(st, None, self.ctx)
-        return Table(self.ctx, h)
+        keep = []; p = pred._c(keep)
+        return self.ctx._new_table("cpb_table_filter", self.h, C.byref(p))
 
     def first_false(self, pred: Predicate) -> int:
         """index of the first row for which the recognisable predicate is false (len(self) if none): cpb_table_first_false"""
         keep = []; p = pred._c(keep); out = C.c_int64()
-        st = self.ctx.lib.cpb_table_first_false(self.ctx.h, self.h, C.byref(p), C.byref(out))
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_table_first_false", self.h, C.byref(p), C.byref(out))
         return out.value
 
     def slice(self, lo: int, hi: int) -> "Table":
-        h = C.c_void_p()
-        st = self.ctx.lib.cpb_table_slice(self.ctx.h, self.h, lo, hi, C.byref(h))
-        if st:
-            _raise(st, None, self.ctx)
-        return Table(self.ctx, h)
+        return self.ctx._new_table("cpb_table_slice", self.h, lo, hi)
 
     def index_on(self, *cols, unique=False) -> "Index":
-        a, keep = _strs(cols); h = C.c_void_p(); e = _abi.Error()
-        st = self.ctx.lib.cpb_index_build(self.ctx.h, self.h, a, len(cols), int(unique), C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        return Index(self.ctx, h, list(cols))
+        a, keep = _strs(cols)
+        return self.ctx._new_index("cpb_index_build", self.h, a, len(cols), int(unique), columns=list(cols))
 
     def join(self, index: "Index", *cols, anti=False) -> "Table":
-        a, keep = _strs(cols); h = C.c_void_p(); e = _abi.Error()
-        fn = self.ctx.lib.cpb_except if anti else self.ctx.lib.cpb_join
-        st = fn(self.ctx.h, self.h, index.h, a, len(cols), C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        return Table(self.ctx, h)
+        a, keep = _strs(cols)
+        return self.ctx._new_table("cpb_except" if anti else "cpb_join", self.h, index.h, a, len(cols))
 
-    def to_csv(self, *cols) -> bytes:
-        a, keep = _strs(cols); p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_to_csv(self.ctx.h, self.h, a, len(cols), C.byref(p), C.byref(n), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
+    def _pinned_bytes(self, name: str, *args) -> bytes:
+        """an entry that returns its bytes in new pinned host memory"""
+        p = C.c_void_p(); n = C.c_uint64()
+        self.ctx._call(name, self.h, *args, C.byref(p), C.byref(n))
         out = C.string_at(p.value, n.value)
         self.ctx.lib.cpb_host_free(self.ctx.h, p)
         return out
+
+    def _device_bytes(self, name: str, *args) -> "DeviceBuffer":
+        """an entry that leaves its bytes in new device memory"""
+        p = C.c_void_p(); n = C.c_uint64()
+        self.ctx._call(name, self.h, *args, C.byref(p), C.byref(n))
+        return DeviceBuffer.adopt(self.ctx, p.value, n.value)
+
+    def to_csv(self, *cols) -> bytes:
+        a, keep = _strs(cols)
+        return self._pinned_bytes("cpb_table_to_csv", a, len(cols))
 
     def to_csv_into(self, dst: "HostBuffer | None", offset: int, *cols, header: bool = True) -> int:
         """one batch of ToCsv into pinned host memory (cpb_table_to_csv_into).  Returns the batch's size in bytes; when
         that exceeds the room left in dst (or dst is None), nothing is written."""
-        a, keep = _strs(cols); n = C.c_uint64(); e = _abi.Error()
-        ptr, cap = (dst.ptr + offset, dst.nbytes - offset) if dst is not None else (None, 0)
-        st = self.ctx.lib.cpb_table_to_csv_into(self.ctx.h, self.h, a, len(cols), int(header), C.c_void_p(ptr), cap, C.byref(n),
-                                                C.byref(e))
-        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
-            return n.value
-        if st:
-            _raise(st, e, self.ctx)
-        return n.value
+        a, keep = _strs(cols)
+        return _into(self.ctx, "cpb_table_to_csv_into", self.h, a, len(cols), int(header), dst=dst, offset=offset)
 
     def to_csv_device(self, *cols) -> "DeviceBuffer":
         """ToCsv with the serialised bytes left in HBM (cpb_table_to_csv_device)"""
-        a, keep = _strs(cols); p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_to_csv_device(self.ctx.h, self.h, a, len(cols), C.byref(p), C.byref(n), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        b = DeviceBuffer.__new__(DeviceBuffer)
-        b.ctx, b.nbytes, b.ptr = self.ctx, n.value, p.value
-        return b
+        a, keep = _strs(cols)
+        return self._device_bytes("cpb_table_to_csv_device", a, len(cols))
 
     def to_json(self, first: bool = True, last: bool = True) -> bytes:
         """DataSource.ToJSON of every column (cpb_table_to_json); first / last: the batch opens / closes the array"""
-        p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_to_json(self.ctx.h, self.h, int(first), int(last), C.byref(p), C.byref(n), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        out = C.string_at(p.value, n.value)
-        self.ctx.lib.cpb_host_free(self.ctx.h, p)
-        return out
+        return self._pinned_bytes("cpb_table_to_json", int(first), int(last))
 
     def to_json_into(self, dst: "HostBuffer | None", offset: int = 0, first: bool = True, last: bool = True) -> int:
         """one batch of a streamed ToJSON into pinned host memory (cpb_table_to_json_into).  Returns the batch's size in
         bytes; when that exceeds the room left in dst (or dst is None), nothing is written."""
-        n = C.c_uint64(); e = _abi.Error()
-        ptr, cap = (dst.ptr + offset, dst.nbytes - offset) if dst is not None else (None, 0)
-        st = self.ctx.lib.cpb_table_to_json_into(self.ctx.h, self.h, int(first), int(last), C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
-        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
-            return n.value
-        if st:
-            _raise(st, e, self.ctx)
-        return n.value
+        return _into(self.ctx, "cpb_table_to_json_into", self.h, int(first), int(last), dst=dst, offset=offset)
 
     def to_json_device(self, first: bool = True, last: bool = True) -> "DeviceBuffer":
         """ToJSON with the serialised bytes left in HBM (cpb_table_to_json_device)"""
-        p = C.c_void_p(); n = C.c_uint64(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_to_json_device(self.ctx.h, self.h, int(first), int(last), C.byref(p), C.byref(n), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        b = DeviceBuffer.__new__(DeviceBuffer)
-        b.ctx, b.nbytes, b.ptr = self.ctx, n.value, p.value
-        return b
+        return self._device_bytes("cpb_table_to_json_device", int(first), int(last))
 
     def values_as_int(self, name: str, strict: bool = True):
         """Row.ValueAsInt (strconv.Atoi, csvplus.go:165-183) of every row of a column, as an int64 CUDA tensor on the
@@ -576,7 +546,7 @@ class Table:
 
     def _values_as(self, name: str, is_float: bool, strict: bool):
         values, status, err = self._convert(name, is_float)
-        if err is not None and (strict or err.kind == 10):  # CPB_E_MISSING_COLUMN fails in both modes
+        if err is not None and (strict or err.kind == _abi.CPB_E_MISSING_COLUMN):  # fails in both modes
             raise err
         return values if strict else (values, status)
 
@@ -593,15 +563,12 @@ class Table:
         ev.record(torch.cuda.current_stream(dev))
         torch.cuda.ExternalStream(self.ctx.stream, device=dev).wait_event(ev)
         b = _enc(name); nbad = C.c_uint64(); e = _abi.Error()
-        fn = self.ctx.lib.cpb_table_column_as_float64 if is_float else self.ctx.lib.cpb_table_column_as_int64
-        st = fn(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), C.c_void_p(status.data_ptr()), C.byref(nbad),
-                C.byref(e))
-        if st == 1:
+        st = self.ctx._call("cpb_table_column_as_float64" if is_float else "cpb_table_column_as_int64", self.h, _abi.Str(b, len(b)),
+                            C.c_void_p(values.data_ptr()), C.c_void_p(status.data_ptr()), C.byref(nbad), err=e, accept=(_abi.CPB_ERR_DATA,))
+        if st:
             err = CsvPlusError(e.msg.decode("utf-8", "replace"), st, e.kind)
             err.row = e.line
             return values, status, err
-        if st:
-            _raise(st, e, self.ctx)
         return values, status, None
 
     def with_column(self, name: str, value, fmt: str | None = None, prec: int = -1) -> "Table":
@@ -614,47 +581,34 @@ class Table:
             if fmt is not None:
                 raise TypeError("with_column: the format of a FormatFloat value is given in FormatFloat")
             value, fmt, prec = value.values, value.fmt, value.prec
-        b = _enc(name); h = C.c_void_p(); e = _abi.Error(); lib = self.ctx.lib
+        b = _enc(name); column = _abi.Str(b, len(b))
         if isinstance(value, (str, bytes)):
             if fmt is not None:
                 raise TypeError("with_column: fmt applies to float64 tensors only")
             v = _enc(value)
-            st = lib.cpb_table_set_literal(self.ctx.h, self.h, _abi.Str(b, len(b)), _abi.Str(v, len(v)), C.byref(h), C.byref(e))
-        else:
-            import torch
-            values = _device_tensor(self, value, (torch.int64, torch.float64), "with_column")
-            if values.dtype == torch.float64:
-                fmt = "g" if fmt is None else fmt
-                _check_format(fmt, prec)
-                st = lib.cpb_table_set_float64(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), fmt.encode(), prec,
-                                               C.byref(h), C.byref(e))
-            else:
-                if fmt is not None:
-                    raise TypeError("with_column: fmt applies to float64 tensors only")
-                st = lib.cpb_table_set_int64(self.ctx.h, self.h, _abi.Str(b, len(b)), C.c_void_p(values.data_ptr()), C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        return Table(self.ctx, h)
+            return self.ctx._new_table("cpb_table_set_literal", self.h, column, _abi.Str(v, len(v)))
+        import torch
+        values = _device_tensor(self, value, (torch.int64, torch.float64), "with_column")
+        if values.dtype == torch.float64:
+            fmt = "g" if fmt is None else fmt
+            _check_format(fmt, prec)
+            return self.ctx._new_table("cpb_table_set_float64", self.h, column, C.c_void_p(values.data_ptr()), fmt.encode(), prec)
+        if fmt is not None:
+            raise TypeError("with_column: fmt applies to float64 tensors only")
+        return self.ctx._new_table("cpb_table_set_int64", self.h, column, C.c_void_p(values.data_ptr()))
 
     def filter_mask(self, mask) -> "Table":
         """the rows where the bool CUDA tensor mask (one value per row) is true, in order: the reference's
         Filter(func(row) bool) with the predicate computed on the GPU"""
         import torch
         keep = _device_tensor(self, mask, (torch.bool,), "filter_mask")
-        h = C.c_void_p(); e = _abi.Error()
-        st = self.ctx.lib.cpb_table_filter_flags(self.ctx.h, self.h, C.c_void_p(keep.data_ptr()), C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
-        return Table(self.ctx, h)
+        return self.ctx._new_table("cpb_table_filter_flags", self.h, C.c_void_p(keep.data_ptr()))
 
     @staticmethod
     def concat(parts: list["Table"]) -> "Table":
         ctx = parts[0].ctx
-        arr = (C.c_void_p * len(parts))(*[p.h for p in parts]); h = C.c_void_p()
-        st = ctx.lib.cpb_table_concat(ctx.h, arr, len(parts), C.byref(h))
-        if st:
-            _raise(st, None, ctx)
-        return Table(ctx, h)
+        arr = (C.c_void_p * len(parts))(*[p.h for p in parts])
+        return ctx._new_table("cpb_table_concat", arr, len(parts))
 
 
 FORMAT_VERBS = "eEfgG"
@@ -716,12 +670,16 @@ def parse_csv(ctx: Context, data, *, on_device=False, nbytes=None, delimiter=","
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
     sa, nspec, pp = _spec_and_pred(spec, pred, keep)
     h = C.c_void_p(); e = _abi.Error()
-    st = ctx.lib.cpb_parse_csv(ctx.h, C.c_void_p(ptr), n, int(dev), C.byref(opts), sa, nspec, pp, C.byref(h), C.byref(e))
-    if st == 1 and h.value:
-        return Table(ctx, h), DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
-    if st:
+    st = ctx._call("cpb_parse_csv", C.c_void_p(ptr), n, int(dev), C.byref(opts), sa, nspec, pp, C.byref(h), err=e, accept=(_abi.CPB_ERR_DATA,))
+    return _rows_before_error(ctx, Table(ctx, h), st, e)
+
+
+def _rows_before_error(ctx: Context, t: "Table | None", st: int, e: _abi.Error) -> tuple:
+    """the outcome of a parse whose status may be CPB_ERR_DATA -> (table of the rows before the error, that error or None);
+    a data error that comes without a table is raised"""
+    if st and (t is None or not t.h.value):
         _raise(st, e, ctx)
-    return Table(ctx, h), None
+    return t, _data_error(e) if st else None
 
 
 def _reader_opts(delimiter=",", comment="", num_fields=0, lazy_quotes=False, trim_leading_space=False,
@@ -764,9 +722,7 @@ def csv_quote_parity(ctx: Context, data, *, nbytes=None, on_device=False) -> int
     keep = []
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
     out = C.c_uint32()
-    st = ctx.lib.cpb_csv_quote_parity(ctx.h, C.c_void_p(ptr), n, int(dev), C.byref(out))
-    if st:
-        _raise(st, None, ctx)
+    ctx._call("cpb_csv_quote_parity", C.c_void_p(ptr), n, int(dev), C.byref(out))
     return out.value
 
 
@@ -777,9 +733,7 @@ def csv_stream_cut(ctx: Context, data, *, nbytes=None, on_device=False, delimite
     keep = []
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
     out = C.c_uint64()
-    st = ctx.lib.cpb_csv_stream_cut(ctx.h, C.c_void_p(ptr), n, int(dev), C.byref(opts), C.byref(out))
-    if st:
-        _raise(st, None, ctx)
+    ctx._call("cpb_csv_stream_cut", C.c_void_p(ptr), n, int(dev), C.byref(opts), C.byref(out))
     return out.value
 
 
@@ -792,13 +746,10 @@ def parse_csv_shard(ctx: Context, data, *, own_bytes: int, shard_index: int, is_
     ptr, n, dev = _input_ptr(data, nbytes, on_device, keep)
     sa, nspec, pp = _spec_and_pred(spec, pred, keep)
     h = C.c_void_p(); e = _abi.Error(); recs = C.c_uint64()
-    st = ctx.lib.cpb_parse_csv_shard(ctx.h, C.c_void_p(ptr), n, int(dev), own_bytes, shard_index, int(is_last), initial_parity, C.byref(opts), sa,
-                                     nspec, pp, C.byref(h), C.byref(recs), C.byref(e))
-    if st == 1 and h.value:
-        return Table(ctx, h), recs.value, DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind)
-    if st:
-        _raise(st, e, ctx)
-    return Table(ctx, h), recs.value, None
+    st = ctx._call("cpb_parse_csv_shard", C.c_void_p(ptr), n, int(dev), own_bytes, shard_index, int(is_last), initial_parity, C.byref(opts), sa,
+                   nspec, pp, C.byref(h), C.byref(recs), err=e, accept=(_abi.CPB_ERR_DATA,))
+    t, err = _rows_before_error(ctx, Table(ctx, h), st, e)
+    return t, recs.value, err
 
 
 # ------------------------------------------------------------------ Index (csvplus.go:610-705)
@@ -817,35 +768,30 @@ class Index:
         return self.ctx.lib.cpb_index_num_rows(self.h)
 
     def table(self) -> Table:
-        h = C.c_void_p()
-        self.ctx.lib.cpb_index_table(self.ctx.h, self.h, C.byref(h))
-        return Table(self.ctx, h)
+        return self.ctx._new_table("cpb_index_table", self.h)
 
     def Iterate(self, fn):  # csvplus.go:618-620
         return TakeTable(self.table(), line_base=0)(fn)
 
     def Find(self, *values) -> "DataSource":  # csvplus.go:625-627
-        a, keep = _strs(values); h = C.c_void_p()
-        st = self.ctx.lib.cpb_index_find(self.ctx.h, self.h, a, len(values), C.byref(h))
-        if st:
-            raise ValueError("too many columns in indexImpl.find()") if st == 2 else CsvPlusError("find failed", st)
-        return TakeTable(Table(self.ctx, h), line_base=0)
+        a, keep = _strs(values)
+        try:
+            return TakeTable(self.ctx._new_table("cpb_index_find", self.h, a, len(values)), line_base=0)
+        except CsvPlusError as e:
+            if e.status != _abi.CPB_ERR_ARG:
+                raise
+            raise ValueError("too many columns in indexImpl.find()") from None
 
     def SubIndex(self, *values) -> "Index":  # csvplus.go:632-641
         if len(values) >= len(self.columns):
             raise ValueError("too many values in SubIndex()")
-        a, keep = _strs(values); h = C.c_void_p()
-        st = self.ctx.lib.cpb_index_sub(self.ctx.h, self.h, a, len(values), C.byref(h))
-        if st:
-            _raise(st, None, self.ctx)
-        return Index(self.ctx, h, self.columns[len(values):])
+        a, keep = _strs(values)
+        return self.ctx._new_index("cpb_index_sub", self.h, a, len(values), columns=self.columns[len(values):])
 
     def dup_groups(self):
         """[lo, hi) sorted-row ranges of every run of >= 2 rows with equal keys (cpb_index_dup_groups) as two int64 arrays"""
         ng = C.c_int64(); lo = C.POINTER(C.c_int64)(); hi = C.POINTER(C.c_int64)()
-        st = self.ctx.lib.cpb_index_dup_groups(self.ctx.h, self.h, C.byref(ng), C.byref(lo), C.byref(hi))
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_index_dup_groups", self.h, C.byref(ng), C.byref(lo), C.byref(hi))
         n = ng.value
         try:
             a = np.ctypeslib.as_array(lo, shape=(max(n, 1),))[:n].copy()
@@ -857,9 +803,7 @@ class Index:
     def dedup_apply(self, keep, bug_compatible: bool = True):
         """keep[g] = sorted position of the row kept for group g, or -1 to drop the group (cpb_index_dedup_apply)"""
         k = np.ascontiguousarray(keep, dtype=np.int64)
-        st = self.ctx.lib.cpb_index_dedup_apply(self.ctx.h, self.h, len(k), k.ctypes.data_as(C.POINTER(C.c_int64)), int(bug_compatible))
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_index_dedup_apply", self.h, len(k), k.ctypes.data_as(C.POINTER(C.c_int64)), int(bug_compatible))
 
     def ResolveDuplicates(self, resolve: Callable[[list[Row]], Row | None], bug_compatible: bool = True):
         """csvplus.go:651-653 / dedup :810-867.  `resolve` gets each group of rows with equal keys and returns the row to
@@ -885,23 +829,15 @@ class Index:
             else:
                 keep[g] = lo[g] + pick
         rt = Table.from_rows(self.ctx, replacements, columns=t.columns) if replacements else None
-        e = _abi.Error()
-        st = self.ctx.lib.cpb_index_dedup_apply2(self.ctx.h, self.h, n, keep.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                 rt.h if rt is not None else None, int(bug_compatible), C.byref(e))
-        if st:
-            _raise(st, e, self.ctx)
+        self.ctx._call("cpb_index_dedup_apply2", self.h, n, keep.ctypes.data_as(C.POINTER(C.c_int64)), rt.h if rt is not None else None,
+                       int(bug_compatible))
 
     def WriteTo(self, fileName: str):  # csvplus.go:655-680: the file is removed on error
         """the index as the reference's encoding/gob file (its key columns, then its rows in stored order), encoded on the
         GPU and written in row-range batches through one pinned buffer.  A path that cannot be created raises the OS
         error and leaves no file; any later error removes the file."""
-        f = open(fileName, "wb")
-        try:
-            with f:
-                self._write_gob(f)
-        except BaseException:
-            os.remove(fileName)
-            raise
+        with _new_file(fileName) as f:
+            self._write_gob(f)
 
     def _write_gob(self, out: io.IOBase):
         # one pinned buffer, sized up front so that the prefix and every batch are serialised in one call each: the prefix
@@ -915,40 +851,16 @@ class Index:
             if rows_bytes > hold[0].nbytes:
                 hold[0].free()
                 hold[:] = [HostBuffer(self.ctx, min(rows_bytes, 1 << 32) + 64)]
-            n, lo, step = len(self), 0, GOB_BATCH_ROWS
-            while lo < n:
-                hi = min(n, lo + step)
-                try:
-                    _write_into(out, hold, self.ctx, lambda buf: self._gob_into(buf, lo, hi))
-                except CsvPlusError as e:
-                    if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
-                        raise
-                    step = (hi - lo) // 2
-                    continue
-                lo = hi
+            _row_batches(len(self), GOB_BATCH_ROWS, lambda lo, hi: _write_into(out, hold, self.ctx, lambda buf: self._gob_into(buf, lo, hi)))
         finally:
             for b in hold:
                 b.free()
 
     def _gob_begin(self, buf: "HostBuffer | None", plen, total) -> int:
-        e = _abi.Error()
-        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
-        st = self.ctx.lib.cpb_index_gob_begin(self.ctx.h, self.h, C.c_void_p(ptr), cap, C.byref(plen), C.byref(total), C.byref(e))
-        if st == 2 and plen.value > cap:  # CPB_ERR_ARG: destination too small
-            return plen.value
-        if st:
-            _raise(st, e, self.ctx)
-        return plen.value
+        return _into(self.ctx, "cpb_index_gob_begin", self.h, dst=buf, size=plen, more=(C.byref(total),))
 
     def _gob_into(self, buf: "HostBuffer | None", lo: int, hi: int) -> int:
-        n = C.c_uint64(); e = _abi.Error()
-        ptr, cap = (buf.ptr, buf.nbytes) if buf is not None else (None, 0)
-        st = self.ctx.lib.cpb_index_gob_into(self.ctx.h, self.h, lo, hi, C.c_void_p(ptr), cap, C.byref(n), C.byref(e))
-        if st == 2 and n.value > cap:  # CPB_ERR_ARG: destination too small
-            return n.value
-        if st:
-            _raise(st, e, self.ctx)
-        return n.value
+        return _into(self.ctx, "cpb_index_gob_into", self.h, lo, hi, dst=buf)
 
 
 def LoadIndex(fileName: str, ctx: Context | None = None) -> Index:  # csvplus.go:683-705
@@ -963,18 +875,14 @@ def LoadIndex(fileName: str, ctx: Context | None = None) -> Index:  # csvplus.go
             got = f.readinto(memoryview(buf.array())[:size]) if size else 0
             if got != size:
                 raise OSError(f"read {fileName}: short read")
-            h = C.c_void_p(); e = _abi.Error()
-            st = ctx.lib.cpb_index_load_gob(ctx.h, C.c_void_p(buf.ptr), size, C.byref(h), C.byref(e))
-            if st:
-                _raise(st, e, ctx)
+            ix = ctx._new_index("cpb_index_load_gob", C.c_void_p(buf.ptr), size, columns=[])
         finally:
             buf.free()
-    cols = []
-    for k in range(ctx.lib.cpb_index_num_keys(h)):
+    for k in range(ctx.lib.cpb_index_num_keys(ix.h)):
         s = _abi.Str()
-        ctx.lib.cpb_index_key_col(h, k, C.byref(s))
-        cols.append(_dec(C.string_at(s.ptr, s.len)))
-    return Index(ctx, h, cols)
+        ctx.lib.cpb_index_key_col(ix.h, k, C.byref(s))
+        ix.columns.append(_dec(C.string_at(s.ptr, s.len)))
+    return ix
 
 
 # ------------------------------------------------------------------ Reader (csvplus.go:922-1146)
@@ -1085,11 +993,8 @@ class _Stream:
         self.ctx, self._keep, self._pushed = ctx, [], None
         o = _reader_opts(**opts)
         sa, nspec, pp = _spec_and_pred(spec, pred, self._keep)  # the predicate is borrowed by the stream until it is freed
-        h = C.c_void_p(); e = _abi.Error()
-        st = ctx.lib.cpb_stream_open(ctx.h, C.byref(o), sa, nspec, pp, C.byref(h), C.byref(e))
-        if st:
-            _raise(st, e, ctx)
-        self.h = h
+        self.h = C.c_void_p()
+        ctx._call("cpb_stream_open", C.byref(o), sa, nspec, pp, C.byref(self.h))
 
     def push(self, piece, last: bool):
         if piece is None:
@@ -1098,19 +1003,13 @@ class _Stream:
             a = piece if isinstance(piece, np.ndarray) else np.frombuffer(piece, np.uint8)
             ptr, n = a.ctypes.data, a.size
         self._pushed = piece  # untouched until the next cpb_stream_next returns
-        st = self.ctx.lib.cpb_stream_push(self.h, C.c_void_p(ptr), n, int(last))
-        if st:
-            _raise(st, None, self.ctx)
+        self.ctx._call("cpb_stream_push", C.c_void_p(ptr), n, int(last), h=self.h)
 
     def next(self):
         h = C.c_void_p(); done = C.c_int(); e = _abi.Error()
-        st = self.ctx.lib.cpb_stream_next(self.h, C.byref(h), C.byref(done), C.byref(e))
-        t = Table(self.ctx, h) if h.value else None
-        if st == 1 and t is not None:
-            return t, DataSourceError(e.line, e.msg.decode("utf-8", "replace"), e.kind), True
-        if st:
-            _raise(st, e, self.ctx)
-        return t, None, bool(done.value)
+        st = self.ctx._call("cpb_stream_next", C.byref(h), C.byref(done), err=e, accept=(_abi.CPB_ERR_DATA,), h=self.h)
+        t, err = _rows_before_error(self.ctx, Table(self.ctx, h) if h.value else None, st, e)
+        return t, err, bool(st or done.value)
 
     def free(self):
         if self.h:
@@ -1467,13 +1366,8 @@ class DataSource:
                 b.free()
 
     def ToCsvFile(self, name: str, *columns):  # csvplus.go:411-443: the file is removed on error
-        try:
-            with open(name, "wb") as f:
-                self.ToCsv(f, *columns)
-        except BaseException:
-            if os.path.exists(name):
-                os.remove(name)
-            raise
+        with _new_file(name) as f:
+            self.ToCsv(f, *columns)
 
     def ToJSON(self, out: io.IOBase):  # csvplus.go:446-474
         """all rows as a JSON array, formatted the way the reference's json.Encoder (SetEscapeHTML(false), no indent) writes
@@ -1503,13 +1397,8 @@ class DataSource:
                 b.free()
 
     def ToJSONFile(self, name: str):  # csvplus.go:477-479
-        try:
-            with open(name, "wb") as f:
-                self.ToJSON(f)
-        except BaseException:
-            if os.path.exists(name):
-                os.remove(name)
-            raise
+        with _new_file(name) as f:
+            self.ToJSON(f)
 
     def ToTensors(self, columns: dict) -> dict:
         """{name: "int" | "float64"} -> {name: CUDA tensor}: Row.ValueAsInt / ValueAsFloat64 of every row of each column,
@@ -1517,23 +1406,14 @@ class DataSource:
         error raised is the one a RowFunc converting the columns in dict order would meet first: the lowest failing row,
         ties to the earlier column (CsvPlusError, .row = the row).  When no row fails, a pending source error is raised:
         the table only holds the rows delivered before it."""
-        kinds = {}
-        for name, kind in columns.items():
-            if kind not in ("int", "float64"):
-                raise ValueError(f"ToTensors: unknown type {kind!r} for column {name!r} (want 'int' or 'float64')")
-            kinds[name] = kind == "float64"
+        kinds = _tensor_kinds(columns, "ToTensors")
         t, err = self._table()
         if t is None:
             import torch
             dev = torch.device("cuda", self._ctx().device)
             out = {name: torch.empty(0, dtype=torch.float64 if f else torch.int64, device=dev) for name, f in kinds.items()}
         else:
-            out, first = {}, None
-            for name, is_float in kinds.items():
-                values, _, e = t._convert(name, is_float)
-                out[name] = values
-                if e is not None and (first is None or e.row < first.row):
-                    first = e
+            out, first = _convert_all(t, kinds)
             if first is not None:
                 raise first
         if err is not None:
@@ -1559,15 +1439,22 @@ class DataSource:
         return t.index_on(*columns, unique=unique)
 
 
-def _tensor_step(t: Table, op, seen: int):
-    """MapTensors / FilterTensors over one batch -> (table, CsvPlusError of the first failing conversion or None)"""
-    kind, kinds, fn = op
+def _convert_all(t: Table, kinds: dict) -> tuple:
+    """Table._convert of every input -> ({name: values}, CsvPlusError of the lowest failing row, ties to the earlier
+    input, or None)"""
     vals, first = {}, None
     for name, is_float in kinds.items():
         values, _, e = t._convert(name, is_float)
         vals[name] = values
         if e is not None and (first is None or e.row < first.row):
             first = e
+    return vals, first
+
+
+def _tensor_step(t: Table, op, seen: int):
+    """MapTensors / FilterTensors over one batch -> (table, CsvPlusError of the first failing conversion or None)"""
+    kind, kinds, fn = op
+    vals, first = _convert_all(t, kinds)
     err = None
     if first is not None:
         err = CsvPlusError(str(first), first.status, first.kind)
@@ -1606,6 +1493,48 @@ def _json_rows(rows: list, first: bool, last: bool) -> bytes:
     return b"".join(parts)
 
 
+@contextlib.contextmanager
+def _new_file(name: str):
+    """name opened for writing; any error while it is written removes it.  A path that cannot be created raises the OS
+    error and leaves nothing behind."""
+    f = open(name, "wb")
+    try:
+        with f:
+            yield f
+    except BaseException:
+        os.remove(name)
+        raise
+
+
+def _into(ctx: Context, name: str, *args, dst: "HostBuffer | None", offset: int = 0, size=None, more: tuple = ()) -> int:
+    """an entry that writes into caller-owned host memory: args are followed by the room of dst from offset on (none when
+    dst is None), the size out-parameter and more.  Returns the size the entry reports; when that exceeds the room the
+    entry answered CPB_ERR_ARG and wrote nothing."""
+    size = C.c_uint64() if size is None else size
+    e = _abi.Error()
+    ptr, cap = (dst.ptr + offset, dst.nbytes - offset) if dst is not None else (None, 0)
+    st = ctx._call(name, *args, C.c_void_p(ptr), cap, C.byref(size), *more, err=e, accept=(_abi.CPB_ERR_ARG,))
+    if st and size.value <= cap:
+        _raise(st, e, ctx)
+    return size.value
+
+
+def _row_batches(n: int, step: int, write: Callable[[int, int], None]):
+    """write(lo, hi) for row ranges of at most step rows that cover [0, n); a range that fails with CPB_E_TOO_LARGE is
+    halved"""
+    lo = 0
+    while lo < n:
+        hi = min(n, lo + step)
+        try:
+            write(lo, hi)
+        except CsvPlusError as e:
+            if e.kind != _abi.CPB_E_TOO_LARGE or hi - lo < 2:
+                raise
+            step = (hi - lo) // 2
+            continue
+        lo = hi
+
+
 def _write_into(out: io.IOBase, hold: list, ctx: Context, serialise: Callable[["HostBuffer | None"], int]):
     """serialise(buf) writes one batch into the pinned buffer buf and returns its size, or writes nothing when the size
     exceeds buf (or buf is None).  The buffer hold[0] is grown to the size reported and the batch serialised again, then
@@ -1625,18 +1554,12 @@ def _write_into(out: io.IOBase, hold: list, ctx: Context, serialise: Callable[["
 def _json_batches(t: Table, out: io.IOBase, first: bool, hold: list):
     """ToJSON of a device table with rows, without the closing `]`: row-range slices of at most JSON_BATCH_ROWS rows, each
     written through the pinned buffer of hold (_write_into).  first: the table opens the array."""
-    n, lo, step = len(t), 0, JSON_BATCH_ROWS
-    while lo < n:
-        hi = min(n, lo + step)
+    n = len(t)
+
+    def write(lo, hi):
         part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
-        try:
-            _write_into(out, hold, t.ctx, lambda buf: part.to_json_into(buf, 0, first and lo == 0, False))
-        except CsvPlusError as e:
-            if e.kind != 13 or hi - lo < 2:  # CPB_E_TOO_LARGE: halve the batch
-                raise
-            step = (hi - lo) // 2
-            continue
-        lo = hi
+        _write_into(out, hold, t.ctx, lambda buf: part.to_json_into(buf, 0, first and lo == 0, False))
+    _row_batches(n, JSON_BATCH_ROWS, write)
 
 
 def Take(src) -> DataSource:  # csvplus.go:252-256

@@ -140,11 +140,77 @@ int translate_exception(Ctx* c, cpb_error* err) {
 }  // namespace cpb
 
 static std::vector<std::string> str_list(const cpb_str* s, int n) {
+    need(n <= 0 || s, "null string list");
     std::vector<std::string> v;
     for (int i = 0; i < n; i++) v.push_back(to_string(s[i]));
     return v;
 }
 static cpb_table* wrap(std::shared_ptr<Table> t) { return new cpb_table{std::move(t)}; }
+
+// the table behind a handle the caller must pass
+static const Table& table_of(const cpb_table* t) {
+    need(t, "null table");
+    return *t->t;
+}
+static Index& index_of(const cpb_index* ix) {
+    need(ix, "null index");
+    return *ix->ix;
+}
+
+// ------------------------------------------------------------------ ToCsv / ToJSON / index file output
+// Where a serialiser's bytes go.  pinned: new pinned host memory, returned in *bytes; into: caller-owned (ideally
+// pinned) host memory of cap bytes at host_dst; device: new device memory, returned in *bytes.
+struct Dest {
+    enum Mode { pinned, into, device } mode;
+    void** bytes; void* host_dst; uint64_t cap;
+    void check() const { need(mode == into ? !cap || host_dst : bytes != nullptr, "null destination"); }
+    uint64_t limit() const { return mode == into ? cap : UINT64_MAX; }  // the most bytes the serialiser may produce
+};
+static void deliver(Ctx* c, const Buf& out, uint64_t total, const Dest& d, const char* too_small) {
+    if (d.mode == Dest::pinned) {
+        void* hp = nullptr;
+        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
+        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        *d.bytes = hp;
+    } else if (d.mode == Dest::into) {
+        if (total > d.cap) throw ArgError{CPB_ERR_ARG, too_small};
+        if (total) {
+            KernelTimer kt(c, "d2h_output", total, 0);
+            CPB_CUDA(cudaMemcpyAsync(d.host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
+        }
+        sync_stream(c);
+    } else {
+        void* dp = nullptr;
+        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
+        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
+        *d.bytes = dp;
+    }
+}
+// One serialiser call: produce(c, room, &total) returns the bytes on the device, or null after its length pass when
+// total exceeds room.  *nbytes = total either way; a destination that is too small gets nothing and the call fails with
+// CPB_ERR_ARG (too_small).
+template <class F> static int serialise(cpb_ctx* h, cpb_error* err, const Dest& d, uint64_t* nbytes, const char* too_small, F&& produce) {
+    return guarded(h, err, [&](Ctx* c) {
+        need(nbytes, "null nbytes");
+        d.check();
+        uint64_t total = 0;
+        Buf out = produce(c, d.limit(), &total);
+        *nbytes = total;
+        deliver(c, out, total, d, too_small);
+        return CPB_OK;
+    });
+}
+
+// *out = make(c, t's table): the entries that derive one table from another (views and computed columns)
+template <class F> static int derived_table(cpb_ctx* h, const cpb_table* t, cpb_table** out, cpb_error* err, F&& make) {
+    return guarded(h, err, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(out, "null out");
+        *out = wrap(make(c, T));
+        return CPB_OK;
+    });
+}
 
 extern "C" {
 
@@ -219,90 +285,79 @@ void* cpb_ctx_stream(cpb_ctx* h) { return h ? (void*)h->c.stream : nullptr; }
 const char* cpb_last_error(cpb_ctx* h) { return h ? h->c.last_error.c_str() : ""; }
 
 int cpb_sync(cpb_ctx* h) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    sync_stream(c);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        sync_stream(c);
+        return CPB_OK;
+    });
 }
 
 int cpb_pool_reserve(cpb_ctx* h, uint64_t nbytes) {
-    if (!h) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (nbytes == 0) return CPB_OK;
-    void* p = nullptr;
-    CPB_CUDA(cudaMallocAsync(&p, nbytes, c->pool, c->stream));
-    CPB_CUDA(cudaFreeAsync(p, c->stream));
-    sync_stream(c);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        if (nbytes == 0) return CPB_OK;
+        void* p = nullptr;
+        CPB_CUDA(cudaMallocAsync(&p, nbytes, c->pool, c->stream));
+        CPB_CUDA(cudaFreeAsync(p, c->stream));
+        sync_stream(c);
+        return CPB_OK;
+    });
 }
 
 int cpb_pool_used_high(cpb_ctx* h, int reset, uint64_t* bytes) {
-    if (!h || !bytes) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    uint64_t v = 0;  // the attribute is a cuuint64_t (64-bit unsigned)
-    if (reset) CPB_CUDA(cudaMemPoolSetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
-    CPB_CUDA(cudaMemPoolGetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
-    *bytes = (uint64_t)v;
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(bytes, "null bytes");
+        uint64_t v = 0;  // the attribute is a cuuint64_t (64-bit unsigned)
+        if (reset) CPB_CUDA(cudaMemPoolSetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
+        CPB_CUDA(cudaMemPoolGetAttribute(c->pool, cudaMemPoolAttrUsedMemHigh, &v));
+        *bytes = (uint64_t)v;
+        return CPB_OK;
+    });
 }
 
 int cpb_host_alloc(cpb_ctx* h, uint64_t n, void** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    CPB_CUDA(cudaMallocHost(out, n ? n : 1));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx*) {
+        need(out, "null out");
+        CPB_CUDA(cudaMallocHost(out, n ? n : 1));
+        return CPB_OK;
+    });
 }
 int cpb_host_free(cpb_ctx* h, void* p) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    sync_stream(c);
-    CPB_CUDA(cudaFreeHost(p));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        sync_stream(c);
+        CPB_CUDA(cudaFreeHost(p));
+        return CPB_OK;
+    });
 }
 int cpb_device_alloc(cpb_ctx* h, uint64_t n, void** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    uint64_t padded = ((n + 15) & ~15ull) + 256;
-    CPB_CUDA(cudaMallocAsync(out, padded, c->pool, c->stream));
-    CPB_CUDA(cudaMemsetAsync((uint8_t*)*out + (n & ~15ull), 0, padded - (n & ~15ull), c->stream));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(out, "null out");
+        uint64_t padded = ((n + 15) & ~15ull) + 256;
+        CPB_CUDA(cudaMallocAsync(out, padded, c->pool, c->stream));
+        CPB_CUDA(cudaMemsetAsync((uint8_t*)*out + (n & ~15ull), 0, padded - (n & ~15ull), c->stream));
+        return CPB_OK;
+    });
 }
 int cpb_device_free(cpb_ctx* h, void* p) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (p) CPB_CUDA(cudaFreeAsync(p, c->stream));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        if (p) CPB_CUDA(cudaFreeAsync(p, c->stream));
+        return CPB_OK;
+    });
 }
-int cpb_memcpy_h2d(cpb_ctx* h, void* dst, const void* src, uint64_t n) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    CPB_CUDA(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, c->stream));
-    sync_stream(c);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+static int copy_sync(cpb_ctx* h, void* dst, const void* src, uint64_t n, cudaMemcpyKind kind) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(!n || (dst && src), "null copy source or destination");
+        CPB_CUDA(cudaMemcpyAsync(dst, src, n, kind, c->stream));
+        sync_stream(c);
+        return CPB_OK;
+    });
 }
-int cpb_memcpy_d2h(cpb_ctx* h, void* dst, const void* src, uint64_t n) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    CPB_CUDA(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
-}
+int cpb_memcpy_h2d(cpb_ctx* h, void* dst, const void* src, uint64_t n) { return copy_sync(h, dst, src, n, cudaMemcpyHostToDevice); }
+int cpb_memcpy_d2h(cpb_ctx* h, void* dst, const void* src, uint64_t n) { return copy_sync(h, dst, src, n, cudaMemcpyDeviceToHost); }
 
 // ------------------------------------------------------------------ parse
 // host input is copied into a device buffer (32 MiB size classes: batches reuse pool blocks) followed by at least 16 zero
 // bytes; device input is used in place
 static const uint8_t* stage_input(Ctx* c, const void* bytes, uint64_t nbytes, int on_device, Buf& staged) {
+    need(!nbytes || bytes, "null input bytes");
     if (on_device) return (const uint8_t*)bytes;
     staged = dev_alloc(c, (nbytes + 32 + (32u << 20) - 1) / (32u << 20) * (32u << 20));  // holds the zeroed 32 bytes too
     CPB_CUDA(cudaMemsetAsync(staged->as<uint8_t>() + (nbytes & ~15ull), 0, 32, c->stream));
@@ -314,6 +369,7 @@ static const uint8_t* stage_input(Ctx* c, const void* bytes, uint64_t nbytes, in
 }
 // the (name, index) pairs of a reader's header spec; a name given twice is an error (csvplus.go:1047-1049)
 static std::vector<std::pair<std::string, int>> header_spec(const cpb_header_col* spec, int nspec) {
+    need(nspec >= 0 && (nspec == 0 || spec), "bad header spec");
     std::vector<std::pair<std::string, int>> sp;
     for (int i = 0; i < nspec; i++) {
         std::string nm = to_string(spec[i].name);
@@ -325,52 +381,45 @@ static std::vector<std::pair<std::string, int>> header_spec(const cpb_header_col
 
 int cpb_parse_csv(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts,
                   const cpb_header_col* spec, int nspec, const cpb_pred* filter, cpb_table** out, cpb_error* err) {
-    if (!h || !out || !opts || (nbytes && !bytes) || nspec < 0) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    auto sp = header_spec(spec, nspec);
-    Buf staged;
-    const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, opts->header_from_first_row ? 2 : 1);
-    *out = wrap(p.table);
-    return p.error ? data_error(err, *p.error) : CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        need(out && opts, "null out or opts");
+        *out = nullptr;
+        auto sp = header_spec(spec, nspec);
+        Buf staged;
+        const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
+        const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, opts->header_from_first_row ? 2 : 1);
+        *out = wrap(p.table);
+        return p.error ? data_error(err, *p.error) : CPB_OK;
+    });
 }
 
 // ------------------------------------------------------------------ streamed input (stream.cu)
 int cpb_stream_open(cpb_ctx* h, const cpb_reader_opts* opts, const cpb_header_col* spec, int nspec, const cpb_pred* filter,
                     cpb_stream** out, cpb_error* err) {
-    if (!h || !out || !opts || nspec < 0) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    *out = new cpb_stream{stream_open(c, *opts, header_spec(spec, nspec), filter)};
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        need(out && opts, "null out or opts");
+        *out = nullptr;
+        *out = new cpb_stream{stream_open(c, *opts, header_spec(spec, nspec), filter)};
+        return CPB_OK;
+    });
 }
 int cpb_stream_push(cpb_stream* st, const void* bytes, uint64_t nbytes, int is_last) {
-    if (!st || (nbytes && !bytes)) return CPB_ERR_ARG;
-    Ctx* c = stream_ctx(st->s); DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    stream_push(st->s, bytes, nbytes, is_last != 0);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(st ? stream_ctx(st->s) : nullptr, nullptr, [&](Ctx*) {
+        need(!nbytes || bytes, "null input bytes");
+        stream_push(st->s, bytes, nbytes, is_last != 0);
+        return CPB_OK;
+    });
 }
 int cpb_stream_next(cpb_stream* st, cpb_table** out, int* done, cpb_error* err) {
-    if (!st || !out || !done) return CPB_ERR_ARG;
-    Ctx* c = stream_ctx(st->s); DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr; *done = 0;
-    CPB_TRY(c, err)
-    bool fin = false;
-    const Parsed p = stream_next(st->s, &fin);
-    *done = fin ? 1 : 0;
-    if (p.table) *out = wrap(p.table);
-    return p.error ? data_error(err, *p.error) : CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(st ? stream_ctx(st->s) : nullptr, err, [&](Ctx*) {
+        need(out && done, "null out or done");
+        *out = nullptr; *done = 0;
+        bool fin = false;
+        const Parsed p = stream_next(st->s, &fin);
+        *done = fin ? 1 : 0;
+        if (p.table) *out = wrap(p.table);
+        return p.error ? data_error(err, *p.error) : CPB_OK;
+    });
 }
 void cpb_stream_free(cpb_stream* st) {
     if (!st) return;
@@ -380,61 +429,61 @@ void cpb_stream_free(cpb_stream* st) {
 }
 
 // ------------------------------------------------------------------ byte-range shards of one file (SURVEY §8e)
-int cpb_csv_quote_parity(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, uint32_t* parity) {
-    if (!h || !parity || (nbytes && !bytes)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    Buf staged;
+// the input of the shard helpers on the device: they read 16 bytes at a time
+static const uint8_t* stage_aligned(Ctx* c, const void* bytes, uint64_t nbytes, int on_device, Buf& staged) {
     const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    if ((reinterpret_cast<uintptr_t>(dev) & 15) != 0) throw ArgError{CPB_ERR_ARG, "device input must be 16-byte aligned"};
-    *parity = quote_parity(c, dev, nbytes);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    need((reinterpret_cast<uintptr_t>(dev) & 15) == 0, "device input must be 16-byte aligned");
+    return dev;
+}
+int cpb_csv_quote_parity(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, uint32_t* parity) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(parity, "null parity");
+        Buf staged;
+        *parity = quote_parity(c, stage_aligned(c, bytes, nbytes, on_device, staged), nbytes);
+        return CPB_OK;
+    });
 }
 int cpb_csv_stream_cut(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, const cpb_reader_opts* opts, uint64_t* cut) {
-    if (!h || !cut || !opts || (nbytes && !bytes)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    Buf staged;
-    const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    if ((reinterpret_cast<uintptr_t>(dev) & 15) != 0) throw ArgError{CPB_ERR_ARG, "device input must be 16-byte aligned"};
-    Buf out = dev_alloc(c, 16);
-    stream_cut(c, dev, nbytes, *opts, out->as<uint64_t>());
-    *cut = read_back<uint64_t>(c, out->p);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(cut && opts, "null cut or opts");
+        Buf staged;
+        const uint8_t* dev = stage_aligned(c, bytes, nbytes, on_device, staged);
+        Buf out = dev_alloc(c, 16);
+        stream_cut(c, dev, nbytes, *opts, out->as<uint64_t>());
+        *cut = read_back<uint64_t>(c, out->p);
+        return CPB_OK;
+    });
 }
 int cpb_parse_csv_shard(cpb_ctx* h, const void* bytes, uint64_t nbytes, int on_device, uint64_t own_bytes, int shard_index, int is_last,
                         uint32_t initial_parity, const cpb_reader_opts* opts, const cpb_header_col* spec, int nspec, const cpb_pred* filter,
                         cpb_table** out, uint64_t* records, cpb_error* err) {
-    if (!h || !out || !opts || (nbytes && !bytes) || nspec < 0 || shard_index < 0) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    std::vector<std::pair<std::string, int>> sp;
-    for (int i = 0; i < nspec; i++) sp.emplace_back(to_string(spec[i].name), spec[i].index);
-    Buf staged;
-    const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
-    const uint64_t base = opts->header_from_first_row ? 2 : 1;
-    const ShardArgs sh{own_bytes, shard_index, is_last != 0, initial_parity};
-    const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, base, &sh);
-    if (records) *records = p.records;
-    *out = wrap(p.table);
-    if (!p.error) return CPB_OK;
-    // the line is LOCAL: (0-based) ordinal of the failing record among this shard's records; the host adds the records
-    // of the shards before it and the reader's base (csvplus.go:1102-1137)
-    DataError local = *p.error;
-    local.line = local.line >= base ? local.line - base : 0;
-    return data_error(err, local);
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) -> int {
+        need(out && opts, "null out or opts");
+        need(shard_index >= 0 && nspec >= 0 && (nspec == 0 || spec), "bad shard index or header spec");
+        *out = nullptr;
+        std::vector<std::pair<std::string, int>> sp;
+        for (int i = 0; i < nspec; i++) sp.emplace_back(to_string(spec[i].name), spec[i].index);
+        Buf staged;
+        const uint8_t* dev = stage_input(c, bytes, nbytes, on_device, staged);
+        const uint64_t base = opts->header_from_first_row ? 2 : 1;
+        const ShardArgs sh{own_bytes, shard_index, is_last != 0, initial_parity};
+        const Parsed p = parse_csv(c, dev, nbytes, *opts, sp, filter, base, &sh);
+        if (records) *records = p.records;
+        *out = wrap(p.table);
+        if (!p.error) return CPB_OK;
+        // the line is LOCAL: (0-based) ordinal of the failing record among this shard's records; the host adds the records
+        // of the shards before it and the reader's base (csvplus.go:1102-1137)
+        DataError local = *p.error;
+        local.line = local.line >= base ? local.line - base : 0;
+        return data_error(err, local);
+    });
 }
 
 // ------------------------------------------------------------------ tables
 int64_t cpb_table_num_rows(const cpb_table* t) { return t ? t->t->nrows : -1; }
 int cpb_table_num_cols(const cpb_table* t) { return t ? (int)t->t->cols.size() : -1; }
 int cpb_table_col_name(const cpb_table* t, int col, cpb_str* out) {
-    if (!t || col < 0 || col >= (int)t->t->cols.size()) return CPB_ERR_ARG;
+    if (!t || !out || col < 0 || col >= (int)t->t->cols.size()) return CPB_ERR_ARG;
     out->ptr = t->t->cols[col].name.data(); out->len = t->t->cols[col].name.size();
     return CPB_OK;
 }
@@ -445,168 +494,168 @@ int cpb_table_col_field(const cpb_table* t, int col) {
 }
 int cpb_table_record_fields(const cpb_table* t) { return t ? t->t->record_fields : -1; }
 
-int cpb_table_col_bytes(cpb_ctx* h, const cpb_table* t, int col, int64_t lo, int64_t hi, uint64_t* nbytes) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    const Table& T = *t->t;
+static void need_rows(const Table& T, int col, int64_t lo, int64_t hi) {
     if (col < 0 || col >= (int)T.cols.size() || lo < 0 || hi < lo || hi > T.nrows) throw ArgError{CPB_ERR_ARG, "bad column/row range"};
-    uint32_t e[2];
-    CPB_CUDA(cudaMemcpyAsync(&e[0], T.cols[col].off() + lo, 4, cudaMemcpyDeviceToHost, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(&e[1], T.cols[col].off() + hi, 4, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    *nbytes = e[1] - e[0];
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+}
+
+int cpb_table_col_bytes(cpb_ctx* h, const cpb_table* t, int col, int64_t lo, int64_t hi, uint64_t* nbytes) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(nbytes, "null nbytes");
+        need_rows(T, col, lo, hi);
+        uint32_t e[2];
+        CPB_CUDA(cudaMemcpyAsync(&e[0], T.cols[col].off() + lo, 4, cudaMemcpyDeviceToHost, c->stream));
+        CPB_CUDA(cudaMemcpyAsync(&e[1], T.cols[col].off() + hi, 4, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        *nbytes = e[1] - e[0];
+        return CPB_OK;
+    });
 }
 
 int cpb_table_fetch_column(cpb_ctx* h, const cpb_table* t, int col, int64_t lo, int64_t hi, int64_t* offsets_out,
                            uint8_t* data_out, uint64_t cap) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    const Table& T = *t->t;
-    if (col < 0 || col >= (int)T.cols.size() || lo < 0 || hi < lo || hi > T.nrows) throw ArgError{CPB_ERR_ARG, "bad column/row range"};
-    size_t cnt = (size_t)(hi - lo) + 1;
-    std::vector<uint32_t> tmp(cnt);
-    CPB_CUDA(cudaMemcpyAsync(tmp.data(), T.cols[col].off() + lo, cnt * 4, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    uint64_t total = tmp[cnt - 1] - tmp[0];
-    if (offsets_out) for (size_t i = 0; i < cnt; i++) offsets_out[i] = (int64_t)(tmp[i] - tmp[0]);
-    if (data_out) {
-        if (total > cap) throw ArgError{CPB_ERR_ARG, "data_out too small"};
-        if (total) {
-            CPB_CUDA(cudaMemcpyAsync(data_out, T.cols[col].bytes() + tmp[0], total, cudaMemcpyDeviceToHost, c->stream));
-            sync_stream(c);
+    return guarded(h, nullptr, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need_rows(T, col, lo, hi);
+        size_t cnt = (size_t)(hi - lo) + 1;
+        std::vector<uint32_t> tmp(cnt);
+        CPB_CUDA(cudaMemcpyAsync(tmp.data(), T.cols[col].off() + lo, cnt * 4, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        uint64_t total = tmp[cnt - 1] - tmp[0];
+        if (offsets_out) for (size_t i = 0; i < cnt; i++) offsets_out[i] = (int64_t)(tmp[i] - tmp[0]);
+        if (data_out) {
+            if (total > cap) throw ArgError{CPB_ERR_ARG, "data_out too small"};
+            if (total) {
+                CPB_CUDA(cudaMemcpyAsync(data_out, T.cols[col].bytes() + tmp[0], total, cudaMemcpyDeviceToHost, c->stream));
+                sync_stream(c);
+            }
         }
-    }
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+        return CPB_OK;
+    });
 }
 
 int cpb_table_column_device(const cpb_table* t, int col, const uint32_t** offsets, const uint8_t** data) {
-    if (!t || col < 0 || col >= (int)t->t->cols.size()) return CPB_ERR_ARG;
+    if (!t || !offsets || !data || col < 0 || col >= (int)t->t->cols.size()) return CPB_ERR_ARG;
     *offsets = t->t->cols[col].off(); *data = t->t->cols[col].bytes();
     return CPB_OK;
 }
 
+// the arguments of a table given as ncols arrays of nrows values
+static void need_columns(int ncols, const cpb_str* names, const void* offsets, const void* data, int64_t nrows, cpb_table** out) {
+    need(out, "null out");
+    need(nrows >= 0 && (ncols <= 0 || (names && offsets && data)), "bad column arrays");
+}
+
 int cpb_table_from_host(cpb_ctx* h, int ncols, const cpb_str* names, const int64_t* const* offsets,
                         const uint8_t* const* data, int64_t nrows, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    auto t = std::make_shared<Table>(); t->ctx = c; t->nrows = nrows;
-    for (int i = 0; i < ncols; i++) {
-        Column col; col.name = to_string(names[i]);
-        std::vector<uint32_t> off((size_t)nrows + 1);
-        for (int64_t r = 0; r <= nrows; r++) {
-            int64_t v = offsets[i][r] - offsets[i][0];
-            if (v < 0 || v > 0xffffffffll) throw DataError{CPB_E_TOO_LARGE, i, 0, false, "column exceeds 4 GiB"};
-            off[(size_t)r] = (uint32_t)v;
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need_columns(ncols, names, offsets, data, nrows, out);
+        auto t = std::make_shared<Table>(); t->ctx = c; t->nrows = nrows;
+        for (int i = 0; i < ncols; i++) {
+            need(offsets[i], "null column offsets");
+            Column col; col.name = to_string(names[i]);
+            std::vector<uint32_t> off((size_t)nrows + 1);
+            for (int64_t r = 0; r <= nrows; r++) {
+                int64_t v = offsets[i][r] - offsets[i][0];
+                if (v < 0 || v > 0xffffffffll) throw DataError{CPB_E_TOO_LARGE, i, 0, false, "column exceeds 4 GiB"};
+                off[(size_t)r] = (uint32_t)v;
+            }
+            col.offsets = dev_alloc(c, off.size() * 4);
+            CPB_CUDA(cudaMemcpyAsync(col.offsets->p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+            uint64_t total = off.back();
+            need(!total || data[i], "null column data");
+            col.data = dev_alloc(c, total + 16);
+            if (total) CPB_CUDA(cudaMemcpyAsync(col.data->p, data[i] + offsets[i][0], total, cudaMemcpyHostToDevice, c->stream));
+            sync_stream(c);
+            t->cols.push_back(col);
         }
-        col.offsets = dev_alloc(c, off.size() * 4);
-        CPB_CUDA(cudaMemcpyAsync(col.offsets->p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
-        uint64_t total = off.back();
-        col.data = dev_alloc(c, total + 16);
-        if (total) CPB_CUDA(cudaMemcpyAsync(col.data->p, data[i] + offsets[i][0], total, cudaMemcpyHostToDevice, c->stream));
-        sync_stream(c);
-        t->cols.push_back(col);
-    }
-    *out = wrap(t);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+        *out = wrap(t);
+        return CPB_OK;
+    });
 }
 
 int cpb_table_from_device(cpb_ctx* h, int ncols, const cpb_str* names, const uint32_t* const* offsets,
                           const uint8_t* const* data, int64_t nrows, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    // the caller's arrays are wrapped without ownership and copied by the concat path, which rebases offsets that do not
-    // start at 0 (row-range views exported by cpb_table_column_device) and reads all extents with one host round trip
-    Table view; view.ctx = c; view.nrows = nrows;
-    for (int i = 0; i < ncols; i++) {
-        Column col; col.name = to_string(names[i]);
-        col.offsets = std::make_shared<DevBuf>(DevBuf::Borrow{}, offsets[i], ((size_t)nrows + 1) * 4);
-        col.data = std::make_shared<DevBuf>(DevBuf::Borrow{}, data[i], 0);
-        view.cols.push_back(col);
-    }
-    *out = wrap(concat_tables(c, {&view}));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need_columns(ncols, names, offsets, data, nrows, out);
+        // the caller's arrays are wrapped without ownership and copied by the concat path, which rebases offsets that do not
+        // start at 0 (row-range views exported by cpb_table_column_device) and reads all extents with one host round trip
+        Table view; view.ctx = c; view.nrows = nrows;
+        for (int i = 0; i < ncols; i++) {
+            need(offsets[i], "null column offsets");
+            Column col; col.name = to_string(names[i]);
+            col.offsets = std::make_shared<DevBuf>(DevBuf::Borrow{}, offsets[i], ((size_t)nrows + 1) * 4);
+            col.data = std::make_shared<DevBuf>(DevBuf::Borrow{}, data[i], 0);
+            view.cols.push_back(col);
+        }
+        *out = wrap(concat_tables(c, {&view}));
+        return CPB_OK;
+    });
 }
 
 int cpb_table_select(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, cpb_table** out, cpb_error* err) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    if (n <= 0) throw ArgError{CPB_ERR_ARG, "no columns specified in SelectColumns()"};  // csvplus.go:512-514
-    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = t->t->nrows; r->first_line = t->t->first_line;
-    for (int i = 0; i < n; i++) {
-        std::string nm = to_string(cols[i]);
-        int k = t->t->find(nm);
-        if (k < 0) {
-            if (t->t->nrows == 0) { *out = wrap(r); r->cols.clear(); return CPB_OK; }  // no rows => Row.Select never runs
-            throw DataError{CPB_E_MISSING_COLUMN, i, t->t->first_line, true, "missing column " + go_quote(nm)};  // csvplus.go:129
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        if (n <= 0) throw ArgError{CPB_ERR_ARG, "no columns specified in SelectColumns()"};  // csvplus.go:512-514
+        auto names = str_list(cols, n);
+        std::vector<int> pick;
+        for (int i = 0; i < n; i++) {
+            int k = T.find(names[i]);
+            if (k < 0) {
+                if (T.nrows == 0) { pick.clear(); break; }  // no rows => Row.Select never runs
+                throw DataError{CPB_E_MISSING_COLUMN, i, T.first_line, true, "missing column " + go_quote(names[i])};  // csvplus.go:129
+            }
+            if (std::find(pick.begin(), pick.end(), k) == pick.end()) pick.push_back(k);  // a Go map holds a name once
         }
-        bool dup = false;
-        for (auto& cc : r->cols) if (cc.name == nm) dup = true;  // a Go map holds a name once
-        if (!dup) r->cols.push_back(t->t->cols[k]);
-    }
-    *out = wrap(r);
-    return CPB_OK;
-    CPB_CATCH(c, err)
+        auto r = table_view(c, T, 0, T.nrows, &pick); r->first_line = T.first_line;
+        return r;
+    });
 }
 
 int cpb_table_drop(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (n <= 0) throw ArgError{CPB_ERR_ARG, "no columns specified in DropColumns()"};  // csvplus.go:494-496
-    auto names = str_list(cols, n);
-    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = t->t->nrows; r->first_line = t->t->first_line;
-    for (auto& col : t->t->cols)
-        if (std::find(names.begin(), names.end(), col.name) == names.end()) r->cols.push_back(col);
-    *out = wrap(r);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return derived_table(h, t, out, nullptr, [&](Ctx* c, const Table& T) {
+        if (n <= 0) throw ArgError{CPB_ERR_ARG, "no columns specified in DropColumns()"};  // csvplus.go:494-496
+        auto names = str_list(cols, n);
+        std::vector<int> pick;
+        for (int k = 0; k < (int)T.cols.size(); k++)
+            if (std::find(names.begin(), names.end(), T.cols[k].name) == names.end()) pick.push_back(k);
+        auto r = table_view(c, T, 0, T.nrows, &pick); r->first_line = T.first_line;
+        return r;
+    });
 }
 
 int cpb_table_slice(cpb_ctx* h, const cpb_table* t, int64_t lo, int64_t hi, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    const Table& T = *t->t;
-    if (lo < 0) lo = 0;
-    if (hi > T.nrows) hi = T.nrows;
-    if (hi < lo) hi = lo;
-    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = hi - lo; r->first_line = T.first_line + (uint64_t)lo;
-    for (auto col : T.cols) { col.row0 += lo; r->cols.push_back(col); }
-    *out = wrap(r);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return derived_table(h, t, out, nullptr, [&](Ctx* c, const Table& T) {
+        if (lo < 0) lo = 0;
+        if (hi > T.nrows) hi = T.nrows;
+        if (hi < lo) hi = lo;
+        auto r = table_view(c, T, lo, hi); r->first_line = T.first_line + (uint64_t)lo;
+        return r;
+    });
 }
 
 int cpb_table_filter(cpb_ctx* h, const cpb_table* t, const cpb_pred* pred, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    *out = wrap(filter_table(c, *t->t, pred));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return derived_table(h, t, out, nullptr, [&](Ctx* c, const Table& T) { return filter_table(c, T, pred); });
 }
 
 int cpb_table_first_false(cpb_ctx* h, const cpb_table* t, const cpb_pred* pred, int64_t* row) {
-    if (!h || !t || !row) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    *row = first_false_row(c, *t->t, pred);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(row, "null row");
+        *row = first_false_row(c, T, pred);
+        return CPB_OK;
+    });
 }
 
 int cpb_table_concat(cpb_ctx* h, const cpb_table* const* parts, int nparts, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (nparts <= 0) throw ArgError{CPB_ERR_ARG, "no parts"};
-    std::vector<const Table*> ps;
-    for (int i = 0; i < nparts; i++) ps.push_back(parts[i]->t.get());
-    *out = wrap(concat_tables(c, ps));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(out, "null out");
+        if (nparts <= 0) throw ArgError{CPB_ERR_ARG, "no parts"};
+        need(parts, "null parts");
+        std::vector<const Table*> ps;
+        for (int i = 0; i < nparts; i++) ps.push_back(&table_of(parts[i]));
+        *out = wrap(concat_tables(c, ps));
+        return CPB_OK;
+    });
 }
 
 void cpb_table_free(cpb_table* t) {
@@ -618,92 +667,88 @@ void cpb_table_free(cpb_table* t) {
 // ------------------------------------------------------------------ index / join
 int cpb_index_build(cpb_ctx* h, const cpb_table* t, const cpb_str* key_cols, int nkeys, int unique, cpb_index** out,
                     cpb_error* err) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    if (nkeys <= 0) throw ArgError{CPB_ERR_ARG, "empty column list in CreateIndex()"};  // csvplus.go:709-710
-    auto keys = str_list(key_cols, nkeys);
-    for (int i = 0; i < nkeys; i++)
-        for (int j = i + 1; j < nkeys; j++)
-            if (keys[i] == keys[j]) throw ArgError{CPB_ERR_ARG, "duplicate column name(s) in CreateIndex()"};  // :714-716
-    *out = new cpb_index{build_index(c, t->t, keys, unique != 0)};
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        need(t && out, "null table or out");
+        *out = nullptr;
+        if (nkeys <= 0) throw ArgError{CPB_ERR_ARG, "empty column list in CreateIndex()"};  // csvplus.go:709-710
+        auto keys = str_list(key_cols, nkeys);
+        for (int i = 0; i < nkeys; i++)
+            for (int j = i + 1; j < nkeys; j++)
+                if (keys[i] == keys[j]) throw ArgError{CPB_ERR_ARG, "duplicate column name(s) in CreateIndex()"};  // :714-716
+        *out = new cpb_index{build_index(c, t->t, keys, unique != 0)};
+        return CPB_OK;
+    });
 }
 int64_t cpb_index_num_rows(const cpb_index* ix) { return ix ? ix->ix->nrows : -1; }
 int cpb_index_num_keys(const cpb_index* ix) { return ix ? (int)ix->ix->key_cols.size() : -1; }
 int cpb_index_table(cpb_ctx* h, const cpb_index* ix, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    *out = wrap(sorted_table(c, *ix->ix));
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        Index& X = index_of(ix);
+        need(out, "null out");
+        *out = wrap(sorted_table(c, X));
+        return CPB_OK;
+    });
+}
+// the stored rows whose leading key columns equal the n values, as a view (all of them when n is 0)
+static std::shared_ptr<Table> rows_with_prefix(Ctx* c, Index& X, const cpb_str* values, int n) {
+    int64_t lo = 0, hi = X.nrows;
+    if (n > 0) find_range(c, X, str_list(values, n), &lo, &hi);
+    return table_view(c, *sorted_table(c, X), lo, hi);
 }
 int cpb_index_find(cpb_ctx* h, const cpb_index* ix, const cpb_str* values, int n, cpb_table** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (n > (int)ix->ix->key_cols.size()) throw ArgError{CPB_ERR_ARG, "too many columns in indexImpl.find()"};  // csvplus.go:876-878
-    int64_t lo = 0, hi = ix->ix->nrows;
-    if (n > 0) find_range(c, *ix->ix, str_list(values, n), &lo, &hi);
-    const Table& T = *sorted_table(c, *ix->ix);
-    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = hi - lo;
-    for (auto col : T.cols) { col.row0 += lo; r->cols.push_back(col); }
-    *out = wrap(r);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        Index& X = index_of(ix);
+        need(out, "null out");
+        if (n > (int)X.key_cols.size()) throw ArgError{CPB_ERR_ARG, "too many columns in indexImpl.find()"};  // csvplus.go:876-878
+        *out = wrap(rows_with_prefix(c, X, values, n));
+        return CPB_OK;
+    });
 }
 int cpb_index_sub(cpb_ctx* h, const cpb_index* ix, const cpb_str* values, int n, cpb_index** out) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (n >= (int)ix->ix->key_cols.size()) throw ArgError{CPB_ERR_ARG, "too many values in SubIndex()"};  // csvplus.go:633-635
-    int64_t lo = 0, hi = ix->ix->nrows;
-    if (n > 0) find_range(c, *ix->ix, str_list(values, n), &lo, &hi);
-    // the slice in the parent's stored order, not re-sorted (csvplus.go:637-640): on a parent in key order it is already
-    // sorted on the remaining key columns; on one out of key order it keeps that order, and the searches follow it
-    auto view = std::make_shared<Table>(); view->ctx = c; view->nrows = hi - lo;
-    for (auto col : sorted_table(c, *ix->ix)->cols) { col.row0 += lo; view->cols.push_back(col); }
-    std::vector<std::string> keys(ix->ix->key_cols.begin() + n, ix->ix->key_cols.end());
-    if (hi == lo) {  // (an empty index also from a parent whose table lacks the key columns)
-        *out = new cpb_index{build_index(c, view, keys, false)};
+    return guarded(h, nullptr, [&](Ctx* c) {
+        Index& X = index_of(ix);
+        need(out, "null out");
+        if (n >= (int)X.key_cols.size()) throw ArgError{CPB_ERR_ARG, "too many values in SubIndex()"};  // csvplus.go:633-635
+        // the slice in the parent's stored order, not re-sorted (csvplus.go:637-640): on a parent in key order it is already
+        // sorted on the remaining key columns; on one out of key order it keeps that order, and the searches follow it
+        auto view = rows_with_prefix(c, X, values, n);
+        std::vector<std::string> keys(X.key_cols.begin() + (n > 0 ? n : 0), X.key_cols.end());
+        if (view->nrows == 0) {  // (an empty index also from a parent whose table lacks the key columns)
+            *out = new cpb_index{build_index(c, view, keys, false)};
+            return CPB_OK;
+        }
+        auto sub = std::make_shared<Index>();
+        sub->ctx = c; sub->key_cols = keys; sub->key_col_idx.assign(keys.size(), -1);
+        index_adopt_rows(c, *sub, view);
+        *out = new cpb_index{sub};
         return CPB_OK;
-    }
-    auto sub = std::make_shared<Index>();
-    sub->ctx = c; sub->key_cols = keys; sub->key_col_idx.assign(keys.size(), -1);
-    index_adopt_rows(c, *sub, view);
-    *out = new cpb_index{sub};
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    });
 }
 int cpb_index_dup_groups(cpb_ctx* h, const cpb_index* ix, int64_t* ngroups, int64_t** lo, int64_t** hi) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    std::vector<int64_t> a, b;
-    index_dup_groups(c, *ix->ix, a, b);
-    *ngroups = (int64_t)a.size();
-    *lo = (int64_t*)malloc((a.size() + 1) * 8); *hi = (int64_t*)malloc((a.size() + 1) * 8);
-    if (!*lo || !*hi) return CPB_ERR_NOMEM;
-    if (!a.empty()) { memcpy(*lo, a.data(), a.size() * 8); memcpy(*hi, b.data(), b.size() * 8); }
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
-}
-int cpb_index_dedup_apply(cpb_ctx* h, cpb_index* ix, int64_t ngroups, const int64_t* keep, int bug_compatible) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    std::vector<int64_t> k(keep, keep + (ngroups > 0 ? ngroups : 0));
-    index_dedup_apply(c, *ix->ix, k, bug_compatible != 0);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) -> int {
+        Index& X = index_of(ix);
+        need(ngroups && lo && hi, "null ngroups, lo or hi");
+        std::vector<int64_t> a, b;
+        index_dup_groups(c, X, a, b);
+        *ngroups = (int64_t)a.size();
+        *lo = (int64_t*)malloc((a.size() + 1) * 8); *hi = (int64_t*)malloc((a.size() + 1) * 8);
+        if (!*lo || !*hi) return CPB_ERR_NOMEM;
+        if (!a.empty()) { memcpy(*lo, a.data(), a.size() * 8); memcpy(*hi, b.data(), b.size() * 8); }
+        return CPB_OK;
+    });
 }
 int cpb_index_dedup_apply2(cpb_ctx* h, cpb_index* ix, int64_t ngroups, const int64_t* keep, const cpb_table* replacements,
                            int bug_compatible, cpb_error* err) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    std::vector<int64_t> k(keep, keep + (ngroups > 0 ? ngroups : 0));
-    index_dedup_apply(c, *ix->ix, k, bug_compatible != 0, replacements ? replacements->t.get() : nullptr);
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        Index& X = index_of(ix);
+        need(ngroups <= 0 || keep, "null keep");
+        std::vector<int64_t> k(keep, keep + (ngroups > 0 ? ngroups : 0));
+        index_dedup_apply(c, X, k, bug_compatible != 0, replacements ? replacements->t.get() : nullptr);
+        return CPB_OK;
+    });
+}
+int cpb_index_dedup_apply(cpb_ctx* h, cpb_index* ix, int64_t ngroups, const int64_t* keep, int bug_compatible) {
+    return cpb_index_dedup_apply2(h, ix, ngroups, keep, nullptr, bug_compatible, nullptr);
 }
 void cpb_index_free(cpb_index* ix) {
     if (!ix) return;
@@ -717,59 +762,19 @@ int cpb_index_key_col(const cpb_index* ix, int k, cpb_str* out) {
     return CPB_OK;
 }
 
-// ------------------------------------------------------------------ index files (gob.cu)
-static void deliver(Ctx* c, const Buf& out, uint64_t total, int mode, void** bytes, void* host_dst, uint64_t cap, const char* too_small);
-int cpb_index_gob_begin(cpb_ctx* h, const cpb_index* ix, void* prefix, uint64_t cap, uint64_t* prefix_len, uint64_t* total_len,
-                        cpb_error* err) {
-    if (!h || !ix || !prefix_len || !total_len || (cap && !prefix)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    const std::string p = gob_prefix(c, *ix->ix, total_len);
-    *prefix_len = p.size();
-    if (p.size() > cap) throw ArgError{CPB_ERR_ARG, "index file prefix destination too small"};
-    memcpy(prefix, p.data(), p.size());
-    return CPB_OK;
-    CPB_CATCH(c, err)
-}
-int cpb_index_gob_into(cpb_ctx* h, const cpb_index* ix, int64_t lo, int64_t hi, void* host_dst, uint64_t cap, uint64_t* nbytes,
-                       cpb_error* err) {
-    if (!h || !ix || !nbytes || (cap && !host_dst)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    if (lo < 0 || hi < lo || hi > ix->ix->nrows) throw ArgError{CPB_ERR_ARG, "bad row range"};
-    uint64_t total = 0;
-    Buf out = gob_rows(c, *ix->ix, (uint64_t)lo, (uint64_t)hi, cap, &total);
-    *nbytes = total;
-    deliver(c, out, total, 1, nullptr, host_dst, cap, "index file destination too small");
-    return CPB_OK;
-    CPB_CATCH(c, err)
-}
-int cpb_index_load_gob(cpb_ctx* h, const void* bytes, uint64_t nbytes, cpb_index** out, cpb_error* err) {
-    if (!h || !out || (nbytes && !bytes)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    std::vector<std::string> keys;
-    *out = new cpb_index{gob_load(c, (const uint8_t*)bytes, nbytes, &keys)};
-    return CPB_OK;
-    CPB_CATCH(c, err)
-}
-
 static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, bool anti,
                        cpb_table** out, cpb_error* err) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *out = nullptr;
-    CPB_TRY(c, err)
-    std::vector<std::string> names = n ? str_list(cols, n) : ix->ix->key_cols;  // natural join, csvplus.go:546-547
-    if (names.size() > ix->ix->key_cols.size())
-        throw ArgError{CPB_ERR_ARG, anti ? "too many source columns in Except()" : "too many source columns in Join()"};  // :548-549, :591-592
-    *out = wrap(join_tables(c, *probe->t, *ix->ix, names, anti));
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        const Table& P = table_of(probe);
+        Index& X = index_of(ix);
+        need(out, "null out");
+        *out = nullptr;
+        std::vector<std::string> names = n ? str_list(cols, n) : X.key_cols;  // natural join, csvplus.go:546-547
+        if (names.size() > X.key_cols.size())
+            throw ArgError{CPB_ERR_ARG, anti ? "too many source columns in Except()" : "too many source columns in Join()"};  // :548-549, :591-592
+        *out = wrap(join_tables(c, P, X, names, anti));
+        return CPB_OK;
+    });
 }
 int cpb_join(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, cpb_table** out, cpb_error* err) {
     return join_common(h, probe, ix, cols, n, false, out, err);
@@ -778,118 +783,108 @@ int cpb_except(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cp
     return join_common(h, probe, ix, cols, n, true, out, err);
 }
 
-// ------------------------------------------------------------------ ToCsv / ToJSON output
-// mode 0: into new pinned host memory, 1: into caller-owned (ideally pinned) host memory of cap bytes, 2: left on the
-// device.  A destination that is too small gets nothing: the call fails with CPB_ERR_ARG (too_small) and *nbytes = the
-// size needed (the serialiser then returns no buffer).
-static void deliver(Ctx* c, const Buf& out, uint64_t total, int mode, void** bytes, void* host_dst, uint64_t cap, const char* too_small) {
-    if (mode == 0) {
-        void* hp = nullptr;
-        CPB_CUDA(cudaMallocHost(&hp, total ? total : 1));
-        if (total) CPB_CUDA(cudaMemcpyAsync(hp, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        sync_stream(c);
-        *bytes = hp;
-    } else if (mode == 1) {
-        if (total > cap) throw ArgError{CPB_ERR_ARG, too_small};
-        if (total) {
-            KernelTimer kt(c, "d2h_output", total, 0);
-            CPB_CUDA(cudaMemcpyAsync(host_dst, out->p, total, cudaMemcpyDeviceToHost, c->stream));
-        }
-        sync_stream(c);
-    } else {
-        void* dp = nullptr;
-        CPB_CUDA(cudaMallocAsync(&dp, total + 16, c->pool, c->stream));
-        if (total) CPB_CUDA(cudaMemcpyAsync(dp, out->p, total, cudaMemcpyDeviceToDevice, c->stream));
-        *bytes = dp;
-    }
+// ------------------------------------------------------------------ index files (gob.cu)
+int cpb_index_gob_begin(cpb_ctx* h, const cpb_index* ix, void* prefix, uint64_t cap, uint64_t* prefix_len, uint64_t* total_len,
+                        cpb_error* err) {
+    return guarded(h, err, [&](Ctx* c) {
+        Index& X = index_of(ix);
+        need(prefix_len && total_len && (!cap || prefix), "null prefix, prefix_len or total_len");
+        const std::string p = gob_prefix(c, X, total_len);
+        *prefix_len = p.size();
+        if (p.size() > cap) throw ArgError{CPB_ERR_ARG, "index file prefix destination too small"};
+        memcpy(prefix, p.data(), p.size());
+        return CPB_OK;
+    });
+}
+int cpb_index_gob_into(cpb_ctx* h, const cpb_index* ix, int64_t lo, int64_t hi, void* host_dst, uint64_t cap, uint64_t* nbytes,
+                       cpb_error* err) {
+    return serialise(h, err, Dest{Dest::into, nullptr, host_dst, cap}, nbytes, "index file destination too small",
+                     [&](Ctx* c, uint64_t room, uint64_t* total) {
+        Index& X = index_of(ix);
+        if (lo < 0 || hi < lo || hi > X.nrows) throw ArgError{CPB_ERR_ARG, "bad row range"};
+        return gob_rows(c, X, (uint64_t)lo, (uint64_t)hi, room, total);
+    });
+}
+int cpb_index_load_gob(cpb_ctx* h, const void* bytes, uint64_t nbytes, cpb_index** out, cpb_error* err) {
+    return guarded(h, err, [&](Ctx* c) {
+        need(out && (!nbytes || bytes), "null out or bytes");
+        *out = nullptr;
+        std::vector<std::string> keys;
+        *out = new cpb_index{gob_load(c, (const uint8_t*)bytes, nbytes, &keys)};
+        return CPB_OK;
+    });
 }
 
 // ------------------------------------------------------------------ ToCsv
-// modes as deliver(); in mode 1 the header line is written only when asked for (a csv.Writer writes it once, before the
-// first batch: csvplus.go:387)
-static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, int mode, void** bytes,
-                         void* host_dst, uint64_t cap, uint64_t* nbytes, cpb_error* err) {
-    if (!h || !t || !nbytes || (mode != 1 && !bytes) || (mode == 1 && cap && !host_dst)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    if (n <= 0) throw ArgError{CPB_ERR_ARG, "empty column list in ToCsv() function"};  // csvplus.go:380-382
-    auto names = str_list(cols, n);
-    std::vector<int> idx;
-    for (int i = 0; i < n; i++) {
-        int k = t->t->find(names[i]);
-        if (k < 0 && t->t->nrows > 0)
-            throw DataError{CPB_E_MISSING_COLUMN, i, t->t->first_line, true, "missing column " + go_quote(names[i])};  // :392, :145
-        idx.push_back(k);
-    }
-    uint64_t total = 0;
-    Buf out = table_to_csv(c, *t->t, idx, names, with_header != 0, mode == 1 ? cap : UINT64_MAX, &total);
-    *nbytes = total;
-    deliver(c, out, total, mode, bytes, host_dst, cap, "ToCsv destination too small");
-    return CPB_OK;
-    CPB_CATCH(c, err)
+// in mode `into` the header line is written only when asked for (a csv.Writer writes it once, before the first batch:
+// csvplus.go:387)
+static int to_csv_common(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, const Dest& d, uint64_t* nbytes,
+                         cpb_error* err) {
+    return serialise(h, err, d, nbytes, "ToCsv destination too small", [&](Ctx* c, uint64_t room, uint64_t* total) {
+        const Table& T = table_of(t);
+        if (n <= 0) throw ArgError{CPB_ERR_ARG, "empty column list in ToCsv() function"};  // csvplus.go:380-382
+        auto names = str_list(cols, n);
+        std::vector<int> idx;
+        for (int i = 0; i < n; i++) {
+            int k = T.find(names[i]);
+            if (k < 0 && T.nrows > 0)
+                throw DataError{CPB_E_MISSING_COLUMN, i, T.first_line, true, "missing column " + go_quote(names[i])};  // :392, :145
+            idx.push_back(k);
+        }
+        return table_to_csv(c, T, idx, names, with_header != 0, room, total);
+    });
 }
 int cpb_table_to_csv_into(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, int with_header, void* host_dst,
                           uint64_t cap, uint64_t* nbytes, cpb_error* err) {
-    return to_csv_common(h, t, cols, n, with_header, 1, nullptr, host_dst, cap, nbytes, err);
+    return to_csv_common(h, t, cols, n, with_header, Dest{Dest::into, nullptr, host_dst, cap}, nbytes, err);
 }
 int cpb_table_to_csv(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, void** bytes, uint64_t* nbytes, cpb_error* err) {
-    return to_csv_common(h, t, cols, n, 1, 0, bytes, nullptr, 0, nbytes, err);
+    return to_csv_common(h, t, cols, n, 1, Dest{Dest::pinned, bytes, nullptr, 0}, nbytes, err);
 }
 int cpb_table_to_csv_device(cpb_ctx* h, const cpb_table* t, const cpb_str* cols, int n, void** bytes, uint64_t* nbytes, cpb_error* err) {
-    return to_csv_common(h, t, cols, n, 1, 2, bytes, nullptr, 0, nbytes, err);
+    return to_csv_common(h, t, cols, n, 1, Dest{Dest::device, bytes, nullptr, 0}, nbytes, err);
 }
 
 // ------------------------------------------------------------------ ToJSON
-// to_host / into host_dst / left on the device, as ToCsv
-static int to_json_common(cpb_ctx* h, const cpb_table* t, int first, int last, int mode, void** bytes, void* host_dst, uint64_t cap,
-                          uint64_t* nbytes, cpb_error* err) {
-    if (!h || !t || !nbytes || (mode != 1 && !bytes) || (mode == 1 && cap && !host_dst)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    uint64_t total = 0;
-    Buf out = table_to_json(c, *t->t, first != 0, last != 0, mode == 1 ? cap : UINT64_MAX, &total);
-    *nbytes = total;
-    deliver(c, out, total, mode, bytes, host_dst, cap, "ToJSON destination too small");
-    return CPB_OK;
-    CPB_CATCH(c, err)
+static int to_json_common(cpb_ctx* h, const cpb_table* t, int first, int last, const Dest& d, uint64_t* nbytes, cpb_error* err) {
+    return serialise(h, err, d, nbytes, "ToJSON destination too small", [&](Ctx* c, uint64_t room, uint64_t* total) {
+        return table_to_json(c, table_of(t), first != 0, last != 0, room, total);
+    });
 }
 int cpb_table_to_json(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void** bytes, uint64_t* nbytes, cpb_error* err) {
-    return to_json_common(h, t, first_batch, last_batch, 0, bytes, nullptr, 0, nbytes, err);
+    return to_json_common(h, t, first_batch, last_batch, Dest{Dest::pinned, bytes, nullptr, 0}, nbytes, err);
 }
 int cpb_table_to_json_into(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void* host_dst, uint64_t cap,
                            uint64_t* nbytes, cpb_error* err) {
-    return to_json_common(h, t, first_batch, last_batch, 1, nullptr, host_dst, cap, nbytes, err);
+    return to_json_common(h, t, first_batch, last_batch, Dest{Dest::into, nullptr, host_dst, cap}, nbytes, err);
 }
 int cpb_table_to_json_device(cpb_ctx* h, const cpb_table* t, int first_batch, int last_batch, void** bytes, uint64_t* nbytes,
                              cpb_error* err) {
-    return to_json_common(h, t, first_batch, last_batch, 2, bytes, nullptr, 0, nbytes, err);
+    return to_json_common(h, t, first_batch, last_batch, Dest{Dest::device, bytes, nullptr, 0}, nbytes, err);
 }
 
 // ------------------------------------------------------------------ numeric columns
 // Row.ValueAsInt / ValueAsFloat64 (csvplus.go:163-205) of every row; the error is the first failing row's
 static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, bool is_float, void* values, uint8_t* status,
                             uint64_t* nbad, cpb_error* err) {
-    if (!h || !t || !nbad || (!values && t->t->nrows > 0)) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    *nbad = 0;
-    CPB_TRY(c, err)
-    const std::string name = to_string(column);
-    const int k = t->t->find(name);
-    if (t->t->nrows == 0) return CPB_OK;
-    if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // :170, :192
-    NumResult r = column_as_number(c, *t->t, k, is_float, values, status);
-    *nbad = r.nbad;
-    if (r.nbad) {
-        const bool range = r.first_status == CPB_NUM_RANGE;
-        throw DataError{range ? CPB_E_NUM_RANGE : CPB_E_NUM_SYNTAX, -1, r.first_row, false,
-                        "column " + go_quote(name) + ": cannot convert " + go_quote(r.first_value) + (is_float ? " to float: " : " to integer: ") +
-                            (range ? "value out of range" : "invalid syntax")};  // :176, :198
-    }
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return guarded(h, err, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(nbad && (values || T.nrows == 0), "null nbad or values");
+        *nbad = 0;
+        const std::string name = to_string(column);
+        const int k = T.find(name);
+        if (T.nrows == 0) return CPB_OK;
+        if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // :170, :192
+        NumResult r = column_as_number(c, T, k, is_float, values, status);
+        *nbad = r.nbad;
+        if (r.nbad) {
+            const bool range = r.first_status == CPB_NUM_RANGE;
+            throw DataError{range ? CPB_E_NUM_RANGE : CPB_E_NUM_SYNTAX, -1, r.first_row, false,
+                            "column " + go_quote(name) + ": cannot convert " + go_quote(r.first_value) + (is_float ? " to float: " : " to integer: ") +
+                                (range ? "value out of range" : "invalid syntax")};  // :176, :198
+        }
+        return CPB_OK;
+    });
 }
 int cpb_table_column_as_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, int64_t* values, uint8_t* status, uint64_t* nbad,
                               cpb_error* err) {
@@ -902,64 +897,45 @@ int cpb_table_column_as_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, 
 
 // ------------------------------------------------------------------ computed columns
 int cpb_table_set_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, const int64_t* dev_values, cpb_table** out, cpb_error* err) {
-    if (!h || !t || !out) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    *out = wrap(table_set_values(c, *t->t, to_string(column), dev_values, false, 'f', 0));
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_values(c, T, to_string(column), dev_values, false, 'f', 0); });
 }
 int cpb_table_set_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, const double* dev_values, char fmt, int prec, cpb_table** out,
                           cpb_error* err) {
-    if (!h || !t || !out) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    *out = wrap(table_set_values(c, *t->t, to_string(column), dev_values, true, fmt, prec));
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_values(c, T, to_string(column), dev_values, true, fmt, prec); });
 }
 int cpb_table_set_literal(cpb_ctx* h, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err) {
-    if (!h || !t || !out) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    *out = wrap(table_set_literal(c, *t->t, to_string(column), to_string(value)));
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_literal(c, T, to_string(column), to_string(value)); });
 }
 int cpb_table_filter_flags(cpb_ctx* h, const cpb_table* t, const uint8_t* dev_keep, cpb_table** out, cpb_error* err) {
-    if (!h || !t || !out) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    clear_error(err);
-    CPB_TRY(c, err)
-    *out = wrap(table_filter_mask(c, *t->t, dev_keep));
-    return CPB_OK;
-    CPB_CATCH(c, err)
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_filter_mask(c, T, dev_keep); });
 }
 
 // ------------------------------------------------------------------ stats
-int cpb_stats_enable(cpb_ctx* h, int on) { DeviceGuard g(&h->c); h->c.stats_on = on != 0; return CPB_OK; }
+int cpb_stats_enable(cpb_ctx* h, int on) {
+    return guarded(h, nullptr, [&](Ctx* c) { c->stats_on = on != 0; return CPB_OK; });
+}
 int cpb_stats_reset(cpb_ctx* h) {
-    DeviceGuard g(&h->c);
-    h->c.drain_events(); h->c.stats.clear();
-    return CPB_OK;
+    return guarded(h, nullptr, [&](Ctx* c) {
+        c->drain_events(); c->stats.clear();
+        return CPB_OK;
+    });
 }
 int cpb_stats_get(cpb_ctx* h, cpb_kstat* out, int cap, int* n) {
-    DeviceGuard g(&h->c);
-    h->c.drain_events();
-    int i = 0;
-    for (auto& kv : h->c.stats) {
-        if (i < cap) {
-            memset(&out[i], 0, sizeof(cpb_kstat));
-            strncpy(out[i].name, kv.first.c_str(), sizeof(out[i].name) - 1);
-            out[i].launches = kv.second.launches; out[i].ms = kv.second.ms; out[i].algo_bytes = kv.second.bytes;
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(n && (cap <= 0 || out), "null n or out");
+        c->drain_events();
+        int i = 0;
+        for (auto& kv : c->stats) {
+            if (i < cap) {
+                memset(&out[i], 0, sizeof(cpb_kstat));
+                strncpy(out[i].name, kv.first.c_str(), sizeof(out[i].name) - 1);
+                out[i].launches = kv.second.launches; out[i].ms = kv.second.ms; out[i].algo_bytes = kv.second.bytes;
+            }
+            i++;
         }
-        i++;
-    }
-    *n = i;
-    return CPB_OK;
+        *n = i;
+        return CPB_OK;
+    });
 }
 uint64_t cpb_kernel_launches(cpb_ctx* h) { return h ? h->c.launches : 0; }
 uint64_t cpb_host_syncs(cpb_ctx* h) { return h ? h->c.host_syncs : 0; }

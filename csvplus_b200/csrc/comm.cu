@@ -217,28 +217,27 @@ using namespace cpb;
 extern "C" {
 
 int cpb_comm_unique_id(uint8_t* id128) {
-    if (!id128) return CPB_ERR_ARG;
-    CPB_TRY(nullptr, nullptr)
-    static_assert(CPB_UNIQUE_ID_BYTES == NCCL_UNIQUE_ID_BYTES, "unique id size");
-    ncclUniqueId id;
-    CPB_NCCL(nccl().GetUniqueId(&id));
-    memcpy(id128, id.internal, NCCL_UNIQUE_ID_BYTES);
-    return CPB_OK;
-    CPB_CATCH(nullptr, nullptr)
+    return translated(nullptr, nullptr, [&] {
+        need(id128, "null id128");
+        static_assert(CPB_UNIQUE_ID_BYTES == NCCL_UNIQUE_ID_BYTES, "unique id size");
+        ncclUniqueId id;
+        CPB_NCCL(nccl().GetUniqueId(&id));
+        memcpy(id128, id.internal, NCCL_UNIQUE_ID_BYTES);
+        return CPB_OK;
+    });
 }
 
 int cpb_comm_init_rank(cpb_ctx* h, int nranks, int rank, const uint8_t* id128) {
-    if (!h || !id128 || nranks < 1 || rank < 0 || rank >= nranks) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (c->comm) throw ArgError{CPB_ERR_ARG, "ctx already has a communicator"};
-    ncclUniqueId id;
-    memcpy(id.internal, id128, NCCL_UNIQUE_ID_BYTES);
-    ncclComm_t comm = nullptr;
-    CPB_NCCL(nccl().CommInitRank(&comm, nranks, id, rank));
-    c->comm = comm; c->nranks = nranks; c->rank = rank; c->comm_owned = true;
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(id128 && nranks >= 1 && rank >= 0 && rank < nranks, "null id128 or bad rank");
+        if (c->comm) throw ArgError{CPB_ERR_ARG, "ctx already has a communicator"};
+        ncclUniqueId id;
+        memcpy(id.internal, id128, NCCL_UNIQUE_ID_BYTES);
+        ncclComm_t comm = nullptr;
+        CPB_NCCL(nccl().CommInitRank(&comm, nranks, id, rank));
+        c->comm = comm; c->nranks = nranks; c->rank = rank; c->comm_owned = true;
+        return CPB_OK;
+    });
 }
 
 int cpb_init_multi(const int* devices, int n, cpb_ctx** out) {
@@ -272,67 +271,66 @@ void cpb_comm_release(cpb::Ctx* c) {  // called by cpb_shutdown
 
 // every rank of the communicator calls it (one process per GPU, or one host thread per ctx)
 int cpb_allgather_table(cpb_ctx* h, const cpb_table* local, cpb_table** out) {
-    if (!h || !local || !out) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    *out = nullptr;
-    CPB_TRY(c, nullptr)
-    GatherJob j{c, local->t.get()};
-    job_begin(j);
-    job_meta_collective(j);
-    job_sizes(j);
-    {
-        KernelTimer kt(c, "allgather_nccl", 0, 0);  // device time of the grouped transfers on the ctx stream
-        CPB_NCCL(nccl().GroupStart());
-        try { job_data_collective(j); } catch (...) { nccl().GroupEnd(); throw; }
-        CPB_NCCL(nccl().GroupEnd());
-    }
-    job_finish(j);
-    *out = new cpb_table{j.out};
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(local && out, "null local or out");
+        *out = nullptr;
+        GatherJob j{c, local->t.get()};
+        job_begin(j);
+        job_meta_collective(j);
+        job_sizes(j);
+        {
+            KernelTimer kt(c, "allgather_nccl", 0, 0);  // device time of the grouped transfers on the ctx stream
+            CPB_NCCL(nccl().GroupStart());
+            try { job_data_collective(j); } catch (...) { nccl().GroupEnd(); throw; }
+            CPB_NCCL(nccl().GroupEnd());
+        }
+        job_finish(j);
+        *out = new cpb_table{j.out};
+        return CPB_OK;
+    });
 }
 
 // single-process form: all n ranks of a cpb_init_multi communicator driven from one host thread (grouped calls)
 int cpb_allgather_tables(cpb_ctx* const* hs, const cpb_table* const* locals, int n, cpb_table** outs) {
     if (!hs || !locals || !outs || n < 1) return CPB_ERR_ARG;
     for (int i = 0; i < n; i++) outs[i] = nullptr;
+    for (int i = 0; i < n; i++) if (!hs[i] || !locals[i]) return CPB_ERR_ARG;  // before any context is locked
     Ctx* c0 = &hs[0]->c;
-    std::vector<std::unique_lock<std::mutex>> locks;
+    std::vector<std::unique_lock<std::mutex>> locks;  // every rank's context, in rank order
     for (int i = 0; i < n; i++) locks.emplace_back(hs[i]->c.mu);
-    CPB_TRY(c0, nullptr)
-    if (n != c0->nranks) throw ArgError{CPB_ERR_ARG, "cpb_allgather_tables needs every rank of the communicator"};
-    std::vector<GatherJob> jobs;
-    for (int i = 0; i < n; i++) jobs.push_back(GatherJob{&hs[i]->c, locals[i]->t.get()});
-    for (auto& j : jobs) job_begin(j);
-    CPB_NCCL(nccl().GroupStart());
-    for (auto& j : jobs) job_meta_collective(j);
-    CPB_NCCL(nccl().GroupEnd());
-    for (auto& j : jobs) job_sizes(j);
-    CPB_NCCL(nccl().GroupStart());
-    try { for (auto& j : jobs) job_data_collective(j); } catch (...) { nccl().GroupEnd(); throw; }
-    CPB_NCCL(nccl().GroupEnd());
-    for (auto& j : jobs) job_finish(j);
-    for (int i = 0; i < n; i++) outs[i] = new cpb_table{jobs[i].out};
-    return CPB_OK;
-    CPB_CATCH(c0, nullptr)
+    return translated(c0, nullptr, [&] {
+        if (n != c0->nranks) throw ArgError{CPB_ERR_ARG, "cpb_allgather_tables needs every rank of the communicator"};
+        std::vector<GatherJob> jobs;
+        for (int i = 0; i < n; i++) jobs.push_back(GatherJob{&hs[i]->c, locals[i]->t.get()});
+        for (auto& j : jobs) job_begin(j);
+        CPB_NCCL(nccl().GroupStart());
+        for (auto& j : jobs) job_meta_collective(j);
+        CPB_NCCL(nccl().GroupEnd());
+        for (auto& j : jobs) job_sizes(j);
+        CPB_NCCL(nccl().GroupStart());
+        try { for (auto& j : jobs) job_data_collective(j); } catch (...) { nccl().GroupEnd(); throw; }
+        CPB_NCCL(nccl().GroupEnd());
+        for (auto& j : jobs) job_finish(j);
+        for (int i = 0; i < n; i++) outs[i] = new cpb_table{jobs[i].out};
+        return CPB_OK;
+    });
 }
 
 // small metadata exchange (host values in, host values out): quote parity / record counts of byte-range shards
 int cpb_allgather_u64(cpb_ctx* h, const uint64_t* in, int count, uint64_t* out) {
-    if (!h || !in || !out || count < 1) return CPB_ERR_ARG;
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (!c->comm) { memcpy(out, in, (size_t)count * 8); return CPB_OK; }
-    Buf a = dev_alloc(c, (size_t)count * 8), b = dev_alloc(c, (size_t)count * 8 * c->nranks);
-    uint64_t* hp = (uint64_t*)c->pinned_scratch((size_t)count * 8 * (c->nranks + 1));
-    memcpy(hp, in, (size_t)count * 8);
-    CPB_CUDA(cudaMemcpyAsync(a->p, hp, (size_t)count * 8, cudaMemcpyHostToDevice, c->stream));
-    CPB_NCCL(nccl().AllGather(a->p, b->p, (size_t)count, ncclUint64, (ncclComm_t)c->comm, c->stream));
-    CPB_CUDA(cudaMemcpyAsync(hp + count, b->p, (size_t)count * 8 * c->nranks, cudaMemcpyDeviceToHost, c->stream));
-    sync_stream(c);
-    memcpy(out, hp + count, (size_t)count * 8 * c->nranks);
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(in && out && count >= 1, "null in or out, or no values");
+        if (!c->comm) { memcpy(out, in, (size_t)count * 8); return CPB_OK; }
+        Buf a = dev_alloc(c, (size_t)count * 8), b = dev_alloc(c, (size_t)count * 8 * c->nranks);
+        uint64_t* hp = (uint64_t*)c->pinned_scratch((size_t)count * 8 * (c->nranks + 1));
+        memcpy(hp, in, (size_t)count * 8);
+        CPB_CUDA(cudaMemcpyAsync(a->p, hp, (size_t)count * 8, cudaMemcpyHostToDevice, c->stream));
+        CPB_NCCL(nccl().AllGather(a->p, b->p, (size_t)count, ncclUint64, (ncclComm_t)c->comm, c->stream));
+        CPB_CUDA(cudaMemcpyAsync(hp + count, b->p, (size_t)count * 8 * c->nranks, cudaMemcpyDeviceToHost, c->stream));
+        sync_stream(c);
+        memcpy(out, hp + count, (size_t)count * 8 * c->nranks);
+        return CPB_OK;
+    });
 }
 
 // the layout arithmetic alone (pure host code; CPU tests call it without a GPU)

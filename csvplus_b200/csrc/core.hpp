@@ -259,10 +259,34 @@ inline Buf dev_alloc(Ctx* c, size_t bytes) {
 
 inline std::string to_string(cpb_str s) { return std::string(s.ptr ? s.ptr : "", (size_t)s.len); }
 
-// exception -> status translation used by every extern "C" body
+// a table over rows [lo, hi) of t that shares t's buffers: every column, or the columns `pick` in that order.
+// first_line stays at its default; the caller sets it where the rows keep the lines of their source
+inline std::shared_ptr<Table> table_view(Ctx* c, const Table& t, int64_t lo, int64_t hi, const std::vector<int>* pick = nullptr) {
+    auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = hi - lo;
+    for (size_t i = 0; i < (pick ? pick->size() : t.cols.size()); i++) {
+        Column col = t.cols[pick ? (size_t)(*pick)[i] : i];
+        col.row0 += lo;
+        r->cols.push_back(col);
+    }
+    return r;
+}
+
+// ------------------------------------------------------------------ the extern "C" boundary
+// A bad argument of an entry point (a null handle, a null out-parameter): CPB_ERR_ARG, `what` in cpb_last_error
+inline void need(bool ok, const char* what) { if (!ok) throw ArgError{CPB_ERR_ARG, what}; }
+// exception -> status translation used by every extern "C" body; c may be null (no context to record the text in)
 int translate_exception(Ctx* c, cpb_error* err);
-#define CPB_TRY(ctx, err) try {
-#define CPB_CATCH(ctx, err) } catch (...) { return ::cpb::translate_exception(ctx, err); }
+template <class F> int translated(Ctx* c, cpb_error* err, F&& body) {
+    try { return body(); } catch (...) { return translate_exception(c, err); }
+}
+// Every entry point that works on a context runs as guarded(ctx, err, body): *err is cleared first, a null context is
+// CPB_ERR_ARG, the context's device is selected and its calls serialised, and body(Ctx*) returns the status or throws
+template <class F> int guarded(Ctx* c, cpb_error* err, F&& body) {
+    clear_error(err);
+    if (!c) return CPB_ERR_ARG;
+    DeviceGuard g(c);
+    return translated(c, err, [&]() -> int { return body(c); });
+}
 
 // ------------------------------------------------------------------ cross-TU operations
 // parse.cu
@@ -384,3 +408,7 @@ struct cpb_ctx { cpb::Ctx c; };
 struct cpb_table { std::shared_ptr<cpb::Table> t; };
 struct cpb_index { std::shared_ptr<cpb::Index> ix; };
 struct cpb_stream { cpb::Stream* s; };
+
+namespace cpb {
+template <class F> int guarded(cpb_ctx* h, cpb_error* err, F&& body) { return guarded(h ? &h->c : nullptr, err, body); }
+}  // namespace cpb

@@ -105,40 +105,40 @@ static uint64_t gcd64(uint64_t a, uint64_t b) { while (b) { uint64_t t = a % b; 
 
 extern "C" int cpb_gen_csv(cpb_ctx* h, int kind, uint64_t seed, uint64_t row_lo, uint64_t row_hi, uint64_t n_cust, uint64_t n_prod,
                            int with_header, int permute, void* dst, uint64_t cap, uint64_t* nbytes) {
-    Ctx* c = &h->c; DeviceGuard g(c);
-    CPB_TRY(c, nullptr)
-    if (kind < 0 || kind > 2 || row_hi < row_lo) throw ArgError{CPB_ERR_ARG, "bad generator arguments"};
-    static const char* headers[3] = {"id,name,surname,born,city,score\n", "order_id,cust_id,prod_id,qty,ts\n", "prod_id,product,price\n"};
-    GenParams gp{};
-    gp.kind = kind; gp.seed = seed; gp.row_lo = row_lo; gp.row_hi = row_hi; gp.n_cust = n_cust ? n_cust : 1; gp.n_prod = n_prod ? n_prod : 1;
-    gp.header_len = with_header ? (uint32_t)strlen(headers[kind]) : 0;
-    if (permute) {
-        uint64_t n = kind == 2 ? gp.n_prod : gp.n_cust;  // ids are a bijection of [0, table size)
-        uint64_t a = (0x9E3779B97F4A7C15ull ^ seed) % n;
-        if (a < 2) a = n > 2 ? 2 : 1;
-        while (gcd64(a, n) != 1) a++;
-        gp.perm_a = a % n; gp.perm_b = (seed * 0x2545F4914F6CDD1Dull) % n; gp.perm_n = n;
-        if (n >= (1ull << 32)) throw ArgError{CPB_ERR_ARG, "permuted tables are limited to 2^32 rows"};
-    }
-    const uint64_t rows = row_hi - row_lo;
-    Buf len = dev_alloc(c, (rows + 1) * 4), total = dev_alloc(c, 8);
-    if (rows) {
-        gen_len_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
-    exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), rows, total->as<uint64_t>());
-    const uint64_t body = read_back<uint64_t>(c, total->p);
-    if (body > 0xffffffffull) throw ArgError{CPB_ERR_ARG, "generate at most 4 GiB per call (split the row range)"};
-    *nbytes = body + gp.header_len;
-    if (dst) {
-        if (*nbytes > cap) throw ArgError{CPB_ERR_ARG, "generator destination too small"};
-        if (gp.header_len) CPB_CUDA(cudaMemcpyAsync(dst, headers[kind], gp.header_len, cudaMemcpyHostToDevice, c->stream));
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(nbytes, "null nbytes");
+        if (kind < 0 || kind > 2 || row_hi < row_lo) throw ArgError{CPB_ERR_ARG, "bad generator arguments"};
+        static const char* headers[3] = {"id,name,surname,born,city,score\n", "order_id,cust_id,prod_id,qty,ts\n", "prod_id,product,price\n"};
+        GenParams gp{};
+        gp.kind = kind; gp.seed = seed; gp.row_lo = row_lo; gp.row_hi = row_hi; gp.n_cust = n_cust ? n_cust : 1; gp.n_prod = n_prod ? n_prod : 1;
+        gp.header_len = with_header ? (uint32_t)strlen(headers[kind]) : 0;
+        if (permute) {
+            uint64_t n = kind == 2 ? gp.n_prod : gp.n_cust;  // ids are a bijection of [0, table size)
+            uint64_t a = (0x9E3779B97F4A7C15ull ^ seed) % n;
+            if (a < 2) a = n > 2 ? 2 : 1;
+            while (gcd64(a, n) != 1) a++;
+            gp.perm_a = a % n; gp.perm_b = (seed * 0x2545F4914F6CDD1Dull) % n; gp.perm_n = n;
+            if (n >= (1ull << 32)) throw ArgError{CPB_ERR_ARG, "permuted tables are limited to 2^32 rows"};
+        }
+        const uint64_t rows = row_hi - row_lo;
+        Buf len = dev_alloc(c, (rows + 1) * 4), total = dev_alloc(c, 8);
         if (rows) {
-            gen_write_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>(), (uint8_t*)dst);
+            gen_len_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>());
             CPB_CUDA(cudaGetLastError());
         }
-        sync_stream(c);
-    }
-    return CPB_OK;
-    CPB_CATCH(c, nullptr)
+        exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), rows, total->as<uint64_t>());
+        const uint64_t body = read_back<uint64_t>(c, total->p);
+        if (body > 0xffffffffull) throw ArgError{CPB_ERR_ARG, "generate at most 4 GiB per call (split the row range)"};
+        *nbytes = body + gp.header_len;
+        if (dst) {
+            if (*nbytes > cap) throw ArgError{CPB_ERR_ARG, "generator destination too small"};
+            if (gp.header_len) CPB_CUDA(cudaMemcpyAsync(dst, headers[kind], gp.header_len, cudaMemcpyHostToDevice, c->stream));
+            if (rows) {
+                gen_write_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>(), (uint8_t*)dst);
+                CPB_CUDA(cudaGetLastError());
+            }
+            sync_stream(c);
+        }
+        return CPB_OK;
+    });
 }

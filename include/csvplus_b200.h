@@ -11,6 +11,8 @@
  *   - extern "C", plain pointers and sizes; no C++/torch types; no exceptions cross the boundary.
  *   - every call returns a cpb_status; data errors additionally fill a cpb_error whose
  *     (line, msg) reproduce the reference's DataSourceError{Line, Err} (csvplus.go:1230-1238).
+ *   - a null ctx, handle or required out-parameter is answered with CPB_ERR_ARG (the reason in cpb_last_error when there
+ *     is a ctx to keep it), never dereferenced; a cpb_error passed in is cleared first.  The *_free calls accept null.
  *   - handles (cpb_ctx / cpb_table / cpb_index) are owned by the library and released by the
  *     matching *_free.  Input byte buffers are borrowed for the duration of the call only.
  *   - every entry point selects the ctx's device (goroutines migrate between OS threads) and
