@@ -325,11 +325,12 @@ void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, u
 struct FlagScan { const uint32_t* flags; uint64_t n; Buf pos; uint64_t count; };  // pos: uint32[n + 1] exclusive scan
 FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n);
 void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out);
-Column gather_column(Ctx* c, const Column& src, const uint32_t* row_ids, int64_t nout);
+// rows row_ids[0, nout) of t (rows 0..nout-1 when row_ids is null: a view compacted into buffers of its own)
 std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout);
+// the rows of t whose flag (uint32 0/1, one per row) is set: scan_flags, compact_flags timed as compact_ids, gather_rows
+std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags);
 std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred);
 int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred);
-Column materialize(Ctx* c, const Column& col, int64_t nrows);  // view -> own compact buffers
 // rows `ids` (positions in `order`) of the index restricted to columns `cols` (row-slot path when it pays, else gather_rows)
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout,
                                          RowOrder order);

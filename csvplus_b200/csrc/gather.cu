@@ -1,5 +1,5 @@
 // gather.cu — column-level primitives shared by Filter / IndexOn / Join:
-//   * device-wide exclusive scan (single pass, decoupled look-back);
+//   * device-wide exclusive scans (single pass, one decoupled look-back chain for every scan);
 //   * string-column gather by row ids (lengths -> scan -> byte copy) = the columnar form of the
 //     per-row map copies the reference makes (Row.Select csvplus.go:122-134, mergeRows :571-583);
 //   * Filter(Like/All/Any/Not) over a materialised table (csvplus.go:276-286, :1243-1293);
@@ -18,7 +18,30 @@ constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_ITEMS = 16;
 constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
 
-// tile state word: bits 63:62 status (0 none, 1 aggregate, 2 inclusive), bits 61:0 value
+// The look-back chain of one tile, run by a whole warp.  Tile t's state word is st[t * stride] (stride NC: the words of
+// NC columns interleaved): bits 63:62 status (0 none, 1 aggregate, 2 inclusive prefix), bits 61:0 the value.  Publishes
+// the tile's total tot, walks the predecessors 32 at a time until one holds its inclusive prefix, publishes this tile's
+// and returns its exclusive prefix (every lane).
+__device__ __forceinline__ unsigned long long lookback(unsigned long long* st, uint32_t stride, uint64_t tile, uint32_t tot) {
+    const int lane = threadIdx.x & 31;
+    if (tile == 0) {
+        if (lane == 0) atomicExch(&st[0], (2ull << 62) | tot);
+        return 0;
+    }
+    if (lane == 0) atomicExch(&st[tile * stride], (1ull << 62) | tot);
+    unsigned long long excl = 0;
+    for (int64_t b = (int64_t)tile - 1;; b -= 32) {
+        const int64_t p = b - lane;
+        unsigned long long s = 2ull << 62;
+        if (p >= 0) { do { s = ld_relaxed_u64((const uint64_t*)&st[p * stride]); } while ((s >> 62) == 0); }
+        const int f = __ffs(__ballot_sync(0xffffffffu, (s >> 62) == 2)) - 1;
+        excl += warp_sum_u64((f < 0 || lane <= f) ? (s & ((1ull << 62) - 1)) : 0ull);
+        if (f >= 0) break;
+    }
+    if (lane == 0) atomicExch(&st[tile * stride], (2ull << 62) | (excl + tot));
+    return excl;
+}
+
 // GATHER: the scanned values are the lengths of the strings picked by `ids` (identity when null) from the offsets
 // array `in` -- the length array of a gather is never materialised.
 template <bool GATHER>
@@ -54,25 +77,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* 
 #pragma unroll
         for (int i = 0; i < SCAN_THREADS / 32; i++) { uint32_t t = s_warp[i]; if (i < warp) woff += t; tot += t; }
         if (warp == 0) {
-            unsigned long long excl = 0;
-            if (tile == 0) {
-                if (lane == 0) atomicExch(&state[0], (2ull << 62) | tot);
-            } else {
-                if (lane == 0) atomicExch(&state[tile], (1ull << 62) | tot);
-                int64_t b = (int64_t)tile - 1;
-                for (;;) {
-                    int64_t p = b - lane;
-                    unsigned long long s = 2ull << 62;
-                    if (p >= 0) { do { s = ld_relaxed_u64((const uint64_t*)&state[p]); } while ((s >> 62) == 0); }
-                    uint32_t incl = __ballot_sync(0xffffffffu, (s >> 62) == 2);
-                    int f = __ffs(incl) - 1;
-                    unsigned long long val = (f < 0 || lane <= f) ? (s & ((1ull << 62) - 1)) : 0ull;
-                    excl += warp_sum_u64(val);
-                    if (f >= 0) break;
-                    b -= 32;
-                }
-                if (lane == 0) atomicExch(&state[tile], (2ull << 62) | (excl + tot));
-            }
+            const unsigned long long excl = lookback(state, 1, tile, tot);
             if (lane == 0) { s_prefix = excl; if (tile == ntiles - 1) { *total = excl + tot; out[n] = (uint32_t)(excl + tot); } }
         }
         __syncthreads();
@@ -201,8 +206,6 @@ __global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32
     }
 }
 
-struct PendingGather { Column col; const Column* src; Buf total; };
-
 // gathers several columns with ONE host synchronisation (totals of all columns read back together)
 static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column*>& srcs, const uint32_t* ids, int64_t nout) {
     std::vector<Column> out(srcs.size());
@@ -229,10 +232,6 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
     return out;
 }
 
-Column gather_column(Ctx* c, const Column& src, const uint32_t* row_ids, int64_t nout) {
-    return gather_columns(c, {&src}, row_ids, nout)[0];
-}
-
 std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout) {
     auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = t.first_line;
     // columns sharing buffers (AssumeHeader aliases) are gathered once
@@ -249,7 +248,18 @@ std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_i
     return r;
 }
 
-Column materialize(Ctx* c, const Column& col, int64_t nrows) { return gather_columns(c, {&col}, nullptr, nrows)[0]; }
+// the rows of t whose flag is set: the flags scanned and counted (one host synchronisation), compacted to row ids
+// (timed as compact_ids) and the rows gathered
+std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags) {
+    const uint64_t n = (uint64_t)t.nrows;
+    const FlagScan s = scan_flags(c, flags, n);
+    Buf ids = dev_alloc(c, (s.count + 1) * 4);
+    {
+        KernelTimer kt(c, "compact_ids", n * 8 + s.count * 4);
+        compact_flags(c, s, 0, ids->as<uint32_t>());
+    }
+    return gather_rows(c, t, ids->as<uint32_t>(), (int64_t)s.count);
+}
 
 // ------------------------------------------------------------------ row slots: one random access per gathered index row
 // A join reads index rows in probe order, i.e. at random: per output column that is one access to the offsets and
@@ -357,9 +367,9 @@ __global__ void __launch_bounds__(256) rowhash_probe_kernel(KeyDesc kd, uint64_t
     if ((threadIdx.x & 31) == 0 && hits) atomicAdd(matches, hits);
 }
 
-// exclusive scans of the NC length fields (8 bits each) of row i's packed lengths in one pass (same chained look-back
-// as scan_u32_kernel; warp c resolves column c).  Src::load(base, n, p) gives the packed lengths of rows
-// [base, base + LS_ITEMS) (0 past n).
+// exclusive scans of the NC length fields (8 bits each) of row i's packed lengths in one pass (warp c runs column c's
+// look-back).  Src::load(base, n, p) gives the packed lengths of rows [base, base + LS_ITEMS) (0 past n).  A body of its
+// own: folded into one kernel with scan_u32_kernel, the scan_gather_len instantiation took 40 registers instead of 32.
 constexpr int LS_ITEMS = 8;
 constexpr int LS_TILE = SCAN_THREADS * LS_ITEMS;
 struct LensById {  // row slots: lens[ids[i]]
@@ -419,26 +429,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const Src src, 
             uint32_t tot = 0;
 #pragma unroll
             for (int i = 0; i < SCAN_THREADS / 32; i++) tot += s_warp[c][i];
-            unsigned long long* st = state + c;  // state[tile * NC + c]
-            unsigned long long excl = 0;
-            if (tile == 0) {
-                if (lane == 0) atomicExch(&st[0], (2ull << 62) | tot);
-            } else {
-                if (lane == 0) atomicExch(&st[tile * NC], (1ull << 62) | tot);
-                int64_t b = (int64_t)tile - 1;
-                for (;;) {
-                    const int64_t q = b - lane;
-                    unsigned long long sv = 2ull << 62;
-                    if (q >= 0) { do { sv = ld_relaxed_u64((const uint64_t*)&st[q * NC]); } while ((sv >> 62) == 0); }
-                    const uint32_t incl = __ballot_sync(0xffffffffu, (sv >> 62) == 2);
-                    const int f = __ffs(incl) - 1;
-                    const unsigned long long val = (f < 0 || lane <= f) ? (sv & ((1ull << 62) - 1)) : 0ull;
-                    excl += warp_sum_u64(val);
-                    if (f >= 0) break;
-                    b -= 32;
-                }
-                if (lane == 0) atomicExch(&st[tile * NC], (2ull << 62) | (excl + tot));
-            }
+            const unsigned long long excl = lookback(state + c, NC, tile, tot);  // state[tile * NC + c]
             if (lane == 0) {
                 s_prefix[c] = excl;
                 if (tile == ntiles - 1) totals[c] = excl + tot;
@@ -812,13 +803,7 @@ std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred
         KernelTimer kt(c, "filter_like", n * 12);
         flags = predicate_flags(c, t, pred);
     }
-    const FlagScan s = scan_flags(c, flags->as<uint32_t>(), n);
-    Buf ids = dev_alloc(c, (s.count + 1) * 4);
-    {
-        KernelTimer kt(c, "compact_ids", n * 8 + s.count * 4);
-        compact_flags(c, s, 0, ids->as<uint32_t>());
-    }
-    return gather_rows(c, t, ids->as<uint32_t>(), (int64_t)s.count);
+    return rows_where(c, t, flags->as<uint32_t>());
 }
 
 // ------------------------------------------------------------------ concat
