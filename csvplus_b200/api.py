@@ -299,11 +299,21 @@ class DeviceBuffer:
 
 
 # ------------------------------------------------------------------ predicates (csvplus.go:1240-1293)
+# what an index key can hold (a set term is an index over its literals): key columns, key image bytes (csvplus_b200.h)
+_MAX_INDEX_KEYS, _MAX_KEY_IMAGE = 16, 4096
+# cpb_str and cpb_pred as numpy records (set terms are lowered in bulk)
+_STR_DTYPE = np.dtype([("ptr", "<u8"), ("len", "<u8")])
+_PRED_DTYPE = np.dtype([("op", "<i4"), ("n", "<i4"), ("keys", "<u8"), ("values", "<u8"), ("children", "<u8")])
+assert _STR_DTYPE.itemsize == C.sizeof(_abi.Str) and _PRED_DTYPE.itemsize == C.sizeof(_abi.Pred)
+
+
 class Predicate:
     """A recognisable predicate: callable on a Row (host) and lowerable to cpb_pred (device)."""
 
     def __init__(self, op: int, match: dict | None = None, kids: list | None = None):
         self.op, self.match, self.kids = op, match or {}, kids or []
+        # computed once per node: a plan that filters batch by batch asks for them on every batch
+        self._sets = self._lowerable = self._lowered = None
 
     def __call__(self, row: Row) -> bool:
         if self.op == 0:
@@ -316,9 +326,11 @@ class Predicate:
 
     def lowerable(self) -> bool:
         """True when the device compiles the tree: every node is a Predicate and the tree stays within the header's
-        CPB_PRED_MAX_* limits.  Terms are counted as if every Like key named a column (a missing one compiles to a constant
-        false), so a tree over missing columns may be declined where the device would have taken it.  A declined tree
-        is evaluated on host rows, as an opaque function is."""
+        CPB_PRED_MAX_* limits, a set term (_set_groups) counting as one term.  Terms are counted as if every Like key named
+        a column (a missing one compiles to a constant false), so a tree over missing columns may be declined where the
+        device would have taken it.  A declined tree is evaluated on host rows, as an opaque function is."""
+        if self._lowerable is not None:
+            return self._lowerable
         terms = ops = 0
 
         def walk(p, depth) -> bool:
@@ -331,28 +343,90 @@ class Predicate:
             if not p.kids:  # All() / Any(): a constant
                 ops += 1
                 return True
-            ops += 1 if p.op == 3 else len(p.kids) - 1
-            return all(walk(k, depth + 1) for k in p.kids)
+            sets = p._set_groups()
+            grouped = {i for _, members in sets for i in members}
+            terms += len(sets); ops += len(sets)  # one term each; its Likes add no depth
+            ops += 1 if p.op == 3 else len(p.kids) - len(grouped) + len(sets) - 1
+            return all(walk(k, depth + 1) for i, k in enumerate(p.kids) if i not in grouped)
 
-        return walk(self, 0) and terms <= _abi.PRED_MAX_TERMS and ops <= _abi.PRED_MAX_OPS
+        self._lowerable = walk(self, 0) and terms <= _abi.PRED_MAX_TERMS and ops <= _abi.PRED_MAX_OPS
+        return self._lowerable
+
+    def _set_groups(self) -> list:
+        """The set terms of an Any node (CPB_PRED_SET_MIN, csvplus_b200.h), as the device forms them: the direct Like children
+        grouped by the set of column names they compare; a group of at least PRED_SET_MIN children whose literals fit an
+        index key image is one term.  -> [(keys in the order of the group's first Like, child positions)], by first child."""
+        if self._sets is None:
+            self._sets = []
+            if self.op == 2 and len(self.kids) >= _abi.PRED_SET_MIN:
+                groups: dict = {}
+                for i, k in enumerate(self.kids):
+                    if isinstance(k, Predicate) and k.op == 0 and 0 < len(k.match) <= _MAX_INDEX_KEYS:
+                        m = k.match  # (a one-column Like is grouped by its name: a str never equals a frozenset)
+                        groups.setdefault(next(iter(m)) if len(m) == 1 else frozenset(m), []).append(i)
+                for members in groups.values():
+                    if len(members) < _abi.PRED_SET_MIN:
+                        continue
+                    keys = list(self.kids[members[0]].match)
+                    widths = [max(len(_enc(self.kids[i].match[key])) for i in members) for key in keys]
+                    if sum(w + (1 if w < 255 else 2 if w < 65535 else 4) for w in widths) <= _MAX_KEY_IMAGE:
+                        self._sets.append((keys, members))
+                self._sets.sort(key=lambda s: s[1][0])
+        return self._sets
 
     def columns(self) -> set:
         """the distinct column names the tree's Like terms compare"""
         return set(self.match).union(*(k.columns() for k in self.kids))
 
     def _c(self, keep: list) -> _abi.Pred:
+        """the cpb_pred tree, lowered once per node; keep receives what must stay alive while the tree is in use"""
+        if self._lowered is None:
+            own: list = []
+            self._lowered = (self._lower(own), own)
+        keep.append(self._lowered)
+        return self._lowered[0]
+
+    def _lower(self, keep: list) -> _abi.Pred:
         p = _abi.Pred()
         p.op = self.op
         if self.op == 0:
             ka, kb = _strs(self.match.keys()); va, vb = _strs(self.match.values())
             keep += [ka, kb, va, vb]
             p.n, p.keys, p.values = len(self.match), ka, va
-        else:
-            kids = [k._c(keep) for k in self.kids]
-            arr = (C.POINTER(_abi.Pred) * max(1, len(kids)))(*[C.pointer(k) for k in kids])
-            keep += [kids, arr]
-            p.n, p.children = len(kids), arr
+            return p
+        ptrs = np.zeros(max(1, len(self.kids)), np.uint64)
+        bulk = np.zeros(len(ptrs), bool)
+        for keys, members in self._set_groups():
+            ptrs[members] = self._lower_group(keys, members, keep)
+            bulk[members] = True
+        for i, k in enumerate(self.kids):
+            if not bulk[i]:
+                ptrs[i] = C.addressof(k._c(keep))
+        arr = (C.POINTER(_abi.Pred) * len(ptrs)).from_buffer(ptrs)
+        keep += [ptrs, arr]
+        p.n, p.children = len(self.kids), arr
         return p
+
+    def _lower_group(self, keys: list, members: list, keep: list) -> np.ndarray:
+        """the Likes of one set term in bulk: every child's pairs in the order of keys, all children on one keys array, the
+        values in one cpb_str array over one byte string, the nodes in one array.  -> the nodes' addresses"""
+        nk, m = len(keys), len(members)
+        ka, kb = _strs(keys)
+        vals = [_enc(self.kids[i].match[k]) for i in members for k in keys]
+        blob = b"".join(vals)
+        lens = np.fromiter(map(len, vals), np.uint64, len(vals))
+        offs = np.zeros(len(vals), np.uint64)
+        np.cumsum(lens[:-1], out=offs[1:])
+        base = np.frombuffer(blob, np.uint8) if blob else np.zeros(1, np.uint8)
+        strs = np.empty(len(vals), _STR_DTYPE)
+        strs["ptr"] = np.uint64(base.ctypes.data) + offs
+        strs["len"] = lens
+        nodes = np.zeros(m, _PRED_DTYPE)
+        nodes["n"] = nk
+        nodes["keys"] = C.addressof(ka)
+        nodes["values"] = np.uint64(strs.ctypes.data) + np.arange(m, dtype=np.uint64) * np.uint64(_STR_DTYPE.itemsize * nk)
+        keep += [ka, kb, blob, base, strs, nodes]
+        return np.uint64(nodes.ctypes.data) + np.arange(m, dtype=np.uint64) * np.uint64(_PRED_DTYPE.itemsize)
 
 
 def Like(match: Row) -> Predicate:

@@ -327,10 +327,17 @@ FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n);
 void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out);
 // rows row_ids[0, nout) of t (rows 0..nout-1 when row_ids is null: a view compacted into buffers of its own)
 std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout);
-// the rows of t whose flag (uint32 0/1, one per row) is set: scan_flags, compact_flags timed as compact_ids, gather_rows
-std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags);
+// the rows of t whose flag (uint32 0/1, one per row) is set: scan_flags, compact_flags timed as compact_ids, gather_rows.
+// first, when given: the position of the first set flag (one more host synchronisation when there is one)
+std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags, uint64_t* first = nullptr);
 std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred);
 int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred);
+struct Compiled;  // pred.cuh
+// The parse of a predicate with set terms (has_set_terms, pred.cuh): p is the unfiltered parse; its rows are filtered with
+// the predicate compiled against its columns (the output columns), reusing *comp when it was compiled against the same
+// names (a stream compiles once and builds its set indexes once).  The error and record counts stay the parse's; row 0's
+// line is the line of the first row kept.
+void filter_parsed(Ctx* c, Parsed& p, const cpb_pred* pred, std::shared_ptr<Compiled>& comp);
 // rows `ids` (positions in `order`) of the index restricted to columns `cols` (row-slot path when it pays, else gather_rows)
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout,
                                          RowOrder order);
@@ -345,6 +352,7 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::
 std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix);  // materialises ix.table on first use
 void ensure_sorted(Ctx* c, Index& ix);                    // sorts a lazily-sorted unique index on first need of the order
 constexpr int MAXKEYS = 16;
+constexpr uint32_t MAX_KEY_IMAGE_BYTES = 4096;  // the longest key image of an index row
 struct KeyDesc {  // key columns + the widths of the order-preserving image (sort.cu)
     int nkeys;
     const uint32_t* off[MAXKEYS];
@@ -362,6 +370,10 @@ void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
 // join.cu.  A join column missing from a non-empty probe table throws DataError.
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti);
+// flag[i] (uint32 0/1) = whether the key of probe row i on the probe columns pidx (the first pidx.size() key columns of
+// ix) is in the index (hit) / is not (!hit): Except's test, and the set terms of a predicate.  A probe value longer than
+// the index column's widest value is not in it.
+Buf key_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, bool hit);
 void find_range(Ctx* c, Index& ix, const std::vector<std::string>& values, int64_t* lo, int64_t* hi);
 bool index_has_duplicates(Ctx* c, Index& ix);  // full-key probe table over the source order + self probe
 // fills ix.derived.rowhash (cols set by the caller) from ix.src.  built: the table is complete; duplicate: some key occurs twice;

@@ -250,7 +250,7 @@ std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_i
 
 // the rows of t whose flag is set: the flags scanned and counted (one host synchronisation), compacted to row ids
 // (timed as compact_ids) and the rows gathered
-std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags) {
+std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags, uint64_t* first) {
     const uint64_t n = (uint64_t)t.nrows;
     const FlagScan s = scan_flags(c, flags, n);
     Buf ids = dev_alloc(c, (s.count + 1) * 4);
@@ -258,6 +258,7 @@ std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags)
         KernelTimer kt(c, "compact_ids", n * 8 + s.count * 4);
         compact_flags(c, s, 0, ids->as<uint32_t>());
     }
+    if (first) *first = s.count ? read_back<uint32_t>(c, ids->p) : 0;
     return gather_rows(c, t, ids->as<uint32_t>(), (int64_t)s.count);
 }
 
@@ -740,11 +741,12 @@ std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, con
 // ------------------------------------------------------------------ Filter over a table
 struct FilterCols { const uint32_t* off[MAXTERMS]; const uint8_t* data[MAXTERMS]; };
 
-__global__ void filter_flags_kernel(FilterCols cols, PredProg prog, const uint8_t* __restrict__ lits, uint32_t* flags, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+// the eq word of row i over the literal terms (the terms in `skip`, set terms, are left 0)
+__device__ __forceinline__ uint32_t literal_terms(const FilterCols& cols, const PredProg& prog, const uint8_t* __restrict__ lits, uint64_t i,
+                                                  uint32_t skip) {
     uint32_t eq = 0;
     for (int t = 0; t < prog.nterms; t++) {
+        if ((skip >> t) & 1u) continue;
         const uint32_t* off = cols.off[t];
         uint32_t s = off[i], len = off[i + 1] - s;
         if (len != prog.term_len[t]) continue;
@@ -754,22 +756,90 @@ __global__ void filter_flags_kernel(FilterCols cols, PredProg prog, const uint8_
         for (uint32_t k = 0; k < len; k++) if (p[k] != l[k]) { ok = false; break; }
         if (ok) eq |= 1u << t;
     }
+    return eq;
+}
+__global__ void filter_flags_kernel(FilterCols cols, PredProg prog, const uint8_t* __restrict__ lits, uint32_t* flags, uint64_t n) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    flags[i] = eval_pred(prog, literal_terms(cols, prog, lits, i, 0u)) ? 1u : 0u;
+}
+// A program with set terms: term t of `sets` takes its bit from hit[t][i], the probe of the term's index (key_flags).
+// (__grid_constant__: the arrays indexed by term are read where the parameters are, not copied to each thread's stack)
+struct SetHits { const uint32_t* hit[MAXTERMS]; };
+__global__ void filter_set_kernel(const __grid_constant__ FilterCols cols, const __grid_constant__ PredProg prog, const uint8_t* __restrict__ lits,
+                                  const __grid_constant__ SetHits hits, uint32_t sets, uint32_t* flags, uint64_t n) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t eq = literal_terms(cols, prog, lits, i, sets);
+    for (uint32_t m = sets; m; m &= m - 1) {
+        const int t = __ffs(m) - 1;
+        eq |= (hits.hit[t][i] & 1u) << t;
+    }
     flags[i] = eval_pred(prog, eq) ? 1u : 0u;
 }
-// flags[i] = 1 when pred holds for row i of t.  The predicate is compiled against t's columns first, so a bad one throws
-// whether or not t has rows; for an empty t nothing is enqueued and the result is null.
-static Buf predicate_flags(Ctx* c, const Table& t, const cpb_pred* pred) {
+
+static Compiled compile_for(const Table& t, const cpb_pred* pred) {
     if (!pred) throw ArgError{CPB_ERR_ARG, "nil predicate"};
     Compiled comp;
     compile_pred(pred, [&](const std::string& key) { return t.find(key); }, comp);
-    const uint64_t n = (uint64_t)t.nrows;
-    if (n == 0) return nullptr;
-    FilterCols fc{};
-    for (int i = 0; i < comp.prog.nterms; i++) { fc.off[i] = t.cols[comp.prog.term_col[i]].off(); fc.data[i] = t.cols[comp.prog.term_col[i]].bytes(); }
+    return comp;
+}
+// the literal terms' columns and the literal pool on the device
+static Buf literal_args(Ctx* c, const Table& t, const Compiled& comp, FilterCols& fc) {
+    for (int i = 0; i < comp.prog.nterms; i++)
+        if (comp.prog.term_col[i] >= 0) { fc.off[i] = t.cols[comp.prog.term_col[i]].off(); fc.data[i] = t.cols[comp.prog.term_col[i]].bytes(); }
     Buf lits = dev_alloc(c, comp.lits.size() + 16);
     if (!comp.lits.empty()) CPB_CUDA(cudaMemcpyAsync(lits->p, comp.lits.data(), comp.lits.size(), cudaMemcpyHostToDevice, c->stream));
+    return lits;
+}
+// flags[i] = 1 when the program of a tree without set terms holds for row i of a non-empty t
+static Buf predicate_flags(Ctx* c, const Table& t, const Compiled& comp) {
+    const uint64_t n = (uint64_t)t.nrows;
+    FilterCols fc{};
+    Buf lits = literal_args(c, t, comp, fc);
     Buf flags = dev_alloc(c, n * 4);
     filter_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(fc, comp.prog, lits->as<uint8_t>(), flags->as<uint32_t>(), n);
+    CPB_CUDA(cudaGetLastError());
+    return flags;
+}
+// IndexOn(keys) over the literal tuples of a set term; the host copy of the literals is released once they are uploaded
+static std::shared_ptr<Index> set_index(Ctx* c, SetTerm& s) {
+    auto lt = std::make_shared<Table>(); lt->ctx = c; lt->nrows = (int64_t)s.rows;
+    uint64_t bytes = 0;
+    for (size_t j = 0; j < s.keys.size(); j++) bytes += s.data[j].size() + s.off[j].size() * 4;
+    {
+        KernelTimer kt(c, "pred_set_upload", bytes, 0);
+        for (size_t j = 0; j < s.keys.size(); j++) {
+            Column col; col.name = s.keys[j];
+            col.offsets = dev_alloc(c, s.off[j].size() * 4);
+            col.data = dev_alloc(c, s.data[j].size() + 16);
+            // (pageable sources: the runtime has staged them when the call returns)
+            CPB_CUDA(cudaMemcpyAsync(col.offsets->p, s.off[j].data(), s.off[j].size() * 4, cudaMemcpyHostToDevice, c->stream));
+            if (!s.data[j].empty()) CPB_CUDA(cudaMemcpyAsync(col.data->p, s.data[j].data(), s.data[j].size(), cudaMemcpyHostToDevice, c->stream));
+            lt->cols.push_back(col);
+        }
+    }
+    s.off.clear(); s.off.shrink_to_fit(); s.data.clear(); s.data.shrink_to_fit();
+    return build_index(c, lt, s.keys, false);
+}
+// flags of a program with set terms over a non-empty t: per set term its index (built on first use) probed with t's
+// columns, then the literal terms and the program in filter_set
+static Buf set_predicate_flags(Ctx* c, const Table& t, Compiled& comp) {
+    const uint64_t n = (uint64_t)t.nrows;
+    SetHits sh{};
+    uint32_t sets = 0;
+    std::vector<Buf> hits;
+    for (SetTerm& s : comp.sets) {
+        if (!s.index) s.index = set_index(c, s);
+        hits.push_back(key_flags(c, t, s.cols, *s.index, true));
+        sh.hit[s.term] = hits.back()->as<uint32_t>();
+        sets |= 1u << s.term;
+    }
+    FilterCols fc{};
+    Buf lits = literal_args(c, t, comp, fc);
+    Buf flags = dev_alloc(c, n * 4);
+    KernelTimer kt(c, "filter_set", n * (4 + 4 * (uint64_t)comp.sets.size() + 4 * (uint64_t)(comp.prog.nterms - (int)comp.sets.size())));
+    filter_set_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(fc, comp.prog, lits->as<uint8_t>(), sh, sets, flags->as<uint32_t>(), n);
     CPB_CUDA(cudaGetLastError());
     return flags;
 }
@@ -780,14 +850,21 @@ __global__ void first_false_kernel(const uint32_t* __restrict__ flags, uint64_t 
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n && flags[i] == 0) atomicMin(out, (unsigned long long)i);
 }
+// The predicate is compiled against t's columns first, so a bad one throws whether or not t has rows.
 int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred) {
+    Compiled comp = compile_for(t, pred);
     const uint64_t n = (uint64_t)t.nrows;
-    if (n == 0) { predicate_flags(c, t, pred); return 0; }  // (checks the predicate)
+    if (n == 0) return 0;
     Buf out = dev_alloc(c, 8);
     CPB_CUDA(cudaMemsetAsync(out->p, 0xff, 8, c->stream));
-    {
+    if (comp.sets.empty()) {
         KernelTimer kt(c, "filter_like", n * 12, 2);
-        Buf flags = predicate_flags(c, t, pred);
+        Buf flags = predicate_flags(c, t, comp);
+        first_false_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(flags->as<uint32_t>(), n, (unsigned long long*)out->p);
+        CPB_CUDA(cudaGetLastError());
+    } else {
+        Buf flags = set_predicate_flags(c, t, comp);
+        KernelTimer kt(c, "first_false", n * 4);
         first_false_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(flags->as<uint32_t>(), n, (unsigned long long*)out->p);
         CPB_CUDA(cudaGetLastError());
     }
@@ -795,15 +872,38 @@ int64_t first_false_row(Ctx* c, const Table& t, const cpb_pred* pred) {
     return first == ~0ull ? (int64_t)n : (int64_t)first;
 }
 
-std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred) {
+// the rows of t for which comp holds; *first (when given) = the position of the first of them in t
+static std::shared_ptr<Table> filter_compiled(Ctx* c, const Table& t, Compiled& comp, uint64_t* first = nullptr) {
     const uint64_t n = (uint64_t)t.nrows;
-    if (n == 0) { predicate_flags(c, t, pred); return gather_rows(c, t, nullptr, 0); }  // (checks the predicate)
+    if (n == 0) { if (first) *first = 0; return gather_rows(c, t, nullptr, 0); }
     Buf flags;
-    {
+    if (comp.sets.empty()) {
         KernelTimer kt(c, "filter_like", n * 12);
-        flags = predicate_flags(c, t, pred);
+        flags = predicate_flags(c, t, comp);
+    } else flags = set_predicate_flags(c, t, comp);
+    return rows_where(c, t, flags->as<uint32_t>(), first);
+}
+
+std::shared_ptr<Table> filter_table(Ctx* c, const Table& t, const cpb_pred* pred) {
+    Compiled comp = compile_for(t, pred);
+    return filter_compiled(c, t, comp);
+}
+
+void filter_parsed(Ctx* c, Parsed& p, const cpb_pred* pred, std::shared_ptr<Compiled>& comp) {
+    const Table& t = *p.table;
+    if (t.nrows == 0) return;
+    std::vector<std::string> names;
+    for (const Column& col : t.cols) names.push_back(col.name);
+    if (!comp || comp->columns != names) {
+        comp = std::make_shared<Compiled>(compile_for(t, pred));
+        comp->columns = std::move(names);
     }
-    return rows_where(c, t, flags->as<uint32_t>());
+    uint64_t first = 0;
+    auto r = filter_compiled(c, t, *comp, &first);
+    r->first_line = t.first_line + first;
+    r->src_field = t.src_field;
+    r->record_fields = t.record_fields;
+    p.table = r;
 }
 
 // ------------------------------------------------------------------ concat

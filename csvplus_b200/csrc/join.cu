@@ -172,9 +172,9 @@ __global__ void expand_pairs_kernel(const uint32_t* __restrict__ lo, const uint3
     uint32_t c = cnt[i], p = pos[i], l = lo[i];
     for (uint32_t j = 0; j < c; j++) { pid[p + j] = (uint32_t)i; iid[p + j] = l + j; }
 }
-__global__ void zero_flag_kernel(const uint32_t* __restrict__ cnt, uint32_t* flag, uint64_t n) {
+__global__ void found_flag_kernel(const uint32_t* __restrict__ cnt, uint32_t want, uint32_t* flag, uint64_t n) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flag[i] = cnt[i] == 0 ? 1u : 0u;
+    if (i < n) flag[i] = (cnt[i] != 0) == (want != 0) ? 1u : 0u;
 }
 
 __global__ void iota_heads_kernel(uint32_t* heads, uint64_t n) {  // heads[i] = i for i in [0, n]
@@ -460,6 +460,38 @@ static Buf rowhash_flags(Ctx* c, const Table& probe, const std::vector<int>& pid
     return flag;
 }
 
+// per probe row the run of index rows matching its key on the first nk key columns: lo / cnt (cnt 0: none), and in
+// flags (32 bytes, zeroed here) the scan total slot [0..1], not_one [2] and the match count [4..5]
+static RowOrder probe_runs(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, uint32_t* lo, uint32_t* cnt, const Buf& flags) {
+    const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
+    const int nk = (int)pidx.size();
+    CPB_CUDA(cudaMemsetAsync(flags->p, 0, 32, c->stream));
+    uint32_t* not_one = flags->as<uint32_t>() + 2;  // [0..1] = scan total
+    const RowOrder order = join_order(ix, nk);
+    if (ni != 0 && order == RowOrder::sorted) ensure_sorted(c, ix);
+    if (ni == 0) {
+        CPB_CUDA(cudaMemsetAsync(cnt, 0, (np + 1) * 4, c->stream));
+    } else if (!ix.in_order) {
+        search_probe(c, probe, pidx, ix, nk, lo, cnt, not_one);
+    } else {
+        const ProbeTable& ht = ensure_hash(c, ix, order, nk);
+        probe_dispatch(c, probe, pidx, ix, ht, order, nk, lo, cnt, not_one);
+    }
+    return order;
+}
+
+Buf key_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& ix, bool hit) {
+    const uint64_t np = (uint64_t)probe.nrows;
+    if (np == 0) return dev_alloc(c, 4);
+    if (ix.derived.rowhash.slots && pidx.size() == ix.key_cols.size()) return rowhash_flags(c, probe, pidx, ix, hit);
+    Buf lo = dev_alloc(c, np * 4), cnt = dev_alloc(c, (np + 1) * 4), flags = dev_alloc(c, 32);
+    probe_runs(c, probe, pidx, ix, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags);
+    Buf flag = dev_alloc(c, np * 4);
+    found_flag_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(cnt->as<uint32_t>(), hit ? 1u : 0u, flag->as<uint32_t>(), np);
+    CPB_CUDA(cudaGetLastError());
+    return flag;
+}
+
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti) {
     const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
     const int nk = (int)cols.size();
@@ -514,12 +546,12 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         r->first_line = probe.first_line;
         return r;
     };
+    if (anti) {
+        Buf miss = key_flags(c, probe, pidx, ix, false);
+        return flagged_rows(probe, scan_flags(c, miss->as<uint32_t>(), np));
+    }
     if (ix.derived.rowhash.slots && nk == (int)ix.key_cols.size()) {
         // a unique index with a row-carrying table joined on its full key: one random access per probe row
-        if (anti) {
-            Buf miss = rowhash_flags(c, probe, pidx, ix, false);
-            return flagged_rows(probe, scan_flags(c, miss->as<uint32_t>(), np));
-        }
         Buf hit;
         FlagScan hits{};  // hits.pos stays null until the hit rows are needed
         std::shared_ptr<Table> gi;
@@ -545,23 +577,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         return flagged_rows(*out, hits);
     }
     Buf lo = dev_alloc(c, np * 4), cnt = dev_alloc(c, (np + 1) * 4), flags = dev_alloc(c, 32);
-    CPB_CUDA(cudaMemsetAsync(flags->p, 0, 32, c->stream));
-    uint32_t* not_one = flags->as<uint32_t>() + 2;  // [0..1] = scan total
-    const RowOrder order = join_order(ix, nk);
-    if (ni != 0 && order == RowOrder::sorted) ensure_sorted(c, ix);
-    if (ni == 0) {
-        CPB_CUDA(cudaMemsetAsync(cnt->p, 0, (np + 1) * 4, c->stream));
-    } else if (!ix.in_order) {
-        search_probe(c, probe, pidx, ix, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
-    } else {
-        const ProbeTable& ht = ensure_hash(c, ix, order, nk);
-        probe_dispatch(c, probe, pidx, ix, ht, order, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), not_one);
-    }
-    if (anti) {
-        Buf flag = dev_alloc(c, np * 4);
-        zero_flag_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(cnt->as<uint32_t>(), flag->as<uint32_t>(), np);
-        return flagged_rows(probe, scan_flags(c, flag->as<uint32_t>(), np));
-    }
+    const RowOrder order = probe_runs(c, probe, pidx, ix, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags);
     const std::vector<uint32_t> hf = read_back<uint32_t>(c, flags->p, 8);
     const uint64_t m = (uint64_t)hf[4] | ((uint64_t)hf[5] << 32);  // counted by the probe kernel (0 when ni == 0)
     // every probe row matched exactly one index row (the usual foreign-key join): the probe-side columns of the

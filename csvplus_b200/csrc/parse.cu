@@ -409,6 +409,13 @@ Parsed run_general(Ctx* c, ParseParams P, const cpb_reader_opts& o, const Substi
 
 Parsed parse_csv(Ctx* c, const uint8_t* in_arg, uint64_t n_arg, const cpb_reader_opts& o_arg, const Spec& spec, const cpb_pred* filter,
                  uint64_t line_base, const ShardArgs* sh) {
+    // set terms are not fused into the scan: the output columns are parsed unfiltered, then filtered
+    if (filter && has_set_terms(filter)) {
+        Parsed p = parse_csv(c, in_arg, n_arg, o_arg, spec, nullptr, line_base, sh);
+        std::shared_ptr<Compiled> comp;
+        filter_parsed(c, p, filter, comp);
+        return p;
+    }
     // encoding/csv readRecord's option validation (SURVEY App. A.2.1)
     if (o_arg.delimiter == o_arg.comment || !valid_delim(o_arg.delimiter) || (o_arg.comment != 0 && !valid_delim(o_arg.comment)))
         return {empty_table(c, spec), DataError{CPB_E_INVALID_DELIM, -1, 1, true, "csv: invalid field or comment delimiter"}};

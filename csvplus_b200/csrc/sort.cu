@@ -375,7 +375,7 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
     }
     const uint32_t kbytes = prefix_bytes(*ix, (int)keys.size()), words = (kbytes + 7) / 8;
     ix->image_words = words;
-    if ((uint64_t)words * 8 > 4096) throw ArgError{CPB_ERR_UNSUPPORTED, "index keys longer than 4 KiB are not supported"};
+    if ((uint64_t)words * 8 > MAX_KEY_IMAGE_BYTES) throw ArgError{CPB_ERR_UNSUPPORTED, "index keys longer than 4 KiB are not supported"};
     // 2. UniqueIndexOn: the duplicate check does not need the order — a probe table over the rows as they are, in which
     //    every key must find itself.  When it passes (the usual case) the sort is left for whoever needs the order.
     Buf img;  // image of the unsorted rows

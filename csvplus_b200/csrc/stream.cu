@@ -18,6 +18,7 @@
 #include <algorithm>
 
 #include "core.hpp"
+#include "pred.cuh"
 #include "util.cuh"
 
 namespace cpb {
@@ -146,6 +147,10 @@ struct Stream {
     cpb_reader_opts o;
     std::vector<std::pair<std::string, int>> spec;
     const cpb_pred* filter;
+    // a filter with set terms filters every batch's table with one compiled program and its set indexes, made for the
+    // first batch with rows (the output columns are the same in every batch)
+    bool set_filter = false;
+    std::shared_ptr<Compiled> comp;
     cudaStream_t copy = nullptr;
     cudaEvent_t copied = nullptr;   // after the last push's copy (the parse waits for it)
     cudaEvent_t freed[2] = {};      // after the last ctx-stream work that read slot k
@@ -222,12 +227,13 @@ struct Stream {
         cpb_reader_opts bo = o;
         if (resolved) bo.header_from_first_row = 0;
         const uint64_t base = resolved ? line_base : (o.header_from_first_row ? 2u : 1u);
-        Parsed p = parse_csv(c, in, cut, bo, spec, filter, base);
+        Parsed p = parse_csv(c, in, cut, bo, spec, set_filter ? nullptr : filter, base);
         if (trial) {
             // a bare quote is an error wherever the record ends; another error only if a later record starts after it
             const bool sure = p.error && p.error->has_line && (p.error->kind == CPB_E_BARE_QUOTE || p.error->line + 1 < base + p.records);
             if (!sure) return {};
         }
+        if (set_filter) filter_parsed(c, p, filter, comp);
         if (!resolved) {
             if (p.no_record && !last_pushed) {
                 p.error.reset();  // only blank / comment lines so far: they hold no record, drop them
@@ -267,6 +273,7 @@ Stream* stream_open(Ctx* c, const cpb_reader_opts& o, std::vector<std::pair<std:
     // invalid options are reported by the first batch's parse, as cpb_parse_csv reports them
     auto s = new Stream{c, o, std::move(spec), filter};
     try {
+        s->set_filter = filter && has_set_terms(filter);
         CPB_CUDA(cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking));
         CPB_CUDA(cudaEventCreateWithFlags(&s->copied, cudaEventDisableTiming));
         for (auto& e : s->freed) CPB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));

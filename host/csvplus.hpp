@@ -107,14 +107,48 @@ struct Predicate {
         }
     }
     // the device compiles the tree: no opaque function in it, within the CPB_PRED_MAX_* limits (every Like pair counted
-    // as a term); a declined tree runs on host rows
+    // as a term, a set term as one); a declined tree runs on host rows
     bool lowerable() const { int terms = 0, ops = 0; return fits(0, terms, ops) && terms <= CPB_PRED_MAX_TERMS && ops <= CPB_PRED_MAX_OPS; }
     bool fits(int depth, int& terms, int& ops) const {
         if (op < 0 || depth > CPB_PRED_MAX_DEPTH) return false;
         if (op == CPB_PRED_LIKE) { terms += (int)match.size(); ops += 2 * (int)match.size() - 1; return true; }
-        ops += kids.empty() || op == CPB_PRED_NOT ? 1 : (int)kids.size() - 1;
-        for (auto& k : kids) if (!k.fits(depth + 1, terms, ops)) return false;
+        if (kids.empty()) { ops += 1; return true; }
+        const std::vector<int> set = set_of();
+        int nsets = 0, grouped = 0;
+        for (size_t i = 0; i < kids.size(); i++) if (set[i] >= 0) { grouped++; if (set[i] >= nsets) nsets = set[i] + 1; }
+        terms += nsets; ops += nsets;  // one term each; its Likes add no depth
+        ops += op == CPB_PRED_NOT ? 1 : (int)kids.size() - grouped + nsets - 1;
+        for (size_t i = 0; i < kids.size(); i++) if (set[i] < 0 && !kids[i].fits(depth + 1, terms, ops)) return false;
         return true;
+    }
+    // The set terms of an Any node (CPB_PRED_SET_MIN, include/csvplus_b200.h): per child the set term it belongs to (0, 1, ...
+    // in the order of their first children), -1 for none.  A group of Likes over one set of column names is a set term when
+    // it has CPB_PRED_SET_MIN children or more and its literals fit an index key image.
+    std::vector<int> set_of() const {
+        std::vector<int> out(kids.size(), -1);
+        if (op != CPB_PRED_ANY || kids.size() < CPB_PRED_SET_MIN) return out;
+        std::map<std::vector<std::string>, std::vector<size_t>> groups;  // key names (sorted: Row is an ordered map) -> children
+        for (size_t i = 0; i < kids.size(); i++) {
+            const Predicate& k = kids[i];
+            if (k.op != CPB_PRED_LIKE || k.match.empty() || k.match.size() > 16) continue;
+            std::vector<std::string> names;
+            for (auto& kv : k.match) names.push_back(kv.first);
+            groups[names].push_back(i);
+        }
+        std::vector<const std::vector<size_t>*> sets;
+        for (auto& g : groups) {
+            if (g.second.size() < CPB_PRED_SET_MIN) continue;
+            uint64_t image = 0;  // the key image of an index over the literals: every value padded to w, then its length
+            for (auto& name : g.first) {
+                uint64_t w = 0;
+                for (size_t i : g.second) w = std::max<uint64_t>(w, kids[i].match.at(name).size());
+                image += w + (w < 255 ? 1 : w < 65535 ? 2 : 4);
+            }
+            if (image <= 4096) sets.push_back(&g.second);
+        }
+        std::sort(sets.begin(), sets.end(), [](auto a, auto b) { return (*a)[0] < (*b)[0]; });
+        for (size_t s = 0; s < sets.size(); s++) for (size_t i : *sets[s]) out[i] = (int)s;
+        return out;
     }
     // the distinct columns the Like terms compare
     void columns(std::vector<std::string>& out) const {
@@ -132,9 +166,13 @@ inline Predicate Not(Predicate k) { Predicate p; p.op = CPB_PRED_NOT; p.kids = {
 inline Predicate Func(std::function<bool(const Row&)> f) { Predicate p; p.fn = std::move(f); return p; }
 
 namespace detail {
-struct CPred {  // owns the cpb_pred tree
+// owns the cpb_pred tree.  The Likes of a set term are lowered in bulk: one keys array for all of them, their values in one
+// array pointing at the Predicate's strings (so the Predicate must outlive the CPred), their nodes in one array.
+struct CPred {
     std::vector<std::unique_ptr<CPred>> kids; std::vector<const cpb_pred*> kid_ptrs;
     std::vector<std::string> ks, vs; std::vector<cpb_str> kstr, vstr; cpb_pred p{};
+    struct Set { std::vector<cpb_str> keys, values; std::vector<cpb_pred> nodes; };
+    std::vector<Set> sets;
     explicit CPred(const Predicate& q) {
         p.op = q.op;
         if (q.op == CPB_PRED_LIKE) {
@@ -142,8 +180,27 @@ struct CPred {  // owns the cpb_pred tree
             for (size_t i = 0; i < ks.size(); i++) { kstr.push_back(cpb_str{ks[i].data(), ks[i].size()}); vstr.push_back(cpb_str{vs[i].data(), vs[i].size()}); }
             p.n = (int)ks.size(); p.keys = kstr.data(); p.values = vstr.data();
         } else {
-            for (auto& k : q.kids) { kids.emplace_back(new CPred(k)); kid_ptrs.push_back(&kids.back()->p); }
-            p.n = (int)kids.size(); p.children = kid_ptrs.data();
+            const std::vector<int> set = q.set_of();
+            std::vector<size_t> nodes, values;  // per set: reserved up front, the nodes and values must not move once pointed at
+            for (size_t i = 0; i < set.size(); i++) {
+                if (set[i] < 0) continue;
+                if (set[i] >= (int)nodes.size()) { nodes.resize(set[i] + 1); values.resize(set[i] + 1); }
+                nodes[set[i]]++; values[set[i]] += q.kids[i].match.size();
+            }
+            sets.resize(nodes.size());
+            for (size_t s = 0; s < sets.size(); s++) { sets[s].nodes.reserve(nodes[s]); sets[s].values.reserve(values[s]); }
+            for (size_t i = 0; i < q.kids.size(); i++) {
+                if (set[i] < 0) { kids.emplace_back(new CPred(q.kids[i])); kid_ptrs.push_back(&kids.back()->p); continue; }
+                Set& s = sets[set[i]];
+                const Row& m = q.kids[i].match;  // (a Row is ordered: every Like of the set has its keys in one order)
+                if (s.keys.empty()) for (auto& kv : m) s.keys.push_back(cpb_str{kv.first.data(), kv.first.size()});
+                cpb_pred node{};
+                node.op = CPB_PRED_LIKE; node.n = (int)m.size(); node.keys = s.keys.data(); node.values = s.values.data() + s.values.size();
+                for (auto& kv : m) s.values.push_back(cpb_str{kv.second.data(), kv.second.size()});
+                s.nodes.push_back(node);
+                kid_ptrs.push_back(&s.nodes.back());
+            }
+            p.n = (int)kid_ptrs.size(); p.children = kid_ptrs.data();
         }
     }
 };

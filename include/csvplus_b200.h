@@ -32,9 +32,24 @@ extern "C" {
 #define CPB_ABI_VERSION 1
 #define CPB_MAX_PARSE_COLS 16 /* columns extracted by one fused parse call (output + predicate columns) */
 /* the largest cpb_pred tree the device compiles; a larger one fails with CPB_ERR_UNSUPPORTED */
-#define CPB_PRED_MAX_TERMS 32 /* Like (column, literal) pairs whose column exists */
-#define CPB_PRED_MAX_OPS 64   /* postfix operations: one per Like pair, per AND / OR / NOT joining them, per empty All / Any */
-#define CPB_PRED_MAX_DEPTH 48 /* All / Any / Not nodes above the deepest node */
+#define CPB_PRED_MAX_TERMS 32 /* Like (column, literal) pairs whose column exists, and set terms */
+#define CPB_PRED_MAX_OPS 64   /* postfix operations: one per Like pair and per set term, per AND / OR / NOT joining them,
+                                 per empty All / Any */
+#define CPB_PRED_MAX_DEPTH 48 /* All / Any / Not nodes above the deepest node (the Likes of a set term add none) */
+/* Set terms (value lists: Any(Like{id: v1}, Like{id: v2}, ...)).  Inside an Any node, the direct Like children that compare
+ * the same SET of column names (key order inside a Like does not matter; a Like naming one column twice never joins a
+ * group) form a group.  A group of at least CPB_PRED_SET_MIN children is one set term: true for a row whose values of
+ * those columns equal, byte for byte, the literals of some child of the group.  It counts as one term and one operation;
+ * the node's other children compile as they would without the group, and everything is ORed.  A set term is evaluated as
+ * an IndexOn over the table of the group's literal tuples, probed as Except probes an index.  So a group is a set term
+ * only when that index can exist:
+ *   - at most 16 columns, and
+ *   - sum over the group's columns of (w + L(w)) <= 4096 bytes, w = the longest literal of the column in bytes,
+ *     L(w) = 1 if w < 255, 2 if w < 65535, else 4 (the key image: every value padded to w, then its length).
+ * A group that fails either compiles as separate Like terms.  When a column of a set term is absent from the row type the
+ * term is a constant false (as each of its Likes would be).  Every tree within the limits above has at most 32 terms, so
+ * no group in it reaches CPB_PRED_SET_MIN: such trees compile exactly as without set terms. */
+#define CPB_PRED_SET_MIN 33
 
 typedef struct cpb_ctx cpb_ctx;
 typedef struct cpb_table cpb_table; /* columnar batch of rows: Arrow-style string columns in HBM */
