@@ -1,5 +1,7 @@
-// format regenerates tests/golden/format_kat.csv with Go's strconv and compares it with the committed file, which the
-// Python restatement (tests/ftoa_oracle.py) wrote.  Unrun here: there is no Go toolchain in this image.
+// format regenerates tests/golden/format_kat.csv and format32_kat.csv with Go's strconv and compares them with the
+// committed files, which the Python restatement (tests/ftoa_oracle.py) wrote.  format32_kat.csv lines are
+// `bits,fmt,prec,expected` with the float32's bits in hex, checked against FormatFloat(float64(x), fmt, prec, 32).
+// Unrun here: there is no Go toolchain in this image.
 //
 //	go run ./format ../../tests/golden
 package main
@@ -15,7 +17,14 @@ import (
 )
 
 func main() {
-	path := filepath.Join(os.Args[1], "format_kat.csv")
+	bad := check(filepath.Join(os.Args[1], "format_kat.csv"), false) + check(filepath.Join(os.Args[1], "format32_kat.csv"), true)
+	if bad != 0 {
+		os.Exit(1)
+	}
+}
+
+// check compares one fixture with strconv; bits32: the float32 fixture.  Returns the lines that differ.
+func check(path string, bits32 bool) int {
 	f, err := os.Open(path)
 	if err != nil {
 		panic(err)
@@ -26,7 +35,16 @@ func main() {
 	for sc.Scan() {
 		p := strings.SplitN(sc.Text(), ",", 5)
 		var got string
-		if p[0] == "i" {
+		if bits32 {
+			p = strings.SplitN(sc.Text(), ",", 4)
+			u, err := strconv.ParseUint(p[0], 16, 32)
+			if err != nil {
+				panic(err)
+			}
+			prec, _ := strconv.Atoi(p[2])
+			got = strconv.FormatFloat(float64(math.Float32frombits(uint32(u))), p[1][0], prec, 32)
+			p = append([]string{"f32"}, p...)
+		} else if p[0] == "i" {
 			v, err := strconv.ParseInt(p[1], 10, 64)
 			if err != nil {
 				panic(err)
@@ -49,8 +67,6 @@ func main() {
 	if err := sc.Err(); err != nil {
 		panic(err)
 	}
-	fmt.Printf("%d lines, %d differ\n", n, bad)
-	if bad != 0 {
-		os.Exit(1)
-	}
+	fmt.Printf("%s: %d lines, %d differ\n", filepath.Base(path), n, bad)
+	return bad
 }

@@ -7,6 +7,12 @@
 // One line per row of the CSV's column `s`: `<Atoi value> <Atoi status> <ParseFloat bits, 16 hex digits> <ParseFloat
 // status>`, status 0 ok, 1 ErrSyntax, 2 ErrRange, values being what strconv returns alongside the error.  Go 1.23
 // (go.mod of the reference).  Never compiled here (no Go toolchain in this image).
+//
+// With -32 it regenerates tests/golden/numeric32_kat.expected from numeric32_kat.csv instead: one line per row,
+// `<ParseFloat(s, 32) bits, 8 hex digits> <status>`:
+//
+//	go run ./numeric -32 ../../tests/golden/numeric32_kat.csv > /tmp/numeric32_kat.expected
+//	cmp ../../tests/golden/numeric32_kat.expected /tmp/numeric32_kat.expected
 package main
 
 import (
@@ -33,7 +39,12 @@ func status(err error) int {
 }
 
 func main() {
-	f, err := os.Open(os.Args[1])
+	args := os.Args[1:]
+	bits32 := len(args) > 0 && args[0] == "-32"
+	if bits32 {
+		args = args[1:]
+	}
+	f, err := os.Open(args[0])
 	if err != nil {
 		log.Fatal(err)
 	}
@@ -46,6 +57,11 @@ func main() {
 		log.Fatal("expected a single column named s")
 	}
 	for _, rec := range records[1:] {
+		if bits32 {
+			x, ferr := strconv.ParseFloat(rec[0], 32)
+			fmt.Printf("%08x %d\n", math.Float32bits(float32(x)), status(ferr))
+			continue
+		}
 		i, ierr := strconv.Atoi(rec[0])
 		x, ferr := strconv.ParseFloat(rec[0], 64)
 		fmt.Printf("%d %d %016x %d\n", i, status(ierr), math.Float64bits(x), status(ferr))

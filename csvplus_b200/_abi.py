@@ -67,8 +67,8 @@ SYMBOLS = [
     "cpb_index_key_col", "cpb_index_gob_begin", "cpb_index_gob_into", "cpb_index_load_gob",
     "cpb_join", "cpb_except", "cpb_table_to_csv", "cpb_table_to_csv_device", "cpb_table_to_csv_into",
     "cpb_table_to_json", "cpb_table_to_json_device", "cpb_table_to_json_into",
-    "cpb_table_column_as_int64", "cpb_table_column_as_float64",
-    "cpb_table_set_int64", "cpb_table_set_float64", "cpb_table_set_literal", "cpb_table_filter_flags",
+    "cpb_table_column_as_int64", "cpb_table_column_as_float64", "cpb_table_column_as_float32",
+    "cpb_table_set_int64", "cpb_table_set_float64", "cpb_table_set_float32", "cpb_table_set_literal", "cpb_table_filter_flags",
     "cpb_comm_unique_id", "cpb_comm_init_rank", "cpb_init_multi", "cpb_comm_size", "cpb_comm_rank", "cpb_allgather_table",
     "cpb_allgather_tables", "cpb_allgather_u64", "cpb_allgather_layout",
     "cpb_stats_enable", "cpb_stats_reset", "cpb_stats_get", "cpb_kernel_launches", "cpb_host_syncs", "cpb_gen_csv",
@@ -154,8 +154,10 @@ def load():
         "cpb_table_to_json_into": (i32, [vp, vp, i32, i32, vp, u64, P(u64), P(Error)]),
         "cpb_table_column_as_int64": (i32, [vp, vp, Str, vp, vp, P(u64), P(Error)]),
         "cpb_table_column_as_float64": (i32, [vp, vp, Str, vp, vp, P(u64), P(Error)]),
+        "cpb_table_column_as_float32": (i32, [vp, vp, Str, vp, vp, P(u64), P(Error)]),
         "cpb_table_set_int64": (i32, [vp, vp, Str, vp, P(vp), P(Error)]),
         "cpb_table_set_float64": (i32, [vp, vp, Str, vp, C.c_char, i32, P(vp), P(Error)]),
+        "cpb_table_set_float32": (i32, [vp, vp, Str, vp, C.c_char, i32, P(vp), P(Error)]),
         "cpb_table_set_literal": (i32, [vp, vp, Str, Str, P(vp), P(Error)]),
         "cpb_table_filter_flags": (i32, [vp, vp, vp, P(vp), P(Error)]),
         "cpb_comm_unique_id": (i32, [vp]),

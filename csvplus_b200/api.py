@@ -612,24 +612,30 @@ class Table:
         ctx's device.  strict: the first failing row raises CsvPlusError with the reference's text (.row = its index), as
         a RowFunc returning the helper's error does; else -> (values, status uint8: 0 ok, 1 ErrSyntax, 2 ErrRange), the
         values being what Go returns alongside each error."""
-        return self._values_as(name, False, strict)
+        return self._values_as(name, "int", strict)
 
     def values_as_float64(self, name: str, strict: bool = True):
         """Row.ValueAsFloat64 (strconv.ParseFloat(s, 64), csvplus.go:187-205): as values_as_int, float64 values"""
-        return self._values_as(name, True, strict)
+        return self._values_as(name, "float64", strict)
 
-    def _values_as(self, name: str, is_float: bool, strict: bool):
-        values, status, err = self._convert(name, is_float)
+    def values_as_float32(self, name: str, strict: bool = True):
+        """strconv.ParseFloat(s, 32) of every row, as ValueAsFloat64's closure calling it would report: as values_as_int,
+        float32 values correctly rounded from the text (not through a float64); the error text is ValueAsFloat64's"""
+        return self._values_as(name, "float32", strict)
+
+    def _values_as(self, name: str, kind: str, strict: bool):
+        values, status, err = self._convert(name, kind)
         if err is not None and (strict or err.kind == _abi.CPB_E_MISSING_COLUMN):  # fails in both modes
             raise err
         return values if strict else (values, status)
 
-    def _convert(self, name: str, is_float: bool):
-        """-> (values, status, CsvPlusError of the first failing row or None); one host synchronisation"""
+    def _convert(self, name: str, kind: str):
+        """kind "int" | "float64" | "float32" -> (values, status, CsvPlusError of the first failing row or None); one host
+        synchronisation"""
         import torch
         dev = torch.device("cuda", self.ctx.device)
         n = len(self)
-        values = torch.empty(n, dtype=torch.float64 if is_float else torch.int64, device=dev)
+        values = torch.empty(n, dtype=getattr(torch, _KIND_DTYPES[kind]), device=dev)
         status = torch.empty(n, dtype=torch.uint8, device=dev)
         # the ctx stream writes into memory torch's current stream allocated: it waits for that stream first; the
         # synchronisation inside the call orders the way back
@@ -637,7 +643,7 @@ class Table:
         ev.record(torch.cuda.current_stream(dev))
         torch.cuda.ExternalStream(self.ctx.stream, device=dev).wait_event(ev)
         b = _enc(name); nbad = C.c_uint64(); e = _abi.Error()
-        st = self.ctx._call("cpb_table_column_as_float64" if is_float else "cpb_table_column_as_int64", self.h, _abi.Str(b, len(b)),
+        st = self.ctx._call("cpb_table_column_as_" + ("int64" if kind == "int" else kind), self.h, _abi.Str(b, len(b)),
                             C.c_void_p(values.data_ptr()), C.c_void_p(status.data_ptr()), C.byref(nbad), err=e, accept=(_abi.CPB_ERR_DATA,))
         if st:
             err = CsvPlusError(e.msg.decode("utf-8", "replace"), st, e.kind)
@@ -650,12 +656,18 @@ class Table:
         set, replaced in place when it exists, else appended; every other column shares this table's buffers.  value is a
         str (the same bytes in every row), an int64 CUDA tensor (strconv.FormatInt(v, 10)), a float64 CUDA tensor
         (strconv.FormatFloat(x, fmt, prec, 64); fmt defaults to 'g', prec -1 gives the shortest digits that read back as x)
-        or a FormatFloat marker.  A tensor holds one value per row; it may be freed as soon as the call returns."""
+        or a FormatFloat marker (the only way to pass a float32 tensor: FormatFloat(x32, bit_size=32)).  A tensor holds
+        one value per row; it may be freed as soon as the call returns."""
+        b = _enc(name); column = _abi.Str(b, len(b))
         if isinstance(value, FormatFloat):
             if fmt is not None:
                 raise TypeError("with_column: the format of a FormatFloat value is given in FormatFloat")
+            if value.bit_size == 32:
+                import torch
+                values = _device_tensor(self, value.values, (torch.float32,), "with_column")
+                return self.ctx._new_table("cpb_table_set_float32", self.h, column, C.c_void_p(values.data_ptr()), value.fmt.encode(),
+                                           value.prec)
             value, fmt, prec = value.values, value.fmt, value.prec
-        b = _enc(name); column = _abi.Str(b, len(b))
         if isinstance(value, (str, bytes)):
             if fmt is not None:
                 raise TypeError("with_column: fmt applies to float64 tensors only")
@@ -696,12 +708,22 @@ def _check_format(fmt, prec):
 
 
 class FormatFloat:
-    """strconv.FormatFloat(x, fmt, prec, 64) of every value of a float64 CUDA tensor: a value for Table.with_column and
-    MapTensors.  fmt is one of e E f g G; prec runs from -1 (the shortest digits that read back as x) to 64."""
+    """strconv.FormatFloat(x, fmt, prec, bit_size) of every value of a CUDA tensor: a value for Table.with_column and
+    MapTensors.  fmt is one of e E f g G; prec runs from -1 (the shortest digits that read back as x) to 64.  bit_size
+    64 takes a float64 tensor, 32 a float32 one (Go's FormatFloat(float64(x), fmt, prec, 32): the shortest digits read
+    back as x as a float32).  As in Go the bit size is explicit: a float64 tensor narrowed with .float() rounds as Go's
+    float32(v) does."""
 
-    def __init__(self, values, fmt: str = "g", prec: int = -1):
+    def __init__(self, values, fmt: str = "g", prec: int = -1, bit_size: int = 64):
         _check_format(fmt, prec)
-        self.values, self.fmt, self.prec = values, fmt, prec
+        if isinstance(bit_size, bool) or bit_size not in (32, 64):
+            raise ValueError(f"FormatFloat: bit size {bit_size!r} (want 32 or 64)")
+        import torch
+        want = torch.float32 if bit_size == 32 else torch.float64
+        if not isinstance(values, torch.Tensor) or values.dtype != want:
+            got = values.dtype if isinstance(values, torch.Tensor) else type(values).__name__
+            raise TypeError(f"FormatFloat: bit size {bit_size} wants a CUDA tensor of {want}, got {got}")
+        self.values, self.fmt, self.prec, self.bit_size = values, fmt, prec, bit_size
 
 
 def _device_tensor(t: Table, x, dtypes: tuple, what: str):
@@ -726,13 +748,15 @@ def _device_tensor(t: Table, x, dtypes: tuple, what: str):
     return x
 
 
+# the value types of ToTensors / MapTensors / FilterTensors inputs -> the name of their tensors' torch dtype
+_KIND_DTYPES = {"int": "int64", "float64": "float64", "float32": "float32"}
+
+
 def _tensor_kinds(inputs: dict, what: str) -> dict:
-    kinds = {}
     for name, kind in inputs.items():
-        if kind not in ("int", "float64"):
-            raise ValueError(f"{what}: unknown type {kind!r} for column {name!r} (want 'int' or 'float64')")
-        kinds[name] = kind == "float64"
-    return kinds
+        if kind not in _KIND_DTYPES:
+            raise ValueError(f"{what}: unknown type {kind!r} for column {name!r} (want 'int', 'float64' or 'float32')")
+    return dict(inputs)
 
 
 def parse_csv(ctx: Context, data, *, on_device=False, nbytes=None, delimiter=",", comment="", num_fields=0, lazy_quotes=False,
@@ -1229,9 +1253,10 @@ class DataSource:
     def DropWhile(self, pred): return self._with(("dropwhile", pred))
 
     def MapTensors(self, inputs: dict, fn):
-        """a device Map (an extension beyond the reference API, like ToTensors): inputs = {column: "int" | "float64"} are
-        converted per batch as ToTensors converts them, fn(dict of CUDA tensors) returns {name: value} and each name is set
-        as Table.with_column sets it (an int64 / float64 tensor with one value per row, a FormatFloat, a str).  fn is called
+        """a device Map (an extension beyond the reference API, like ToTensors): inputs = {column: "int" | "float64" |
+        "float32"} are converted per batch as ToTensors converts them, fn(dict of CUDA tensors) returns {name: value} and
+        each name is set as Table.with_column sets it (an int64 / float64 tensor with one value per row, a FormatFloat, a
+        str; a float32 result goes through FormatFloat(x, bit_size=32)).  fn is called
         once per non-empty batch and must be row-wise.  A conversion error (the lowest failing row, ties to the earlier
         input) ends the plan there like a source error: the rows before it flow on and the sink raises CsvPlusError with
         .row = the row's ordinal among the rows that reached the step."""
@@ -1475,8 +1500,9 @@ class DataSource:
             self.ToJSON(f)
 
     def ToTensors(self, columns: dict) -> dict:
-        """{name: "int" | "float64"} -> {name: CUDA tensor}: Row.ValueAsInt / ValueAsFloat64 of every row of each column,
-        converted on the GPU (an extension beyond the reference API, like TakeTable).  The plan is evaluated once.  The
+        """{name: "int" | "float64" | "float32"} -> {name: CUDA tensor}: Row.ValueAsInt / ValueAsFloat64 (or ParseFloat(s,
+        32), Table.values_as_float32) of every row of each column, converted on the GPU (an extension beyond the reference
+        API, like TakeTable).  The plan is evaluated once.  The
         error raised is the one a RowFunc converting the columns in dict order would meet first: the lowest failing row,
         ties to the earlier column (CsvPlusError, .row = the row).  When no row fails, a pending source error is raised:
         the table only holds the rows delivered before it."""
@@ -1485,7 +1511,7 @@ class DataSource:
         if t is None:
             import torch
             dev = torch.device("cuda", self._ctx().device)
-            out = {name: torch.empty(0, dtype=torch.float64 if f else torch.int64, device=dev) for name, f in kinds.items()}
+            out = {name: torch.empty(0, dtype=getattr(torch, _KIND_DTYPES[k]), device=dev) for name, k in kinds.items()}
         else:
             out, first = _convert_all(t, kinds)
             if first is not None:
@@ -1517,8 +1543,8 @@ def _convert_all(t: Table, kinds: dict) -> tuple:
     """Table._convert of every input -> ({name: values}, CsvPlusError of the lowest failing row, ties to the earlier
     input, or None)"""
     vals, first = {}, None
-    for name, is_float in kinds.items():
-        values, _, e = t._convert(name, is_float)
+    for name, kind in kinds.items():
+        values, _, e = t._convert(name, kind)
         vals[name] = values
         if e is not None and (first is None or e.row < first.row):
             first = e

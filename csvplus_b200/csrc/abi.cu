@@ -864,9 +864,11 @@ int cpb_table_to_json_device(cpb_ctx* h, const cpb_table* t, int first_batch, in
 }
 
 // ------------------------------------------------------------------ numeric columns
-// Row.ValueAsInt / ValueAsFloat64 (csvplus.go:163-205) of every row; the error is the first failing row's
-static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, bool is_float, void* values, uint8_t* status,
+// Row.ValueAsInt / ValueAsFloat64 (csvplus.go:163-205), and ParseFloat(s, 32) in the same closure, of every row; the
+// error is the first failing row's
+static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, NumKind kind, void* values, uint8_t* status,
                             uint64_t* nbad, cpb_error* err) {
+    const bool is_float = kind != NumKind::Int64;
     return guarded(h, err, [&](Ctx* c) {
         const Table& T = table_of(t);
         need(nbad && (values || T.nrows == 0), "null nbad or values");
@@ -875,7 +877,7 @@ static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, bool
         const int k = T.find(name);
         if (T.nrows == 0) return CPB_OK;
         if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // :170, :192
-        NumResult r = column_as_number(c, T, k, is_float, values, status);
+        NumResult r = column_as_number(c, T, k, kind, values, status);
         *nbad = r.nbad;
         if (r.nbad) {
             const bool range = r.first_status == CPB_NUM_RANGE;
@@ -888,20 +890,34 @@ static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, bool
 }
 int cpb_table_column_as_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, int64_t* values, uint8_t* status, uint64_t* nbad,
                               cpb_error* err) {
-    return column_as_common(h, t, column, false, values, status, nbad, err);
+    return column_as_common(h, t, column, NumKind::Int64, values, status, nbad, err);
 }
 int cpb_table_column_as_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, double* values, uint8_t* status, uint64_t* nbad,
                                 cpb_error* err) {
-    return column_as_common(h, t, column, true, values, status, nbad, err);
+    return column_as_common(h, t, column, NumKind::Float64, values, status, nbad, err);
+}
+int cpb_table_column_as_float32(cpb_ctx* h, const cpb_table* t, cpb_str column, float* values, uint8_t* status, uint64_t* nbad,
+                                cpb_error* err) {
+    return column_as_common(h, t, column, NumKind::Float32, values, status, nbad, err);
 }
 
 // ------------------------------------------------------------------ computed columns
 int cpb_table_set_int64(cpb_ctx* h, const cpb_table* t, cpb_str column, const int64_t* dev_values, cpb_table** out, cpb_error* err) {
-    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_values(c, T, to_string(column), dev_values, false, 'f', 0); });
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        return table_set_values(c, T, to_string(column), dev_values, NumKind::Int64, 'f', 0);
+    });
 }
 int cpb_table_set_float64(cpb_ctx* h, const cpb_table* t, cpb_str column, const double* dev_values, char fmt, int prec, cpb_table** out,
                           cpb_error* err) {
-    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_values(c, T, to_string(column), dev_values, true, fmt, prec); });
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        return table_set_values(c, T, to_string(column), dev_values, NumKind::Float64, fmt, prec);
+    });
+}
+int cpb_table_set_float32(cpb_ctx* h, const cpb_table* t, cpb_str column, const float* dev_values, char fmt, int prec, cpb_table** out,
+                          cpb_error* err) {
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        return table_set_values(c, T, to_string(column), dev_values, NumKind::Float32, fmt, prec);
+    });
 }
 int cpb_table_set_literal(cpb_ctx* h, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err) {
     return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_set_literal(c, T, to_string(column), to_string(value)); });

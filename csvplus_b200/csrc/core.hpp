@@ -397,17 +397,30 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
 // json.cu: ToJSON of every column (keys in bytewise order); '[' before the first row when first, ']' appended when last;
 // room as table_to_csv
 Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, uint64_t* nbytes);
-// numeric.cu: strconv.Atoi / ParseFloat(s, 64) of every row of column `col` into device values (+ nullable status)
+// numeric.cu / format.cu: the device value types of the numeric columns: int64 (Atoi / FormatInt(v, 10)), float64 and
+// float32 (ParseFloat / FormatFloat with bitSize 64 and 32)
+enum class NumKind { Int64, Float64, Float32 };
+// an IEEE binary format as strconv's floatInfo describes it; W holds the bits
+template <int MANT, int EXPB, typename W>
+struct FloatFormat {
+    typedef W word;
+    static constexpr int mantbits = MANT, expbits = EXPB, bias = (1 << (EXPB - 1)) - 1;
+    static constexpr uint64_t frac = (1ull << MANT) - 1, expmax = (1ull << EXPB) - 1;
+    static constexpr uint64_t inf = expmax << MANT, sign = 1ull << (MANT + EXPB);
+};
+typedef FloatFormat<52, 11, uint64_t> Float64Format;
+typedef FloatFormat<23, 8, uint32_t> Float32Format;
+// numeric.cu: strconv.Atoi / ParseFloat(s, 64 or 32) of every row of column `col` into device values (+ nullable status)
 struct NumResult {
     uint64_t nbad = 0, nrare = 0;  // failing rows, rows the exact (rare) path converted
     uint64_t first_row = 0;        // lowest failing row, its status and (up to 480 of) its bytes
     int first_status = 0;
     std::string first_value;
 };
-NumResult column_as_number(Ctx* c, const Table& t, int col, bool is_float, void* values, uint8_t* status);
+NumResult column_as_number(Ctx* c, const Table& t, int col, NumKind kind, void* values, uint8_t* status);
 // format.cu: computed columns.  t with column `name` set (replaced in place, else appended; the other columns share t's
-// buffers) to strconv.FormatInt(v, 10) / FormatFloat(x, fmt, prec, 64) of the n device values, or to one literal value
-std::shared_ptr<Table> table_set_values(Ctx* c, const Table& t, const std::string& name, const void* values, bool is_float, char fmt, int prec);
+// buffers) to strconv.FormatInt(v, 10) / FormatFloat(x, fmt, prec, 64 or 32) of the n device values, or to one literal value
+std::shared_ptr<Table> table_set_values(Ctx* c, const Table& t, const std::string& name, const void* values, NumKind kind, char fmt, int prec);
 std::shared_ptr<Table> table_set_literal(Ctx* c, const Table& t, const std::string& name, const std::string& value);
 // the rows of t whose keep byte is nonzero, in order
 std::shared_ptr<Table> table_filter_mask(Ctx* c, const Table& t, const uint8_t* keep);

@@ -256,21 +256,36 @@ public:
     // nullable (CPB_NUM_OK / _SYNTAX / _RANGE).  Returns the failing rows; strict: the first one throws Error with the
     // reference's text, as a RowFunc returning the helper's error.  An absent column throws in both modes.
     uint64_t ValuesAsInt(const std::string& column, int64_t* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
-        return convert(column, false, dev_values, dev_status, strict);
+        return convert(column, strict, [&](cpb_str c, uint64_t* nbad, cpb_error* e) {
+            return cpb_table_column_as_int64(detail::ctx(), h_.get(), c, dev_values, dev_status, nbad, e);
+        });
     }
     uint64_t ValuesAsFloat64(const std::string& column, double* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
-        return convert(column, true, dev_values, dev_status, strict);
+        return convert(column, strict, [&](cpb_str c, uint64_t* nbad, cpb_error* e) {
+            return cpb_table_column_as_float64(detail::ctx(), h_.get(), c, dev_values, dev_status, nbad, e);
+        });
+    }
+    // strconv.ParseFloat(s, 32) in the same closure: float values correctly rounded from the text, ValueAsFloat64's errors
+    uint64_t ValuesAsFloat32(const std::string& column, float* dev_values, uint8_t* dev_status = nullptr, bool strict = true) const {
+        return convert(column, strict, [&](cpb_str c, uint64_t* nbad, cpb_error* e) {
+            return cpb_table_column_as_float32(detail::ctx(), h_.get(), c, dev_values, dev_status, nbad, e);
+        });
     }
     // Map(func(row) Row { row[column] = value; return row }) on the GPU: a table with `column` set (replaced in place, else
     // appended; every other column shares this table's buffers).  dev_values[size()] is device memory read on the ctx
-    // stream: strconv.FormatInt(v, 10), strconv.FormatFloat(x, fmt, prec, 64) (fmt e E f g G, prec -1..64), or one
-    // literal value in every row.  A column of 4 GiB or more throws.
+    // stream: strconv.FormatInt(v, 10), strconv.FormatFloat(x, fmt, prec, 64) (fmt e E f g G, prec -1..64), for float
+    // values FormatFloat(float64(x), fmt, prec, 32), or one literal value in every row.  A column of 4 GiB or more throws.
     Table WithColumn(const std::string& column, const int64_t* dev_values) const {
         return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) { return cpb_table_set_int64(detail::ctx(), h_.get(), c, dev_values, out, e); });
     }
     Table WithColumn(const std::string& column, const double* dev_values, char fmt = 'g', int prec = -1) const {
         return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
             return cpb_table_set_float64(detail::ctx(), h_.get(), c, dev_values, fmt, prec, out, e);
+        });
+    }
+    Table WithColumn(const std::string& column, const float* dev_values, char fmt = 'g', int prec = -1) const {
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
+            return cpb_table_set_float32(detail::ctx(), h_.get(), c, dev_values, fmt, prec, out, e);
         });
     }
     Table WithColumn(const std::string& column, const std::string& value) const {
@@ -289,11 +304,10 @@ private:
         detail::check(call(cpb_str{column.data(), column.size()}, &out, &e), e);
         return Table(out);
     }
-    uint64_t convert(const std::string& column, bool is_float, void* values, uint8_t* status, bool strict) const {
+    template <class Call>
+    uint64_t convert(const std::string& column, bool strict, Call call) const {
         cpb_error e{}; uint64_t nbad = 0;
-        const cpb_str c{column.data(), column.size()};
-        const int st = is_float ? cpb_table_column_as_float64(detail::ctx(), h_.get(), c, (double*)values, status, &nbad, &e)
-                                : cpb_table_column_as_int64(detail::ctx(), h_.get(), c, (int64_t*)values, status, &nbad, &e);
+        const int st = call(cpb_str{column.data(), column.size()}, &nbad, &e);
         if (st == CPB_ERR_DATA && (strict || e.kind == CPB_E_MISSING_COLUMN)) throw Error(e.msg);
         if (st != CPB_OK && st != CPB_ERR_DATA) throw Error(e.msg[0] ? e.msg : cpb_last_error(detail::ctx()));
         return nbad;

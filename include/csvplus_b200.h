@@ -328,11 +328,15 @@ int cpb_table_to_json_into(cpb_ctx* ctx, const cpb_table* t, int first_batch, in
  * or +-Inf for a range error); status[nrows] is nullable (CPB_NUM_*); *nbad = failing rows.
  * nbad > 0: CPB_ERR_DATA, kind CPB_E_NUM_SYNTAX / CPB_E_NUM_RANGE of the first failing row, err->line = that row
  * (0-based), has_line = 0, msg = the reference's text.  An absent column on a non-empty table: CPB_ERR_DATA,
- * CPB_E_MISSING_COLUMN, line 0, has_line = 0.  A float column converts at most 2^32 - 1 rows per call. */
+ * CPB_E_MISSING_COLUMN, line 0, has_line = 0.  A float column converts at most 2^32 - 1 rows per call.
+ * column_as_float32: strconv.ParseFloat(s, 32) into float values, correctly rounded to float32 (never through a
+ * double); otherwise as column_as_float64, with the same error text ("... to float: ..."). */
 enum { CPB_NUM_OK = 0, CPB_NUM_SYNTAX = 1, CPB_NUM_RANGE = 2 };
 int cpb_table_column_as_int64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, int64_t* values, uint8_t* status,
                               uint64_t* nbad, cpb_error* err);
 int cpb_table_column_as_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, double* values, uint8_t* status,
+                                uint64_t* nbad, cpb_error* err);
+int cpb_table_column_as_float32(cpb_ctx* ctx, const cpb_table* t, cpb_str column, float* values, uint8_t* status,
                                 uint64_t* nbad, cpb_error* err);
 
 /* ------------------------------------------------------------------ computed columns
@@ -343,13 +347,18 @@ int cpb_table_column_as_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column
  *   set_int64  : strconv.FormatInt(v, 10).
  *   set_float64: strconv.FormatFloat(x, fmt, prec, 64), byte for byte; fmt one of e E f g G, prec -1..64 (-1: the
  *                shortest digits that read back as x).  Another fmt or prec: CPB_ERR_ARG, nothing computed.
+ *   set_float32: strconv.FormatFloat(float64(x), fmt, prec, 32) of float values: as set_float64, the shortest digits
+ *                being those that read back as x as a float32.
  *   set_literal: value in every row.
  * One column stays below 4 GiB: a column of 4 GiB or more fails with CPB_ERR_DATA / CPB_E_TOO_LARGE (checked on the
  * exact 64-bit total, before any offset is written).  Host synchronisations: none for an empty table; for set_float64
- * one, or two when some row needs the exact big-integer path (its kernel, format_rare, then shows in cpb_stats_get).
+ * one, or two when some row needs the exact big-integer path (its kernel, format_rare, then shows in cpb_stats_get);
+ * the same for set_float32, whose kernels show as format_float32 / format_rare32.
  * filter_flags: the rows whose dev_keep[row] byte is nonzero, in order (dev_keep[nrows] read on the ctx stream). */
 int cpb_table_set_int64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const int64_t* dev_values, cpb_table** out, cpb_error* err);
 int cpb_table_set_float64(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const double* dev_values, char fmt, int prec,
+                          cpb_table** out, cpb_error* err);
+int cpb_table_set_float32(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const float* dev_values, char fmt, int prec,
                           cpb_table** out, cpb_error* err);
 int cpb_table_set_literal(cpb_ctx* ctx, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err);
 int cpb_table_filter_flags(cpb_ctx* ctx, const cpb_table* t, const uint8_t* dev_keep, cpb_table** out, cpb_error* err);

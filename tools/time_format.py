@@ -1,9 +1,11 @@
 """FormatInt / FormatFloat timing: python tools/time_format.py [rows]
 
   shapes (values already in HBM): FormatInt of ids, FormatFloat(price*qty, 'f', 2) and FormatFloat(x, 'g', -1) of random
-  finite doubles;
-  per shape: kernel ms per call (format_int / format_float, format_rare when rows took the exact path, the offset scan,
-  format_write), algorithmic bytes (8 B of value per row + 4 B of offset per row + the output bytes) over the sum of
+  finite doubles, each float shape followed by its float32 leg (the same prices as float32 with bitSize 32; random
+  finite float32 bits);
+  per shape: kernel ms per call (format_int / format_float / format_float32, format_rare / format_rare32 when rows took
+  the exact path, the offset scan, format_write), algorithmic bytes (8 B of value per row (4 B for float32) + 4 B of
+  offset per row + the output bytes) over the sum of
   kernel times against the H100 SXM data-sheet 3.35 TB/s, each kernel's own bytes over its time, the call's wall time
   and host synchronisations per call;
   then a MapTensors step end to end against the host Transform closure it replaces, at 1 M rows, both through ToCsv."""
@@ -39,14 +41,18 @@ def base(n):
 
 
 def report(label, t, values, fmt=None, prec=-1, reps=5):
+    if isinstance(values, cp.FormatFloat):  # the format is in the marker
+        vbytes, kw = values.values.element_size(), {}
+    else:
+        vbytes, kw = values.element_size(), {"fmt": fmt, "prec": prec}
     for _ in range(2):
-        out = t.with_column("v", values, fmt=fmt, prec=prec)
+        out = t.with_column("v", values, **kw)
     ctx.stats(enable=True, reset=True)
     s0 = ctx.host_syncs()
     torch.cuda.synchronize(dev)
     w0 = time.perf_counter()
     for _ in range(reps):
-        out = t.with_column("v", values, fmt=fmt, prec=prec)
+        out = t.with_column("v", values, **kw)
     wall = (time.perf_counter() - w0) / reps
     syncs = (ctx.host_syncs() - s0) / reps
     st = ctx.stats(); ctx.stats(enable=False)
@@ -54,7 +60,7 @@ def report(label, t, values, fmt=None, prec=-1, reps=5):
     nb = C.c_uint64()
     ctx.lib.cpb_table_col_bytes(ctx.h, out.h, out.columns.index("v"), 0, n, C.byref(nb))
     out_total = nb.value
-    algo = 8 * n + 4 * (n + 1) + out_total
+    algo = vbytes * n + 4 * (n + 1) + out_total
     kms = sum(v["ms"] for k, v in st.items()) / reps
     print(f"{label}: {n} rows, {out_total / n:.1f} B per row, {kms:.3f} ms of kernels per call, wall {wall * 1e3:.3f} ms per call, "
           f"{syncs:.0f} host sync(s) per call; algo {algo / 1e9:.3f} GB -> {algo / (kms * 1e-3) / 1e9:.0f} GB/s = "
@@ -71,10 +77,14 @@ report("FormatInt(id)", t, torch.arange(rows, dtype=torch.int64, device=dev) * 7
 price = torch.randint(1, 100_000, (rows,), device=dev, generator=g).to(torch.float64) / 100
 qty = torch.randint(1, 50, (rows,), device=dev, generator=g).to(torch.float64)
 report("FormatFloat(price*qty, 'f', 2)", t, price * qty, "f", 2)
+report("FormatFloat(price*qty, 'f', 2, 32)", t, cp.FormatFloat((price * qty).float(), "f", 2, bit_size=32))
 x = torch.randint(-2**63, 2**63 - 1, (rows,), dtype=torch.int64, device=dev, generator=g).view(torch.float64)
 x = torch.where(torch.isfinite(x), x, torch.zeros_like(x))
 report("FormatFloat(x, 'g', -1), random bits", t, x, "g", -1)
-del t, price, qty, x
+x32 = torch.randint(-2**31, 2**31 - 1, (rows,), dtype=torch.int32, device=dev, generator=g).view(torch.float32)
+x32 = torch.where(torch.isfinite(x32), x32, torch.zeros_like(x32))
+report("FormatFloat(x, 'g', -1, 32), random bits", t, cp.FormatFloat(x32, "g", -1, bit_size=32))
+del t, price, qty, x, x32
 
 # a MapTensors step against the host Transform closure, end to end through ToCsv, at 1 M rows
 n1 = 1_000_000

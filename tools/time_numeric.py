@@ -1,10 +1,10 @@
-"""ValueAsInt / ValueAsFloat64 timing: python tools/time_numeric.py [rows]
+"""ValueAsInt / ValueAsFloat64 / ParseFloat(s, 32) timing: python tools/time_numeric.py [rows]
 
-  columns: qty, cust_id, order_id of generated orders (int), price of products and score of people (float64), and a
-  hard-float column of 17-25-digit values (float64);
-  per column: kernel ms per call (numeric_int / numeric_float + numeric_rare), algorithmic bytes (offsets + value bytes +
-  8 B of output + 1 B of status per row) over kernel time against the H100 SXM data-sheet 3.35 TB/s, rows that took the
-  exact path, and host synchronisations per call;
+  columns: qty, cust_id, order_id of generated orders (int), price of products and score of people (float64, then the
+  same column as float32 beside it), and a hard-float column of 17-25-digit values (float64, then float32);
+  per column: kernel ms per call (numeric_int / numeric_float + numeric_rare, numeric_float32 + numeric_rare32),
+  algorithmic bytes (offsets + value bytes + 8 B of output (4 B for float32) + 1 B of status per row) over kernel time
+  against the H100 SXM data-sheet 3.35 TB/s, rows that took the exact path, and host synchronisations per call;
   then the host path the conversion replaces (Table.rows() + int() / float()) at 1 M rows."""
 import os
 import random
@@ -25,8 +25,8 @@ except OSError:
     print("nvidia-smi not available", flush=True)
 
 
-def timed(t, name, is_float, reps=5):
-    conv = t.values_as_float64 if is_float else t.values_as_int
+def timed(t, name, kind, reps=5):
+    conv = {"int": t.values_as_int, "float64": t.values_as_float64, "float32": t.values_as_float32}[kind]
     for _ in range(2):
         conv(name, strict=False)
     ctx.stats(enable=True, reset=True)
@@ -38,8 +38,8 @@ def timed(t, name, is_float, reps=5):
     return {k: (v["ms"] / reps, v["algo_bytes"] / reps) for k, v in st.items()}, syncs
 
 
-def report(label, t, name, is_float):
-    st, syncs = timed(t, name, is_float)
+def report(label, t, name, kind):
+    st, syncs = timed(t, name, kind)
     total = sum(ms for ms, _ in st.values())
     print(f"{label}: {len(t)} rows, {total:.3f} ms of kernels per call, {syncs:.0f} host sync(s) per call", flush=True)
     for k, (ms, b) in sorted(st.items()):
@@ -50,19 +50,25 @@ def report(label, t, name, is_float):
 orders = ctx.gen_csv("orders", (0, rows), n_cust=rows // 10, n_prod=1000)
 to, _ = cp.parse_csv(ctx, orders, spec=[("order_id", -1), ("cust_id", -1), ("qty", -1)])
 for c in ("qty", "cust_id", "order_id"):
-    report(f"orders.{c} (int)", to, c, False)
+    report(f"orders.{c} (int)", to, c, "int")
 products = ctx.gen_csv("products", (0, rows), n_prod=rows)
 tp, _ = cp.parse_csv(ctx, products, spec=[("price", -1)])
-report("products.price (float64)", tp, "price", True)
+report("products.price (float64)", tp, "price", "float64")
+report("products.price (float32)", tp, "price", "float32")
 people = ctx.gen_csv("people", (0, rows))
 tq, _ = cp.parse_csv(ctx, people, spec=[("score", -1)])
-report("people.score (float64)", tq, "score", True)
+report("people.score (float64)", tq, "score", "float64")
+report("people.score (float32)", tq, "score", "float32")
 # hard floats: 17-25 significant digits with exponents across the range
 rng = random.Random(5)
 nh = min(rows, 2_000_000)
 hard = [f"{rng.randint(1, 9)}.{rng.randrange(10 ** 24):024d}"[: rng.randint(18, 26)] + f"e{rng.randint(-300, 300)}" for _ in range(nh)]
 th = cp.Table.from_rows(ctx, [{"h": v} for v in hard], columns=["h"])
-report(f"hard floats, 17-25 digits (float64, {nh} rows)", th, "h", True)
+report(f"hard floats, 17-25 digits (float64, {nh} rows)", th, "h", "float64")
+hard32 = [v[: v.index("e")] + f"e{rng.randint(-40, 35)}" for v in hard]  # the same digits inside float32's range
+th32 = cp.Table.from_rows(ctx, [{"h": v} for v in hard32], columns=["h"])
+report(f"hard floats, 17-25 digits, exponents -40..35 (float64, {nh} rows)", th32, "h", "float64")
+report(f"hard floats, 17-25 digits, exponents -40..35 (float32, {nh} rows)", th32, "h", "float32")
 
 n1 = min(rows, 1_000_000)
 small = to.slice(0, n1)
