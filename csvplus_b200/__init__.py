@@ -5,11 +5,11 @@ of include/csvplus_b200.h).  This package is the thin host mirror of the referen
 (csvplus.go) over that ABI; it never computes results on the CPU and fails loudly when the CUDA
 library or a GPU is missing.
 """
-from .api import (All, Any, Context, CsvPlusError, DataSource, DataSourceError, DeviceBuffer, FormatFloat, FromBytes,  # noqa: F401
+from .api import (All, Any, Categories, Context, CsvPlusError, DataSource, DataSourceError, DeviceBuffer, FormatFloat, FromBytes,  # noqa: F401
                   FromFile, FromReadCloser, FromReader, HostBuffer, Index, Like, LoadIndex, Not, Predicate, Reader, Row, StopIterationEOF,
                   Table, Take, TakeRows, TakeTable, csv_quote_parity, csv_stream_cut, parse_csv, parse_csv_shard)
 
-__all__ = ["All", "Any", "Context", "CsvPlusError", "DataSource", "DataSourceError", "DeviceBuffer", "FormatFloat", "FromBytes", "FromFile",
+__all__ = ["All", "Any", "Categories", "Context", "CsvPlusError", "DataSource", "DataSourceError", "DeviceBuffer", "FormatFloat", "FromBytes", "FromFile",
            "FromReadCloser", "FromReader", "HostBuffer", "Index", "Like", "LoadIndex", "Not", "Predicate", "Reader", "Row",
            "StopIterationEOF", "Table", "Take", "TakeRows", "TakeTable", "csv_quote_parity", "csv_stream_cut", "parse_csv",
            "parse_csv_shard"]

@@ -637,11 +637,7 @@ class Table:
         n = len(self)
         values = torch.empty(n, dtype=getattr(torch, _KIND_DTYPES[kind]), device=dev)
         status = torch.empty(n, dtype=torch.uint8, device=dev)
-        # the ctx stream writes into memory torch's current stream allocated: it waits for that stream first; the
-        # synchronisation inside the call orders the way back
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(dev))
-        torch.cuda.ExternalStream(self.ctx.stream, device=dev).wait_event(ev)
+        _ctx_waits_for_torch(self.ctx, dev)
         b = _enc(name); nbad = C.c_uint64(); e = _abi.Error()
         st = self.ctx._call("cpb_table_column_as_" + ("int64" if kind == "int" else kind), self.h, _abi.Str(b, len(b)),
                             C.c_void_p(values.data_ptr()), C.c_void_p(status.data_ptr()), C.byref(nbad), err=e, accept=(_abi.CPB_ERR_DATA,))
@@ -651,14 +647,46 @@ class Table:
             return values, status, err
         return values, status, None
 
+    def values_as_codes(self, name: str) -> "Categories":
+        """categorical codes of a column, computed on the GPU (pandas.factorize(sort=False)): .codes, an int64 CUDA tensor
+        on the ctx's device, holds each row's rank among the column's distinct values in order of first appearance, and
+        .dictionary is a new Table of one column `name` whose row k holds the value of code k.  Values are equal when
+        their bytes are; there is no length limit.  The codes belong to this table.  A missing column raises
+        CsvPlusError as values_as_int does.  One call, two host synchronisations."""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        codes = torch.empty(len(self), dtype=torch.int64, device=dev)
+        _ctx_waits_for_torch(self.ctx, dev)
+        b = _enc(name); h = C.c_void_p()
+        self._checked_row("cpb_table_column_codes", _abi.Str(b, len(b)), C.c_void_p(codes.data_ptr()), C.byref(h))
+        return Categories(codes, Table(self.ctx, h))
+
+    def _checked_row(self, name: str, *args) -> None:
+        """an entry whose data error names a row in err.line: raised as CsvPlusError with .row = that row"""
+        e = _abi.Error()
+        st = self.ctx._call(name, self.h, *args, err=e, accept=(_abi.CPB_ERR_DATA,))
+        if st:
+            err = CsvPlusError(e.msg.decode("utf-8", "replace"), st, e.kind)
+            err.row = e.line
+            raise err
+
     def with_column(self, name: str, value, fmt: str | None = None, prec: int = -1) -> "Table":
         """the reference's Map(func(row) Row { row[name] = value; return row }) on the GPU: a new table with column `name`
         set, replaced in place when it exists, else appended; every other column shares this table's buffers.  value is a
         str (the same bytes in every row), an int64 CUDA tensor (strconv.FormatInt(v, 10)), a float64 CUDA tensor
         (strconv.FormatFloat(x, fmt, prec, 64); fmt defaults to 'g', prec -1 gives the shortest digits that read back as x)
-        or a FormatFloat marker (the only way to pass a float32 tensor: FormatFloat(x32, bit_size=32)).  A tensor holds
-        one value per row; it may be freed as soon as the call returns."""
+        or a FormatFloat marker (the only way to pass a float32 tensor: FormatFloat(x32, bit_size=32)), or Categories:
+        the dictionary's value at each row's code (a code outside the dictionary raises CsvPlusError with .row = the
+        lowest such row).  A tensor holds one value per row; it may be freed as soon as the call returns."""
         b = _enc(name); column = _abi.Str(b, len(b))
+        if isinstance(value, Categories):
+            if fmt is not None:
+                raise TypeError("with_column: fmt applies to float64 tensors only")
+            import torch
+            codes = _device_tensor(self, value.codes, (torch.int64,), "with_column")
+            h = C.c_void_p()
+            self._checked_row("cpb_table_set_codes", column, C.c_void_p(codes.data_ptr()), value.dictionary.h, C.byref(h))
+            return Table(self.ctx, h)
         if isinstance(value, FormatFloat):
             if fmt is not None:
                 raise TypeError("with_column: the format of a FormatFloat value is given in FormatFloat")
@@ -726,6 +754,27 @@ class FormatFloat:
         self.values, self.fmt, self.prec, self.bit_size = values, fmt, prec, bit_size
 
 
+class Categories:
+    """categorical codes of a string column (Table.values_as_codes, the "category" kind of ToTensors): codes, an int64
+    CUDA tensor with one code per row, and dictionary, a Table of one column whose row k holds the value of code k.
+    Table.with_column(name, Categories(codes, dictionary)) (or a MapTensors result) sets each row to the dictionary's
+    value at its code, so a torch-computed remap (dictionary permuted, codes mapped) comes back as a string column."""
+
+    def __init__(self, codes, dictionary: Table):
+        if not isinstance(dictionary, Table):
+            raise TypeError(f"Categories: the dictionary is a Table, got {type(dictionary).__name__}")
+        self.codes, self.dictionary = codes, dictionary
+
+
+def _ctx_waits_for_torch(ctx: "Context", dev) -> None:
+    """the ctx stream writes into memory torch's current stream allocated: it waits for that stream first; the
+    synchronisation inside the call orders the way back"""
+    import torch
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(dev))
+    torch.cuda.ExternalStream(ctx.stream, device=dev).wait_event(ev)
+
+
 def _device_tensor(t: Table, x, dtypes: tuple, what: str):
     """x as a contiguous 1-D CUDA tensor of one of dtypes with one value per row of t, on t's device, ready to be read on
     the ctx stream: the ctx stream waits for torch's current stream (where x was produced), and x's memory is not reused
@@ -752,10 +801,16 @@ def _device_tensor(t: Table, x, dtypes: tuple, what: str):
 _KIND_DTYPES = {"int": "int64", "float64": "float64", "float32": "float32"}
 
 
-def _tensor_kinds(inputs: dict, what: str) -> dict:
+def _tensor_kinds(inputs: dict, what: str, category: bool = False) -> dict:
+    """the inputs checked; category: "category" is accepted (ToTensors only: MapTensors / FilterTensors convert each
+    batch on its own, and codes numbered per batch would not match from one batch to the next)"""
     for name, kind in inputs.items():
-        if kind not in _KIND_DTYPES:
-            raise ValueError(f"{what}: unknown type {kind!r} for column {name!r} (want 'int', 'float64' or 'float32')")
+        if kind == "category" and not category:
+            raise ValueError(f"{what}: 'category' is not an input type (column {name!r}): inputs are converted batch by batch and "
+                             "codes would differ between batches; take codes with ToTensors or Table.values_as_codes")
+        if kind not in _KIND_DTYPES and kind != "category":
+            raise ValueError(f"{what}: unknown type {kind!r} for column {name!r} (want 'int', 'float64', 'float32'"
+                             + (" or 'category')" if category else ")"))
     return dict(inputs)
 
 
@@ -1256,7 +1311,9 @@ class DataSource:
         """a device Map (an extension beyond the reference API, like ToTensors): inputs = {column: "int" | "float64" |
         "float32"} are converted per batch as ToTensors converts them, fn(dict of CUDA tensors) returns {name: value} and
         each name is set as Table.with_column sets it (an int64 / float64 tensor with one value per row, a FormatFloat, a
-        str; a float32 result goes through FormatFloat(x, bit_size=32)).  fn is called
+        str, Categories; a float32 result goes through FormatFloat(x, bit_size=32)).  "category" is not an input type:
+        inputs are converted batch by batch, and codes numbered per batch would differ between batches (ValueError);
+        take codes once with ToTensors.  fn is called
         once per non-empty batch and must be row-wise.  A conversion error (the lowest failing row, ties to the earlier
         input) ends the plan there like a source error: the rows before it flow on and the sink raises CsvPlusError with
         .row = the row's ordinal among the rows that reached the step."""
@@ -1264,7 +1321,7 @@ class DataSource:
 
     def FilterTensors(self, inputs: dict, fn):
         """a device Filter: as MapTensors, fn returns a bool CUDA tensor with one value per row; the rows where it is true
-        are kept"""
+        are kept.  As for MapTensors, "category" is not an input type (codes would differ between batches)."""
         return self._with(("filtertensors", _tensor_kinds(inputs, "FilterTensors"), fn))
 
     def DropColumns(self, *columns):
@@ -1500,18 +1557,21 @@ class DataSource:
             self.ToJSON(f)
 
     def ToTensors(self, columns: dict) -> dict:
-        """{name: "int" | "float64" | "float32"} -> {name: CUDA tensor}: Row.ValueAsInt / ValueAsFloat64 (or ParseFloat(s,
-        32), Table.values_as_float32) of every row of each column, converted on the GPU (an extension beyond the reference
-        API, like TakeTable).  The plan is evaluated once.  The
+        """{name: "int" | "float64" | "float32" | "category"} -> {name: CUDA tensor or Categories}: Row.ValueAsInt /
+        ValueAsFloat64 (or ParseFloat(s, 32), Table.values_as_float32) of every row of each column, converted on the GPU
+        (an extension beyond the reference API, like TakeTable); "category" gives Table.values_as_codes of the column.
+        The plan is evaluated once, so the codes cover every row of the result.  The
         error raised is the one a RowFunc converting the columns in dict order would meet first: the lowest failing row,
         ties to the earlier column (CsvPlusError, .row = the row).  When no row fails, a pending source error is raised:
         the table only holds the rows delivered before it."""
-        kinds = _tensor_kinds(columns, "ToTensors")
+        kinds = _tensor_kinds(columns, "ToTensors", category=True)
         t, err = self._table()
         if t is None:
             import torch
-            dev = torch.device("cuda", self._ctx().device)
-            out = {name: torch.empty(0, dtype=getattr(torch, _KIND_DTYPES[k]), device=dev) for name, k in kinds.items()}
+            ctx = self._ctx()
+            dev = torch.device("cuda", ctx.device)
+            out = {name: Categories(torch.empty(0, dtype=torch.int64, device=dev), Table.from_rows(ctx, [], [name])) if k == "category"
+                   else torch.empty(0, dtype=getattr(torch, _KIND_DTYPES[k]), device=dev) for name, k in kinds.items()}
         else:
             out, first = _convert_all(t, kinds)
             if first is not None:
@@ -1544,7 +1604,13 @@ def _convert_all(t: Table, kinds: dict) -> tuple:
     input, or None)"""
     vals, first = {}, None
     for name, kind in kinds.items():
-        values, _, e = t._convert(name, kind)
+        if kind == "category":  # (its only error is a missing column, at row 0)
+            try:
+                values, e = t.values_as_codes(name), None
+            except CsvPlusError as x:
+                values, e = None, x
+        else:
+            values, _, e = t._convert(name, kind)
         vals[name] = values
         if e is not None and (first is None or e.row < first.row):
             first = e

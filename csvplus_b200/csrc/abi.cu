@@ -926,6 +926,32 @@ int cpb_table_filter_flags(cpb_ctx* h, const cpb_table* t, const uint8_t* dev_ke
     return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) { return table_filter_mask(c, T, dev_keep); });
 }
 
+// ------------------------------------------------------------------ categorical codes
+int cpb_table_column_codes(cpb_ctx* h, const cpb_table* t, cpb_str column, int64_t* dev_codes, cpb_table** dictionary, cpb_error* err) {
+    return guarded(h, err, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(dictionary && (dev_codes || T.nrows == 0), "null dictionary or codes");
+        const std::string name = to_string(column);
+        const int k = T.find(name);
+        if (T.nrows == 0) {
+            auto d = std::make_shared<Table>(); d->ctx = c;
+            Column col = empty_column(c); col.name = name;
+            d->cols.push_back(col);
+            *dictionary = wrap(d);
+            return CPB_OK;
+        }
+        if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // as column_as_int64
+        *dictionary = wrap(column_codes(c, T, k, dev_codes));
+        return CPB_OK;
+    });
+}
+int cpb_table_set_codes(cpb_ctx* h, const cpb_table* t, cpb_str column, const int64_t* dev_codes, const cpb_table* dictionary,
+                        cpb_table** out, cpb_error* err) {
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        return table_set_codes(c, T, to_string(column), dev_codes, table_of(dictionary));
+    });
+}
+
 // ------------------------------------------------------------------ stats
 int cpb_stats_enable(cpb_ctx* h, int on) {
     return guarded(h, nullptr, [&](Ctx* c) { c->stats_on = on != 0; return CPB_OK; });

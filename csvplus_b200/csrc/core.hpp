@@ -422,8 +422,18 @@ NumResult column_as_number(Ctx* c, const Table& t, int col, NumKind kind, void* 
 // buffers) to strconv.FormatInt(v, 10) / FormatFloat(x, fmt, prec, 64 or 32) of the n device values, or to one literal value
 std::shared_ptr<Table> table_set_values(Ctx* c, const Table& t, const std::string& name, const void* values, NumKind kind, char fmt, int prec);
 std::shared_ptr<Table> table_set_literal(Ctx* c, const Table& t, const std::string& name, const std::string& value);
+// t with column `name` set to col (its row0 reset), replaced in place, else appended; a column of no rows
+std::shared_ptr<Table> with_column(const Table& t, const std::string& name, Column col);
+Column empty_column(Ctx* c);
 // the rows of t whose keep byte is nonzero, in order
 std::shared_ptr<Table> table_filter_mask(Ctx* c, const Table& t, const uint8_t* keep);
+// codes.cu: categorical codes.  column_codes: codes[r] = the rank of row r's value of column col among the column's
+// distinct values in order of first appearance (int64, device memory, written on the ctx stream before the call's last
+// host synchronisation); returns the dictionary, one column named as col whose row k holds the value of code k.
+// table_set_codes: t with column `name` set to dict's only column at codes[r] (under with_column's rules); a code
+// outside [0, rows of dict) throws DataError CPB_E_BAD_CODE with line = the lowest such row.
+std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* codes);
+std::shared_ptr<Table> table_set_codes(Ctx* c, const Table& t, const std::string& name, const int64_t* codes, const Table& dict);
 
 }  // namespace cpb
 

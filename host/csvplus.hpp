@@ -271,6 +271,15 @@ public:
             return cpb_table_column_as_float32(detail::ctx(), h_.get(), c, dev_values, dev_status, nbad, e);
         });
     }
+    // categorical codes of a column (pandas.factorize(sort=False)), computed on the GPU: dev_codes[size()] (caller-owned
+    // device memory) gets each row's rank among the column's distinct values in order of first appearance, complete
+    // when the call returns; the returned table is the dictionary, one column named `column` whose row k holds the value
+    // of code k.  Codes belong to this table.  An absent column throws the error ValuesAsInt throws.
+    Table ValuesAsCodes(const std::string& column, int64_t* dev_codes) const {
+        cpb_table* out = nullptr; cpb_error e{};
+        detail::check(cpb_table_column_codes(detail::ctx(), h_.get(), cpb_str{column.data(), column.size()}, dev_codes, &out, &e), e);
+        return Table(out);
+    }
     // Map(func(row) Row { row[column] = value; return row }) on the GPU: a table with `column` set (replaced in place, else
     // appended; every other column shares this table's buffers).  dev_values[size()] is device memory read on the ctx
     // stream: strconv.FormatInt(v, 10), strconv.FormatFloat(x, fmt, prec, 64) (fmt e E f g G, prec -1..64), for float
@@ -286,6 +295,13 @@ public:
     Table WithColumn(const std::string& column, const float* dev_values, char fmt = 'g', int prec = -1) const {
         return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
             return cpb_table_set_float32(detail::ctx(), h_.get(), c, dev_values, fmt, prec, out, e);
+        });
+    }
+    // the value of dictionary's only column at dev_codes[row] (int64, device memory read on the ctx stream) in every row: a
+    // code outside the dictionary throws, naming the lowest such row.  WithColumn(c, ValuesAsCodes(c, codes), codes) is c.
+    Table WithColumn(const std::string& column, const int64_t* dev_codes, const Table& dictionary) const {
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
+            return cpb_table_set_codes(detail::ctx(), h_.get(), c, dev_codes, dictionary.get(), out, e);
         });
     }
     Table WithColumn(const std::string& column, const std::string& value) const {

@@ -90,7 +90,8 @@ typedef enum cpb_err_kind {
     CPB_E_UNSUPPORTED = 15,
     CPB_E_NUM_SYNTAX = 16,      /* csvplus.go:176/:198  cannot convert %q to integer|float: invalid syntax */
     CPB_E_NUM_RANGE = 17,       /* csvplus.go:176/:198  ...: value out of range */
-    CPB_E_GOB = 18              /* LoadIndex (csvplus.go:683-705): the file is not an index gob stream ("EOF", "unexpected EOF", ...) */
+    CPB_E_GOB = 18,             /* LoadIndex (csvplus.go:683-705): the file is not an index gob stream ("EOF", "unexpected EOF", ...) */
+    CPB_E_BAD_CODE = 19         /* cpb_table_set_codes: a categorical code outside the dictionary's rows */
 } cpb_err_kind;
 
 typedef struct cpb_error {
@@ -362,6 +363,24 @@ int cpb_table_set_float32(cpb_ctx* ctx, const cpb_table* t, cpb_str column, cons
                           cpb_table** out, cpb_error* err);
 int cpb_table_set_literal(cpb_ctx* ctx, const cpb_table* t, cpb_str column, cpb_str value, cpb_table** out, cpb_error* err);
 int cpb_table_filter_flags(cpb_ctx* ctx, const cpb_table* t, const uint8_t* dev_keep, cpb_table** out, cpb_error* err);
+
+/* ------------------------------------------------------------------ categorical codes (pandas.factorize(sort=False))
+ * column_codes: dev_codes[r] (int64, device memory written on the ctx stream) = the rank of row r's value of `column`
+ * among the column's distinct values in order of first appearance; values are equal when their bytes are (no length
+ * limit, no Unicode normalisation, the empty value is a value).  *dictionary = a new table of one column named
+ * `column`: row k holds the value of code k (max code + 1 rows).  The result depends only on the column's bytes and
+ * row order.  Codes belong to this table: another batch numbers its values afresh.  An empty table gives a dictionary
+ * of no rows and writes nothing.  An absent column on a non-empty table: CPB_ERR_DATA, CPB_E_MISSING_COLUMN, line 0,
+ * has_line = 0 (as column_as_int64).  A table of 2^31 rows or more: CPB_ERR_DATA / CPB_E_TOO_LARGE.  Host
+ * synchronisations: two; the codes are complete when the call returns.
+ * set_codes: *out = t with `column` set to dictionary's only column at dev_codes[r] (int64[nrows], device memory read
+ * on the ctx stream), replaced in place or appended as set_int64 sets it.  A dictionary without exactly one column:
+ * CPB_ERR_ARG.  A code outside [0, rows of dictionary): CPB_ERR_DATA, CPB_E_BAD_CODE, err->line = the lowest such
+ * row (0-based), has_line = 0, and no table.  set_codes(t, c, column_codes(t, c)) reproduces column c byte for byte. */
+int cpb_table_column_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, int64_t* dev_codes, cpb_table** dictionary,
+                           cpb_error* err);
+int cpb_table_set_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const int64_t* dev_codes, const cpb_table* dictionary,
+                        cpb_table** out, cpb_error* err);
 
 /* ------------------------------------------------------------------ multi-GPU (SURVEY §8e)
  * The probe stream shards by row range with no data-path collective; the one exchange step is the all-gather of the
