@@ -112,7 +112,7 @@ def _strs(items: Iterable) -> tuple:
 
 def _raise(st: int, err: _abi.Error, ctx=None):
     msg = err.msg.decode("utf-8", "replace") if err is not None else ""
-    if st == _abi.CPB_ERR_DATA:
+    if st == _abi.CPB_ERR_DATA and err is not None:  # (an entry without a cpb_error* reports through cpb_last_error)
         if err.has_line:
             raise _data_error(err)
         raise CsvPlusError(msg, st, err.kind)

@@ -318,7 +318,9 @@ Parsed stream_next(Stream* s, bool* done);  // table null: no complete record ye
 void stream_free(Stream* s);
 Ctx* stream_ctx(Stream* s);
 // gather.cu
-void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, uint64_t* total_dev);  // out[n] = total
+// out[i] = in[0] + ... + in[i-1] modulo 2^32 (out may alias in; out[n] = the total modulo 2^32); *total_dev = the exact
+// 64-bit total for any input (below 2^62), so a caller that checks it against 0xFFFFFFFF before it uses out[] is sound
+void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, uint64_t* total_dev);
 // compaction of 0/1 flags into the ascending list of the set positions, in two calls so that the caller allocates the
 // output in between: scan_flags scans the flags and reads the count back (one host synchronisation); compact_flags
 // writes out[j] = (j-th set position) + add and the sentinel out[count] = n + add, so out holds count + 1 entries

@@ -20,15 +20,17 @@ constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
 
 // The look-back chain of one tile, run by a whole warp.  Tile t's state word is st[t * stride] (stride NC: the words of
 // NC columns interleaved): bits 63:62 status (0 none, 1 aggregate, 2 inclusive prefix), bits 61:0 the value.  Publishes
-// the tile's total tot, walks the predecessors 32 at a time until one holds its inclusive prefix, publishes this tile's
-// and returns its exclusive prefix (every lane).
-__device__ __forceinline__ unsigned long long lookback(unsigned long long* st, uint32_t stride, uint64_t tile, uint32_t tot) {
+// the tile's total tot(), walks the predecessors 32 at a time until one holds its inclusive prefix, publishes this tile's
+// and returns its exclusive prefix (every lane).  (tot is called where the total is needed: a caller may read it again
+// from shared memory rather than hold it in registers through the walk.)
+template <class Tot>
+__device__ __forceinline__ unsigned long long lookback(unsigned long long* st, uint32_t stride, uint64_t tile, Tot tot) {
     const int lane = threadIdx.x & 31;
     if (tile == 0) {
-        if (lane == 0) atomicExch(&st[0], (2ull << 62) | tot);
+        if (lane == 0) atomicExch(&st[0], (2ull << 62) | tot());
         return 0;
     }
-    if (lane == 0) atomicExch(&st[tile * stride], (1ull << 62) | tot);
+    if (lane == 0) atomicExch(&st[tile * stride], (1ull << 62) | tot());
     unsigned long long excl = 0;
     for (int64_t b = (int64_t)tile - 1;; b -= 32) {
         const int64_t p = b - lane;
@@ -38,18 +40,21 @@ __device__ __forceinline__ unsigned long long lookback(unsigned long long* st, u
         excl += warp_sum_u64((f < 0 || lane <= f) ? (s & ((1ull << 62) - 1)) : 0ull);
         if (f >= 0) break;
     }
-    if (lane == 0) atomicExch(&st[tile * stride], (2ull << 62) | (excl + tot));
+    if (lane == 0) atomicExch(&st[tile * stride], (2ull << 62) | (excl + tot()));
     return excl;
 }
 
 // GATHER: the scanned values are the lengths of the strings picked by `ids` (identity when null) from the offsets
 // array `in` -- the length array of a gather is never materialised.
+// The offsets out[] are sums modulo 2^32 (a caller uses them only when the total fits); *total is exact.  The thread,
+// warp and tile sums are kept in 32 bits plus a count of their wraps past 2^32: a sum of non-negative addends has
+// wrapped exactly when it is smaller than the addend just added.  A few long rows wrap one tile's sum.
 template <bool GATHER>
 __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* __restrict__ in, const uint32_t* __restrict__ ids,
                                                                 uint32_t* out, uint64_t n, unsigned long long* state,
                                                                 uint32_t* ticket, unsigned long long* total) {
     __shared__ uint32_t s_tile;
-    __shared__ uint32_t s_warp[SCAN_THREADS / 32];
+    __shared__ unsigned long long s_warp[SCAN_THREADS / 32];  // the warps' exact sums
     __shared__ unsigned long long s_prefix;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint64_t ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
@@ -60,7 +65,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* 
         if (tile >= ntiles) break;
         const uint64_t base = tile * SCAN_TILE + (uint64_t)tid * SCAN_ITEMS;
         uint32_t v[SCAN_ITEMS];
-        uint32_t sum = 0;
+        uint32_t sum = 0, wraps = 0;
 #pragma unroll
         for (int i = 0; i < SCAN_ITEMS; i++) {
             v[i] = 0;
@@ -69,19 +74,28 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* 
                 else v[i] = in[base + i];
             }
             sum += v[i];
+            wraps += sum < v[i];
         }
         uint32_t inc = warp_incl_scan(sum);
-        if (lane == 31) s_warp[warp] = inc;
+        wraps = __reduce_add_sync(0xffffffffu, wraps + (inc < sum));  // the warp's wraps: its threads' and its scan's
+        if (lane == 31) s_warp[warp] = ((unsigned long long)wraps << 32) | inc;
         __syncthreads();
-        uint32_t woff = 0, tot = 0;
-#pragma unroll
-        for (int i = 0; i < SCAN_THREADS / 32; i++) { uint32_t t = s_warp[i]; if (i < warp) woff += t; tot += t; }
         if (warp == 0) {
+            // the tile's exact total, read from s_warp where it is needed: a 64-bit total held through the look-back
+            // took 40 registers instead of 32 (6 CTAs per SM instead of 8)
+            auto tot = [&] {
+                unsigned long long t = 0;
+#pragma unroll
+                for (int i = 0; i < SCAN_THREADS / 32; i++) t += ((volatile unsigned long long*)s_warp)[i];
+                return t;
+            };
             const unsigned long long excl = lookback(state, 1, tile, tot);
-            if (lane == 0) { s_prefix = excl; if (tile == ntiles - 1) { *total = excl + tot; out[n] = (uint32_t)(excl + tot); } }
+            if (lane == 0) { s_prefix = excl; if (tile == ntiles - 1) { const unsigned long long all = excl + tot(); *total = all; out[n] = (uint32_t)all; } }
         }
         __syncthreads();
-        uint32_t run = (uint32_t)s_prefix + woff + (inc - sum);
+        uint32_t run = (uint32_t)s_prefix + (inc - sum);
+#pragma unroll
+        for (int i = 0; i < SCAN_THREADS / 32; i++) if (i < warp) run += (uint32_t)s_warp[i];
 #pragma unroll
         for (int i = 0; i < SCAN_ITEMS; i++) { if (base + i < n) out[base + i] = run; run += v[i]; }
         __syncthreads();
@@ -218,8 +232,9 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
         scan_impl(c, nullptr, srcs[k]->off(), ids, o, (uint64_t)nout, totals->as<uint64_t>() + k);
     }
     const std::vector<uint64_t> tot = read_back<uint64_t>(c, totals->p, srcs.size());
-    for (size_t k = 0; k < srcs.size(); k++) {
+    for (size_t k = 0; k < srcs.size(); k++)  // every column checked before any is copied: a refused gather writes nothing
         if (tot[k] > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, (int)k, 0, false, "a result column exceeds 4 GiB; process in smaller batches"};
+    for (size_t k = 0; k < srcs.size(); k++) {
         out[k].data = dev_alloc(c, tot[k] + 16);
         if (nout && tot[k]) {
             KernelTimer kt(c, "gather_copy", 2 * tot[k] + (uint64_t)nout * 12);
@@ -371,6 +386,7 @@ __global__ void __launch_bounds__(256) rowhash_probe_kernel(KeyDesc kd, uint64_t
 // exclusive scans of the NC length fields (8 bits each) of row i's packed lengths in one pass (warp c runs column c's
 // look-back).  Src::load(base, n, p) gives the packed lengths of rows [base, base + LS_ITEMS) (0 past n).  A body of its
 // own: folded into one kernel with scan_u32_kernel, the scan_gather_len instantiation took 40 registers instead of 32.
+// Its 32-bit sums cannot wrap: a tile's column sum is at most 255 bytes x LS_TILE rows (522 240).
 constexpr int LS_ITEMS = 8;
 constexpr int LS_TILE = SCAN_THREADS * LS_ITEMS;
 struct LensById {  // row slots: lens[ids[i]]
@@ -430,7 +446,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lens_kernel(const Src src, 
             uint32_t tot = 0;
 #pragma unroll
             for (int i = 0; i < SCAN_THREADS / 32; i++) tot += s_warp[c][i];
-            const unsigned long long excl = lookback(state + c, NC, tile, tot);  // state[tile * NC + c]
+            const unsigned long long excl = lookback(state + c, NC, tile, [=] { return (unsigned long long)tot; });  // state[tile * NC + c]
             if (lane == 0) {
                 s_prefix[c] = excl;
                 if (tile == ntiles - 1) totals[c] = excl + tot;

@@ -25,8 +25,8 @@ __host__ __device__ inline bool first_rune_is_space(const uint8_t* p, uint32_t n
     if (c == 0xE3 && n >= 3) return p[1] == 0x80 && p[2] == 0x80;
     return false;
 }
-// returns output length of one field; *quoted tells whether it is written in quotes
-__host__ __device__ inline uint32_t field_out_len(const uint8_t* p, uint32_t n, bool* quoted) {
+// returns output length of one field (up to 2n + 2, so 64 bits); *quoted tells whether it is written in quotes
+__host__ __device__ inline uint64_t field_out_len(const uint8_t* p, uint32_t n, bool* quoted) {
     *quoted = false;
     if (n == 0) return 0;
     uint32_t nq = 0; bool need = (n == 2 && p[0] == '\\' && p[1] == '.');
@@ -37,11 +37,11 @@ __host__ __device__ inline uint32_t field_out_len(const uint8_t* p, uint32_t n, 
     }
     if (!need) need = first_rune_is_space(p, n);
     *quoted = need;
-    return need ? n + nq + 2 : n;
+    return need ? (uint64_t)n + nq + 2 : n;
 }
 __host__ __device__ inline uint32_t field_write(const uint8_t* p, uint32_t n, uint8_t* d) {
-    bool q; uint32_t len = field_out_len(p, n, &q);
-    if (!q) { for (uint32_t i = 0; i < n; i++) d[i] = p[i]; return len; }
+    bool q; field_out_len(p, n, &q);
+    if (!q) { for (uint32_t i = 0; i < n; i++) d[i] = p[i]; return n; }
     uint32_t k = 0;
     d[k++] = '"';
     for (uint32_t i = 0; i < n; i++) { if (p[i] == '"') d[k++] = '"'; d[k++] = p[i]; }
@@ -49,16 +49,18 @@ __host__ __device__ inline uint32_t field_write(const uint8_t* p, uint32_t n, ui
     return k;
 }
 
+// len[r] = output bytes of row r, saturated at 0xFFFFFFFF (the host then reports CPB_E_TOO_LARGE): a row of quotes
+// doubles in length, and a column may be named more than once
 __global__ void csv_row_len_kernel(WriteCols wc, uint64_t n, uint32_t* len) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
-    uint32_t total = (uint32_t)wc.n;  // n-1 commas + newline
+    uint64_t total = (uint64_t)wc.n;  // n-1 commas + newline
     for (int k = 0; k < wc.n; k++) {
         uint32_t s = wc.off[k][r], l = wc.off[k][r + 1] - s;
         bool q;
         total += field_out_len(wc.data[k] + s, l, &q);
     }
-    len[r] = total;
+    len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
 }
 constexpr int CW_WARPS = 8;
 constexpr int CW_STAGE = 4096;
@@ -98,7 +100,8 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     }
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
     const uint64_t body = read_back<uint64_t>(c, tot->p);
-    if (body > 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToCsv output exceeds 4 GiB; write in smaller batches"};
+    // (one row of 0xFFFFFFFF bytes may be a saturated longer one: refused as well)
+    if (body > 0xffffffffull || (n == 1 && body == 0xffffffffull)) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToCsv output exceeds 4 GiB; write in smaller batches"};
     *nbytes = header.size() + body;
     if (*nbytes > room) return nullptr;
     Buf out = dev_alloc(c, header.size() + body + 16);
