@@ -17,6 +17,7 @@ PRED_SET_MIN = 33    # CPB_PRED_SET_MIN
 # the cpb_status and cpb_err_kind values the host layer tells apart (tests check them against the header's enums)
 CPB_ERR_DATA = 1
 CPB_ERR_ARG = 2
+CPB_ERR_UNSUPPORTED = 4
 CPB_E_MISSING_COLUMN = 10
 CPB_E_TOO_LARGE = 13
 CPB_E_BAD_CODE = 19
@@ -70,7 +71,7 @@ SYMBOLS = [
     "cpb_table_to_json", "cpb_table_to_json_device", "cpb_table_to_json_into",
     "cpb_table_column_as_int64", "cpb_table_column_as_float64", "cpb_table_column_as_float32",
     "cpb_table_set_int64", "cpb_table_set_float64", "cpb_table_set_float32", "cpb_table_set_literal", "cpb_table_filter_flags",
-    "cpb_table_column_codes", "cpb_table_set_codes",
+    "cpb_table_column_codes", "cpb_table_set_codes", "cpb_table_set_sprintf", "cpb_table_sprintf_into",
     "cpb_comm_unique_id", "cpb_comm_init_rank", "cpb_init_multi", "cpb_comm_size", "cpb_comm_rank", "cpb_allgather_table",
     "cpb_allgather_tables", "cpb_allgather_u64", "cpb_allgather_layout",
     "cpb_stats_enable", "cpb_stats_reset", "cpb_stats_get", "cpb_kernel_launches", "cpb_host_syncs", "cpb_gen_csv",
@@ -164,6 +165,8 @@ def load():
         "cpb_table_filter_flags": (i32, [vp, vp, vp, P(vp), P(Error)]),
         "cpb_table_column_codes": (i32, [vp, vp, Str, vp, P(vp), P(Error)]),
         "cpb_table_set_codes": (i32, [vp, vp, Str, vp, vp, P(vp), P(Error)]),
+        "cpb_table_set_sprintf": (i32, [vp, vp, Str, Str, P(Str), i32, P(vp), P(Error)]),
+        "cpb_table_sprintf_into": (i32, [vp, vp, Str, P(Str), i32, vp, u64, P(u64), P(Error)]),
         "cpb_comm_unique_id": (i32, [vp]),
         "cpb_comm_init_rank": (i32, [vp, i32, i32, vp]),
         "cpb_init_multi": (i32, [P(i32), i32, P(vp)]),

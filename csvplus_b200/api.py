@@ -28,6 +28,9 @@ Row = dict  # map[string]string, csvplus.go:59 (values are str; bytes survive vi
 # rows per cpb_table_to_json_into call when DataSource.ToJSON writes a device table: one call produces < 4 GiB, and
 # about 2.4 GB for joined rows of ~150 B.  A batch that is still too large is split in halves.
 JSON_BATCH_ROWS = 1 << 24
+# rows per cpb_table_sprintf_into call of DataSource.ToText (one call produces < 4 GiB; a batch that is still too large is
+# halved)
+TEXT_BATCH_ROWS = 1 << 24
 # rows per cpb_index_gob_into call of Index.WriteTo (one call produces < 4 GiB; a batch that is still too large is halved)
 GOB_BATCH_ROWS = 1 << 24
 # bytes per host push of an input (FromFile / FromReader / host FromBytes, cpb_stream_*): one batch is parsed per push, so
@@ -607,6 +610,13 @@ class Table:
         """ToJSON with the serialised bytes left in HBM (cpb_table_to_json_device)"""
         return self._device_bytes("cpb_table_to_json_device", int(first), int(last))
 
+    def sprintf_into(self, dst: "HostBuffer | None", offset: int, format, *cols) -> int:
+        """fmt.Sprintf(format, v...) of every row (v: the row's values of cols), the texts back to back, into pinned host
+        memory (cpb_table_sprintf_into).  Returns their size in bytes; when that exceeds the room left in dst (or dst is
+        None), nothing is written.  A refused format raises ValueError; a missing column DataSourceError, as ToCsv."""
+        with _format_refusal():
+            return _into(self.ctx, "cpb_table_sprintf_into", self.h, *Sprintf(format, *cols)._args(), dst=dst, offset=offset)
+
     def values_as_int(self, name: str, strict: bool = True):
         """Row.ValueAsInt (strconv.Atoi, csvplus.go:165-183) of every row of a column, as an int64 CUDA tensor on the
         ctx's device.  strict: the first failing row raises CsvPlusError with the reference's text (.row = its index), as
@@ -677,8 +687,15 @@ class Table:
         (strconv.FormatFloat(x, fmt, prec, 64); fmt defaults to 'g', prec -1 gives the shortest digits that read back as x)
         or a FormatFloat marker (the only way to pass a float32 tensor: FormatFloat(x32, bit_size=32)), or Categories:
         the dictionary's value at each row's code (a code outside the dictionary raises CsvPlusError with .row = the
-        lowest such row).  A tensor holds one value per row; it may be freed as soon as the call returns."""
+        lowest such row), or Sprintf: fmt.Sprintf(format, v...) of each row's values of the named columns (a refused
+        format raises ValueError, a missing column CsvPlusError).  A tensor holds one value per row; it may be freed as
+        soon as the call returns."""
         b = _enc(name); column = _abi.Str(b, len(b))
+        if isinstance(value, Sprintf):
+            if fmt is not None:
+                raise TypeError("with_column: the format of a Sprintf value is given in Sprintf")
+            with _format_refusal():
+                return self.ctx._new_table("cpb_table_set_sprintf", self.h, column, *value._args())
         if isinstance(value, Categories):
             if fmt is not None:
                 raise TypeError("with_column: fmt applies to float64 tensors only")
@@ -764,6 +781,34 @@ class Categories:
         if not isinstance(dictionary, Table):
             raise TypeError(f"Categories: the dictionary is a Table, got {type(dictionary).__name__}")
         self.codes, self.dictionary = codes, dictionary
+
+
+class Sprintf:
+    """fmt.Sprintf(format, v[0], v[1], ...) of every row, v = the row's values of `columns` (Row.SelectValues; a column may
+    be named twice): a value for Table.with_column and MapTensors.  The format is str or bytes; the library accepts
+    literal bytes, %% and %[-][width][.prec]s / %v (width and precision at most 1000000, counted in runes as Go counts
+    them), with exactly one verb per column.  Anything else raises ValueError when the value is used, with the library's
+    message naming the byte offset."""
+
+    def __init__(self, format, *columns):
+        self.format, self.columns = _enc(format), tuple(columns)
+
+    def _args(self) -> tuple:
+        """(format, column list, count) as the ABI takes them; the list keeps its bytes alive"""
+        a, keep = _strs(self.columns)
+        a._keep = keep
+        return _abi.Str(self.format, len(self.format)), a, len(self.columns)
+
+
+@contextlib.contextmanager
+def _format_refusal():
+    """a format the library refuses (CPB_ERR_UNSUPPORTED) raises ValueError with its message"""
+    try:
+        yield
+    except CsvPlusError as e:
+        if e.status == _abi.CPB_ERR_UNSUPPORTED:
+            raise ValueError(str(e)) from None
+        raise
 
 
 def _ctx_waits_for_torch(ctx: "Context", dev) -> None:
@@ -1311,7 +1356,8 @@ class DataSource:
         """a device Map (an extension beyond the reference API, like ToTensors): inputs = {column: "int" | "float64" |
         "float32"} are converted per batch as ToTensors converts them, fn(dict of CUDA tensors) returns {name: value} and
         each name is set as Table.with_column sets it (an int64 / float64 tensor with one value per row, a FormatFloat, a
-        str, Categories; a float32 result goes through FormatFloat(x, bit_size=32)).  "category" is not an input type:
+        str, Categories, Sprintf; a float32 result goes through FormatFloat(x, bit_size=32)).  A Sprintf reads the batch's
+        columns as they were before the step, a column the same result replaces included.  "category" is not an input type:
         inputs are converted batch by batch, and codes numbered per batch would differ between batches (ValueError);
         take codes once with ToTensors.  fn is called
         once per non-empty batch and must be row-wise.  A conversion error (the lowest failing row, ties to the earlier
@@ -1323,6 +1369,12 @@ class DataSource:
         """a device Filter: as MapTensors, fn returns a bool CUDA tensor with one value per row; the rows where it is true
         are kept.  As for MapTensors, "category" is not an input type (codes would differ between batches)."""
         return self._with(("filtertensors", _tensor_kinds(inputs, "FilterTensors"), fn))
+
+    def Sprintf(self, column: str, format, *columns):
+        """a device Map (an extension beyond the reference API, like MapTensors): every row's `column` set to
+        fmt.Sprintf(format, v...) of its values of `columns`, as Table.with_column(column, Sprintf(format, *columns))
+        sets it, batch by batch"""
+        return self._with(("sprintf", column, Sprintf(format, *columns)))
 
     def DropColumns(self, *columns):
         if len(columns) == 0:
@@ -1392,7 +1444,7 @@ class DataSource:
         stop = False
         for i, op in enumerate(ops):
             kind = op[0]
-            device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop", "maptensors", "filtertensors")
+            device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop", "maptensors", "filtertensors", "sprintf")
                          or (kind in ("filter", "takewhile", "dropwhile") and isinstance(op[1], Predicate) and op[1].lowerable()))
             if device_ok:
                 if state[0] == "rows":
@@ -1406,6 +1458,7 @@ class DataSource:
                     elif kind == "filter": t = t.filter(op[1])
                     elif kind == "join": t = t.join(op[1], *op[2])
                     elif kind == "except": t = t.join(op[1], *op[2], anti=True)
+                    elif kind == "sprintf": t = t.with_column(op[1], op[2])
                     elif kind == "top":  # note: the reference pulls one extra row (SURVEY §Q8)
                         seen = carry.get(i, 0)
                         t = t.slice(0, min(len(t), max(0, op[1] - seen)))
@@ -1556,6 +1609,29 @@ class DataSource:
         with _new_file(name) as f:
             self.ToJSON(f)
 
+    def ToText(self, out: io.IOBase, format, *columns):
+        """what a RowFunc calling fmt.Fprintf(out, format, v...) for every row writes, v = the row's values of columns
+        (an extension beyond the reference's sinks, which write CSV and JSON): every row's text in row order, no header
+        and no separator.  A device table is formatted by the GPU in row-range batches through one pinned buffer; rows
+        left on the host go through Table.from_rows first.  Rows delivered before a source error are written, then the
+        error is raised, as ToCsv does.  A refused format raises ValueError (see Sprintf); a missing column raises
+        DataSourceError as ToCsv reports it."""
+        hold: list = []  # the pinned buffer every batch is formatted into
+        try:
+            for state, err, _ in self._batches():
+                t = self._as_table(state)
+                if t is not None:
+                    _text_batches(t, out, format, columns, hold)
+                if err is not None:
+                    raise err
+        finally:
+            for b in hold:
+                b.free()
+
+    def ToTextFile(self, name: str, format, *columns):  # as ToCsvFile: the file is removed on error
+        with _new_file(name) as f:
+            self.ToText(f, format, *columns)
+
     def ToTensors(self, columns: dict) -> dict:
         """{name: "int" | "float64" | "float32" | "category"} -> {name: CUDA tensor or Categories}: Row.ValueAsInt /
         ValueAsFloat64 (or ParseFloat(s, 32), Table.values_as_float32) of every row of each column, converted on the GPU
@@ -1632,11 +1708,25 @@ def _tensor_step(t: Table, op, seen: int):
         if kind == "maptensors":
             if not isinstance(res, dict):
                 raise TypeError(f"MapTensors: fn must return a dict of column values, got {type(res).__name__}")
-            for name, value in res.items():
-                t = t.with_column(name, value)
+            t = _set_results(t, res)
         else:
             t = t.filter_mask(res)
     return t, err
+
+
+def _set_results(t: Table, res: dict) -> Table:
+    """t with every column of res set in dict order.  A Sprintf reads t's columns as they were before: one that names a
+    column set before it in res is computed first into a column of its own name and copied into place in order."""
+    staged, set_before = {}, set()
+    for name, value in res.items():
+        if isinstance(value, Sprintf) and set_before & set(value.columns):
+            staged[name] = "\0sprintf%d\0%s" % (len(staged), name)
+        set_before.add(name)
+    for name, tmp in staged.items():
+        t = t.with_column(tmp, res[name])
+    for name, value in res.items():
+        t = t.with_column(name, Sprintf("%s", staged[name]) if name in staged else value)
+    return t.drop(*staged.values()) if staged else t
 
 
 def _concat(tables: list) -> "Table | None":
@@ -1726,6 +1816,19 @@ def _json_batches(t: Table, out: io.IOBase, first: bool, hold: list):
         part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
         _write_into(out, hold, t.ctx, lambda buf: part.to_json_into(buf, 0, first and lo == 0, False))
     _row_batches(n, JSON_BATCH_ROWS, write)
+
+
+def _text_batches(t: Table, out: io.IOBase, format, columns: tuple, hold: list):
+    """Table.sprintf_into of a device table in row-range slices of at most TEXT_BATCH_ROWS rows, each written through the
+    pinned buffer of hold (_write_into).  A table of no rows still has its format and columns checked."""
+    n = len(t)
+    if n == 0:
+        t.sprintf_into(None, 0, format, *columns)
+
+    def write(lo, hi):
+        part = t if (lo, hi) == (0, n) else t.slice(lo, hi)
+        _write_into(out, hold, t.ctx, lambda buf: part.sprintf_into(buf, 0, format, *columns))
+    _row_batches(n, TEXT_BATCH_ROWS, write)
 
 
 def Take(src) -> DataSource:  # csvplus.go:252-256

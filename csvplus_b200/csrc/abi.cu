@@ -952,6 +952,21 @@ int cpb_table_set_codes(cpb_ctx* h, const cpb_table* t, cpb_str column, const in
     });
 }
 
+// ------------------------------------------------------------------ Sprintf columns and text
+int cpb_table_set_sprintf(cpb_ctx* h, const cpb_table* t, cpb_str column, cpb_str format, const cpb_str* args, int nargs, cpb_table** out,
+                          cpb_error* err) {
+    return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
+        return table_set_sprintf(c, T, to_string(column), to_string(format), str_list(args, nargs));
+    });
+}
+int cpb_table_sprintf_into(cpb_ctx* h, const cpb_table* t, cpb_str format, const cpb_str* args, int nargs, void* host_dst, uint64_t cap,
+                           uint64_t* nbytes, cpb_error* err) {
+    return serialise(h, err, Dest{Dest::into, nullptr, host_dst, cap}, nbytes, "Sprintf destination too small",
+                     [&](Ctx* c, uint64_t room, uint64_t* total) {
+                         return table_sprintf(c, table_of(t), to_string(format), str_list(args, nargs), room, total);
+                     });
+}
+
 // ------------------------------------------------------------------ stats
 int cpb_stats_enable(cpb_ctx* h, int on) {
     return guarded(h, nullptr, [&](Ctx* c) { c->stats_on = on != 0; return CPB_OK; });

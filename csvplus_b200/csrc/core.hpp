@@ -436,6 +436,15 @@ std::shared_ptr<Table> table_filter_mask(Ctx* c, const Table& t, const uint8_t* 
 // outside [0, rows of dict) throws DataError CPB_E_BAD_CODE with line = the lowest such row.
 std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* codes);
 std::shared_ptr<Table> table_set_codes(Ctx* c, const Table& t, const std::string& name, const int64_t* codes, const Table& dict);
+// sprintf.cu: fmt.Sprintf(format, v...) of every row, v = the row's values of columns cols (a name may repeat).  The
+// format is compiled first: one outside the accepted subset, or whose verb count is not cols.size(), throws ArgError
+// CPB_ERR_UNSUPPORTED naming the byte offset.  A column t lacks (on a table with rows) throws DataError
+// CPB_E_MISSING_COLUMN: as column_as_int64 reports it for table_set_sprintf, as ToCsv does for table_sprintf.
+// table_set_sprintf: t with column `name` set to the texts (under with_column's rules); table_sprintf: the texts
+// back to back (room as table_to_csv).  A result of 4 GiB or more throws CPB_E_TOO_LARGE after the length pass.
+std::shared_ptr<Table> table_set_sprintf(Ctx* c, const Table& t, const std::string& name, const std::string& format,
+                                         const std::vector<std::string>& cols);
+Buf table_sprintf(Ctx* c, const Table& t, const std::string& format, const std::vector<std::string>& cols, uint64_t room, uint64_t* nbytes);
 
 }  // namespace cpb
 

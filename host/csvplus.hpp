@@ -308,6 +308,16 @@ public:
         const cpb_str v{value.data(), value.size()};
         return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) { return cpb_table_set_literal(detail::ctx(), h_.get(), c, v, out, e); });
     }
+    // Map(func(row) Row { v, _ := row.SelectValues(cols...); row[column] = fmt.Sprintf(format, v[0], ...); return row }) on
+    // the GPU.  format: literal bytes, %% and %[-][width][.prec]s / %v, one verb per column (cpb_table_set_sprintf); a
+    // refused format, a missing column or a column of 4 GiB or more throws.
+    Table WithSprintf(const std::string& column, const std::string& format, const std::vector<std::string>& cols) const {
+        const detail::Strs a(cols);
+        const cpb_str f{format.data(), format.size()};
+        return set(column, [&](cpb_str c, cpb_table** out, cpb_error* e) {
+            return cpb_table_set_sprintf(detail::ctx(), h_.get(), c, f, a.v.data(), (int)cols.size(), out, e);
+        });
+    }
     // the rows whose dev_keep[row] byte (device memory, size() bytes) is nonzero, in order
     Table FilterMask(const uint8_t* dev_keep) const {
         cpb_table* out = nullptr; cpb_error e{};
@@ -570,6 +580,47 @@ public:
             return true;
         });
         out << (opened ? "]" : "[]");
+    }
+    // ToText: what a RowFunc calling fmt.Fprintf(out, format, v...) for every row writes (v: the row's values of cols),
+    // formatted on the GPU in row-range batches (each < 4 GiB; a batch that is still too large is halved) into one reused
+    // pinned buffer.  Delivered rows are written before a source error is thrown, as ToCsv does.
+    void ToText(std::ostream& out, const std::string& format, const std::vector<std::string>& cols) const {
+        const detail::Strs a(cols);
+        const cpb_str f{format.data(), format.size()};
+        detail::Pinned buf;
+        each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool) {
+            const int64_t n = t.size();
+            int64_t lo = 0, step = int64_t(1) << 24;
+            do {  // (a table of no rows still has its format and columns checked)
+                const int64_t hi = std::min(n, lo + step);
+                Table p = (lo == 0 && hi == n) ? t : t.slice(lo, hi);
+                bool too_large = false;
+                try {
+                    buf.write(out, [&](void* dst, uint64_t cap, uint64_t* w, cpb_error* e) {
+                        const int st = cpb_table_sprintf_into(detail::ctx(), p.get(), f, a.v.data(), (int)cols.size(), dst, cap, w, e);
+                        too_large = st == CPB_ERR_DATA && e->kind == CPB_E_TOO_LARGE;
+                        return st;
+                    });
+                } catch (const Error&) {
+                    if (!too_large || hi - lo < 2) throw;
+                    step = (hi - lo) / 2;  // halve the batch
+                    continue;
+                }
+                lo = hi;
+            } while (lo < n);
+            if (err) throw *err;
+            return true;
+        });
+    }
+    // ToTextFile: ToText into a new file, removed on error (as ToCsvFile)
+    void ToTextFile(const std::string& name, const std::string& format, const std::vector<std::string>& cols) const {
+        try {
+            std::ofstream f(name, std::ios::binary | std::ios::trunc);
+            if (!f) throw Error("open " + name + ": " + strerror(errno));
+            ToText(f, format, cols);
+            f.close();
+            if (!f) throw Error("write " + name + " failed");
+        } catch (...) { std::remove(name.c_str()); throw; }
     }
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }

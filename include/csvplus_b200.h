@@ -382,6 +382,28 @@ int cpb_table_column_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, int
 int cpb_table_set_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const int64_t* dev_codes, const cpb_table* dictionary,
                         cpb_table** out, cpb_error* err);
 
+/* ------------------------------------------------------------------ formatted rows (fmt.Sprintf of string columns)
+ * Every row's text is fmt.Sprintf(format, v[0], ..., v[nargs-1]), v = the row's values of the columns args (Row.SelectValues,
+ * csvplus.go:138-149; a column may be named more than once).  The accepted format language is the subset of Go's fmt whose
+ * output for string operands is fixed:
+ *   - literal bytes, copied verbatim (NUL and invalid UTF-8 included), and %% (bare);
+ *   - %[-...][width][.[prec]]s and the same with v: width and prec decimal, at most 1000000, a bare '.' is precision 0;
+ *     precision keeps the first prec runes, width pads with spaces to width runes (left-aligned with '-'), runes being
+ *     utf8.DecodeRune's (a byte outside a valid sequence is one rune of one byte).
+ * Anything else — another verb, the flags 0 + # and space, '*', explicit argument indexes, flags or width on %%, a lone
+ * trailing '%', a verb count other than nargs, more than 64 verbs, a format longer than 4096 bytes — fails with
+ * CPB_ERR_UNSUPPORTED before any kernel runs, the message naming the byte offset.  A column the table lacks (on a table
+ * with rows) fails with CPB_ERR_DATA / CPB_E_MISSING_COLUMN "missing column %q".
+ *   set_sprintf: *out = t with `column` set to the texts, replaced in place or appended as set_int64 sets it; the missing
+ *                column is reported as column_as_int64 reports it (line 0, has_line = 0).  One host synchronisation.
+ *   sprintf_into: the texts of every row back to back (no header, no separator: the format carries its own newline), the
+ *                contract of cpb_table_to_csv_into; the missing column is reported as cpb_table_to_csv reports it.
+ * One call produces less than 4 GiB (else CPB_ERR_DATA / CPB_E_TOO_LARGE, nothing written: format row-range slices). */
+int cpb_table_set_sprintf(cpb_ctx* ctx, const cpb_table* t, cpb_str column, cpb_str format, const cpb_str* args, int nargs,
+                          cpb_table** out, cpb_error* err);
+int cpb_table_sprintf_into(cpb_ctx* ctx, const cpb_table* t, cpb_str format, const cpb_str* args, int nargs, void* host_dst,
+                           uint64_t cap, uint64_t* nbytes, cpb_error* err);
+
 /* ------------------------------------------------------------------ multi-GPU (SURVEY §8e)
  * The probe stream shards by row range with no data-path collective; the one exchange step is the all-gather of the
  * build-side columns (each rank parses 1/N of the build file) so that every rank can build the full Index
