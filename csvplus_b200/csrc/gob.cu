@@ -21,9 +21,10 @@
 // The rows of the index are taken in its stored order (sorted_table).  A message of 8 GiB or more (encoding/gob's tooBig
 // on 64-bit), or a rows slice above 8 GiB of Go maps, is refused before anything is written, as gob's encoder refuses it.
 //
-// Encode: gob_row_len (bytes per row) -> exclusive_scan_u32 -> gob_write (warp_write_rows of rowwrite.cuh) over a
-// keyed-column table whose names are uint(len name) name.  The prefix (type definitions, columns, rows header) is built
-// here on the host; the rows are written in row-range batches (each < 4 GiB) by cpb_index_gob_into.
+// Encode: the row type GobRows through the row serialiser driver of rowwrite.cuh (gob_row_len, which also sums the
+// lengths exactly -> exclusive_scan_u32 -> gob_write) over a keyed-column table whose names are uint(len name) name.
+// The prefix (type definitions, columns, rows header) is built here on the host; the rows are written in row-range
+// batches (each < 4 GiB) by cpb_index_gob_into.
 //
 // Decode: the host parses the type definitions (any ids, any order), the columns value, the rows message header and the
 // first row (k and the column set).  The rows body is uploaded once.  A row has no marker and its start depends on every
@@ -122,24 +123,31 @@ static std::string map_def(const std::string& name, int64_t id, int64_t key, int
 }
 
 // ------------------------------------------------------------------ encode kernels
-// len[r] = bytes of row r, saturated at 0xFFFFFFFF (then *sum is >= 4 GiB too); *sum += the exact 64-bit total.  The
-// 32-bit scan of the lengths is run only when that total is below 4 GiB, so no partial sum of it can wrap.
-__global__ void gob_row_len_kernel(const KeyedCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len,
-                                   unsigned long long* sum) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint64_t total = 0;
-    if (r < n) {
-        total = row_const;
+// a row: uint(k), then every pair uint(len name) name (pre-encoded) uint(len value) value
+struct GobRows : KeyedRows {
+    __device__ uint64_t len(uint64_t r) const {
+        uint64_t total = row_const;
         for (int k = 0; k < ncols; k++) {
             const uint32_t* off = cols[k].off;
             const uint32_t l = off[r + 1] - off[r];
             total += gob_uint_len(l) + l;
         }
-        len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
+        return total;
     }
-    total = warp_sum_u64(total);
-    if ((threadIdx.x & 31) == 0 && total) atomicAdd(sum, (unsigned long long)total);
-}
+    __device__ void write(uint64_t r, uint8_t* q, const Tables& t) const {
+        q += gob_put_uint(q, (uint64_t)ncols);
+        for (int k = 0; k < ncols; k++) {
+            const KeyedCol c = t.cols[k];
+            for (uint32_t j = 0; j < c.key_len; j++) q[j] = t.keys[c.key + j];
+            q += c.key_len;
+            const uint32_t s = c.off[r], l = c.off[r + 1] - s;
+            q += gob_put_uint(q, l);
+            const uint8_t* p = c.data + s;
+            for (uint32_t j = 0; j < l; j++) q[j] = p[j];
+            q += l;
+        }
+    }
+};
 // out[y] += the exact 64-bit sum of v[y * stride + i], i < n (blockIdx.y = y)
 __global__ void gob_sum_kernel(const uint32_t* __restrict__ v, uint64_t n, uint64_t stride, unsigned long long* out) {
     const uint32_t* p = v + (uint64_t)blockIdx.y * stride;
@@ -149,55 +157,27 @@ __global__ void gob_sum_kernel(const uint32_t* __restrict__ v, uint64_t n, uint6
     if ((threadIdx.x & 31) == 0 && s) atomicAdd(out + blockIdx.y, (unsigned long long)s);
 }
 
-// the keyed-column table is copied to shared memory when it fits (meta_smem)
-constexpr int GB_WARPS = 8;
-constexpr int GB_STAGE = 4096;
-constexpr uint32_t GB_STAGE_BYTES = GB_WARPS * (GB_STAGE + 16);
-constexpr uint32_t GB_META_SMEM = 16384;
-__global__ void __launch_bounds__(GB_WARPS * 32) gob_write_kernel(const KeyedCol* cols, const uint8_t* keys, int ncols, uint32_t meta_bytes,
-                                                                  int meta_smem, uint64_t n, const uint32_t* __restrict__ pos, uint8_t* out) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    stage_keyed_cols(smem + GB_STAGE_BYTES, meta_smem, meta_bytes, cols, keys);
-    warp_write_rows<GB_WARPS, GB_STAGE>(smem, n, pos, out, [&](uint64_t r, uint8_t* q) {
-        q += gob_put_uint(q, (uint64_t)ncols);
-        for (int k = 0; k < ncols; k++) {
-            const KeyedCol c = cols[k];
-            for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
-            q += c.key_len;
-            const uint32_t s = c.off[r], l = c.off[r + 1] - s;
-            q += gob_put_uint(q, l);
-            const uint8_t* p = c.data + s;
-            for (uint32_t j = 0; j < l; j++) q[j] = p[j];
-            q += l;
-        }
-    });
-}
-
 // the keyed columns of rows [lo, hi) of the index's stored rows
 struct GobMeta {
     std::shared_ptr<Table> t;  // the stored rows, kept alive while the kernels read them
     KeyedCols kc;
-    uint64_t row_const = 0;    // uint(k) + every pre-encoded name
 };
 static GobMeta gob_meta(Ctx* c, Index& ix, uint64_t lo) {
     GobMeta m;
     m.t = sorted_table(c, ix);
     m.kc = keyed_cols(c, *m.t, lo, [](std::string& keys, const std::string& name, int) { put_str(keys, name); });
-    m.row_const = gob_uint_len((uint64_t)m.kc.ncols) + (m.kc.meta_bytes - m.kc.keys_at);
     return m;
 }
+// uint(k) + every pre-encoded name: the bytes of a row besides its values
+static GobRows gob_row_type(const KeyedCols& kc) { return GobRows{KeyedRows(kc, gob_uint_len((uint64_t)kc.ncols) + (kc.meta_bytes - kc.keys_at))}; }
 
-// row lengths of rows [lo, lo + n) into len (n + 1 entries, not yet scanned); *out = {exact total bytes, value bytes}
+// row lengths of rows [lo, lo + n) into len (n + 1 entries, not yet scanned); *out = {exact total bytes, value bytes}.
+// The 32-bit scan of the lengths is run only when that total is below 4 GiB, so no partial sum of it can wrap.
 static void gob_lengths(Ctx* c, const GobMeta& m, uint64_t n, Buf& len, uint64_t out[2]) {
     len = dev_alloc(c, (n + 1) * 4);
     Buf tot = dev_alloc(c, 16);
     CPB_CUDA(cudaMemsetAsync(tot->p, 0, 16, c->stream));
-    if (n) {
-        KernelTimer kt(c, "gob_row_len", n * 4 * (m.kc.ncols + 1));
-        gob_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(m.kc.md->as<KeyedCol>(), m.kc.ncols, m.row_const, n, len->as<uint32_t>(),
-                                                                 tot->as<unsigned long long>());
-        CPB_CUDA(cudaGetLastError());
-    }
+    row_lengths<true>(c, gob_row_type(m.kc), n, len->as<uint32_t>(), "gob_row_len", n * 4 * (m.kc.ncols + 1), tot->as<unsigned long long>());
     keyed_value_bytes(c, m.kc, n, tot->as<unsigned long long>() + 1);
     const std::vector<uint64_t> h = read_back<uint64_t>(c, tot->p, 2);
     out[0] = h[0]; out[1] = h[1];
@@ -235,23 +215,13 @@ Buf gob_rows(Ctx* c, Index& ix, uint64_t lo, uint64_t hi, uint64_t room, uint64_
     Buf len;
     uint64_t t[2];
     gob_lengths(c, m, n, len, t);
-    if (t[0] >= 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "index rows batch exceeds 4 GiB; write in smaller batches"};
+    check_body(t[0], n, MAX_BODY - 1, "index rows batch exceeds 4 GiB; write in smaller batches");
     *nbytes = t[0];
     if (*nbytes > room) return nullptr;
     Buf tot = dev_alloc(c, 8);
     exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());  // every partial sum < 4 GiB
     Buf out = dev_alloc(c, t[0] + 16);
-    if (n) {
-        const KeyedCols& kc = m.kc;
-        KernelTimer kt(c, "gob_write", t[1] + n * 4 * (kc.ncols + 1) + t[0]);
-        const bool meta_smem = kc.meta_bytes <= GB_META_SMEM;
-        const uint32_t smem = GB_STAGE_BYTES + (meta_smem ? kc.meta_bytes : 0);
-        CPB_CUDA(cudaFuncSetAttribute(gob_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GB_STAGE_BYTES + GB_META_SMEM));
-        const uint32_t blocks = (uint32_t)std::min<uint64_t>((n + GB_WARPS * 32 - 1) / (GB_WARPS * 32), (uint64_t)c->sm_count * 8);
-        gob_write_kernel<<<blocks, GB_WARPS * 32, smem, c->stream>>>(kc.md->as<KeyedCol>(), kc.md->as<uint8_t>() + kc.keys_at, kc.ncols,
-                                                                     kc.meta_bytes, meta_smem, n, len->as<uint32_t>(), out->as<uint8_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
+    row_write<4096>(c, gob_row_type(m.kc), n, len->as<uint32_t>(), out->as<uint8_t>(), "gob_write", t[1] + n * 4 * (m.kc.ncols + 1) + t[0], 8);
     return out;
 }
 

@@ -15,8 +15,9 @@
 //
 // One call serialises one table or one row-range batch of a larger result: first_batch puts '[' before its first row
 // (else ','), last_batch appends ']'.  An empty batch writes only those brackets, so first = last = 1 gives "[]".
-// Kernels: json_row_len (bytes per row) -> exclusive_scan_u32 -> json_write (warp_write_rows of rowwrite.cuh).  The
-// columns are a keyed-column table (rowwrite.cuh) whose names are the key prefixes, so there is no column limit.
+// The row type JsonRows through the row serialiser driver of rowwrite.cuh (json_row_len -> exclusive_scan_u32 ->
+// json_write).  The columns are a keyed-column table (rowwrite.cuh) whose names are the key prefixes, so there is no
+// column limit.
 #include <algorithm>
 #include <numeric>
 
@@ -43,21 +44,6 @@ __device__ __forceinline__ bool json_plain(const uint8_t* p, uint32_t n) {
         if ((x | ((x - 0x20 * L) & ~x) | ((q - L) & ~q) | ((b - L) & ~b)) & H) return false;
     }
     return true;
-}
-
-// length of the valid UTF-8 sequence (utf8.DecodeRune) starting at p, 0 if none; p[0] >= 0x80, rem >= 1 bytes readable
-__host__ __device__ inline uint32_t utf8_seq(const uint8_t* p, uint64_t rem) {
-    const uint8_t c = p[0];
-    uint32_t w;
-    uint8_t lo = 0x80, hi = 0xBF;
-    if (c < 0xC2) return 0;
-    if (c < 0xE0) w = 2;
-    else if (c < 0xF0) { w = 3; if (c == 0xE0) lo = 0xA0; else if (c == 0xED) hi = 0x9F; }
-    else if (c < 0xF5) { w = 4; if (c == 0xF0) lo = 0x90; else if (c == 0xF4) hi = 0x8F; }
-    else return 0;
-    if (rem < w || p[1] < lo || p[1] > hi) return 0;
-    for (uint32_t j = 2; j < w; j++) if ((p[j] & 0xC0) != 0x80) return 0;
-    return w;
 }
 
 __host__ __device__ inline void put6(uint8_t* d, uint8_t a, uint8_t b, uint8_t c, uint8_t e) {
@@ -96,38 +82,29 @@ __host__ __device__ inline uint64_t json_escape(const uint8_t* p, uint64_t n, ui
     return k;
 }
 
-// len[r] = output bytes of row r, saturated at 0xFFFFFFFF (the host then reports CPB_E_TOO_LARGE)
-__global__ void json_row_len_kernel(const KeyedCol* __restrict__ cols, int ncols, uint64_t row_const, uint64_t n, uint32_t* len) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    uint64_t total = row_const;
-    for (int k = 0; k < ncols; k++) {
-        const uint32_t* off = cols[k].off;
-        const uint32_t s = off[r], l = off[r + 1] - s;
-        const uint8_t* p = cols[k].data + s;
-        total += json_plain(p, l) ? l : json_escape(p, l, nullptr);
-    }
-    len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
-}
-
 // A JSON row repeats every key, so it is several times longer than the CSV line of the same row (about 120-150 B for a
 // joined orders x customers row): the stage holds 32 rows of up to 190 B, where ToCsv's 4 KB would send most such
-// groups down the direct path.  The keyed-column table is copied to shared memory when it fits (meta_smem).
-constexpr int JW_WARPS = 8;
-constexpr int JW_STAGE = 6144;
-constexpr uint32_t JW_STAGE_BYTES = JW_WARPS * (JW_STAGE + 16);
-constexpr uint32_t JW_META_SMEM = 16384;
-__global__ void __launch_bounds__(JW_WARPS * 32) json_write_kernel(const KeyedCol* cols, const uint8_t* keys, int ncols, uint32_t meta_bytes,
-                                                                   int meta_smem, uint8_t first_byte, uint64_t n,
-                                                                   const uint32_t* __restrict__ pos, uint8_t* out) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    stage_keyed_cols(smem + JW_STAGE_BYTES, meta_smem, meta_bytes, cols, keys);
-    warp_write_rows<JW_WARPS, JW_STAGE>(smem, n, pos, out, [&](uint64_t r, uint8_t* q) {
+// groups down the direct path.
+constexpr uint32_t JW_STAGE = 6144;
+// a row: first_byte ('[' or ',') for row 0, else ','; then the pairs between braces, and '\n'
+struct JsonRows : KeyedRows {
+    uint8_t first_byte;
+    __device__ uint64_t len(uint64_t r) const {
+        uint64_t total = row_const;
+        for (int k = 0; k < ncols; k++) {
+            const uint32_t* off = cols[k].off;
+            const uint32_t s = off[r], l = off[r + 1] - s;
+            const uint8_t* p = cols[k].data + s;
+            total += json_plain(p, l) ? l : json_escape(p, l, nullptr);
+        }
+        return total;
+    }
+    __device__ void write(uint64_t r, uint8_t* q, const Tables& t) const {
         *q++ = r == 0 ? first_byte : ',';
         *q++ = '{';
         for (int k = 0; k < ncols; k++) {
-            const KeyedCol c = cols[k];
-            for (uint32_t j = 0; j < c.key_len; j++) q[j] = keys[c.key + j];
+            const KeyedCol c = t.cols[k];
+            for (uint32_t j = 0; j < c.key_len; j++) q[j] = t.keys[c.key + j];
             q += c.key_len;
             const uint32_t s = c.off[r], l = c.off[r + 1] - s;
             const uint8_t* p = c.data + s;
@@ -136,8 +113,8 @@ __global__ void __launch_bounds__(JW_WARPS * 32) json_write_kernel(const KeyedCo
             *q++ = '"';
         }
         q[0] = '}'; q[1] = '\n';
-    });
-}
+    }
+};
 
 // ---- the keyed-column table of rowwrite.cuh (ToJSON and Index.WriteTo)
 __global__ void keyed_value_bytes_kernel(const KeyedCol* cols, int ncols, uint64_t n, unsigned long long* out) {
@@ -199,34 +176,17 @@ Buf table_to_json(Ctx* c, const Table& t, bool first, bool last, uint64_t room, 
     const KeyedCols kc = keyed_cols(c, t, 0, json_key);
     const int ncols = kc.ncols;
     // '['/',' '{' '}' '\n', the key prefixes and the closing quote of every value
-    const uint64_t row_const = 4 + (kc.meta_bytes - kc.keys_at) + ncols;
-    const KeyedCol* dcols = kc.md->as<KeyedCol>();
-
+    const JsonRows rows{KeyedRows(kc, 4 + (kc.meta_bytes - kc.keys_at) + ncols), (uint8_t)(first ? '[' : ',')};
     Buf len = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 16);
-    {
-        KernelTimer kt(c, "json_row_len", n * 4 * (ncols + 1));
-        json_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dcols, ncols, row_const, n, len->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
+    row_lengths(c, rows, n, len->as<uint32_t>(), "json_row_len", n * 4 * (ncols + 1));
     keyed_value_bytes(c, kc, n, tot->as<unsigned long long>() + 1);
-    exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
-    const std::vector<uint64_t> ht = read_back<uint64_t>(c, tot->p, 2);
+    const std::vector<uint64_t> ht = row_offsets(c, len->as<uint32_t>(), n, tot->as<uint64_t>(), 2, MAX_BODY - 1,
+                                                 "ToJSON output exceeds 4 GiB; write in smaller batches");
     const uint64_t body = ht[0], value_bytes = ht[1];
-    if (body >= 0xffffffffull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToJSON output exceeds 4 GiB; write in smaller batches"};
     *nbytes = body + (last ? 1 : 0);
     if (*nbytes > room) return nullptr;
     Buf out = dev_alloc(c, body + 1 + 16);
-    {
-        KernelTimer kt(c, "json_write", value_bytes + n * 4 * (ncols + 1) + body);
-        const bool meta_smem = kc.meta_bytes <= JW_META_SMEM;
-        const uint32_t smem = JW_STAGE_BYTES + (meta_smem ? kc.meta_bytes : 0);
-        CPB_CUDA(cudaFuncSetAttribute(json_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, JW_STAGE_BYTES + JW_META_SMEM));
-        const uint32_t blocks = (uint32_t)std::min<uint64_t>((n + JW_WARPS * 32 - 1) / (JW_WARPS * 32), (uint64_t)c->sm_count * 8);
-        json_write_kernel<<<blocks, JW_WARPS * 32, smem, c->stream>>>(dcols, kc.md->as<uint8_t>() + kc.keys_at, ncols, kc.meta_bytes,
-                                                                      meta_smem, first ? '[' : ',', n, len->as<uint32_t>(),
-                                                                      out->as<uint8_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
+    row_write<JW_STAGE>(c, rows, n, len->as<uint32_t>(), out->as<uint8_t>(), "json_write", value_bytes + n * 4 * (ncols + 1) + body, 8);
     if (last) CPB_CUDA(cudaMemsetAsync(out->as<uint8_t>() + body, ']', 1, c->stream));
     return out;
 }

@@ -12,18 +12,16 @@
 //   format longer than SP_MAXLIT bytes) is refused by sprintf_compile with CPB_ERR_UNSUPPORTED before any launch.
 //
 // The format compiles once, on the host, into pieces: a literal slice of the format's bytes (adjacent literals and %%
-// merged) or a verb (its column, width, precision, alignment).  Two kernels, shaped like ToCsv's (write.cu):
+// merged) or a verb (its column, width, precision, alignment).  The row type SprintfRows runs through the row serialiser
+// driver of rowwrite.cuh, as ToCsv's does:
 //   sprintf_len:   one thread per row: the literal bytes (a constant) plus each verb's bytes; a verb with a precision walks
 //                  at most prec runes, a verb with a width counts the runes of its (truncated) value unless the value has at
-//                  least 4 * width bytes (then it has at least width runes and needs no padding).  Summed in 64 bits and
-//                  saturated at 0xFFFFFFFF, as csv_row_len does.
+//                  least 4 * width bytes (then it has at least width runes and needs no padding).
 //   exclusive_scan_u32 of the lengths (the offsets) and its exact 64-bit total, read back once: a total of 2^32 or more,
 //                  or one row of exactly 0xFFFFFFFF bytes (which may be a saturated longer one), is CPB_E_TOO_LARGE before
 //                  anything else is allocated.
-//   sprintf_write: the warp-staged row writer (rowwrite.cuh); every block first copies the piece table and the literal
-//                  bytes into shared memory.
-#include <algorithm>
-
+//   sprintf_write: the warp-staged row writer; every block first copies the piece table and the literal bytes into
+//                  shared memory.
 #include "core.hpp"
 #include "rowwrite.cuh"
 
@@ -35,20 +33,10 @@ constexpr uint32_t SP_MAXLIT = 4096;          // bytes of a format
 constexpr uint32_t SP_MAXNUM = 1000000;       // the largest width or precision
 constexpr uint32_t SP_NO_PREC = 0xFFFFFFFFu;  // a verb without a precision
 
-// Go's utf8.DecodeRune: the bytes of the rune starting at p (n > 0 bytes left); 1 for a byte that starts no valid sequence
+// the bytes of the rune utf8.DecodeRune reads at p (n > 0 bytes left): 1 for a byte that starts no valid sequence
 __host__ __device__ __forceinline__ uint32_t rune_bytes(const uint8_t* p, uint32_t n) {
-    const uint8_t c = p[0];
-    if (c < 0xC2) return 1;  // ASCII, a continuation byte, or an overlong lead C0 / C1
-    if (c <= 0xDF) return n >= 2 && (p[1] & 0xC0) == 0x80 ? 2 : 1;
-    if (c <= 0xEF) {
-        const uint8_t lo = c == 0xE0 ? 0xA0 : 0x80, hi = c == 0xED ? 0x9F : 0xBF;
-        return n >= 3 && p[1] >= lo && p[1] <= hi && (p[2] & 0xC0) == 0x80 ? 3 : 1;
-    }
-    if (c <= 0xF4) {
-        const uint8_t lo = c == 0xF0 ? 0x90 : 0x80, hi = c == 0xF4 ? 0x8F : 0xBF;
-        return n >= 4 && p[1] >= lo && p[1] <= hi && (p[2] & 0xC0) == 0x80 && (p[3] & 0xC0) == 0x80 ? 4 : 1;
-    }
-    return 1;
+    const uint32_t w = utf8_seq(p, n);
+    return w ? w : 1;
 }
 
 // one verb of a row: *keep = the value's bytes that are written (truncateString), returns the padding spaces (padString)
@@ -69,15 +57,6 @@ __host__ __device__ __forceinline__ uint32_t verb_layout(const uint8_t* p, uint3
     return runes < width ? width - runes : 0;
 }
 
-// the verbs of a compiled format as kernel parameters: verb v reads column off[v] / data[v]
-struct SpVerbs {
-    int n;
-    uint32_t lit_total;  // literal bytes of a row
-    const uint32_t* off[SP_MAXV];
-    const uint8_t* data[SP_MAXV];
-    uint32_t width[SP_MAXV], prec[SP_MAXV];
-    uint64_t left;       // bit v: verb v is left-aligned ('-')
-};
 // a piece of the format: verb >= 0, or the literal bytes [lit, lit + len) of the literal blob
 struct SpPiece { int32_t verb; uint32_t lit, len, pad_; };
 
@@ -162,90 +141,89 @@ static SpFormat sprintf_compile(const std::string& f, int nargs) {
     return r;
 }
 
-__device__ __forceinline__ uint64_t sprintf_row_len(const SpVerbs& sv, uint64_t r) {
-    uint64_t total = sv.lit_total;
-    for (int v = 0; v < sv.n; v++) {
-        const uint32_t s = sv.off[v][r], l = sv.off[v][r + 1] - s;
-        uint32_t keep;
-        const uint32_t pad = verb_layout(sv.data[v] + s, l, sv.width[v], sv.prec[v], &keep);
-        total += (uint64_t)keep + pad;
-    }
-    return total;
-}
-
-__global__ void sprintf_len_kernel(const SpVerbs sv, uint64_t n, uint32_t* __restrict__ len) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const uint64_t total = sprintf_row_len(sv, r);
-    len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
-}
-
-constexpr int SW_WARPS = 8;
 constexpr uint32_t SW_STAGE = 4096;
-__global__ void __launch_bounds__(SW_WARPS * 32) sprintf_write_kernel(const SpVerbs sv, const SpPiece* __restrict__ gpieces, int npieces,
-                                                                      const uint8_t* __restrict__ glit, uint64_t n,
-                                                                      const uint32_t* __restrict__ pos, uint8_t* out) {
-    __shared__ __align__(16) uint8_t stage_all[SW_WARPS][SW_STAGE + 16];
-    __shared__ SpPiece pieces[SP_MAXP];
-    __shared__ uint8_t lit[SP_MAXLIT];
-    for (int i = threadIdx.x; i < npieces; i += blockDim.x) pieces[i] = gpieces[i];
-    for (uint32_t i = threadIdx.x; i < sv.lit_total; i += blockDim.x) lit[i] = glit[i];
-    __syncthreads();
-    warp_write_rows<SW_WARPS, SW_STAGE>(&stage_all[0][0], n, pos, out, [&](uint64_t r, uint8_t* q) {
+// a row: the pieces of a compiled format; verb v reads column off[v] / data[v].  Every block copies the piece table and
+// the literal bytes into shared memory, at their largest size whatever the format.
+struct SprintfRows {
+    int n;
+    uint32_t lit_total;  // literal bytes of a row
+    const uint32_t* off[SP_MAXV];
+    const uint8_t* data[SP_MAXV];
+    uint32_t width[SP_MAXV], prec[SP_MAXV];
+    uint64_t left;       // bit v: verb v is left-aligned ('-')
+    const SpPiece* pieces; int npieces;
+    const uint8_t* lit;
+
+    __device__ uint64_t len(uint64_t r) const {
+        uint64_t total = lit_total;
+        for (int v = 0; v < n; v++) {
+            const uint32_t s = off[v][r], l = off[v][r + 1] - s;
+            uint32_t keep;
+            const uint32_t pad = verb_layout(data[v] + s, l, width[v], prec[v], &keep);
+            total += (uint64_t)keep + pad;
+        }
+        return total;
+    }
+
+    struct Tables { const SpPiece* pieces; const uint8_t* lit; };
+    static constexpr uint32_t TABLE_BYTES = SP_MAXP * sizeof(SpPiece) + SP_MAXLIT;
+    static constexpr bool TAIL_VARIES = false;
+    uint32_t tail() const { return TABLE_BYTES; }
+    __device__ Tables stage(uint8_t* sm) const {
+        SpPiece* sp = reinterpret_cast<SpPiece*>(sm);
+        uint8_t* sl = sm + SP_MAXP * sizeof(SpPiece);
+        for (int i = threadIdx.x; i < npieces; i += blockDim.x) sp[i] = pieces[i];
+        for (uint32_t i = threadIdx.x; i < lit_total; i += blockDim.x) sl[i] = lit[i];
+        __syncthreads();
+        return {sp, sl};
+    }
+
+    __device__ void write(uint64_t r, uint8_t* q, const Tables& t) const {
         for (int k = 0; k < npieces; k++) {
-            const SpPiece pc = pieces[k];
+            const SpPiece pc = t.pieces[k];
             if (pc.verb < 0) {
-                for (uint32_t i = 0; i < pc.len; i++) *q++ = lit[pc.lit + i];
+                for (uint32_t i = 0; i < pc.len; i++) *q++ = t.lit[pc.lit + i];
                 continue;
             }
             const int v = pc.verb;
-            const uint32_t s = sv.off[v][r], l = sv.off[v][r + 1] - s;
-            const uint8_t* p = sv.data[v] + s;
+            const uint32_t s = off[v][r], l = off[v][r + 1] - s;
+            const uint8_t* p = data[v] + s;
             uint32_t keep;
-            const uint32_t pad = verb_layout(p, l, sv.width[v], sv.prec[v], &keep);
-            const bool left = (sv.left >> v) & 1;
-            if (!left) for (uint32_t i = 0; i < pad; i++) *q++ = ' ';
+            const uint32_t pad = verb_layout(p, l, width[v], prec[v], &keep);
+            const bool left_aligned = (left >> v) & 1;
+            if (!left_aligned) for (uint32_t i = 0; i < pad; i++) *q++ = ' ';
             for (uint32_t i = 0; i < keep; i++) *q++ = p[i];
-            if (left) for (uint32_t i = 0; i < pad; i++) *q++ = ' ';
+            if (left_aligned) for (uint32_t i = 0; i < pad; i++) *q++ = ' ';
         }
-    });
-}
-
-// lengths, scan and the one readback: *body = the exact total; len (n + 1 entries) then holds the offsets
-static uint64_t sprintf_sizes(Ctx* c, const SpVerbs& sv, uint64_t n, uint32_t* len, const char* what) {
-    Buf tot = dev_alloc(c, 8);
-    if (n) {
-        KernelTimer kt(c, "sprintf_len", n * 4 * (sv.n + 1));
-        sprintf_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(sv, n, len);
-        CPB_CUDA(cudaGetLastError());
     }
-    exclusive_scan_u32(c, len, len, n, tot->as<uint64_t>());
-    const uint64_t body = read_back<uint64_t>(c, tot->p);
-    if (body > 0xffffffffull || (n == 1 && body == 0xffffffffull))
-        throw DataError{CPB_E_TOO_LARGE, -1, 0, false, std::string(what) + " would hold 4 GiB or more: format row-range slices"};
-    return body;
+};
+
+// the lengths of the n rows into len (n + 1 entries), which then holds the offsets; returns the exact total
+static uint64_t sprintf_sizes(Ctx* c, const SprintfRows& rows, uint64_t n, uint32_t* len, const std::string& what) {
+    Buf tot = dev_alloc(c, 8);
+    row_lengths(c, rows, n, len, "sprintf_len", n * 4 * (rows.n + 1));
+    return row_offsets(c, len, n, tot->as<uint64_t>(), 1, MAX_BODY, what + " would hold 4 GiB or more: format row-range slices")[0];
 }
 
-static void sprintf_write(Ctx* c, const SpFormat& f, const SpVerbs& sv, uint64_t n, const uint32_t* pos, uint64_t body, uint8_t* out) {
+static void sprintf_write(Ctx* c, const SpFormat& f, SprintfRows rows, uint64_t n, const uint32_t* pos, uint64_t body, uint8_t* out) {
     if (!n) return;
     const size_t pbytes = f.pieces.size() * sizeof(SpPiece);
     Buf meta = dev_alloc(c, pbytes + f.lit.size());
     // (pageable source: the copy is staged before the call returns, so the host table may go away)
     CPB_CUDA(cudaMemcpyAsync(meta->p, f.pieces.data(), pbytes, cudaMemcpyHostToDevice, c->stream));
     if (!f.lit.empty()) CPB_CUDA(cudaMemcpyAsync(meta->as<uint8_t>() + pbytes, f.lit.data(), f.lit.size(), cudaMemcpyHostToDevice, c->stream));
-    KernelTimer kt(c, "sprintf_write", 2 * body + n * 4 * (sv.n + 1));
-    const uint32_t wblocks = (uint32_t)std::min<uint64_t>((n + SW_WARPS * 32 - 1) / (SW_WARPS * 32), (uint64_t)c->sm_count * 16);
-    sprintf_write_kernel<<<wblocks, SW_WARPS * 32, 0, c->stream>>>(sv, meta->as<SpPiece>(), (int)f.pieces.size(), meta->as<uint8_t>() + pbytes,
-                                                                   n, pos, out);
-    CPB_CUDA(cudaGetLastError());
+    rows.pieces = meta->as<SpPiece>();
+    rows.npieces = (int)f.pieces.size();
+    rows.lit = meta->as<uint8_t>() + pbytes;
+    row_write<SW_STAGE>(c, rows, n, pos, out, "sprintf_write", 2 * body + n * 4 * (rows.n + 1), 16);
 }
 
 // the format compiled for the columns `names` of t, and their positions in t.  A column t lacks is Row.SelectValues's
 // `missing column %q` (csvplus.go:138-149), for a table with rows only: as ToCsv reports it (column index, row 0) for a
 // sink, as column_as_int64 does (no row) for a computed column.
-static SpVerbs sprintf_prepare(const Table& t, const std::string& format, const std::vector<std::string>& names, bool sink, SpFormat& f) {
+static SprintfRows sprintf_prepare(const Table& t, const std::string& format, const std::vector<std::string>& names, bool sink, SpFormat& f) {
     f = sprintf_compile(format, (int)names.size());
-    SpVerbs sv{};
+    SprintfRows sv{};
     sv.n = f.nverbs;
     sv.lit_total = (uint32_t)f.lit.size();
     sv.left = f.left;
@@ -265,12 +243,12 @@ static SpVerbs sprintf_prepare(const Table& t, const std::string& format, const 
 std::shared_ptr<Table> table_set_sprintf(Ctx* c, const Table& t, const std::string& name, const std::string& format,
                                          const std::vector<std::string>& cols) {
     SpFormat f;
-    const SpVerbs sv = sprintf_prepare(t, format, cols, false, f);
+    const SprintfRows sv = sprintf_prepare(t, format, cols, false, f);
     const uint64_t n = (uint64_t)t.nrows;
     if (n == 0) return with_column(t, name, empty_column(c));
     Column col;
     col.offsets = dev_alloc(c, (n + 1) * 4);
-    const uint64_t body = sprintf_sizes(c, sv, n, col.offsets->as<uint32_t>(), ("column " + go_quote(name)).c_str());
+    const uint64_t body = sprintf_sizes(c, sv, n, col.offsets->as<uint32_t>(), "column " + go_quote(name));
     col.data = dev_alloc(c, body + 16);
     sprintf_write(c, f, sv, n, col.offsets->as<uint32_t>(), body, col.data->as<uint8_t>());
     return with_column(t, name, col);
@@ -278,7 +256,7 @@ std::shared_ptr<Table> table_set_sprintf(Ctx* c, const Table& t, const std::stri
 
 Buf table_sprintf(Ctx* c, const Table& t, const std::string& format, const std::vector<std::string>& cols, uint64_t room, uint64_t* nbytes) {
     SpFormat f;
-    const SpVerbs sv = sprintf_prepare(t, format, cols, true, f);
+    const SprintfRows sv = sprintf_prepare(t, format, cols, true, f);
     const uint64_t n = (uint64_t)t.nrows;
     Buf len = dev_alloc(c, (n + 1) * 4);
     const uint64_t body = sprintf_sizes(c, sv, n, len->as<uint32_t>(), "Sprintf output");

@@ -2,16 +2,13 @@
 // encoding/csv.Writer (comma ',', UseCRLF=false; SURVEY App. B): header line, then one line per row
 // with the named columns in caller order.  A field is quoted iff it is non-empty and (it is `\.` or
 // contains , " \r \n or its first rune is unicode.IsSpace); inside quotes " is doubled.
-// Two kernels: per-row output length -> exclusive scan -> serialisation through warp_write_rows (rowwrite.cuh).
-#include <algorithm>
-
+// The row type CsvRows through the row serialiser driver of rowwrite.cuh.
 #include "core.hpp"
 #include "rowwrite.cuh"
 
 namespace cpb {
 
 constexpr int MAXW = 64;  // columns per ToCsv call
-struct WriteCols { int n; const uint32_t* off[MAXW]; const uint8_t* data[MAXW]; };
 
 __host__ __device__ inline bool first_rune_is_space(const uint8_t* p, uint32_t n) {
     uint8_t c = p[0];
@@ -49,32 +46,28 @@ __host__ __device__ inline uint32_t field_write(const uint8_t* p, uint32_t n, ui
     return k;
 }
 
-// len[r] = output bytes of row r, saturated at 0xFFFFFFFF (the host then reports CPB_E_TOO_LARGE): a row of quotes
-// doubles in length, and a column may be named more than once
-__global__ void csv_row_len_kernel(WriteCols wc, uint64_t n, uint32_t* len) {
-    uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    uint64_t total = (uint64_t)wc.n;  // n-1 commas + newline
-    for (int k = 0; k < wc.n; k++) {
-        uint32_t s = wc.off[k][r], l = wc.off[k][r + 1] - s;
-        bool q;
-        total += field_out_len(wc.data[k] + s, l, &q);
+// a row: the named columns in caller order, each field through the quoting rule, then '\n'.  A row of quotes doubles
+// in length, and a column may be named more than once.
+struct CsvRows : NoTables {
+    int n; const uint32_t* off[MAXW]; const uint8_t* data[MAXW];
+    __device__ uint64_t len(uint64_t r) const {
+        uint64_t total = (uint64_t)n;  // n-1 commas + newline
+        for (int k = 0; k < n; k++) {
+            const uint32_t s = off[k][r], l = off[k][r + 1] - s;
+            bool q;
+            total += field_out_len(data[k] + s, l, &q);
+        }
+        return total;
     }
-    len[r] = total > 0xffffffffull ? 0xffffffffu : (uint32_t)total;
-}
-constexpr int CW_WARPS = 8;
-constexpr int CW_STAGE = 4096;
-__global__ void __launch_bounds__(CW_WARPS * 32) csv_row_write_kernel(WriteCols wc, uint64_t n, const uint32_t* __restrict__ pos, uint8_t* out) {
-    __shared__ __align__(16) uint8_t stage_all[CW_WARPS][CW_STAGE + 16];
-    warp_write_rows<CW_WARPS, CW_STAGE>(&stage_all[0][0], n, pos, out, [&](uint64_t r, uint8_t* q) {
-        for (int k = 0; k < wc.n; k++) {
+    __device__ void write(uint64_t r, uint8_t* q, Tables) const {
+        for (int k = 0; k < n; k++) {
             if (k) *q++ = ',';
-            const uint32_t s = wc.off[k][r], l = wc.off[k][r + 1] - s;
-            q += field_write(wc.data[k] + s, l, q);
+            const uint32_t s = off[k][r], l = off[k][r + 1] - s;
+            q += field_write(data[k] + s, l, q);
         }
         *q = '\n';
-    });
-}
+    }
+};
 
 Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std::vector<std::string>& names, bool with_header,
                  uint64_t room, uint64_t* nbytes) {
@@ -89,29 +82,18 @@ Buf table_to_csv(Ctx* c, const Table& t, const std::vector<int>& cols, const std
     }
     if (with_header) header += '\n';
     const uint64_t n = (uint64_t)t.nrows;
-    WriteCols wc{};
-    wc.n = (int)cols.size();
-    for (int k = 0; k < wc.n && n; k++) { wc.off[k] = t.cols[cols[k]].off(); wc.data[k] = t.cols[cols[k]].bytes(); }
+    CsvRows rows{};
+    rows.n = (int)cols.size();
+    for (int k = 0; k < rows.n && n; k++) { rows.off[k] = t.cols[cols[k]].off(); rows.data[k] = t.cols[cols[k]].bytes(); }
     Buf len = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8);
-    if (n) {
-        KernelTimer kt(c, "csv_row_len", n * 4 * (wc.n + 1));
-        csv_row_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(wc, n, len->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
-    }
-    exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), n, tot->as<uint64_t>());
-    const uint64_t body = read_back<uint64_t>(c, tot->p);
-    // (one row of 0xFFFFFFFF bytes may be a saturated longer one: refused as well)
-    if (body > 0xffffffffull || (n == 1 && body == 0xffffffffull)) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "ToCsv output exceeds 4 GiB; write in smaller batches"};
+    row_lengths(c, rows, n, len->as<uint32_t>(), "csv_row_len", n * 4 * (rows.n + 1));
+    const uint64_t body = row_offsets(c, len->as<uint32_t>(), n, tot->as<uint64_t>(), 1, MAX_BODY,
+                                      "ToCsv output exceeds 4 GiB; write in smaller batches")[0];
     *nbytes = header.size() + body;
     if (*nbytes > room) return nullptr;
     Buf out = dev_alloc(c, header.size() + body + 16);
     CPB_CUDA(cudaMemcpyAsync(out->p, header.data(), header.size(), cudaMemcpyHostToDevice, c->stream));
-    if (n) {
-        KernelTimer kt(c, "csv_write", 2 * body + n * 4 * (wc.n + 1));
-        const uint32_t wblocks = (uint32_t)std::min<uint64_t>((n + CW_WARPS * 32 - 1) / (CW_WARPS * 32), (uint64_t)c->sm_count * 16);
-        csv_row_write_kernel<<<wblocks, CW_WARPS * 32, 0, c->stream>>>(wc, n, len->as<uint32_t>(), out->as<uint8_t>() + header.size());
-        CPB_CUDA(cudaGetLastError());
-    }
+    row_write<4096>(c, rows, n, len->as<uint32_t>(), out->as<uint8_t>() + header.size(), "csv_write", 2 * body + n * 4 * (rows.n + 1), 16);
     return out;
 }
 
