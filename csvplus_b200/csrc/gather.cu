@@ -351,6 +351,9 @@ __global__ void __launch_bounds__(256) rowhash_probe_kernel(KeyDesc kd, uint64_t
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x) {
         unsigned long long k0; uint32_t k1;
         uint64_t s = rh_start(kd, i, nslots, k0, k1);
+#ifdef RH_DIAG_SEQ_SLOT  // diagnostic (tools/prof_rowhash.py): a sequential slot instead of the key's
+        s = i % nslots;
+#endif
         uint4 h = rh_header(slots, s), v = __ldg(&slots[s].pay);  // one sector, both halves
         const uint64_t s0 = s;
         const bool found = rh_walk(slots, rmask, k0, k1, s, h);

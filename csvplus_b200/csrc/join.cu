@@ -334,8 +334,9 @@ static void search_probe(Ctx* c, const Table& probe, const std::vector<int>& pid
 struct PayCols { int nc; const uint32_t* off[RH_MAXC]; const uint8_t* data[RH_MAXC]; };
 __global__ void __launch_bounds__(256) rowhash_scatter_kernel(KeyDesc kd, PayCols pc, uint64_t n, RowSlot* slots, uint64_t nslots,
                                                               uint32_t rshift, uint32_t* fill) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
+    const uint64_t r0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r0 - (threadIdx.x & 31u) >= n) return;  // whole warps only: pairs of lanes exchange their images below
+    const uint64_t r = r0 < n ? r0 : n - 1;     // (a row past n is read, not stored)
     unsigned long long w0, w1, w2;
     pack3(kd, r, w0, w1, w2);
     unsigned long long pa = 0, pb = 0;
@@ -350,12 +351,37 @@ __global__ void __launch_bounds__(256) rowhash_scatter_kernel(KeyDesc kd, PayCol
         hdr |= l << (5 * j);
         pos += l;
     }
+#ifdef RH_DIAG_NO_PAYLOAD  // diagnostic (tools/prof_rowhash.py): the key alone
+    pa = pb = 0; hdr = RH_OCCUPIED;
+#endif
     const uint64_t g = slot_of(hash3(w0, w1, 0ull), nslots) >> rshift;
-    const uint32_t p = atomicAdd(&fill[g], 1u);
-    if (p >> rshift) return;  // the region overflows: rowhash_region reports it
+#ifdef RH_DIAG_NO_ATOMIC  // diagnostic: the position from the row number, the fill counts untouched
+    const uint32_t p = (uint32_t)r & ((1u << rshift) - 1u);
+#else
+    const uint32_t p = r0 < n ? atomicAdd(&fill[g], 1u) : ~0u;
+#endif
+    bool ok = r0 < n && !(p >> rshift);  // a region given more than it holds: rowhash_region reports it
+#ifdef RH_DIAG_NO_STORE  // diagnostic: no image store (kept live by a store no row makes)
+    ok = ok && ((pa ^ pb ^ w0) + hdr) == 0x9E3779B97F4A7C15ull;
+#endif
+    // A row's image is one 32-byte sector.  Written as two 16-byte halves by one lane, each store instruction of a warp
+    // sends 32 half sectors to L2; instead lanes 2i and 2i + 1 write lane 2i's image in the first store and lane
+    // 2i + 1's in the second, so each store is 16 whole sectors (one shuffle of the half each lane lacks).  Evict-last:
+    // a region's frontier line stays in L2 until its later images fill it.
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
     uint4* d = reinterpret_cast<uint4*>(&slots[(g << rshift) + p]);
-    d[0] = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)(w1 >> 32), hdr);
-    d[1] = make_uint4((uint32_t)pa, (uint32_t)(pa >> 32), (uint32_t)pb, (uint32_t)(pb >> 32));
+    const uint4 h4 = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)(w1 >> 32), hdr);
+    const uint4 p4 = make_uint4((uint32_t)pa, (uint32_t)(pa >> 32), (uint32_t)pb, (uint32_t)(pb >> 32));
+    const bool odd = threadIdx.x & 1u;
+    uint4 x = odd ? h4 : p4;  // what the other lane of the pair stores: the odd lane's header, the even lane's payload
+    x.x = __shfl_xor_sync(~0u, x.x, 1); x.y = __shfl_xor_sync(~0u, x.y, 1); x.z = __shfl_xor_sync(~0u, x.z, 1); x.w = __shfl_xor_sync(~0u, x.w, 1);
+    uint4* dp = reinterpret_cast<uint4*>(__shfl_xor_sync(~0u, reinterpret_cast<unsigned long long>(d), 1));
+    const bool okp = __shfl_xor_sync(~0u, ok ? 1u : 0u, 1) != 0u;
+    uint4* d1 = odd ? dp + 1 : d; const uint4 v1 = odd ? x : h4; const bool ok1 = odd ? okp : ok;  // the even lane's row
+    uint4* d2 = odd ? d + 1 : dp; const uint4 v2 = odd ? p4 : x; const bool ok2 = odd ? ok : okp;  // the odd lane's row
+    if (ok1) asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(d1), "r"(v1.x), "r"(v1.y), "r"(v1.z), "r"(v1.w), "l"(pol) : "memory");
+    if (ok2) asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(d2), "r"(v2.x), "r"(v2.y), "r"(v2.z), "r"(v2.w), "l"(pol) : "memory");
 }
 constexpr int RH_THREADS = 256, RH_UNROLL = 2;  // staged images in flight per thread
 __global__ void __launch_bounds__(RH_THREADS) rowhash_region_kernel(RowSlot* slots, uint64_t nslots, uint64_t nregions, uint32_t rshift,
