@@ -164,29 +164,6 @@ __global__ void __launch_bounds__(CW_WARPS * 32) codes_insert_kernel(const ValCo
     }
 }
 
-__global__ void codes_flags_kernel(const uint32_t* __restrict__ slots, uint64_t n, uint32_t* rep, uint32_t* __restrict__ flags) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint32_t f = slots[rep[i]];
-    rep[i] = f;
-    flags[i] = f == (uint32_t)i;
-}
-
-__global__ void codes_write_kernel(const uint32_t* __restrict__ rep, const uint32_t* __restrict__ pos, uint64_t n, int64_t* __restrict__ codes) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) codes[i] = pos[rep[i]];
-}
-
-__global__ void codes_check_kernel(const int64_t* __restrict__ codes, uint64_t n, uint64_t nd, uint32_t* __restrict__ ids,
-                                   unsigned long long* bad) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int64_t k = codes[i];
-    const bool ok = k >= 0 && (uint64_t)k < nd;
-    ids[i] = ok ? (uint32_t)k : 0;
-    if (!ok) atomicMin(bad, (unsigned long long)i);
-}
-
 std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* codes) {
     const uint64_t n = (uint64_t)t.nrows;
     const std::vector<int> pick{col};
@@ -212,10 +189,17 @@ std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* co
                                                                       rep->as<uint32_t>());
         CPB_CUDA(cudaGetLastError());
     }
+    uint32_t* r = rep->as<uint32_t>();
     {
+        // r[i] = the first row of row i's value; flags: the rows that are first
         KernelTimer kt(c, "codes_flags", n * 16);
-        codes_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(slots->as<uint32_t>(), n, rep->as<uint32_t>(), flags->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
+        const uint32_t* sl = slots->as<uint32_t>();
+        uint32_t* fl = flags->as<uint32_t>();
+        each_row(c, n, [=] __device__(uint64_t i) {
+            const uint32_t f = sl[r[i]];
+            r[i] = f;
+            fl[i] = f == (uint32_t)i;
+        });
     }
     const FlagScan s = scan_flags(c, flags->as<uint32_t>(), n);
     Buf first = dev_alloc(c, (s.count + 1) * 4);
@@ -225,8 +209,8 @@ std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* co
     }
     {
         KernelTimer kt(c, "codes_write", n * 16);
-        codes_write_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(rep->as<uint32_t>(), s.pos->as<uint32_t>(), n, codes);
-        CPB_CUDA(cudaGetLastError());
+        const uint32_t* pos = s.pos->as<uint32_t>();
+        each_row(c, n, [=] __device__(uint64_t i) { codes[i] = pos[r[i]]; });
     }
     if (s.count == n) {  // every value distinct: the column is its own dictionary; the codes are complete on return
         sync_stream(c);
@@ -245,9 +229,16 @@ std::shared_ptr<Table> table_set_codes(Ctx* c, const Table& t, const std::string
     Buf ids = dev_alloc(c, n * 4), bad = dev_alloc(c, 8);
     CPB_CUDA(cudaMemsetAsync(bad->p, 0xff, 8, c->stream));
     {
+        // ids[i] = code i, or 0 where it is outside the dictionary; *first_bad = the first such row
         KernelTimer kt(c, "codes_check", n * 12);
-        codes_check_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(codes, n, nd, ids->as<uint32_t>(), (unsigned long long*)bad->p);
-        CPB_CUDA(cudaGetLastError());
+        uint32_t* id = ids->as<uint32_t>();
+        unsigned long long* first_bad = (unsigned long long*)bad->p;
+        each_row(c, n, [=] __device__(uint64_t i) {
+            const int64_t k = codes[i];
+            const bool ok = k >= 0 && (uint64_t)k < nd;
+            id[i] = ok ? (uint32_t)k : 0;
+            if (!ok) atomicMin(first_bad, (unsigned long long)i);
+        });
     }
     const uint64_t row = read_back<uint64_t>(c, bad->p);
     if (row != ~0ull) {

@@ -19,6 +19,7 @@
 #include <mutex>
 
 #include "core.hpp"
+#include "util.cuh"
 
 namespace cpb {
 
@@ -82,16 +83,6 @@ NcclApi& nccl() {
 struct Seg { uint64_t row_base, byte_base, rows, first_off; };
 constexpr int MAX_RANKS = 64;
 struct RebaseParams { int nranks; Seg seg[MAX_RANKS]; uint64_t total_rows, total_bytes; };
-
-// out[row_base_q + i] = in_q[i] - first_off_q + byte_base_q ; out[total_rows] = total_bytes
-__global__ void gather_rebase_kernel(uint32_t* off, RebaseParams rp) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i > rp.total_rows) return;
-    if (i == rp.total_rows) { off[i] = (uint32_t)rp.total_bytes; return; }
-    int q = 0;
-    while (q + 1 < rp.nranks && i >= rp.seg[q + 1].row_base) q++;
-    off[i] = (uint32_t)((uint64_t)off[i] - rp.seg[q].first_off + rp.seg[q].byte_base);
-}
 
 // meta per column: (first offset, end offset) of the rows of this view
 constexpr int MAX_GATHER_COLS = 128;
@@ -202,8 +193,13 @@ void job_finish(GatherJob& j) {
         for (int q = 0; q < R; q++)
             rp.seg[q] = Seg{row_base[q], byte_base[(size_t)k * (R + 1) + q], j.meta[(size_t)q * M], j.meta[(size_t)q * M + 1 + 2 * k]};
         KernelTimer kt(c, "gather_rebase", (row_base[R] + 1) * 8);
-        gather_rebase_kernel<<<nblk(row_base[R] + 1, 256), 256, 0, c->stream>>>(j.out->cols[k].offsets->as<uint32_t>(), rp);
-        CPB_CUDA(cudaGetLastError());
+        // off[row_base_q + i] = in_q[i] - first_off_q + byte_base_q ; off[total_rows] = total_bytes
+        uint32_t* off = j.out->cols[k].offsets->as<uint32_t>();
+        each_row(c, rp.total_rows + 1, [=] __device__(uint64_t i) {
+            int q = 0;
+            while (q + 1 < rp.nranks && i >= rp.seg[q + 1].row_base) q++;
+            off[i] = i == rp.total_rows ? (uint32_t)rp.total_bytes : (uint32_t)((uint64_t)off[i] - rp.seg[q].first_off + rp.seg[q].byte_base);
+        });
         moved += rp.total_bytes + rp.total_rows * 4;
     }
     if (c->stats_on) { c->stats["allgather_bytes"].bytes += moved; c->stats["allgather_bytes"].launches += 1; }

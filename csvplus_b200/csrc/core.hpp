@@ -327,6 +327,8 @@ void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, u
 struct FlagScan { const uint32_t* flags; uint64_t n; Buf pos; uint64_t count; };  // pos: uint32[n + 1] exclusive scan
 FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n);
 void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out);
+// flag[i] (uint32 0/1) = whether v[i] is nonzero (nonzero) / is zero (!nonzero)
+void nonzero_flags(Ctx* c, const uint32_t* v, uint64_t n, bool nonzero, uint32_t* flag);
 // rows row_ids[0, nout) of t (rows 0..nout-1 when row_ids is null: a view compacted into buffers of its own)
 std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout);
 // the rows of t whose flag (uint32 0/1, one per row) is set: scan_flags, compact_flags timed as compact_ids, gather_rows.
@@ -369,6 +371,7 @@ void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const s
 uint32_t prefix_bytes(const Index& ix, int nk);  // image bytes covered by the first nk key columns
 // head[i] = 1 when the first pbytes image bytes of row i differ from those of row i - 1 (row 0 always)
 void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head);
+void iota_u32(Ctx* c, uint32_t* p, uint64_t n);  // p[i] = i for i in [0, n)
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
 // join.cu.  A join column missing from a non-empty probe table throws DataError.
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti);

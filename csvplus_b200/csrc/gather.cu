@@ -133,10 +133,9 @@ void exclusive_scan_u32(Ctx* c, const uint32_t* in, uint32_t* out, uint64_t n, u
 }
 
 // ------------------------------------------------------------------ compaction of flags (scan_flags / compact_flags)
-__global__ void compact_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t* out, uint64_t n, uint32_t add) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) out[pos[i]] = (uint32_t)i + add;
-    if (i == 0) out[pos[n]] = (uint32_t)n + add;  // sentinel: the end of the last run when the flags mark run heads
+void nonzero_flags(Ctx* c, const uint32_t* v, uint64_t n, bool nonzero, uint32_t* flag) {
+    const uint32_t want = nonzero ? 1u : 0u;  // (captured as a word: a captured bool compiles to two more instructions)
+    each_row(c, n, [=] __device__(uint64_t i) { flag[i] = (v[i] != 0) == (want != 0) ? 1u : 0u; });
 }
 FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n) {
     FlagScan s{flags, n, dev_alloc(c, (n + 1) * 4), 0};
@@ -146,9 +145,13 @@ FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n) {
     return s;
 }
 void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out) {
-    if (s.n == 0) return;
-    compact_kernel<<<nblk(s.n, 256), 256, 0, c->stream>>>(s.flags, s.pos->as<uint32_t>(), out, s.n, add);
-    CPB_CUDA(cudaGetLastError());
+    const uint32_t *flags = s.flags, *pos = s.pos->as<uint32_t>();
+    const uint64_t n = s.n;
+    const uint32_t end = (uint32_t)n + add;  // sentinel: the end of the last run when the flags mark run heads
+    each_row(c, n, [=] __device__(uint64_t i) {
+        if (flags[i]) out[pos[i]] = (uint32_t)i + add;
+        if (i == 0) out[pos[n]] = end;
+    });
 }
 
 // ------------------------------------------------------------------ gather by row ids
@@ -926,11 +929,6 @@ void filter_parsed(Ctx* c, Parsed& p, const cpb_pred* pred, std::shared_ptr<Comp
 }
 
 // ------------------------------------------------------------------ concat
-__global__ void rebase_offsets_kernel(const uint32_t* __restrict__ in, uint32_t* out, uint64_t n, uint32_t add) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i <= n) out[i] = in[i] - in[0] + add;  // also writes the sentinel (overwritten by the next part's first entry: same value)
-}
-
 std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& parts) {
     const Table& first = *parts[0];
     for (auto* p : parts) {
@@ -964,8 +962,11 @@ std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& pa
             uint32_t b0 = ext[2 * (p * K + k)], b1 = ext[2 * (p * K + k) + 1];
             uint64_t pr = (uint64_t)parts[p]->nrows;
             KernelTimer kt(c, "concat", (uint64_t)(b1 - b0) * 2 + pr * 8);
-            rebase_offsets_kernel<<<nblk(pr + 1, 256), 256, 0, c->stream>>>(parts[p]->cols[k].off(), col.offsets->as<uint32_t>() + row, pr, (uint32_t)byte);
-            CPB_CUDA(cudaGetLastError());
+            // the part's offsets rebased to where its bytes go, its end included (the next part's first entry: same value)
+            const uint32_t* in = parts[p]->cols[k].off();
+            uint32_t* out = col.offsets->as<uint32_t>() + row;
+            const uint32_t add = (uint32_t)byte;
+            each_row(c, pr + 1, [=] __device__(uint64_t i) { out[i] = in[i] - in[0] + add; });
             if (b1 > b0) CPB_CUDA(cudaMemcpyAsync(col.data->as<uint8_t>() + byte, parts[p]->cols[k].bytes() + b0, b1 - b0, cudaMemcpyDeviceToDevice, c->stream));
             row += pr; byte += b1 - b0;
         }

@@ -83,18 +83,20 @@ __device__ void emit_row(const GenParams& g, uint64_t row, Emit& e) {
     e.ch('\n');
 }
 
-__global__ void gen_len_kernel(GenParams g, uint32_t* len) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g.row_lo + i >= g.row_hi) return;
-    Emit e{nullptr};
-    emit_row(g, g.row_lo + i, e);
-    len[i] = e.n;
+static void gen_lengths(Ctx* c, const GenParams& g, uint32_t* len) {
+    each_row(c, g.row_hi - g.row_lo, [=] __device__(uint64_t i) {
+        Emit e{nullptr};
+        emit_row(g, g.row_lo + i, e);
+        len[i] = e.n;
+    });
 }
-__global__ void gen_write_kernel(GenParams g, const uint32_t* __restrict__ off, uint8_t* dst) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g.row_lo + i >= g.row_hi) return;
-    Emit e{dst + g.header_len + off[i]};
-    emit_row(g, g.row_lo + i, e);
+// the rows at dst + header_len + off[i] (off: the scanned lengths)
+static void gen_write(Ctx* c, const GenParams& g, const uint32_t* off, uint8_t* dst) {
+    uint8_t* body = dst + g.header_len;
+    each_row(c, g.row_hi - g.row_lo, [=] __device__(uint64_t i) {
+        Emit e{body + off[i]};
+        emit_row(g, g.row_lo + i, e);
+    });
 }
 
 }  // namespace cpb
@@ -122,10 +124,7 @@ extern "C" int cpb_gen_csv(cpb_ctx* h, int kind, uint64_t seed, uint64_t row_lo,
         }
         const uint64_t rows = row_hi - row_lo;
         Buf len = dev_alloc(c, (rows + 1) * 4), total = dev_alloc(c, 8);
-        if (rows) {
-            gen_len_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>());
-            CPB_CUDA(cudaGetLastError());
-        }
+        gen_lengths(c, gp, len->as<uint32_t>());
         exclusive_scan_u32(c, len->as<uint32_t>(), len->as<uint32_t>(), rows, total->as<uint64_t>());
         const uint64_t body = read_back<uint64_t>(c, total->p);
         if (body > 0xffffffffull) throw ArgError{CPB_ERR_ARG, "generate at most 4 GiB per call (split the row range)"};
@@ -133,10 +132,7 @@ extern "C" int cpb_gen_csv(cpb_ctx* h, int kind, uint64_t seed, uint64_t row_lo,
         if (dst) {
             if (*nbytes > cap) throw ArgError{CPB_ERR_ARG, "generator destination too small"};
             if (gp.header_len) CPB_CUDA(cudaMemcpyAsync(dst, headers[kind], gp.header_len, cudaMemcpyHostToDevice, c->stream));
-            if (rows) {
-                gen_write_kernel<<<nblk(rows, 256), 256, 0, c->stream>>>(gp, len->as<uint32_t>(), (uint8_t*)dst);
-                CPB_CUDA(cudaGetLastError());
-            }
+            gen_write(c, gp, len->as<uint32_t>(), (uint8_t*)dst);
             sync_stream(c);
         }
         return CPB_OK;

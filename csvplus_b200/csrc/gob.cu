@@ -274,18 +274,6 @@ __global__ void gob_cand_kernel(const uint8_t* __restrict__ b, uint64_t L, uint6
     for (uint64_t x = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; x < w; x += (uint64_t)gridDim.x * blockDim.x)
         flag[x] = gob_row_end(b, L, s + x, ks, nullptr, nullptr, 0, 0) != 0 ? 1u : 0u;
 }
-// succ[i] = candidate index of the end of candidate i's row: END = C when the row ends at or past the window's end
-// (cpos[C] = w is the compaction's sentinel), DEAD when its end is not a candidate
-__global__ void gob_succ_kernel(const uint8_t* __restrict__ b, uint64_t L, uint64_t s, uint32_t w, GobKeys ks,
-                                const uint32_t* __restrict__ cpos, uint64_t C, uint32_t* succ) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= C) return;
-    const uint64_t e = gob_row_end(b, L, s + cpos[i], ks, nullptr, nullptr, 0, 0) - s;
-    if (e >= w) { succ[i] = (uint32_t)C; return; }
-    uint64_t lo = i + 1, hi = C;  // e > cpos[i]: the lower bound of e in cpos(i, C]
-    while (lo < hi) { const uint64_t h = lo + (hi - lo) / 2; if (cpos[h] < e) lo = h + 1; else hi = h; }
-    succ[i] = cpos[lo] == e ? (uint32_t)lo : GOB_DEAD;
-}
 // exit[i] = the first node past i's chunk on i's path (a later candidate, END or DEAD)
 __global__ void gob_exit_kernel(const uint32_t* __restrict__ succ, uint64_t C, uint32_t* exit) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -323,27 +311,7 @@ __global__ void gob_mark_kernel(const uint8_t* __restrict__ b, uint64_t L, uint6
         if (succ[x] == C) *next = gob_row_end(b, L, s + cpos[x], ks, nullptr, nullptr, 0, 0);
     }
 }
-__global__ void gob_rowstart_kernel(const uint32_t* __restrict__ cpos, const uint32_t* __restrict__ rid, uint64_t n, uint64_t s,
-                                    uint64_t* out) {
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < n) out[j] = s + cpos[rid[j]];
-}
-__global__ void gob_extract_kernel(const uint8_t* __restrict__ b, uint64_t L, GobKeys ks, const uint64_t* __restrict__ start, uint64_t R,
-                                   uint32_t* lens, uint64_t* vpos) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < R) gob_row_end(b, L, start[r], ks, lens, vpos, R, r);
-}
 struct GobOut { uint32_t* off; uint8_t* data; };
-__global__ void gob_copy_kernel(const uint8_t* __restrict__ b, const uint32_t* __restrict__ lens, const uint64_t* __restrict__ vpos,
-                                const GobOut* __restrict__ outs, uint32_t k, uint64_t R) {
-    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= R * k) return;
-    const uint64_t j = t / R, r = t - j * R;
-    const uint32_t l = lens[t];
-    const uint8_t* src = b + vpos[t];
-    uint8_t* d = outs[j].data + outs[j].off[r];
-    for (uint32_t i = 0; i < l; i++) d[i] = src[i];
-}
 
 // ------------------------------------------------------------------ decode, host side
 [[noreturn]] static void gob_fail(const std::string& msg) { throw DataError{CPB_E_GOB, -1, 0, false, msg}; }
@@ -506,12 +474,20 @@ std::shared_ptr<Index> gob_load(Ctx* c, const uint8_t* bytes, uint64_t nbytes, s
             CPB_CUDA(cudaMemsetAsync(mark->p, 0, C * 4 + 4, c->stream));
             CPB_CUDA(cudaMemsetAsync(st->p, 0, 16, c->stream));
             unsigned long long* ok = st->as<unsigned long long>();
+            const uint32_t* cp = cpos->as<uint32_t>();
             {
                 KernelTimer kt(c, "gob_path", C * 28, 4);
-                if (C) {
-                    gob_succ_kernel<<<nblk(C, 256), 256, 0, c->stream>>>(b, L, s, w, ks, cpos->as<uint32_t>(), C, succ->as<uint32_t>());
-                    gob_exit_kernel<<<nblk(nchunks, 128), 128, 0, c->stream>>>(succ->as<uint32_t>(), C, exits->as<uint32_t>());
-                }
+                // sc[i] = candidate index of the end of candidate i's row: END = C when the row ends at or past the window's
+                // end (cp[C] = w is the compaction's sentinel), DEAD when its end is not a candidate
+                uint32_t* sc = succ->as<uint32_t>();
+                each_row(c, C, [=] __device__(uint64_t i) {
+                    const uint64_t e = gob_row_end(b, L, s + cp[i], ks, nullptr, nullptr, 0, 0) - s;
+                    if (e >= w) { sc[i] = (uint32_t)C; return; }
+                    uint64_t lo = i + 1, hi = C;  // e > cp[i]: the lower bound of e in cp(i, C]
+                    while (lo < hi) { const uint64_t h = lo + (hi - lo) / 2; if (cp[h] < e) lo = h + 1; else hi = h; }
+                    sc[i] = cp[lo] == e ? (uint32_t)lo : GOB_DEAD;
+                });
+                if (C) gob_exit_kernel<<<nblk(nchunks, 128), 128, 0, c->stream>>>(succ->as<uint32_t>(), C, exits->as<uint32_t>());
                 gob_stitch_kernel<<<1, 1, 0, c->stream>>>(cpos->as<uint32_t>(), exits->as<uint32_t>(), C, entry->as<uint32_t>(), ok);
                 if (C)
                     gob_mark_kernel<<<nblk(nchunks, 128), 128, 0, c->stream>>>(b, L, s, ks, cpos->as<uint32_t>(), succ->as<uint32_t>(),
@@ -524,11 +500,9 @@ std::shared_ptr<Index> gob_load(Ctx* c, const uint8_t* bytes, uint64_t nbytes, s
                 gob_fail("index file: the rows do not decode as " + std::to_string(nrows) + " rows of one column set");
             Buf rid = dev_alloc(c, (ms.count + 1) * 4);
             compact_flags(c, ms, 0, rid->as<uint32_t>());
-            if (ms.count) {
-                gob_rowstart_kernel<<<nblk(ms.count, 256), 256, 0, c->stream>>>(cpos->as<uint32_t>(), rid->as<uint32_t>(), ms.count, s,
-                                                                                start->as<uint64_t>() + R);
-                CPB_CUDA(cudaGetLastError());
-            }
+            const uint32_t* row = rid->as<uint32_t>();
+            uint64_t* at = start->as<uint64_t>() + R;
+            each_row(c, ms.count, [=] __device__(uint64_t j) { at[j] = s + cp[row[j]]; });
             R += ms.count;
             s = h[1];
         }
@@ -538,7 +512,10 @@ std::shared_ptr<Index> gob_load(Ctx* c, const uint8_t* bytes, uint64_t nbytes, s
         CPB_CUDA(cudaMemsetAsync(tots->p, 0, k * 8 + 8, c->stream));
         {
             KernelTimer kt(c, "gob_extract", L + R * (8 + 12 * (uint64_t)k));
-            gob_extract_kernel<<<nblk(R, 256), 256, 0, c->stream>>>(b, L, ks, start->as<uint64_t>(), R, lens->as<uint32_t>(), vpos->as<uint64_t>());
+            const uint64_t* row_start = start->as<uint64_t>();
+            uint32_t* ln = lens->as<uint32_t>();
+            uint64_t* vp = vpos->as<uint64_t>();
+            each_row(c, R, [=] __device__(uint64_t r) { gob_row_end(b, L, row_start[r], ks, ln, vp, R, r); });
             if (k) gob_sum_kernel<<<dim3((uint32_t)std::min<uint64_t>(nblk(R, 256), (uint64_t)c->sm_count * 4), k), 256, 0, c->stream>>>(
                 lens->as<uint32_t>(), R, R, tots->as<unsigned long long>());
             CPB_CUDA(cudaGetLastError());
@@ -559,8 +536,17 @@ std::shared_ptr<Index> gob_load(Ctx* c, const uint8_t* bytes, uint64_t nbytes, s
             Buf douts = dev_alloc(c, k * sizeof(GobOut));
             CPB_CUDA(cudaMemcpyAsync(douts->p, houts.data(), k * sizeof(GobOut), cudaMemcpyHostToDevice, c->stream));
             KernelTimer kt(c, "gob_copy", 2 * all + R * k * 12);
-            gob_copy_kernel<<<nblk(R * k, 256), 256, 0, c->stream>>>(b, lens->as<uint32_t>(), vpos->as<uint64_t>(), douts->as<GobOut>(), k, R);
-            CPB_CUDA(cudaGetLastError());
+            // thread t copies the value of column t / R of row t % R
+            const uint32_t* ln = lens->as<uint32_t>();
+            const uint64_t* vp = vpos->as<uint64_t>();
+            const GobOut* outs = douts->as<GobOut>();
+            each_row(c, R * k, [=] __device__(uint64_t t) {
+                const uint64_t j = t / R, r = t - j * R;
+                const uint32_t l = ln[t];
+                const uint8_t* src = b + vp[t];
+                uint8_t* d = outs[j].data + outs[j].off[r];
+                for (uint32_t i = 0; i < l; i++) d[i] = src[i];
+            });
             sync_stream(c);  // houts is pageable host memory
         }
     } else {

@@ -165,23 +165,6 @@ __global__ void __launch_bounds__(256) join_probe16_kernel(KeyDesc kd, uint64_t 
     add_matches(not_one, matches);
 }
 
-__global__ void expand_pairs_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ pos,
-                                    uint32_t* pid, uint32_t* iid, uint64_t np) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= np) return;
-    uint32_t c = cnt[i], p = pos[i], l = lo[i];
-    for (uint32_t j = 0; j < c; j++) { pid[p + j] = (uint32_t)i; iid[p + j] = l + j; }
-}
-__global__ void found_flag_kernel(const uint32_t* __restrict__ cnt, uint32_t want, uint32_t* flag, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flag[i] = (cnt[i] != 0) == (want != 0) ? 1u : 0u;
-}
-
-__global__ void iota_heads_kernel(uint32_t* heads, uint64_t n) {  // heads[i] = i for i in [0, n]
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i <= n) heads[i] = (uint32_t)i;
-}
-
 // The order a join on the first nk key columns uses: a lazily sorted unique index joined on its full key is probed
 // over the rows as they were given (no sort needed); everything else over the sorted rows.
 static RowOrder join_order(const Index& ix, int nk) {
@@ -219,8 +202,7 @@ static ProbeTable& ensure_hash(Ctx* c, Index& ix, RowOrder order, int nk, uint32
         // no host round trip for the number of distinct keys
         ht.nheads = n;
         ht.heads = dev_alloc_owned(ix.ctx, c, (n + 1) * 4);
-        iota_heads_kernel<<<nblk(n + 1, 256), 256, 0, c->stream>>>(ht.heads->as<uint32_t>(), n);
-        CPB_CUDA(cudaGetLastError());
+        iota_u32(c, ht.heads->as<uint32_t>(), n + 1);
     } else {
         Buf head = dev_alloc(c, (n + 1) * 4);
         {
@@ -513,8 +495,7 @@ Buf key_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& i
     Buf lo = dev_alloc(c, np * 4), cnt = dev_alloc(c, (np + 1) * 4), flags = dev_alloc(c, 32);
     probe_runs(c, probe, pidx, ix, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags);
     Buf flag = dev_alloc(c, np * 4);
-    found_flag_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(cnt->as<uint32_t>(), hit ? 1u : 0u, flag->as<uint32_t>(), np);
-    CPB_CUDA(cudaGetLastError());
+    nonzero_flags(c, cnt->as<uint32_t>(), np, hit, flag->as<uint32_t>());
     return flag;
 }
 
@@ -622,10 +603,14 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     exclusive_scan_u32(c, cnt->as<uint32_t>(), pos->as<uint32_t>(), np, flags->as<uint64_t>());
     Buf pid = dev_alloc(c, m * 4), iid = dev_alloc(c, m * 4);
     {
+        // probe row i's run of index rows [lo[i], lo[i] + cnt[i]) as the pairs pos[i] onwards
         KernelTimer kt(c, "join_pairs", np * 12 + m * 8);
-        expand_pairs_kernel<<<nblk(np, 256), 256, 0, c->stream>>>(lo->as<uint32_t>(), cnt->as<uint32_t>(), pos->as<uint32_t>(), pid->as<uint32_t>(),
-                                                                  iid->as<uint32_t>(), np);
-        CPB_CUDA(cudaGetLastError());
+        const uint32_t *run_lo = lo->as<uint32_t>(), *run_cnt = cnt->as<uint32_t>(), *at = pos->as<uint32_t>();
+        uint32_t *probe_id = pid->as<uint32_t>(), *index_id = iid->as<uint32_t>();
+        each_row(c, np, [=] __device__(uint64_t i) {
+            const uint32_t k = run_cnt[i], p = at[i], l = run_lo[i];
+            for (uint32_t j = 0; j < k; j++) { probe_id[p + j] = (uint32_t)i; index_id[p + j] = l + j; }
+        });
     }
     Table pt; pt.ctx = c; pt.nrows = (int64_t)np;
     for (auto* p : pcols) pt.cols.push_back(*p);
@@ -641,10 +626,6 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
 // Every row probes the full-key table built over the rows themselves: with unique keys row r finds r.  Two rows with
 // the same key occupy two slots of one probe sequence, so at least one of them finds the other: a duplicate exists
 // iff some row does not find itself.
-__global__ void self_check_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ cnt, uint64_t n, uint32_t* flag) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && (cnt[i] != 1u || lo[i] != (uint32_t)i)) *flag = 1u;  // benign race: every writer stores 1
-}
 bool index_has_duplicates(Ctx* c, Index& ix) {
     const uint64_t n = (uint64_t)ix.nrows;
     const int nk = (int)ix.key_cols.size();
@@ -657,8 +638,11 @@ bool index_has_duplicates(Ctx* c, Index& ix) {
     probe_dispatch(c, *ix.src, ix.key_col_idx, ix, ht, RowOrder::source, nk, lo->as<uint32_t>(), cnt->as<uint32_t>(), flags->as<uint32_t>() + 2);
     {
         KernelTimer kt(c, "unique_check", n * 8);
-        self_check_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(lo->as<uint32_t>(), cnt->as<uint32_t>(), n, flags->as<uint32_t>() + 8);
-        CPB_CUDA(cudaGetLastError());
+        const uint32_t *run_lo = lo->as<uint32_t>(), *run_cnt = cnt->as<uint32_t>();
+        uint32_t* dup = flags->as<uint32_t>() + 8;
+        each_row(c, n, [=] __device__(uint64_t i) {
+            if (run_cnt[i] != 1u || run_lo[i] != (uint32_t)i) *dup = 1u;  // benign race: every writer stores 1
+        });
     }
     return read_back<uint32_t>(c, flags->as<uint32_t>() + 8) != 0;
 }

@@ -56,13 +56,12 @@ constexpr int RS_THREADS = 256;
 constexpr int RS_ITEMS = 8;
 constexpr int RS_TILE = RS_THREADS * RS_ITEMS;
 
-__global__ void iota_kernel(uint32_t* p, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) p[i] = (uint32_t)i;
+void iota_u32(Ctx* c, uint32_t* p, uint64_t n) {
+    each_row(c, n, [=] __device__(uint64_t i) { p[i] = (uint32_t)i; });
 }
-__global__ void gather_u64_kernel(const uint64_t* __restrict__ src, const uint32_t* __restrict__ idx, uint64_t* dst, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = src[idx[i]];
+// dst[i] = src[idx[i]]
+static void gather_u64(Ctx* c, const uint64_t* src, const uint32_t* idx, uint64_t* dst, uint64_t n) {
+    each_row(c, n, [=] __device__(uint64_t i) { dst[i] = src[idx[i]]; });
 }
 // histogram of all 8 bytes of every key: hist[b * 256 + v]
 __global__ void hist8_kernel(const uint64_t* __restrict__ keys, uint64_t n, uint32_t* hist) {
@@ -143,7 +142,7 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint64_
 // host round trip for the whole sort (round 1: one per image word).
 static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
     Buf permA = dev_alloc(c, n * 4), permB = dev_alloc(c, n * 4), keyA = dev_alloc(c, n * 8), keyB = dev_alloc(c, n * 8);
-    iota_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(permA->as<uint32_t>(), n);
+    iota_u32(c, permA->as<uint32_t>(), n);
     const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;
     const uint32_t nblocks = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 4);
     const uint64_t tpb = (ntiles + nblocks - 1) / nblocks;
@@ -167,8 +166,7 @@ static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t
         if (!any) continue;  // the whole word is constant
         {
             KernelTimer kt(c, "sort_gather_word", n * 20);
-            gather_u64_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(image + (uint64_t)w * n, permA->as<uint32_t>(), keyA->as<uint64_t>(), n);
-            CPB_CUDA(cudaGetLastError());
+            gather_u64(c, image + (uint64_t)w * n, permA->as<uint32_t>(), keyA->as<uint64_t>(), n);
         }
         *traffic += n * 20;
         for (int b = 0; b < 8; b++) {
@@ -187,38 +185,11 @@ static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t
 }
 
 // ------------------------------------------------------------------ adjacent compare (unique check, groups)
-__global__ void head_flags_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, uint32_t* head) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    head[i] = (i == 0 || !prefix_equal(image, n, i, image, n, i - 1, pbytes)) ? 1u : 0u;
-}
 void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head) {
-    head_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(image, n, pbytes, head);
-    CPB_CUDA(cudaGetLastError());
+    each_row(c, n, [=] __device__(uint64_t i) { head[i] = (i == 0 || !prefix_equal(image, n, i, image, n, i - 1, pbytes)) ? 1u : 0u; });
 }
-__global__ void first_dup_kernel(const uint32_t* __restrict__ head, uint64_t n, unsigned long long* first) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 1 && i < n && head[i] == 0) atomicMin(first, (unsigned long long)i);
-}
-// group start: head && next is not head; group end (exclusive hi = i+1): !head && (last || next is head)
-__global__ void group_flags_kernel(const uint32_t* __restrict__ head, uint64_t n, uint32_t* gs, uint32_t* ge) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    bool h = head[i] != 0, nh = (i + 1 == n) || head[i + 1] != 0;
-    gs[i] = (h && !nh) ? 1u : 0u;
-    ge[i] = (!h && nh) ? 1u : 0u;
-}
-__global__ void singleton_flags_kernel(const uint32_t* __restrict__ head, uint64_t n, uint32_t* keep) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    bool h = head[i] != 0, nh = (i + 1 == n) || head[i + 1] != 0;
-    keep[i] = (h && nh) ? 1u : 0u;
-}
-__global__ void set_flags_kernel(const int64_t* __restrict__ rows, uint64_t m, uint32_t* keep, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m && rows[i] >= 0 && (uint64_t)rows[i] < n) keep[rows[i]] = 1u;
-}
-__global__ void clear_one_kernel(uint32_t* keep, uint64_t i) { keep[i] = 0; }
+// nonzero when the row after row i starts a run of equal keys; past the last row, one always starts
+__device__ __forceinline__ uint32_t next_head(const uint32_t* head, uint64_t last, uint64_t i) { return i == last ? 1u : head[i + 1]; }
 
 void describe_keys(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, KeyDesc& kd) {
     kd.nkeys = (int)kidx.size();
@@ -294,9 +265,7 @@ static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vecto
 // rows ids[0..m) of a key image of n_src rows, as an image of m rows
 static Buf gather_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n_src, const uint32_t* ids, uint64_t m) {
     Buf out = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)words * m) * 8);
-    for (uint32_t w = 0; w < words && m; w++)
-        gather_u64_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(image + (uint64_t)w * n_src, ids, out->as<uint64_t>() + (uint64_t)w * m, m);
-    CPB_CUDA(cudaGetLastError());
+    for (uint32_t w = 0; w < words; w++) gather_u64(c, image + (uint64_t)w * n_src, ids, out->as<uint64_t>() + (uint64_t)w * m, m);
     return out;
 }
 
@@ -418,9 +387,10 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> tp, const std:
         CPB_CUDA(cudaMemsetAsync(first->p, 0xff, 8, c->stream));
         {
             KernelTimer kt(c, "unique_check", (uint64_t)words * n * 8, 2);
-            head_flags(c, simg, n, words * 8, head->as<uint32_t>());
-            first_dup_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, (unsigned long long*)first->p);
-            CPB_CUDA(cudaGetLastError());
+            uint32_t* hd = head->as<uint32_t>();
+            unsigned long long* fd = (unsigned long long*)first->p;
+            head_flags(c, simg, n, words * 8, hd);
+            each_row(c, n, [=] __device__(uint64_t i) { if (i >= 1 && hd[i] == 0) atomicMin(fd, (unsigned long long)i); });
         }
         const uint64_t fd = read_back<uint64_t>(c, first->p);
         if (fd != ~0ull) {
@@ -463,11 +433,6 @@ __global__ void dup_walk_kernel(const uint64_t* __restrict__ image, uint64_t n, 
     }
     *ngroups = g;
 }
-__global__ void not_flags_kernel(const uint32_t* __restrict__ head, uint64_t n, uint32_t* out) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = head[i] ? 0u : 1u;
-}
-
 void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<int64_t>& hi) {
     lo.clear(); hi.clear();
     const uint64_t n = (uint64_t)ix.nrows;
@@ -480,15 +445,22 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
         return out;
     };
     Buf head = dev_alloc(c, n * 4), gs = dev_alloc(c, n * 4);
+    uint32_t* hd = head->as<uint32_t>();
     uint64_t ng = 0, ne = 0;
     Buf los, his;
     if (ix.in_order) {  // a group is a run of equal keys: its first row is a head followed by a non-head, and so on
         Buf ge = dev_alloc(c, n * 4);
         {
             KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 12, 2);
-            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
-            group_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>(), ge->as<uint32_t>());
-            CPB_CUDA(cudaGetLastError());
+            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, hd);
+            // group start: a head followed by a non-head; group end (exclusive hi = i + 1): a non-head followed by a head
+            uint32_t *s = gs->as<uint32_t>(), *e = ge->as<uint32_t>();
+            const uint64_t last = n - 1;
+            each_row(c, n, [=] __device__(uint64_t i) {
+                const bool h = hd[i] != 0, nh = next_head(hd, last, i) != 0;
+                s[i] = (h && !nh) ? 1u : 0u;
+                e[i] = (!h && nh) ? 1u : 0u;
+            });
         }
         los = compact(gs, 0, &ng);
         his = compact(ge, 1, &ne);
@@ -496,9 +468,8 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
     } else {
         {
             KernelTimer kt(c, "dedup_segments", (uint64_t)ix.image_words * n * 8 + n * 8, 2);
-            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
-            not_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, gs->as<uint32_t>());
-            CPB_CUDA(cudaGetLastError());
+            head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, hd);
+            nonzero_flags(c, hd, n, false, gs->as<uint32_t>());
         }
         uint64_t npairs = 0;
         Buf pairs = compact(gs, 0, &npairs);
@@ -522,35 +493,6 @@ void index_dup_groups(Ctx* c, Index& ix, std::vector<int64_t>& lo, std::vector<i
     lo.assign(a.begin(), a.end()); hi.assign(b.begin(), b.end());
 }
 
-// indexImpl.dedup (csvplus.go:810-867) with the resolver's choices already made on the host.
-// keep[g] >= 0: stored position of the row kept for group g; -1: the group is dropped (the resolver returned an "empty"
-// row, :845); <= -2: the resolver returned a row that is not one of the group's rows — row (-2 - keep[g]) of `repl`
-// takes the place of the group (:846 stores whatever row came back; the index is NOT re-sorted, exactly like the reference).
-// The rows kept: every row outside the groups, the chosen row of each group, in stored order — except that the walk
-// never copies the last row when no group covers it (SURVEY §Q1, bug_compatible).
-// keep[i] = 1 for the rows outside the groups [lo, hi) (ascending, disjoint)
-__global__ void uncovered_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ hi, uint64_t ng, uint64_t n, uint32_t* keep) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint64_t a = 0, b = ng;  // groups starting at or before i
-    while (a < b) { const uint64_t h = a + (b - a) / 2; if (lo[h] <= i) a = h + 1; else b = h; }
-    keep[i] = (a == 0 || i >= hi[a - 1]) ? 1u : 0u;
-}
-__global__ void patch_ids_kernel(const uint32_t* __restrict__ pos, const int64_t* __restrict__ at, const uint32_t* __restrict__ with, uint64_t m, uint32_t* ids) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m) ids[pos[at[i]]] = with[i];
-}
-
-// *out = 1 when some row's key image is below the previous row's
-__global__ void order_check_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t words, uint32_t* out) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i == 0 || i >= n) return;
-    for (uint32_t w = 0; w < words; w++) {
-        const uint64_t a = image[(uint64_t)w * n + i - 1], b = image[(uint64_t)w * n + i];
-        if (a != b) { if (a > b) *out = 1u; return; }  // benign race: every writer stores 1
-    }
-}
-
 void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt) {
     const uint64_t m = (uint64_t)nt->nrows;
     nt->first_line = 0;
@@ -566,14 +508,28 @@ void index_adopt_rows(Ctx* c, Index& ix, std::shared_ptr<Table> nt) {
         Buf flag = dev_alloc(c, 8);
         CPB_CUDA(cudaMemsetAsync(flag->p, 0, 8, c->stream));
         {
+            // *out = 1 when some row's key image is below the previous row's
             KernelTimer kt(c, "order_check", m * words * 8);
-            order_check_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(ix.image->as<uint64_t>(), m, words, flag->as<uint32_t>());
-            CPB_CUDA(cudaGetLastError());
+            const uint64_t* image = ix.image->as<uint64_t>();
+            uint32_t* out = flag->as<uint32_t>();
+            each_row(c, m, [=] __device__(uint64_t i) {
+                if (i == 0) return;
+                for (uint32_t w = 0; w < words; w++) {
+                    const uint64_t a = image[(uint64_t)w * m + i - 1], b = image[(uint64_t)w * m + i];
+                    if (a != b) { if (a > b) *out = 1u; return; }  // benign race: every writer stores 1
+                }
+            });
         }
         ix.in_order = read_back<uint32_t>(c, flag->p) == 0;
     }
 }
 
+// indexImpl.dedup (csvplus.go:810-867) with the resolver's choices already made on the host.
+// keep[g] >= 0: stored position of the row kept for group g; -1: the group is dropped (the resolver returned an "empty"
+// row, :845); <= -2: the resolver returned a row that is not one of the group's rows — row (-2 - keep[g]) of `repl`
+// takes the place of the group (:846 stores whatever row came back; the index is NOT re-sorted, exactly like the reference).
+// The rows kept: every row outside the groups, the chosen row of each group, in stored order — except that the walk
+// never copies the last row when no group covers it (SURVEY §Q1, bug_compatible).
 void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, bool bug_compatible, const Table* repl) {
     const uint64_t n = (uint64_t)ix.nrows;
     if (n < 2 || keep_in.empty()) return;  // no duplicate group: the reference returns early (:820-822)
@@ -601,12 +557,18 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
     // flag = the rows outside the groups.  In key order the groups are the runs of equal keys, so those are the rows
     // that are heads of runs of one; out of key order they come from the groups the walk found.
     Buf flag = dev_alloc(c, n * 4);
+    uint32_t* fl = flag->as<uint32_t>();
     bool last_outside = false;
     if (ix.in_order) {
         Buf head = dev_alloc(c, n * 4);
-        head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, head->as<uint32_t>());
-        singleton_flags_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(head->as<uint32_t>(), n, flag->as<uint32_t>());
-        if (bug_compatible) last_outside = read_back<uint32_t>(c, head->as<uint32_t>() + (n - 1)) != 0;
+        uint32_t* hd = head->as<uint32_t>();
+        head_flags(c, ix.image->as<uint64_t>(), n, ix.image_words * 8, hd);
+        const uint64_t last = n - 1;
+        each_row(c, n, [=] __device__(uint64_t i) {
+            const bool h = hd[i] != 0, nh = next_head(hd, last, i) != 0;
+            fl[i] = (h && nh) ? 1u : 0u;
+        });
+        if (bug_compatible) last_outside = read_back<uint32_t>(c, hd + (n - 1)) != 0;
     } else {
         std::vector<uint32_t> lh(lo.begin(), lo.end()), hh(hi.begin(), hi.end());
         Buf dlo = dev_alloc(c, (lh.size() + 1) * 4), dhi = dev_alloc(c, (hh.size() + 1) * 4);
@@ -614,15 +576,22 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
             CPB_CUDA(cudaMemcpyAsync(dlo->p, lh.data(), lh.size() * 4, cudaMemcpyHostToDevice, c->stream));
             CPB_CUDA(cudaMemcpyAsync(dhi->p, hh.data(), hh.size() * 4, cudaMemcpyHostToDevice, c->stream));
         }
-        uncovered_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(dlo->as<uint32_t>(), dhi->as<uint32_t>(), lh.size(), n, flag->as<uint32_t>());
+        // the rows outside the groups [lo, hi) (ascending, disjoint)
+        const uint32_t *glo = dlo->as<uint32_t>(), *ghi = dhi->as<uint32_t>();
+        const uint64_t ng = lh.size();
+        each_row(c, n, [=] __device__(uint64_t i) {
+            uint64_t a = 0, b = ng;  // groups starting at or before i
+            while (a < b) { const uint64_t h = a + (b - a) / 2; if (glo[h] <= i) a = h + 1; else b = h; }
+            fl[i] = (a == 0 || i >= ghi[a - 1]) ? 1u : 0u;
+        });
         last_outside = hi.empty() || (uint64_t)hi.back() < n;
         sync_stream(c);  // lh / hh are pageable host vectors
     }
     Buf kd = dev_alloc(c, keep.size() * 8);
     CPB_CUDA(cudaMemcpyAsync(kd->p, keep.data(), keep.size() * 8, cudaMemcpyHostToDevice, c->stream));
-    set_flags_kernel<<<nblk(keep.size(), 256), 256, 0, c->stream>>>(kd->as<int64_t>(), keep.size(), flag->as<uint32_t>(), n);
-    if (bug_compatible && last_outside) clear_one_kernel<<<1, 1, 0, c->stream>>>(flag->as<uint32_t>(), n - 1);
-    CPB_CUDA(cudaGetLastError());
+    const int64_t* rows = kd->as<int64_t>();
+    each_row(c, keep.size(), [=] __device__(uint64_t i) { if (rows[i] >= 0 && (uint64_t)rows[i] < n) fl[rows[i]] = 1u; });
+    if (bug_compatible && last_outside) CPB_CUDA(cudaMemsetAsync(fl + (n - 1), 0, 4, c->stream));
     // compaction of the kept positions (the scanned positions are needed again to patch replacement ids in)
     const FlagScan kept = scan_flags(c, flag->as<uint32_t>(), n);
     const uint64_t m = kept.count;
@@ -633,8 +602,10 @@ void index_dedup_apply(Ctx* c, Index& ix, const std::vector<int64_t>& keep_in, b
         Buf dp = dev_alloc(c, rpos.size() * 8), dr = dev_alloc(c, rid.size() * 4);
         CPB_CUDA(cudaMemcpyAsync(dp->p, rpos.data(), rpos.size() * 8, cudaMemcpyHostToDevice, c->stream));
         CPB_CUDA(cudaMemcpyAsync(dr->p, rid.data(), rid.size() * 4, cudaMemcpyHostToDevice, c->stream));
-        patch_ids_kernel<<<nblk(rpos.size(), 256), 256, 0, c->stream>>>(kept.pos->as<uint32_t>(), dp->as<int64_t>(), dr->as<uint32_t>(), rpos.size(), ids->as<uint32_t>());
-        CPB_CUDA(cudaGetLastError());
+        const uint32_t *pos = kept.pos->as<uint32_t>(), *with = dr->as<uint32_t>();
+        const int64_t* at = dp->as<int64_t>();
+        uint32_t* id = ids->as<uint32_t>();
+        each_row(c, rpos.size(), [=] __device__(uint64_t i) { id[pos[at[i]]] = with[i]; });
         // rows [0, n) = the index, rows [n, n + repl) = the replacement rows in the index's column order
         Table rsel; rsel.ctx = c; rsel.nrows = repl->nrows;
         for (auto& col : ix.table->cols) rsel.cols.push_back(repl->cols[repl->find(col.name)]);

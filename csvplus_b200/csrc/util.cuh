@@ -1,10 +1,27 @@
-// util.cuh — device-side helpers (sm_90a): mbarrier + bulk-async (TMA 1-D) staging, gpu-scope
-// acquire/release for the decoupled look-back chains, warp scans, key-image compare.
+// util.cuh — device-side helpers (sm_90a): the one-thread-per-row launcher, mbarrier + bulk-async (TMA 1-D) staging,
+// gpu-scope acquire/release for the decoupled look-back chains, warp scans, key-image compare.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "core.hpp"
+
 namespace cpb {
+
+// ---- one thread per row: f(i) for every i in [0, n)
+template <class F>
+__global__ void __launch_bounds__(256) each_row_kernel(uint64_t n, F f) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) f(i);
+}
+// Launches each_row_kernel on c's stream and checks the launch; nothing is launched for n == 0 (a grid of no blocks is a
+// launch error).  f is a [=] __device__ (uint64_t i) lambda that captures plain values and device pointers.
+template <class F>
+void each_row(Ctx* c, uint64_t n, F f) {
+    if (n == 0) return;
+    each_row_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, f);
+    CPB_CUDA(cudaGetLastError());
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
