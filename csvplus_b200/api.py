@@ -783,6 +783,18 @@ class Categories:
         self.codes, self.dictionary = codes, dictionary
 
 
+class Groups:
+    """the result of DataSource.GroupBy: table, a Table of the key columns in the order given with one row per group
+    (the key values of the group's first row), and values, {output name: CUDA tensor with one value per group} (int64 for
+    count and "int" inputs, float64 for "float64" inputs)."""
+
+    def __init__(self, table: Table, values: dict):
+        self.table, self.values = table, values
+
+    def __len__(self):
+        return len(self.table)
+
+
 class Sprintf:
     """fmt.Sprintf(format, v[0], v[1], ...) of every row, v = the row's values of `columns` (Row.SelectValues; a column may
     be named twice): a value for Table.with_column and MapTensors.  The format is str or bytes; the library accepts
@@ -1656,6 +1668,47 @@ class DataSource:
             raise err
         return out
 
+    def GroupBy(self, keys, aggs: dict) -> "Groups":
+        """per-group aggregates computed on the GPU (an extension beyond the reference API, like ToTensors): what a RowFunc
+        folding the plan's rows in order into a map keyed by the values of `keys` computes.  keys: a non-empty sequence
+        of distinct column names; aggs: {output name: (op, column, kind) or ("count",)}, op one of count sum min max first
+        last, kind "int" (Row.ValueAsInt, int64) or "float64" (Row.ValueAsFloat64).  Rows are in one group when every key
+        column holds equal bytes; groups are numbered in order of first appearance.  sum of "int" wraps as Go's int64 +=;
+        sum of "float64" is acc += v in row order from +0.0, bit for bit; min / max of "float64" fold with Go's
+        math.Min / math.Max; first / last take the group's first / last row.  The plan is consumed batch by batch: device
+        memory holds the groups and one batch, never the whole input.  A conversion error raises the CsvPlusError
+        ToTensors would raise for the inputs in aggs order (.row = the row's ordinal among the rows reaching the sink),
+        after the rows before it are folded; a source error is raised after the delivered rows are folded.  Rows left on
+        the host (after an opaque Map or Filter(func)) go through Table.from_rows first."""
+        keys = _group_keys(keys)
+        specs = _group_aggs(aggs)
+        ctx = self._ctx()
+        ka, kkeep = _strs(keys)
+        arr = (_abi.Agg * max(1, len(specs)))()
+        keep = []
+        for i, (op, column, kind) in enumerate(specs.values()):
+            b = _enc(column)
+            keep.append(b)
+            arr[i] = _abi.Agg(_abi.CPB_AGG_OPS[op], _abi.CPB_AGG_KINDS[kind], _abi.Str(b, len(b)))
+        h = C.c_void_p()
+        ctx._call("cpb_groups_open", ka, len(keys), arr, len(specs), C.byref(h))
+        try:
+            seen = 0
+            for state, err, _ in self._batches():
+                t = self._as_table(state)
+                if t is not None and len(t):
+                    e = _abi.Error()
+                    if ctx._call("cpb_groups_push", h, t.h, err=e, accept=(_abi.CPB_ERR_DATA,)):
+                        x = CsvPlusError(e.msg.decode("utf-8", "replace"), _abi.CPB_ERR_DATA, e.kind)
+                        x.row = seen + e.line
+                        raise x
+                    seen += len(t)
+                if err is not None:
+                    raise err
+            return _groups_result(ctx, h, specs)
+        finally:
+            ctx._call("cpb_groups_free", h)
+
     def IndexOn(self, *columns) -> Index:  # csvplus.go:529-531
         return self._index(columns, False)
 
@@ -1673,6 +1726,48 @@ class DataSource:
         if t is None:
             t = Table.from_rows(self._ctx(), [], list(columns))
         return t.index_on(*columns, unique=unique)
+
+
+def _group_keys(keys) -> list:
+    if isinstance(keys, (str, bytes)):
+        raise ValueError("GroupBy: keys is a sequence of column names, not one name")
+    keys = list(keys)
+    if len(keys) == 0:
+        raise ValueError("empty column list in GroupBy()")
+    if len(set(keys)) != len(keys):
+        raise ValueError("duplicate column name(s) in GroupBy()")
+    return keys
+
+
+def _group_aggs(aggs: dict) -> dict:
+    """{name: (op, column, kind)}: every aggregate checked, count as ("count", "", "int")"""
+    out = {}
+    for name, spec in dict(aggs).items():
+        spec = tuple(spec) if isinstance(spec, (tuple, list)) else (spec,)
+        if spec == ("count",):
+            out[name] = ("count", "", "int")
+            continue
+        if len(spec) != 3 or spec[0] not in _abi.CPB_AGG_OPS or spec[0] == "count":
+            raise ValueError(f"GroupBy: aggregate {name!r} is {spec!r} (want (op, column, kind) with op one of sum min max first "
+                             "last, or ('count',))")
+        if spec[2] not in _abi.CPB_AGG_KINDS:
+            raise ValueError(f"GroupBy: unknown type {spec[2]!r} for aggregate {name!r} (want 'int' or 'float64')")
+        out[name] = spec
+    return out
+
+
+def _groups_result(ctx: Context, h, specs: dict) -> "Groups":
+    import torch
+    dev = torch.device("cuda", ctx.device)
+    th, n = C.c_void_p(), C.c_uint64()
+    ctx._call("cpb_groups_result", h, C.byref(th), C.byref(n))
+    values = {}
+    for i, (name, (op, _, kind)) in enumerate(specs.items()):
+        v = torch.empty(n.value, dtype=torch.float64 if kind == "float64" and op != "count" else torch.int64, device=dev)
+        _ctx_waits_for_torch(ctx, dev)
+        ctx._call("cpb_groups_values", h, i, C.c_void_p(v.data_ptr()))
+        values[name] = v
+    return Groups(Table(ctx, th), values)
 
 
 def _convert_all(t: Table, kinds: dict) -> tuple:

@@ -868,7 +868,6 @@ int cpb_table_to_json_device(cpb_ctx* h, const cpb_table* t, int first_batch, in
 // error is the first failing row's
 static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, NumKind kind, void* values, uint8_t* status,
                             uint64_t* nbad, cpb_error* err) {
-    const bool is_float = kind != NumKind::Int64;
     return guarded(h, err, [&](Ctx* c) {
         const Table& T = table_of(t);
         need(nbad && (values || T.nrows == 0), "null nbad or values");
@@ -879,12 +878,7 @@ static int column_as_common(cpb_ctx* h, const cpb_table* t, cpb_str column, NumK
         if (k < 0) throw DataError{CPB_E_MISSING_COLUMN, -1, 0, false, "missing column " + go_quote(name)};  // :170, :192
         NumResult r = column_as_number(c, T, k, kind, values, status);
         *nbad = r.nbad;
-        if (r.nbad) {
-            const bool range = r.first_status == CPB_NUM_RANGE;
-            throw DataError{range ? CPB_E_NUM_RANGE : CPB_E_NUM_SYNTAX, -1, r.first_row, false,
-                            "column " + go_quote(name) + ": cannot convert " + go_quote(r.first_value) + (is_float ? " to float: " : " to integer: ") +
-                                (range ? "value out of range" : "invalid syntax")};  // :176, :198
-        }
+        if (r.nbad) throw number_error(name, kind, r);
         return CPB_OK;
     });
 }
@@ -949,6 +943,51 @@ int cpb_table_set_codes(cpb_ctx* h, const cpb_table* t, cpb_str column, const in
                         cpb_table** out, cpb_error* err) {
     return derived_table(h, t, out, err, [&](Ctx* c, const Table& T) {
         return table_set_codes(c, T, to_string(column), dev_codes, table_of(dictionary));
+    });
+}
+
+// ------------------------------------------------------------------ GroupBy
+static Groups& groups_of(Ctx* c, const cpb_groups* g) {
+    need(g, "null groups");
+    need(groups_ctx(*g->g) == c, "groups of another context");
+    return *g->g;
+}
+int cpb_groups_open(cpb_ctx* h, const cpb_str* keys, int nkeys, const cpb_agg* aggs, int naggs, cpb_groups** out) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        need(out && (naggs <= 0 || aggs), "null out or aggregates");
+        std::vector<GroupAgg> ag;
+        for (int i = 0; i < naggs; i++) ag.push_back(GroupAgg{aggs[i].op, aggs[i].kind, to_string(aggs[i].column)});
+        *out = new cpb_groups{groups_open(c, str_list(keys, nkeys), ag)};
+        return CPB_OK;
+    });
+}
+int cpb_groups_push(cpb_ctx* h, cpb_groups* g, const cpb_table* t, cpb_error* err) {
+    return guarded(h, err, [&](Ctx* c) {
+        groups_push(c, groups_of(c, g), table_of(t));
+        return CPB_OK;
+    });
+}
+int cpb_groups_result(cpb_ctx* h, const cpb_groups* g, cpb_table** keys, uint64_t* ngroups) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        const Groups& G = groups_of(c, g);
+        need(keys && ngroups, "null keys or ngroups");
+        *keys = wrap(groups_keys(c, G));
+        *ngroups = groups_count(G);
+        return CPB_OK;
+    });
+}
+int cpb_groups_values(cpb_ctx* h, const cpb_groups* g, int i, void* dev_dst) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        groups_values(c, groups_of(c, g), i, dev_dst);
+        return CPB_OK;
+    });
+}
+int cpb_groups_free(cpb_ctx* h, cpb_groups* g) {
+    return guarded(h, nullptr, [&](Ctx* c) {
+        groups_of(c, g);
+        groups_free(g->g);
+        delete g;
+        return CPB_OK;
     });
 }
 

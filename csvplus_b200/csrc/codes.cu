@@ -4,8 +4,8 @@
 //   length, any bytes, the empty value included.
 //
 // Distinct pass.  An open-addressing table of uint32 row ids in HBM: nslots = the power of two >= 2 n (load factor
-// between 1/4 and 1/2, at least 64 slots), 0xFFFFFFFF = empty, linear probing from hash & (nslots - 1).  The hash is
-// 64 bits over the value's 8-byte little-endian words (the last one zero-padded): the sum of fmix64(word ^ (i + 1) *
+// between 1/4 and 1/2, at least 64 slots), 0xFFFFFFFF = empty, linear probing from hash & (nslots - 1).  The hash
+// (keyhash.cuh) is 64 bits over the value's 8-byte little-endian words (the last one zero-padded): the sum of fmix64(word ^ (i + 1) *
 // golden) over the words, finished with the length.  A sum does not depend on which lane added which word, so one
 // thread or a whole warp computes the same hash.  A row claims an empty slot with atomicCAS; a slot whose row has the
 // same hash is compared byte for byte (a hash is never taken as equality), and on equal bytes the row is folded in
@@ -39,48 +39,13 @@
 #include <algorithm>
 
 #include "core.hpp"
+#include "keyhash.cuh"
 #include "util.cuh"
 
 namespace cpb {
 
 constexpr uint32_t EMPTY_SLOT = 0xFFFFFFFFu;
-constexpr uint32_t LONG_BYTES = 128;
 constexpr int CW_WARPS = 8;
-
-__device__ __forceinline__ uint64_t fmix64(uint64_t k) {
-    k ^= k >> 33; k *= 0xff51afd7ed558ccdull;
-    k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull;
-    k ^= k >> 33;
-    return k;
-}
-__device__ __forceinline__ uint64_t word_mix(uint64_t w, uint32_t i) { return fmix64(w ^ ((uint64_t)(i + 1) * 0x9E3779B97F4A7C15ull)); }
-__device__ __forceinline__ uint64_t hash_finish(uint64_t sum, uint32_t len) { return fmix64(sum + (uint64_t)len * 0xC2B2AE3D27D4EB4Full); }
-
-// word i (bytes [8i, min(8i + 8, len)), little-endian, zero-padded) of the len bytes at sp, from aligned 8-byte loads:
-// the aligned word holding a byte of the value never crosses a page, so nothing past the value's last word is read
-__device__ __forceinline__ uint64_t word_at(const uint8_t* sp, uint32_t len, uint32_t i) {
-    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(sp) & 7u), sh = mis * 8, rem = len - 8 * i;
-    const unsigned long long* wp = reinterpret_cast<const unsigned long long*>(sp - mis) + i;
-    uint64_t v = __ldg(wp) >> sh;
-    if (sh && mis + rem > 8) v |= (uint64_t)__ldg(wp + 1) << (64 - sh);
-    if (rem < 8) v &= (1ull << (8 * rem)) - 1;
-    return v;
-}
-__device__ __forceinline__ bool equal_thread(const uint8_t* a, const uint8_t* b, uint32_t len) {
-    const uint32_t nw = (len + 7) / 8;
-    for (uint32_t w = 0; w < nw; w++) if (word_at(a, len, w) != word_at(b, len, w)) return false;
-    return true;
-}
-__device__ __forceinline__ bool equal_warp(const uint8_t* a, const uint8_t* b, uint32_t len, int lane) {
-    const uint32_t nw = (len + 7) / 8;
-    bool diff = false;
-    for (uint32_t w0 = 0; w0 < nw; w0 += 32) {
-        const uint32_t w = w0 + lane;
-        if (w < nw) diff = word_at(a, len, w) != word_at(b, len, w);
-        if (__any_sync(0xffffffffu, diff)) return false;
-    }
-    return true;
-}
 
 struct ValCol { const uint32_t* off; const uint8_t* data; };
 

@@ -353,6 +353,9 @@ std::shared_ptr<Table> rowhash_gather(Ctx* c, Index& ix, const Table& probe, con
                                       uint64_t* matches);
 // sort.cu.  A missing key column (of a non-empty table) or a duplicate key of a unique index throws DataError.
 std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::vector<std::string>& keys, bool unique);
+// stable sort of the row ids 0..n-1 by image words [0, words) (word w of row r at image[w * n + r], compared as unsigned
+// integers): the buffer of the sorted ids.  One host synchronisation (the digit histograms); *traffic += bytes moved.
+Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic);
 std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix);  // materialises ix.table on first use
 void ensure_sorted(Ctx* c, Index& ix);                    // sorts a lazily-sorted unique index on first need of the order
 constexpr int MAXKEYS = 16;
@@ -423,6 +426,8 @@ struct NumResult {
     std::string first_value;
 };
 NumResult column_as_number(Ctx* c, const Table& t, int col, NumKind kind, void* values, uint8_t* status);
+// the reference's error for the first failing row of r (r.nbad > 0) in column `name` (csvplus.go:176, :198); line = the row
+DataError number_error(const std::string& name, NumKind kind, const NumResult& r);
 // format.cu: computed columns.  t with column `name` set (replaced in place, else appended; the other columns share t's
 // buffers) to strconv.FormatInt(v, 10) / FormatFloat(x, fmt, prec, 64 or 32) of the n device values, or to one literal value
 std::shared_ptr<Table> table_set_values(Ctx* c, const Table& t, const std::string& name, const void* values, NumKind kind, char fmt, int prec);
@@ -439,6 +444,20 @@ std::shared_ptr<Table> table_filter_mask(Ctx* c, const Table& t, const uint8_t* 
 // outside [0, rows of dict) throws DataError CPB_E_BAD_CODE with line = the lowest such row.
 std::shared_ptr<Table> column_codes(Ctx* c, const Table& t, int col, int64_t* codes);
 std::shared_ptr<Table> table_set_codes(Ctx* c, const Table& t, const std::string& name, const int64_t* codes, const Table& dict);
+// groupby.cu: GroupBy state that persists across pushes (DESIGN §3.14).  groups_open checks keys (1..MAXKEYS, distinct)
+// and aggregates (ArgError); groups_push folds a table's rows: a key column T lacks throws DataError CPB_E_MISSING_COLUMN
+// at line 0, a failing conversion its number_error after the rows before it are folded (an aggregate column T lacks
+// counts as failing at row 0).  groups_keys: the key rows of the groups in group order; groups_values: aggregate i of
+// every group (8 B each) copied into device memory dst, complete on return.
+struct GroupAgg { int op; int kind; std::string column; };
+struct Groups;
+Groups* groups_open(Ctx* c, const std::vector<std::string>& keys, const std::vector<GroupAgg>& aggs);
+void groups_push(Ctx* c, Groups& g, const Table& t);
+std::shared_ptr<Table> groups_keys(Ctx* c, const Groups& g);
+uint64_t groups_count(const Groups& g);
+void groups_values(Ctx* c, const Groups& g, int i, void* dst);
+Ctx* groups_ctx(const Groups& g);
+void groups_free(Groups* g);
 // sprintf.cu: fmt.Sprintf(format, v...) of every row, v = the row's values of columns cols (a name may repeat).  The
 // format is compiled first: one outside the accepted subset, or whose verb count is not cols.size(), throws ArgError
 // CPB_ERR_UNSUPPORTED naming the byte offset.  A column t lacks (on a table with rows) throws DataError
@@ -458,6 +477,7 @@ struct cpb_ctx { cpb::Ctx c; };
 struct cpb_table { std::shared_ptr<cpb::Table> t; };
 struct cpb_index { std::shared_ptr<cpb::Index> ix; };
 struct cpb_stream { cpb::Stream* s; };
+struct cpb_groups { cpb::Groups* g; };
 
 namespace cpb {
 template <class F> int guarded(cpb_ctx* h, cpb_error* err, F&& body) { return guarded(h ? &h->c : nullptr, err, body); }

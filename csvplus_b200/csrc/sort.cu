@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint64_
 // Which digits are constant over the whole column (their pass would be the identity) does not depend on the order of
 // the rows: the byte histograms of ALL image words are taken from the unsorted image up front and read back with one
 // host round trip for the whole sort (round 1: one per image word).
-static Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
+Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
     Buf permA = dev_alloc(c, n * 4), permB = dev_alloc(c, n * 4), keyA = dev_alloc(c, n * 8), keyB = dev_alloc(c, n * 8);
     iota_u32(c, permA->as<uint32_t>(), n);
     const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;

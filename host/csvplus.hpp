@@ -500,6 +500,30 @@ inline Reader FromString(std::string data) {
     });
 }
 
+// ---------------------------------------------------------------- GroupBy
+// one aggregate of DataSource::GroupBy: op CPB_AGG_COUNT .. CPB_AGG_LAST over column, converted as Row.ValueAsInt
+// (CPB_AGG_INT) or Row.ValueAsFloat64 (CPB_AGG_FLOAT64); count takes neither
+struct Agg { std::string name; int op; std::string column; int kind = CPB_AGG_INT; };
+// the result of DataSource::GroupBy: Keys(), the key columns with one row per group in order of first appearance, and
+// per aggregate a device array of one value per group (int64 for count and int inputs, double for float64 inputs),
+// owned by this object
+class Groups {
+public:
+    Table Keys() const { return keys_; }
+    uint64_t size() const { return n_; }
+    const int64_t* Int(const std::string& name) const { return (const int64_t*)at(name); }
+    const double* Float64(const std::string& name) const { return (const double*)at(name); }
+private:
+    friend class DataSource;
+    const void* at(const std::string& name) const {
+        auto it = values_.find(name);
+        if (it == values_.end()) throw std::out_of_range("no aggregate " + name);
+        return it->second.get();
+    }
+    Table keys_; uint64_t n_ = 0;
+    std::map<std::string, std::shared_ptr<void>> values_;
+};
+
 // ---------------------------------------------------------------- DataSource (csvplus.go:207-608)
 class DataSource {
     struct Op { int kind; Predicate pred; std::vector<std::string> cols; std::shared_ptr<Index> index; uint64_t n = 0; std::function<Row(const Row&)> map; };
@@ -621,6 +645,38 @@ public:
             f.close();
             if (!f) throw Error("write " + name + " failed");
         } catch (...) { std::remove(name.c_str()); throw; }
+    }
+    // per-group aggregates on the GPU (an extension beyond the reference API): what a RowFunc folding the rows in order
+    // into a map keyed by the values of keys computes (cpb_groups_*).  Batch by batch: device memory holds the groups and
+    // one batch.  A conversion error throws Error with the reference's text after the rows before it are folded; a
+    // source error is thrown after the delivered rows are folded.
+    Groups GroupBy(const std::vector<std::string>& keys, const std::vector<Agg>& aggs) const {
+        if (keys.empty()) throw std::logic_error("empty column list in GroupBy()");
+        for (size_t i = 0; i < keys.size(); i++) for (size_t j = i + 1; j < keys.size(); j++) if (keys[i] == keys[j]) throw std::logic_error("duplicate column name(s) in GroupBy()");
+        cpb_ctx* c = detail::ctx();
+        detail::Strs k(keys);
+        std::vector<cpb_agg> a;
+        for (auto& x : aggs) a.push_back(cpb_agg{x.op, x.kind, cpb_str{x.column.data(), x.column.size()}});
+        cpb_groups* g = nullptr;
+        if (cpb_groups_open(c, k.v.data(), (int)keys.size(), a.data(), (int)a.size(), &g) != CPB_OK) throw Error(cpb_last_error(c));
+        std::shared_ptr<cpb_groups> hold(g, [c](cpb_groups* p) { cpb_groups_free(c, p); });
+        each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool) {
+            cpb_error e{};
+            detail::check(cpb_groups_push(c, g, t.get(), &e), e);
+            if (err) throw *err;
+            return true;
+        });
+        Groups out;
+        cpb_table* kt = nullptr;
+        if (cpb_groups_result(c, g, &kt, &out.n_) != CPB_OK) throw Error(cpb_last_error(c));
+        out.keys_ = Table(kt);
+        for (size_t i = 0; i < aggs.size(); i++) {
+            void* p = nullptr;
+            if (cpb_device_alloc(c, out.n_ * 8 + 8, &p) != CPB_OK) throw Error(cpb_last_error(c));
+            out.values_[aggs[i].name] = std::shared_ptr<void>(p, [c](void* q) { cpb_device_free(c, q); });
+            if (cpb_groups_values(c, g, (int)i, p) != CPB_OK) throw Error(cpb_last_error(c));
+        }
+        return out;
     }
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }

@@ -382,6 +382,35 @@ int cpb_table_column_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, int
 int cpb_table_set_codes(cpb_ctx* ctx, const cpb_table* t, cpb_str column, const int64_t* dev_codes, const cpb_table* dictionary,
                         cpb_table** out, cpb_error* err);
 
+/* ------------------------------------------------------------------ GroupBy (per-key aggregates over pushed tables)
+ * A groups object folds the rows of every table pushed into it, in push order, as a Go RowFunc folding them in that order
+ * would.  Groups: rows whose key columns hold equal bytes, numbered in order of first appearance.  Aggregates (op, kind,
+ * column): CPB_AGG_COUNT (rows; kind and column ignored), _SUM (int: int64 +=, wrapping; float64: acc += v from +0.0 in
+ * row order, rounded to nearest per addition), _MIN / _MAX (float64: Go's math.Min / math.Max), _FIRST / _LAST (the value
+ * of the group's first / last row).  Inputs are Row.ValueAsInt (CPB_AGG_INT, int64) / ValueAsFloat64 (CPB_AGG_FLOAT64).
+ * open: 1 to 16 distinct key columns, at most 32 aggregates, else CPB_ERR_ARG.
+ * push: a key column t lacks (t with rows): CPB_ERR_DATA / CPB_E_MISSING_COLUMN, line 0, nothing folded.  A conversion
+ * error: the lowest failing row of t (ties to the earlier aggregate; an absent aggregate column fails at row 0), with the
+ * error column_as_int64 / _float64 reports, err->line = that row of t; the rows before it are folded.  A table of 2^32
+ * rows or more, or more than 2^32 - 1 groups in all: CPB_ERR_DATA / CPB_E_TOO_LARGE.  Host synchronisations per push:
+ * one per aggregate with a column, two (the miss count, the sort), two more when some row starts a new group.
+ * result: *keys = a table of the key columns (named and ordered as opened), row g holding group g's key; *ngroups.
+ * values: aggregate i of every group (int64 for count and int inputs, float64 for float64 inputs; 8 * ngroups bytes) into
+ * device memory dev_dst, complete when the call returns.  A groups object belongs to the context that opened it. */
+typedef struct cpb_groups cpb_groups;
+enum { CPB_AGG_COUNT = 0, CPB_AGG_SUM = 1, CPB_AGG_MIN = 2, CPB_AGG_MAX = 3, CPB_AGG_FIRST = 4, CPB_AGG_LAST = 5 };
+enum { CPB_AGG_INT = 0, CPB_AGG_FLOAT64 = 1 };
+typedef struct cpb_agg {
+    int32_t op;   /* CPB_AGG_COUNT .. CPB_AGG_LAST */
+    int32_t kind; /* CPB_AGG_INT / CPB_AGG_FLOAT64 */
+    cpb_str column;
+} cpb_agg;
+int cpb_groups_open(cpb_ctx* ctx, const cpb_str* keys, int nkeys, const cpb_agg* aggs, int naggs, cpb_groups** out);
+int cpb_groups_push(cpb_ctx* ctx, cpb_groups* g, const cpb_table* t, cpb_error* err);
+int cpb_groups_result(cpb_ctx* ctx, const cpb_groups* g, cpb_table** keys, uint64_t* ngroups);
+int cpb_groups_values(cpb_ctx* ctx, const cpb_groups* g, int i, void* dev_dst);
+int cpb_groups_free(cpb_ctx* ctx, cpb_groups* g);
+
 /* ------------------------------------------------------------------ formatted rows (fmt.Sprintf of string columns)
  * Every row's text is fmt.Sprintf(format, v[0], ..., v[nargs-1]), v = the row's values of the columns args (Row.SelectValues,
  * csvplus.go:138-149; a column may be named more than once).  The accepted format language is the subset of Go's fmt whose
