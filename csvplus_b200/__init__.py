@@ -6,10 +6,11 @@ of include/csvplus_b200.h).  This package is the thin host mirror of the referen
 library or a GPU is missing.
 """
 from .api import (All, Any, Categories, Context, CsvPlusError, DataSource, DataSourceError, DeviceBuffer, FormatFloat, FromBytes,  # noqa: F401
-                  FromFile, FromReadCloser, FromReader, Groups, HostBuffer, Index, Like, LoadIndex, Not, Predicate, Reader, Row, Sprintf,
+                  FromFile, FromReadCloser, FromReader, Groups, HostBuffer, Index, Like, LoadIndex, MAX_ORDER_KEYS, Not,
+                  ORDER_KINDS, Predicate, Reader, Row, Sprintf,
                   StopIterationEOF, Table, Take, TakeRows, TakeTable, csv_quote_parity, csv_stream_cut, parse_csv, parse_csv_shard)
 
 __all__ = ["All", "Any", "Categories", "Context", "CsvPlusError", "DataSource", "DataSourceError", "DeviceBuffer", "FormatFloat", "FromBytes", "FromFile",
-           "FromReadCloser", "FromReader", "Groups", "HostBuffer", "Index", "Like", "LoadIndex", "Not", "Predicate", "Reader", "Row",
+           "FromReadCloser", "FromReader", "Groups", "HostBuffer", "Index", "Like", "LoadIndex", "MAX_ORDER_KEYS", "Not", "ORDER_KINDS", "Predicate", "Reader", "Row",
            "Sprintf", "StopIterationEOF", "Table", "Take", "TakeRows", "TakeTable", "csv_quote_parity", "csv_stream_cut", "parse_csv",
            "parse_csv_shard"]

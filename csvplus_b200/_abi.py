@@ -24,6 +24,9 @@ CPB_E_BAD_CODE = 19
 # GroupBy aggregates (cpb_agg): ops and input kinds
 CPB_AGG_OPS = {"count": 0, "sum": 1, "min": 2, "max": 3, "first": 4, "last": 5}
 CPB_AGG_KINDS = {"int": 0, "float64": 1}
+# OrderBy key kinds (cpb_order_key)
+CPB_ORDER_KINDS = {"str": 0, "int": 1, "float64": 2}
+MAX_ORDER_KEYS = 16  # the most keys of one cpb_table_order_by
 
 
 class Str(C.Structure):
@@ -57,6 +60,10 @@ class Agg(C.Structure):
     _fields_ = [("op", C.c_int32), ("kind", C.c_int32), ("column", Str)]
 
 
+class OrderKey(C.Structure):
+    _fields_ = [("column", Str), ("kind", C.c_int32), ("descending", C.c_int32)]
+
+
 class KStat(C.Structure):
     _fields_ = [("name", C.c_char * 48), ("launches", C.c_uint64), ("ms", C.c_double), ("algo_bytes", C.c_uint64)]
 
@@ -80,6 +87,7 @@ SYMBOLS = [
     "cpb_table_set_int64", "cpb_table_set_float64", "cpb_table_set_float32", "cpb_table_set_literal", "cpb_table_filter_flags",
     "cpb_table_column_codes", "cpb_table_set_codes", "cpb_table_set_sprintf", "cpb_table_sprintf_into",
     "cpb_groups_open", "cpb_groups_push", "cpb_groups_result", "cpb_groups_values", "cpb_groups_free",
+    "cpb_table_order_by",
     "cpb_comm_unique_id", "cpb_comm_init_rank", "cpb_init_multi", "cpb_comm_size", "cpb_comm_rank", "cpb_allgather_table",
     "cpb_allgather_tables", "cpb_allgather_u64", "cpb_allgather_layout",
     "cpb_stats_enable", "cpb_stats_reset", "cpb_stats_get", "cpb_kernel_launches", "cpb_host_syncs", "cpb_gen_csv",
@@ -180,6 +188,7 @@ def load():
         "cpb_groups_result": (i32, [vp, vp, P(vp), P(u64)]),
         "cpb_groups_values": (i32, [vp, vp, i32, vp]),
         "cpb_groups_free": (i32, [vp, vp]),
+        "cpb_table_order_by": (i32, [vp, vp, P(OrderKey), i32, u64, vp, P(vp), P(Error)]),
         "cpb_comm_unique_id": (i32, [vp]),
         "cpb_comm_init_rank": (i32, [vp, i32, i32, vp]),
         "cpb_init_multi": (i32, [P(i32), i32, P(vp)]),

@@ -38,6 +38,9 @@ GOB_BATCH_ROWS = 1 << 24
 # push.  128 MiB: on an H100 the streamed orders join of DESIGN §3.7 ran as fast as at 64 MiB with half the host
 # synchronisations, and slower with larger batches (less copy / compute overlap).
 STREAM_BATCH_BYTES = 128 << 20
+# DataSource.OrderBy: the key kinds, and the most keys of one order
+ORDER_KINDS = tuple(_abi.CPB_ORDER_KINDS)
+MAX_ORDER_KEYS = _abi.MAX_ORDER_KEYS
 
 
 def _enc(s) -> bytes:
@@ -563,6 +566,27 @@ class Table:
     def index_on(self, *cols, unique=False) -> "Index":
         a, keep = _strs(cols)
         return self.ctx._new_index("cpb_index_build", self.h, a, len(cols), int(unique), columns=list(cols))
+
+    def order_by(self, *keys, limit: int | None = None, before: "Table | None" = None) -> "Table":
+        """the rows in the order DataSource.OrderBy(*keys) gives them (keys as there), as a new Table; limit: only the
+        first `limit` rows of that order (all of them when None).  before: rows with this table's columns that precede
+        its rows (the result of an earlier call), ordered together with them.  A failing conversion raises CsvPlusError
+        with .row = the row of this table."""
+        specs = _order_keys(keys)
+        arr = (_abi.OrderKey * len(specs))()
+        keep = []
+        for i, (column, kind, desc) in enumerate(specs):
+            b = _enc(column)
+            keep.append(b)
+            arr[i] = _abi.OrderKey(_abi.Str(b, len(b)), _abi.CPB_ORDER_KINDS[kind], int(desc))
+        h, e = C.c_void_p(), _abi.Error()
+        lim = (1 << 64) - 1 if limit is None else max(0, int(limit))
+        if self.ctx._call("cpb_table_order_by", self.h, arr, len(specs), lim, before.h if before is not None else None, C.byref(h),
+                          err=e, accept=(_abi.CPB_ERR_DATA,)):
+            x = CsvPlusError(e.msg.decode("utf-8", "replace"), _abi.CPB_ERR_DATA, e.kind)
+            x.row = e.line
+            raise x
+        return Table(self.ctx, h)
 
     def join(self, index: "Index", *cols, anti=False) -> "Table":
         a, keep = _strs(cols)
@@ -1349,7 +1373,8 @@ class DataSource:
     """A lazily evaluated plan: source + operations.  Calling it with a RowFunc pulls the rows."""
 
     def __init__(self, source, ops: tuple = ()):
-        self._src, self._ops = source, ops  # source: Reader | ("table", Table, line_base) | ("rows", list[Row])
+        # source: Reader | ("table", Table, line_base) | ("rows", list[Row]) | ("ordered", DataSource, keys)
+        self._src, self._ops = source, ops
 
     def _with(self, op) -> "DataSource":
         return DataSource(self._src, self._ops + (op,))
@@ -1388,6 +1413,20 @@ class DataSource:
         sets it, batch by batch"""
         return self._with(("sprintf", column, Sprintf(format, *columns)))
 
+    def OrderBy(self, *keys) -> "DataSource":
+        """the plan's rows in a stable order on the GPU (an extension beyond the reference API, like GroupBy): what Go's
+        slices.SortStableFunc gives with a comparator chaining the keys left to right (cmp.Or of one cmp.Compare per
+        key).  A key is a column name (ascending "str"), (column, kind) or (column, kind, "asc" | "desc"); kind "str"
+        compares the bytes (strings.Compare, IndexOn's order), "int" Row.ValueAsInt, "float64" Row.ValueAsFloat64 as
+        cmp.Compare does (every NaN below every number, -0 == +0).  "desc" reverses that key (NaNs last); rows equal in
+        every key keep plan order.  The plan before OrderBy is consumed completely before any row flows on; the
+        operations after it run on the ordered rows.  OrderBy(...).Top(n) keeps only n rows on the device as the batches
+        are read (memory for n rows and one batch); any other plan orders the materialised rows, as IndexOn does.
+        Errors, raised before any row is delivered: a failing conversion raises the CsvPlusError ToTensors raises for the
+        key columns in key order (.row = the row's ordinal among the rows reaching OrderBy; a missing key column fails at
+        row 0); a source error is raised after the rows before it are read, and a conversion error in those rows wins."""
+        return DataSource(("ordered", self, tuple((c, k, "desc" if d else "asc") for c, k, d in _order_keys(keys))))
+
     def DropColumns(self, *columns):
         if len(columns) == 0:
             raise ValueError("no columns specified in DropColumns()")
@@ -1415,6 +1454,8 @@ class DataSource:
             return s.ctx
         if s[0] == "table":
             return s[1].ctx
+        if s[0] == "ordered":
+            return s[1]._ctx()
         return Context.default()
 
     def _batches(self):
@@ -1443,12 +1484,38 @@ class DataSource:
             finally:
                 src.close()
             return
-        if s[0] == "table":
+        if s[0] == "ordered":
+            state = ("table", self._ordered(s[1], list(s[2]), ops[0][1] if ops and ops[0][0] == "top" else None))
+        elif s[0] == "table":
             state = ("table", s[1])
         else:
             state = ("rows", [dict(r) for r in s[1]])  # iterate() clones, csvplus.go:230
         state, err, _ = self._apply(state, None, ops, carry)
         yield state, err, False
+
+    def _ordered(self, up: "DataSource", keys: list, top: "int | None") -> "Table | None":
+        """the rows of plan `up` ordered by keys (None: it delivers no table); top: only the first top rows are needed,
+        and the batches are folded into them one by one.  Errors are raised here, before any row flows on."""
+        if top is None:
+            t, err = up._table()
+            if t is not None:
+                t = t.order_by(*keys)
+            if err is not None:
+                raise err
+            return t
+        out, seen = None, 0
+        for state, err, _ in up._batches():
+            t = up._as_table(state)
+            if t is not None and (out is None or len(t)):
+                try:
+                    out = t.order_by(*keys, limit=top, before=out)
+                except CsvPlusError as x:
+                    x.row = seen + x.row
+                    raise
+                seen += len(t)
+            if err is not None:
+                raise err
+        return out
 
     def _apply(self, state, err, ops, carry: dict):
         """the operations over one batch -> (state, err, stop); carry: per-operation state across batches"""
@@ -1726,6 +1793,28 @@ class DataSource:
         if t is None:
             t = Table.from_rows(self._ctx(), [], list(columns))
         return t.index_on(*columns, unique=unique)
+
+
+def _order_keys(keys) -> list:
+    """the keys of OrderBy as [(column, kind, descending)], every rule checked (ValueError)"""
+    out = []
+    for k in keys:
+        spec = (k,) if isinstance(k, str) else tuple(k) if isinstance(k, (tuple, list)) else None
+        if spec is None or not 1 <= len(spec) <= 3 or not isinstance(spec[0], str):
+            raise ValueError(f"OrderBy: key {k!r} is not a column name, (column, kind) or (column, kind, direction)")
+        column, kind, direction = (spec + ("str", "asc")[len(spec) - 1:])[:3]
+        if kind not in _abi.CPB_ORDER_KINDS:
+            raise ValueError(f"OrderBy: unknown kind {kind!r} for key {column!r} (want 'str', 'int' or 'float64')")
+        if direction not in ("asc", "desc"):
+            raise ValueError(f"OrderBy: unknown direction {direction!r} for key {column!r} (want 'asc' or 'desc')")
+        out.append((column, kind, direction == "desc"))
+    if not out:
+        raise ValueError("empty key list in OrderBy()")
+    if len({c for c, _, _ in out}) != len(out):
+        raise ValueError("duplicate column name(s) in OrderBy()")
+    if len(out) > MAX_ORDER_KEYS:
+        raise ValueError(f"OrderBy: more than {MAX_ORDER_KEYS} keys")
+    return out
 
 
 def _group_keys(keys) -> list:

@@ -991,6 +991,20 @@ int cpb_groups_free(cpb_ctx* h, cpb_groups* g) {
     });
 }
 
+// ------------------------------------------------------------------ OrderBy
+int cpb_table_order_by(cpb_ctx* h, const cpb_table* t, const cpb_order_key* keys, int nkeys, uint64_t limit, const cpb_table* before,
+                       cpb_table** out, cpb_error* err) {
+    return guarded(h, err, [&](Ctx* c) {
+        const Table& T = table_of(t);
+        need(out && (nkeys <= 0 || keys), "null out or keys");
+        *out = nullptr;
+        std::vector<OrderKey> ks;
+        for (int i = 0; i < nkeys; i++) ks.push_back(OrderKey{to_string(keys[i].column), keys[i].kind, keys[i].descending != 0});
+        *out = wrap(order_table(c, T, ks, limit, before ? &table_of(before) : nullptr));
+        return CPB_OK;
+    });
+}
+
 // ------------------------------------------------------------------ Sprintf columns and text
 int cpb_table_set_sprintf(cpb_ctx* h, const cpb_table* t, cpb_str column, cpb_str format, const cpb_str* args, int nargs, cpb_table** out,
                           cpb_error* err) {

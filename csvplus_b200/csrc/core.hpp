@@ -356,6 +356,15 @@ std::shared_ptr<Index> build_index(Ctx* c, std::shared_ptr<Table> t, const std::
 // stable sort of the row ids 0..n-1 by image words [0, words) (word w of row r at image[w * n + r], compared as unsigned
 // integers): the buffer of the sorted ids.  One host synchronisation (the digit histograms); *traffic += bytes moved.
 Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic);
+// the first k rows (0 < k < n) of that order without sorting: ascending row ids uint32[k + 1] (the last entry n).  MSD
+// radix select with every digit's choice made on the device; one host synchronisation (the digit histograms)
+Buf select_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t k, uint64_t* traffic);
+// rows ids[0..m) of a key image of n_src rows, as an image of m rows
+Buf gather_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n_src, const uint32_t* ids, uint64_t m);
+// per key column the longest value of rows [0, n) of t: the column widths of the key image (one host synchronisation).
+// With `row_cols` (at most 4 columns), *row_max = their longest row, from the same readback.
+std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n, const std::vector<int>* row_cols = nullptr,
+                                 uint32_t* row_max = nullptr);
 std::shared_ptr<Table> sorted_table(Ctx* c, Index& ix);  // materialises ix.table on first use
 void ensure_sorted(Ctx* c, Index& ix);                    // sorts a lazily-sorted unique index on first need of the order
 constexpr int MAXKEYS = 16;
@@ -376,6 +385,8 @@ uint32_t prefix_bytes(const Index& ix, int nk);  // image bytes covered by the f
 void head_flags(Ctx* c, const uint64_t* image, uint64_t n, uint32_t pbytes, uint32_t* head);
 void iota_u32(Ctx* c, uint32_t* p, uint64_t n);  // p[i] = i for i in [0, n)
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
+// the same image written to dst (word w of row r at dst[w * t.nrows + r])
+void pack_into(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint64_t* dst);
 // join.cu.  A join column missing from a non-empty probe table throws DataError.
 std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti);
 // flag[i] (uint32 0/1) = whether the key of probe row i on the probe columns pidx (the first pidx.size() key columns of
@@ -458,6 +469,14 @@ uint64_t groups_count(const Groups& g);
 void groups_values(Ctx* c, const Groups& g, int i, void* dst);
 Ctx* groups_ctx(const Groups& g);
 void groups_free(Groups* g);
+// order.cu: OrderBy (DESIGN §3.16).  The first `limit` rows (every row when limit >= rows) of the stable order of
+// before ‖ t (before: null, or rows with t's columns that precede t's in plan order) under the keys, compared left to
+// right: CPB_ORDER_STR as strings.Compare, _INT as Row.ValueAsInt, _FLOAT64 as cmp.Compare of Row.ValueAsFloat64.
+// Keys: 1..MAXKEYS distinct columns of a known kind, else ArgError.  t's values are converted before anything is ordered:
+// the lowest failing row (ties to the earlier key; a key column t lacks fails at row 0) throws its number_error with line
+// = the row of t.  Rows come back with first_line 0, as an index's rows.
+struct OrderKey { std::string column; int kind; bool descending; };
+std::shared_ptr<Table> order_table(Ctx* c, const Table& t, const std::vector<OrderKey>& keys, uint64_t limit, const Table* before);
 // sprintf.cu: fmt.Sprintf(format, v...) of every row, v = the row's values of columns cols (a name may repeat).  The
 // format is compiled first: one outside the accepted subset, or whose verb count is not cols.size(), throws ArgError
 // CPB_ERR_UNSUPPORTED naming the byte offset.  A column t lacks (on a table with rows) throws DataError

@@ -136,17 +136,11 @@ __global__ void __launch_bounds__(RS_THREADS) radix_scatter_kernel(const uint64_
     }
 }
 
-// Stable sort of `perm` (row ids) by image words [0, words): returns the buffer holding the sorted ids.
-// Which digits are constant over the whole column (their pass would be the identity) does not depend on the order of
-// the rows: the byte histograms of ALL image words are taken from the unsorted image up front and read back with one
-// host round trip for the whole sort (round 1: one per image word).
-Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
-    Buf permA = dev_alloc(c, n * 4), permB = dev_alloc(c, n * 4), keyA = dev_alloc(c, n * 8), keyB = dev_alloc(c, n * 8);
-    iota_u32(c, permA->as<uint32_t>(), n);
-    const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;
-    const uint32_t nblocks = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 4);
-    const uint64_t tpb = (ntiles + nblocks - 1) / nblocks;
-    Buf hist = dev_alloc(c, (size_t)words * 8 * 256 * 4), counts = dev_alloc(c, (256ull * nblocks + 1) * 4), tot = dev_alloc(c, 8);
+// skip[w * 8 + b] = 1 when byte b (0 = least significant) of image word w is the same in every row, so that a radix pass
+// over it would be the identity.  Which digits are constant does not depend on the order of the rows: the byte
+// histograms of ALL image words are taken up front and read back with one host round trip.
+static std::vector<uint8_t> constant_digits(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
+    Buf hist = dev_alloc(c, (size_t)words * 8 * 256 * 4);
     CPB_CUDA(cudaMemsetAsync(hist->p, 0, (size_t)words * 8 * 256 * 4, c->stream));
     {
         KernelTimer kt(c, "sort_hist", n * 8 * words, (int)words);
@@ -160,6 +154,19 @@ Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uin
     for (uint32_t w = 0; w < words; w++)
         for (int b = 0; b < 8; b++)
             for (int v = 0; v < 256; v++) if (hh[((size_t)w * 8 + b) * 256 + v] == n) skip[(size_t)w * 8 + b] = 1;
+    return skip;
+}
+
+// Stable sort of `perm` (row ids) by image words [0, words): returns the buffer holding the sorted ids.  Constant digits
+// (constant_digits) are not passed over (round 1: one host round trip per image word).
+Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t* traffic) {
+    Buf permA = dev_alloc(c, n * 4), permB = dev_alloc(c, n * 4), keyA = dev_alloc(c, n * 8), keyB = dev_alloc(c, n * 8);
+    iota_u32(c, permA->as<uint32_t>(), n);
+    const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;
+    const uint32_t nblocks = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 4);
+    const uint64_t tpb = (ntiles + nblocks - 1) / nblocks;
+    Buf counts = dev_alloc(c, (256ull * nblocks + 1) * 4), tot = dev_alloc(c, 8);
+    const std::vector<uint8_t> skip = constant_digits(c, image, words, n, traffic);
     for (int w = (int)words - 1; w >= 0; w--) {
         bool any = false;
         for (int b = 0; b < 8; b++) any = any || !skip[(size_t)w * 8 + b];
@@ -182,6 +189,119 @@ Buf sort_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uin
         }
     }
     return permA;
+}
+
+// ------------------------------------------------------------------ top-k selection: MSD radix select
+// The threshold is found digit by digit, most significant first, on the device: a pass histograms one digit of the rows
+// still in the running (their higher digits equal the threshold's so far) and a one-block step picks the bucket that
+// holds the need-th of them.  st[r] holds row r's digit of the last pass, or SEL_OUT once the row left the running: pass
+// p + 1 keeps the rows whose digit is the bucket pass p chose, so no pass reads an earlier word again.
+constexpr uint16_t SEL_OUT = 0xFFFF;
+struct SelState {
+    uint64_t need;    // rows still to take among those equal to the threshold so far
+    uint32_t choice;  // the bucket the last pass chose
+    uint32_t first;   // no pass has run yet: every row is in the running
+    uint32_t done;    // the chosen bucket is taken whole: the threshold is known as far as it matters
+};
+__global__ void __launch_bounds__(256) select_hist_kernel(const uint64_t* __restrict__ word, uint64_t n, int shift, uint16_t* __restrict__ st,
+                                                          const SelState* __restrict__ s, uint32_t* __restrict__ hist) {
+    if (s->done) return;
+    __shared__ uint32_t sh[256];
+    sh[threadIdx.x] = 0;
+    __syncthreads();
+    const bool first = s->first != 0;
+    const uint32_t prev = s->choice;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (!first) {
+            const uint16_t v = st[i];
+            if (v != prev) {
+                if (v != SEL_OUT) st[i] = SEL_OUT;
+                continue;
+            }
+        }
+        const uint32_t d = (uint32_t)(word[i] >> shift) & 0xffu;
+        st[i] = (uint16_t)d;
+        atomicAdd(&sh[d], 1u);
+    }
+    __syncthreads();
+    if (sh[threadIdx.x]) atomicAdd(&hist[threadIdx.x], sh[threadIdx.x]);
+}
+// one block of 256 threads: the bucket d holding the need-th row in the running; its digit goes into the threshold and
+// its mask, need becomes the rank within d, and hist is cleared for the next pass
+__global__ void __launch_bounds__(256) select_choose_kernel(uint32_t* __restrict__ hist, SelState* __restrict__ s, uint64_t* __restrict__ thr,
+                                                            uint64_t* __restrict__ mask, int shift) {
+    __shared__ uint32_t sc[256];
+    const uint32_t t = threadIdx.x, h = hist[t];
+    const bool live = !s->done;
+    const uint64_t need = s->need;
+    sc[t] = h;
+    __syncthreads();
+    for (uint32_t d = 1; d < 256; d <<= 1) {  // inclusive scan
+        const uint32_t v = t >= d ? sc[t - d] : 0;
+        __syncthreads();
+        sc[t] += v;
+        __syncthreads();
+    }
+    const uint64_t below = sc[t] - h;
+    if (live && h && below < need && need <= below + h) {
+        s->need = need - below;
+        s->choice = t;
+        s->first = 0;
+        s->done = need - below == h;
+        *thr |= (uint64_t)t << shift;
+        *mask |= 0xffull << shift;
+    }
+    hist[t] = 0;
+}
+
+// The first k rows (0 < k < n) of the order (image words [0, words) as unsigned integers, then row), as ascending row
+// ids uint32[k + 1] (the last entry is n).  One host synchronisation (constant_digits).
+Buf select_by_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n, uint64_t k, uint64_t* traffic) {
+    const std::vector<uint8_t> skip = constant_digits(c, image, words, n, traffic);
+    Buf st = dev_alloc(c, n * 2), state = dev_alloc(c, sizeof(SelState)), hist = dev_alloc(c, 256 * 4),
+        thr = dev_alloc(c, (size_t)words * 16);
+    uint64_t* th = thr->as<uint64_t>();
+    uint64_t* mk = th + words;  // the digits of the threshold that are known (constant digits never are: every row has them)
+    const SelState s0{k, 0, 1, 0};
+    CPB_CUDA(cudaMemcpyAsync(state->p, &s0, sizeof s0, cudaMemcpyHostToDevice, c->stream));
+    CPB_CUDA(cudaMemsetAsync(hist->p, 0, 256 * 4, c->stream));
+    CPB_CUDA(cudaMemsetAsync(thr->p, 0, (size_t)words * 16, c->stream));
+    SelState* sp = state->as<SelState>();
+    {
+        int passes = 0;
+        for (uint32_t w = 0; w < words; w++)
+            for (int b = 0; b < 8; b++) passes += !skip[(size_t)w * 8 + b];
+        KernelTimer kt(c, "select_pass", n * 12 * (uint64_t)passes, 2 * passes);
+        for (uint32_t w = 0; w < words; w++)
+            for (int b = 7; b >= 0; b--) {
+                if (skip[(size_t)w * 8 + b]) continue;
+                select_hist_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(image + (uint64_t)w * n, n, 8 * b, st->as<uint16_t>(), sp,
+                                                                            hist->as<uint32_t>());
+                select_choose_kernel<<<1, 256, 0, c->stream>>>(hist->as<uint32_t>(), sp, th + w, mk + w, 8 * b);
+            }
+        CPB_CUDA(cudaGetLastError());
+    }
+    st.reset();
+    // the rows below the threshold, and the first `need` rows equal to it in row order: k rows, as the choices made sure
+    Buf lt = dev_alloc(c, n * 4), eq = dev_alloc(c, n * 4), pos = dev_alloc(c, (n + 1) * 4), tot = dev_alloc(c, 8), ids = dev_alloc(c, (k + 1) * 4);
+    {
+        KernelTimer kt(c, "select_take", n * (8 * (uint64_t)words + 40), 4);
+        uint32_t *l = lt->as<uint32_t>(), *e = eq->as<uint32_t>(), *ep = pos->as<uint32_t>();
+        each_row(c, n, [=] __device__(uint64_t i) {
+            int r = 0;
+            for (uint32_t w = 0; w < words && r == 0; w++) {
+                const uint64_t m = mk[w], x = image[(uint64_t)w * n + i] & m, y = th[w] & m;
+                r = x < y ? -1 : x > y ? 1 : 0;
+            }
+            l[i] = r < 0; e[i] = r == 0;
+        });
+        exclusive_scan_u32(c, e, ep, n, tot->as<uint64_t>());
+        each_row(c, n, [=] __device__(uint64_t i) { l[i] = l[i] || (e[i] && ep[i] < sp->need); });
+        exclusive_scan_u32(c, l, ep, n, tot->as<uint64_t>());  // (the ranks among the equal rows are used up)
+        compact_flags(c, FlagScan{l, n, pos, k}, 0, ids->as<uint32_t>());
+    }
+    *traffic += n * 12 * 8 * (uint64_t)words + n * (8 * (uint64_t)words + 40);
+    return ids;
 }
 
 // ------------------------------------------------------------------ adjacent compare (unique check, groups)
@@ -216,14 +336,19 @@ Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const
     KeyDesc kd{};
     describe_keys(c, t, kidx, width, kd);
     *words_out = kd.words;
-    uint64_t n = (uint64_t)t.nrows;
-    Buf img = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)kd.words * n) * 8);
+    Buf img = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)kd.words * (uint64_t)t.nrows) * 8);
+    pack_into(c, t, kidx, width, img->as<uint64_t>());
+    return img;
+}
+void pack_into(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint64_t* dst) {
+    KeyDesc kd{};
+    describe_keys(c, t, kidx, width, kd);
+    const uint64_t n = (uint64_t)t.nrows;
     if (n && kd.words) {
         KernelTimer kt(c, "key_pack", n * kd.words * 8);
-        key_pack_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(kd, n, img->as<uint64_t>());
+        key_pack_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(kd, n, dst);
         CPB_CUDA(cudaGetLastError());
     }
-    return img;
 }
 
 // the longest row of up to 4 columns taken together (the bytes of all their values in one row)
@@ -242,8 +367,8 @@ __global__ void max_row_bytes_kernel(RowCols rc, uint64_t n, uint32_t* out) {
 
 // per key column the longest value of rows [0, n) of t: the column widths of the key image.  With `row_cols` (at most
 // 4 columns), *row_max = their longest row, from the same readback.
-static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n,
-                                        const std::vector<int>* row_cols = nullptr, uint32_t* row_max = nullptr) {
+std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vector<int>& key_cols, uint64_t n, const std::vector<int>* row_cols,
+                                 uint32_t* row_max) {
     const size_t nk = key_cols.size();
     Buf wd = dev_alloc(c, (nk + 1) * 4);
     CPB_CUDA(cudaMemsetAsync(wd->p, 0, (nk + 1) * 4, c->stream));
@@ -263,7 +388,7 @@ static std::vector<uint32_t> key_widths(Ctx* c, const Table& t, const std::vecto
 }
 
 // rows ids[0..m) of a key image of n_src rows, as an image of m rows
-static Buf gather_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n_src, const uint32_t* ids, uint64_t m) {
+Buf gather_image(Ctx* c, const uint64_t* image, uint32_t words, uint64_t n_src, const uint32_t* ids, uint64_t m) {
     Buf out = dev_alloc(c, std::max<uint64_t>(1, (uint64_t)words * m) * 8);
     for (uint32_t w = 0; w < words; w++) gather_u64(c, image + (uint64_t)w * n_src, ids, out->as<uint64_t>() + (uint64_t)w * m, m);
     return out;

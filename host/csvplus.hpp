@@ -208,6 +208,10 @@ struct CPred {
 
 // ---------------------------------------------------------------- Table / Index handles
 class Index;
+// one key of DataSource::OrderBy / Table::OrderBy: column compared as kind (CPB_ORDER_STR: strings.Compare, _INT:
+// Row.ValueAsInt, _FLOAT64: cmp.Compare of Row.ValueAsFloat64, every NaN first), the comparison reversed when descending
+struct OrderKey { std::string column; int kind = CPB_ORDER_STR; bool descending = false; };
+
 class Table {
 public:
     explicit Table(cpb_table* h = nullptr) : h_(h, cpb_table_free) {}
@@ -233,6 +237,15 @@ public:
     Table slice(int64_t lo, int64_t hi) const {  // a row-range view (cpb_table_slice)
         cpb_table* out = nullptr;
         if (cpb_table_slice(detail::ctx(), h_.get(), lo, hi, &out) != CPB_OK) throw Error(cpb_last_error(detail::ctx()));
+        return Table(out);
+    }
+    // the first `limit` rows of the stable order of before ‖ these rows under keys (cpb_table_order_by); before: rows with
+    // these columns that precede them, or null.  A failing conversion throws Error with the reference's text.
+    Table OrderBy(const std::vector<OrderKey>& keys, uint64_t limit = UINT64_MAX, const Table* before = nullptr) const {
+        std::vector<cpb_order_key> k;
+        for (auto& x : keys) k.push_back(cpb_order_key{cpb_str{x.column.data(), x.column.size()}, x.kind, x.descending ? 1 : 0});
+        cpb_table* out = nullptr; cpb_error e{};
+        detail::check(cpb_table_order_by(detail::ctx(), h_.get(), k.data(), (int)k.size(), limit, before ? before->get() : nullptr, &out, &e), e);
         return Table(out);
     }
     static Table from_rows(const std::vector<Row>& rows) {  // TakeRows, csvplus.go:218
@@ -531,6 +544,23 @@ class DataSource {
 public:
     explicit DataSource(Reader r) : reader_(new Reader(std::move(r))) {}
     explicit DataSource(Table t) : table_(new Table(std::move(t))) {}
+    // the plan's rows in a stable order on the GPU (an extension beyond the reference API, like GroupBy): Go's
+    // slices.SortStableFunc with cmp.Or of one cmp.Compare per key.  The plan before it is consumed completely before any
+    // row flows on.  OrderBy(keys).Top(n) folds the batches into their first n rows as they are read (device memory for n
+    // rows and one batch); any other plan orders the materialised rows.  A conversion error throws Error, a source error
+    // DataSourceError, before any row is delivered.
+    DataSource OrderBy(std::vector<OrderKey> keys) const {
+        if (keys.empty()) throw std::logic_error("empty key list in OrderBy()");
+        if (keys.size() > 16) throw std::logic_error("OrderBy: more than 16 keys");
+        for (size_t i = 0; i < keys.size(); i++) {
+            if (keys[i].kind < CPB_ORDER_STR || keys[i].kind > CPB_ORDER_FLOAT64) throw std::logic_error("OrderBy: unknown key kind");
+            for (size_t j = i + 1; j < keys.size(); j++) if (keys[i].column == keys[j].column) throw std::logic_error("duplicate column name(s) in OrderBy()");
+        }
+        DataSource d;
+        d.up_ = std::make_shared<const DataSource>(*this);
+        d.keys_ = std::move(keys);
+        return d;
+    }
     DataSource Filter(Predicate p) const { return with({FILTER, std::move(p)}); }
     DataSource Map(std::function<Row(const Row&)> f) const { Op o{MAP}; o.map = std::move(f); return with(std::move(o)); }
     DataSource Top(uint64_t n) const { Op o{TOP}; o.n = n; return with(std::move(o)); }
@@ -681,6 +711,24 @@ public:
     Index IndexOn(const std::vector<std::string>& cols) const { return index(cols, false); }
     Index UniqueIndexOn(const std::vector<std::string>& cols) const { return index(cols, true); }
 private:
+    DataSource() = default;
+    // the rows of up_ in the order of keys_; top: only the first *top rows are needed, folded batch by batch
+    Table ordered(const uint64_t* top) const {
+        if (!top) {
+            std::unique_ptr<DataSourceError> err;
+            Table t = up_->run(&err);
+            t = t.OrderBy(keys_);
+            if (err) throw *err;
+            return t;
+        }
+        Table out;
+        up_->each([&](Table& t, std::unique_ptr<DataSourceError>& err, bool) {
+            if (!out.get() || t.size()) out = t.OrderBy(keys_, *top, out.get() ? &out : nullptr);
+            if (err) throw *err;
+            return true;
+        });
+        return out;
+    }
     DataSource with(Op o) const { DataSource d = *this; d.ops_.push_back(std::move(o)); return d; }
     Index index(const std::vector<std::string>& cols, bool unique) const {
         if (cols.empty()) throw std::logic_error("empty column list in CreateIndex()");
@@ -750,9 +798,12 @@ private:
                                          ? &ops_[0].pred : nullptr;
             if (fused) first = 1;
             reader_->batches(fused, apply);
+        } else if (up_) {
+            apply(ordered(!ops_.empty() && ops_[0].kind == TOP ? &ops_[0].n : nullptr), nullptr, false);
         } else apply(*table_, nullptr, false);
     }
     std::shared_ptr<Reader> reader_; std::shared_ptr<Table> table_; std::vector<Op> ops_;
+    std::shared_ptr<const DataSource> up_; std::vector<OrderKey> keys_;  // an ordered plan: up_'s rows by keys_
 };
 
 inline DataSource Take(const Reader& r) { return DataSource(r); }                          // csvplus.go:252

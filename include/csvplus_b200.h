@@ -411,6 +411,35 @@ int cpb_groups_result(cpb_ctx* ctx, const cpb_groups* g, cpb_table** keys, uint6
 int cpb_groups_values(cpb_ctx* ctx, const cpb_groups* g, int i, void* dev_dst);
 int cpb_groups_free(cpb_ctx* ctx, cpb_groups* g);
 
+/* ------------------------------------------------------------------ OrderBy (stable multi-key order, first `limit` rows)
+ * The order is Go's slices.SortStableFunc with a comparator chaining the keys left to right (cmp.Or of one cmp.Compare
+ * per key): CPB_ORDER_STR compares the value's bytes (strings.Compare, IndexOn's order), _INT compares Row.ValueAsInt as
+ * int64, _FLOAT64 compares Row.ValueAsFloat64 as cmp.Compare does (every NaN below every number and all NaNs equal,
+ * -0 == +0).  descending != 0 reverses that key (cmp.Compare(b, a): NaNs last).  Rows equal in every key keep their order.
+ * keys: 1 to 16 distinct columns of a known kind, else CPB_ERR_ARG.
+ * *out = the first `limit` rows (all of them when limit >= rows) of that order of before ‖ t; before (nullable) holds
+ * rows that precede t's rows in plan order, with t's columns, so that a stream of batches is folded into its first
+ * `limit` rows as out = order_by(batch, limit, before = the previous out).  The rows of *out are numbered from 0.
+ * Every value of t is converted before anything is ordered: the lowest failing row (ties to the earlier key) is
+ * CPB_ERR_DATA with the error cpb_table_column_as_int64 / _float64 reports, err->line = the row of t; a key column t
+ * lacks (t with rows) is CPB_E_MISSING_COLUMN at line 0.  A key image over 4 KiB is CPB_ERR_UNSUPPORTED; t of 2^32 rows
+ * or more CPB_ERR_DATA / CPB_E_TOO_LARGE.
+ * Host synchronisations, with S = 1 when some key is a string key (else 0) and I = the int and float64 keys, for t of n
+ * rows with columns and k = min(limit, n) > 0, without before:
+ *   select route (2k <= n: radix select, then a sort of the k rows): S + I + 3
+ *   sort route (otherwise: the whole image sorted, the first k gathered):  S + I + 2
+ *   (k == 0: S + I)
+ * With before: S + I for t; when k < n, 2 more (t's k rows selected or sorted, then gathered); 1 for the concatenation;
+ * then the union ordered as above (S + I + its route). */
+enum { CPB_ORDER_STR = 0, CPB_ORDER_INT = 1, CPB_ORDER_FLOAT64 = 2 };
+typedef struct cpb_order_key {
+    cpb_str column;
+    int32_t kind;      /* CPB_ORDER_STR / _INT / _FLOAT64 */
+    int32_t descending;
+} cpb_order_key;
+int cpb_table_order_by(cpb_ctx* ctx, const cpb_table* t, const cpb_order_key* keys, int nkeys, uint64_t limit,
+                       const cpb_table* before, cpb_table** out, cpb_error* err);
+
 /* ------------------------------------------------------------------ formatted rows (fmt.Sprintf of string columns)
  * Every row's text is fmt.Sprintf(format, v[0], ..., v[nargs-1]), v = the row's values of the columns args (Row.SelectValues,
  * csvplus.go:138-149; a column may be named more than once).  The accepted format language is the subset of Go's fmt whose
