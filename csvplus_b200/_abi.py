@@ -81,7 +81,7 @@ SYMBOLS = [
     "cpb_index_build", "cpb_index_num_rows", "cpb_index_num_keys", "cpb_index_table", "cpb_index_find", "cpb_index_sub",
     "cpb_index_dup_groups", "cpb_index_dedup_apply", "cpb_index_dedup_apply2", "cpb_free", "cpb_index_free",
     "cpb_index_key_col", "cpb_index_gob_begin", "cpb_index_gob_into", "cpb_index_load_gob",
-    "cpb_join", "cpb_except", "cpb_table_to_csv", "cpb_table_to_csv_device", "cpb_table_to_csv_into",
+    "cpb_join", "cpb_except", "cpb_left_join", "cpb_table_to_csv", "cpb_table_to_csv_device", "cpb_table_to_csv_into",
     "cpb_table_to_json", "cpb_table_to_json_device", "cpb_table_to_json_into",
     "cpb_table_column_as_int64", "cpb_table_column_as_float64", "cpb_table_column_as_float32",
     "cpb_table_set_int64", "cpb_table_set_float64", "cpb_table_set_float32", "cpb_table_set_literal", "cpb_table_filter_flags",
@@ -165,6 +165,7 @@ def load():
         "cpb_index_load_gob": (i32, [vp, vp, u64, P(vp), P(Error)]),
         "cpb_join": (i32, [vp, vp, vp, P(Str), i32, P(vp), P(Error)]),
         "cpb_except": (i32, [vp, vp, vp, P(Str), i32, P(vp), P(Error)]),
+        "cpb_left_join": (i32, [vp, vp, vp, P(Str), i32, P(vp), P(Error)]),
         "cpb_table_to_csv": (i32, [vp, vp, P(Str), i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_csv_device": (i32, [vp, vp, P(Str), i32, P(vp), P(u64), P(Error)]),
         "cpb_table_to_csv_into": (i32, [vp, vp, P(Str), i32, i32, vp, u64, P(u64), P(Error)]),

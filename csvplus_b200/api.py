@@ -588,9 +588,12 @@ class Table:
             raise x
         return Table(self.ctx, h)
 
-    def join(self, index: "Index", *cols, anti=False) -> "Table":
+    def join(self, index: "Index", *cols, anti=False, left=False) -> "Table":
+        """Join (anti: Except; left: LeftJoin) of this table's rows against index on cols"""
+        if anti and left:
+            raise ValueError("join: anti and left exclude each other")
         a, keep = _strs(cols)
-        return self.ctx._new_table("cpb_except" if anti else "cpb_join", self.h, index.h, a, len(cols))
+        return self.ctx._new_table("cpb_except" if anti else "cpb_left_join" if left else "cpb_join", self.h, index.h, a, len(cols))
 
     def _pinned_bytes(self, name: str, *args) -> bytes:
         """an entry that returns its bytes in new pinned host memory"""
@@ -1442,6 +1445,19 @@ class DataSource:
             raise ValueError("too many source columns in Join()")
         return self._with(("join", index, columns))
 
+    def LeftJoin(self, index: Index, *columns):
+        """Join that keeps every row (an extension beyond the reference API, like GroupBy and OrderBy).  columns as for
+        Join: none is a natural join on the index key names, fewer than the index keys a prefix match.  Rows in plan
+        order: a row Join gives k >= 1 rows gives exactly those rows (mergeRows(indexRow, row), the row winning name
+        collisions); any other row gives one row, its own values plus "" in every column only the index contributes --
+        what Row.SafeGetValue(col, "") reads from the row alone.  An index key column named differently from the row's
+        join column is such a column (LeftJoin(customers, "cust_id") leaves the index's "id" empty on a miss).  The
+        columns are Join's, so the matched rows taken in order are Join's result.  Streamed batch by batch like Join,
+        with Join's errors: a missing join column raises DataSourceError at row 0."""
+        if len(columns) > len(index.columns):
+            raise ValueError("too many source columns in LeftJoin()")
+        return self._with(("leftjoin", index, columns))
+
     def Except(self, index: Index, *columns):
         if len(columns) > len(index.columns):
             raise ValueError("too many source columns in Except()")
@@ -1523,7 +1539,7 @@ class DataSource:
         stop = False
         for i, op in enumerate(ops):
             kind = op[0]
-            device_ok = (kind in ("select", "dropcols", "join", "except", "top", "drop", "maptensors", "filtertensors", "sprintf")
+            device_ok = (kind in ("select", "dropcols", "join", "leftjoin", "except", "top", "drop", "maptensors", "filtertensors", "sprintf")
                          or (kind in ("filter", "takewhile", "dropwhile") and isinstance(op[1], Predicate) and op[1].lowerable()))
             if device_ok:
                 if state[0] == "rows":
@@ -1536,6 +1552,7 @@ class DataSource:
                     elif kind == "dropcols": t = t.drop(*op[1])
                     elif kind == "filter": t = t.filter(op[1])
                     elif kind == "join": t = t.join(op[1], *op[2])
+                    elif kind == "leftjoin": t = t.join(op[1], *op[2], left=True)
                     elif kind == "except": t = t.join(op[1], *op[2], anti=True)
                     elif kind == "sprintf": t = t.with_column(op[1], op[2])
                     elif kind == "top":  # note: the reference pulls one extra row (SURVEY §Q8)
@@ -1563,7 +1580,7 @@ class DataSource:
                                 carry[i] = False
                             t = t.slice(k, len(t))
                 except DataSourceError as e:
-                    if err is None or kind in ("select", "join", "except"):
+                    if err is None or kind in ("select", "join", "leftjoin", "except"):
                         return ("rows", []), e, True
                     raise
                 if kind == "top":

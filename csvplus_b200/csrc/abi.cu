@@ -762,7 +762,7 @@ int cpb_index_key_col(const cpb_index* ix, int k, cpb_str* out) {
     return CPB_OK;
 }
 
-static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, bool anti,
+static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, JoinMode mode,
                        cpb_table** out, cpb_error* err) {
     return guarded(h, err, [&](Ctx* c) {
         const Table& P = table_of(probe);
@@ -770,17 +770,22 @@ static int join_common(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, 
         need(out, "null out");
         *out = nullptr;
         std::vector<std::string> names = n ? str_list(cols, n) : X.key_cols;  // natural join, csvplus.go:546-547
-        if (names.size() > X.key_cols.size())
-            throw ArgError{CPB_ERR_ARG, anti ? "too many source columns in Except()" : "too many source columns in Join()"};  // :548-549, :591-592
-        *out = wrap(join_tables(c, P, X, names, anti));
+        if (names.size() > X.key_cols.size())  // :548-549, :591-592
+            throw ArgError{CPB_ERR_ARG, mode == JoinMode::anti   ? "too many source columns in Except()"
+                                        : mode == JoinMode::left ? "too many source columns in LeftJoin()"
+                                                                 : "too many source columns in Join()"};
+        *out = wrap(join_tables(c, P, X, names, mode));
         return CPB_OK;
     });
 }
 int cpb_join(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, cpb_table** out, cpb_error* err) {
-    return join_common(h, probe, ix, cols, n, false, out, err);
+    return join_common(h, probe, ix, cols, n, JoinMode::inner, out, err);
 }
 int cpb_except(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, cpb_table** out, cpb_error* err) {
-    return join_common(h, probe, ix, cols, n, true, out, err);
+    return join_common(h, probe, ix, cols, n, JoinMode::anti, out, err);
+}
+int cpb_left_join(cpb_ctx* h, const cpb_table* probe, const cpb_index* ix, const cpb_str* cols, int n, cpb_table** out, cpb_error* err) {
+    return join_common(h, probe, ix, cols, n, JoinMode::left, out, err);
 }
 
 // ------------------------------------------------------------------ index files (gob.cu)

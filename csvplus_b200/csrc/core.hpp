@@ -329,8 +329,10 @@ FlagScan scan_flags(Ctx* c, const uint32_t* flags, uint64_t n);
 void compact_flags(Ctx* c, const FlagScan& s, uint32_t add, uint32_t* out);
 // flag[i] (uint32 0/1) = whether v[i] is nonzero (nonzero) / is zero (!nonzero)
 void nonzero_flags(Ctx* c, const uint32_t* v, uint64_t n, bool nonzero, uint32_t* flag);
-// rows row_ids[0, nout) of t (rows 0..nout-1 when row_ids is null: a view compacted into buffers of its own)
-std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout);
+// rows row_ids[0, nout) of t (rows 0..nout-1 when row_ids is null: a view compacted into buffers of its own).  miss: an
+// id NO_ROW gives a row of empty values (its own kernel instantiations, so the plain gather carries no such test)
+constexpr uint32_t NO_ROW = 0xffffffffu;
+std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout, bool miss = false);
 // the rows of t whose flag (uint32 0/1, one per row) is set: scan_flags, compact_flags timed as compact_ids, gather_rows.
 // first, when given: the position of the first set flag (one more host synchronisation when there is one)
 std::shared_ptr<Table> rows_where(Ctx* c, const Table& t, const uint32_t* flags, uint64_t* first = nullptr);
@@ -342,9 +344,10 @@ struct Compiled;  // pred.cuh
 // names (a stream compiles once and builds its set indexes once).  The error and record counts stay the parse's; row 0's
 // line is the line of the first row kept.
 void filter_parsed(Ctx* c, Parsed& p, const cpb_pred* pred, std::shared_ptr<Compiled>& comp);
-// rows `ids` (positions in `order`) of the index restricted to columns `cols` (row-slot path when it pays, else gather_rows)
+// rows `ids` (positions in `order`) of the index restricted to columns `cols` (row-slot path when it pays, else gather_rows);
+// miss: an id NO_ROW gives empty values
 std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout,
-                                         RowOrder order);
+                                         RowOrder order, bool miss = false);
 std::shared_ptr<Table> concat_tables(Ctx* c, const std::vector<const Table*>& parts);
 // full-key join against ix.derived.rowhash: payload columns `cols` (source column numbers, a non-empty subset of its cols)
 // for every probe row, empty where the row finds no key; *matches = probe rows that found their key.  One random access
@@ -387,8 +390,10 @@ void iota_u32(Ctx* c, uint32_t* p, uint64_t n);  // p[i] = i for i in [0, n)
 Buf pack_with_widths(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint32_t* words_out);
 // the same image written to dst (word w of row r at dst[w * t.nrows + r])
 void pack_into(Ctx* c, const Table& t, const std::vector<int>& kidx, const std::vector<uint32_t>& width, uint64_t* dst);
-// join.cu.  A join column missing from a non-empty probe table throws DataError.
-std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti);
+// join.cu.  A join column missing from a non-empty probe table throws DataError.  inner: Join; anti: Except; left:
+// LeftJoin (Join's rows, and every probe row Join drops kept once with its index-only columns empty)
+enum class JoinMode { inner, anti, left };
+std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, JoinMode mode);
 // flag[i] (uint32 0/1) = whether the key of probe row i on the probe columns pidx (the first pidx.size() key columns of
 // ix) is in the index (hit) / is not (!hit): Except's test, and the set terms of a predicate.  A probe value longer than
 // the index column's widest value is not in it.

@@ -45,14 +45,13 @@ __device__ __forceinline__ unsigned long long lookback(unsigned long long* st, u
 }
 
 // GATHER: the scanned values are the lengths of the strings picked by `ids` (identity when null) from the offsets
-// array `in` -- the length array of a gather is never materialised.
+// array `in` -- the length array of a gather is never materialised.  MISS (with GATHER): an id NO_ROW has length 0.
 // The offsets out[] are sums modulo 2^32 (a caller uses them only when the total fits); *total is exact.  The thread,
 // warp and tile sums are kept in 32 bits plus a count of their wraps past 2^32: a sum of non-negative addends has
 // wrapped exactly when it is smaller than the addend just added.  A few long rows wrap one tile's sum.
-template <bool GATHER>
-__global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* __restrict__ in, const uint32_t* __restrict__ ids,
-                                                                uint32_t* out, uint64_t n, unsigned long long* state,
-                                                                uint32_t* ticket, unsigned long long* total) {
+template <bool GATHER, bool MISS>
+__device__ __forceinline__ void scan_u32_tiles(const uint32_t* __restrict__ in, const uint32_t* __restrict__ ids, uint32_t* out, uint64_t n,
+                                               unsigned long long* state, uint32_t* ticket, unsigned long long* total) {
     __shared__ uint32_t s_tile;
     __shared__ unsigned long long s_warp[SCAN_THREADS / 32];  // the warps' exact sums
     __shared__ unsigned long long s_prefix;
@@ -70,7 +69,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* 
         for (int i = 0; i < SCAN_ITEMS; i++) {
             v[i] = 0;
             if (base + i < n) {
-                if (GATHER) { const uint32_t r = ids ? ids[base + i] : (uint32_t)(base + i); v[i] = in[r + 1] - in[r]; }
+                if (GATHER) { const uint32_t r = ids ? ids[base + i] : (uint32_t)(base + i); v[i] = MISS && r == NO_ROW ? 0u : in[r + 1] - in[r]; }
                 else v[i] = in[base + i];
             }
             sum += v[i];
@@ -101,13 +100,26 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* 
         __syncthreads();
     }
 }
+template <bool GATHER>
+__global__ void __launch_bounds__(SCAN_THREADS) scan_u32_kernel(const uint32_t* __restrict__ in, const uint32_t* __restrict__ ids,
+                                                                uint32_t* out, uint64_t n, unsigned long long* state,
+                                                                uint32_t* ticket, unsigned long long* total) {
+    scan_u32_tiles<GATHER, false>(in, ids, out, n, state, ticket, total);
+}
+// the lengths of a gather whose ids may be NO_ROW (LeftJoin's index side)
+__global__ void __launch_bounds__(SCAN_THREADS) scan_miss_len_kernel(const uint32_t* __restrict__ in, const uint32_t* __restrict__ ids,
+                                                                     uint32_t* out, uint64_t n, unsigned long long* state,
+                                                                     uint32_t* ticket, unsigned long long* total) {
+    scan_u32_tiles<true, true>(in, ids, out, n, state, ticket, total);
+}
 
 __global__ void scan_empty_kernel(uint32_t* out, unsigned long long* total) { out[0] = 0; *total = 0; }
 
 // out may alias in; out has n+1 entries (out[n] = total, truncated to 32 bits); *total_dev holds the 64-bit total.
-// gather_off != nullptr: scan the lengths off[ids[i]+1]-off[ids[i]] instead of `in` (ids may be null = identity).
+// gather_off != nullptr: scan the lengths off[ids[i]+1]-off[ids[i]] instead of `in` (ids may be null = identity; with
+// miss, an id NO_ROW has length 0).
 static void scan_impl(Ctx* c, const uint32_t* in, const uint32_t* gather_off, const uint32_t* ids, uint32_t* out, uint64_t n,
-                      uint64_t* total_dev) {
+                      uint64_t* total_dev, bool miss = false) {
     if (n == 0) {
         KernelTimer kt(c, "scan_u32", 0);
         scan_empty_kernel<<<1, 1, 0, c->stream>>>(out, (unsigned long long*)total_dev);
@@ -121,7 +133,8 @@ static void scan_impl(Ctx* c, const uint32_t* in, const uint32_t* gather_off, co
     uint32_t grid = (uint32_t)std::min<uint64_t>(ntiles, (uint64_t)c->sm_count * 8);
     if (gather_off) {
         KernelTimer kt(c, "scan_gather_len", n * (ids ? 16 : 12));
-        scan_u32_kernel<true><<<grid, SCAN_THREADS, 0, c->stream>>>(gather_off, ids, out, n, state, ticket, (unsigned long long*)total_dev);
+        if (miss) scan_miss_len_kernel<<<grid, SCAN_THREADS, 0, c->stream>>>(gather_off, ids, out, n, state, ticket, (unsigned long long*)total_dev);
+        else scan_u32_kernel<true><<<grid, SCAN_THREADS, 0, c->stream>>>(gather_off, ids, out, n, state, ticket, (unsigned long long*)total_dev);
     } else {
         KernelTimer kt(c, "scan_u32", n * 8);
         scan_u32_kernel<false><<<grid, SCAN_THREADS, 0, c->stream>>>(in, nullptr, out, n, state, ticket, (unsigned long long*)total_dev);
@@ -193,9 +206,11 @@ __device__ __forceinline__ void warp_store_stage(uint8_t* gb, const uint8_t* sta
 }
 constexpr int GW_WARPS = 8;
 constexpr int GW_STAGE = 2048;  // bytes staged per warp; longer groups take the direct path
-__global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32_t* __restrict__ src_off, const uint8_t* __restrict__ src,
-                                                                    const uint32_t* __restrict__ ids, const uint32_t* __restrict__ dst_off,
-                                                                    uint8_t* __restrict__ dst, uint64_t n) {
+// (MISS: an id NO_ROW is an empty value)
+template <bool MISS>
+__device__ __forceinline__ void gather_copy_groups(const uint32_t* __restrict__ src_off, const uint8_t* __restrict__ src,
+                                                   const uint32_t* __restrict__ ids, const uint32_t* __restrict__ dst_off,
+                                                   uint8_t* __restrict__ dst, uint64_t n) {
     __shared__ __align__(16) uint8_t stage_all[GW_WARPS][GW_STAGE + 16];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint8_t* stage = stage_all[warp];
@@ -205,7 +220,8 @@ __global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32
         uint32_t s = 0, len = 0, d = 0;
         if (i < n) {
             const uint32_t r = ids ? ids[i] : (uint32_t)i;
-            s = src_off[r]; len = src_off[r + 1] - s; d = dst_off[i];
+            if (!MISS || r != NO_ROW) { s = src_off[r]; len = src_off[r + 1] - s; }
+            d = dst_off[i];
         }
         const uint32_t d0 = __shfl_sync(0xffffffffu, d, 0);
         const uint64_t last = (g * 32 + 31 < n ? g * 32 + 31 : n - 1) - g * 32;
@@ -222,9 +238,20 @@ __global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32
         }
     }
 }
+__global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_kernel(const uint32_t* __restrict__ src_off, const uint8_t* __restrict__ src,
+                                                                    const uint32_t* __restrict__ ids, const uint32_t* __restrict__ dst_off,
+                                                                    uint8_t* __restrict__ dst, uint64_t n) {
+    gather_copy_groups<false>(src_off, src, ids, dst_off, dst, n);
+}
+__global__ void __launch_bounds__(GW_WARPS * 32) gather_copy_miss_kernel(const uint32_t* __restrict__ src_off, const uint8_t* __restrict__ src,
+                                                                         const uint32_t* __restrict__ ids, const uint32_t* __restrict__ dst_off,
+                                                                         uint8_t* __restrict__ dst, uint64_t n) {
+    gather_copy_groups<true>(src_off, src, ids, dst_off, dst, n);
+}
 
-// gathers several columns with ONE host synchronisation (totals of all columns read back together)
-static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column*>& srcs, const uint32_t* ids, int64_t nout) {
+// gathers several columns with ONE host synchronisation (totals of all columns read back together); miss: an id NO_ROW
+// is an empty value
+static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column*>& srcs, const uint32_t* ids, int64_t nout, bool miss) {
     std::vector<Column> out(srcs.size());
     if (srcs.empty()) return out;
     Buf totals = dev_alloc(c, srcs.size() * 8);
@@ -232,7 +259,7 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
         out[k].name = srcs[k]->name;
         out[k].offsets = dev_alloc(c, ((size_t)nout + 1) * 4);
         uint32_t* o = out[k].offsets->as<uint32_t>();
-        scan_impl(c, nullptr, srcs[k]->off(), ids, o, (uint64_t)nout, totals->as<uint64_t>() + k);
+        scan_impl(c, nullptr, srcs[k]->off(), ids, o, (uint64_t)nout, totals->as<uint64_t>() + k, miss);
     }
     const std::vector<uint64_t> tot = read_back<uint64_t>(c, totals->p, srcs.size());
     for (size_t k = 0; k < srcs.size(); k++)  // every column checked before any is copied: a refused gather writes nothing
@@ -242,7 +269,11 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
         if (nout && tot[k]) {
             KernelTimer kt(c, "gather_copy", 2 * tot[k] + (uint64_t)nout * 12);
             const uint32_t gblocks = (uint32_t)std::min<uint64_t>(((uint64_t)nout + GW_WARPS * 32 - 1) / (GW_WARPS * 32), (uint64_t)c->sm_count * 16);
-            gather_copy_kernel<<<gblocks, GW_WARPS * 32, 0, c->stream>>>(srcs[k]->off(), srcs[k]->bytes(), ids,
+            if (miss)
+                gather_copy_miss_kernel<<<gblocks, GW_WARPS * 32, 0, c->stream>>>(srcs[k]->off(), srcs[k]->bytes(), ids,
+                                                                                   out[k].offsets->as<uint32_t>(), out[k].data->as<uint8_t>(), (uint64_t)nout);
+            else
+                gather_copy_kernel<<<gblocks, GW_WARPS * 32, 0, c->stream>>>(srcs[k]->off(), srcs[k]->bytes(), ids,
                                                                               out[k].offsets->as<uint32_t>(), out[k].data->as<uint8_t>(), (uint64_t)nout);
             CPB_CUDA(cudaGetLastError());
         }
@@ -250,7 +281,7 @@ static std::vector<Column> gather_columns(Ctx* c, const std::vector<const Column
     return out;
 }
 
-std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout) {
+std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_ids, int64_t nout, bool miss) {
     auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = t.first_line;
     // columns sharing buffers (AssumeHeader aliases) are gathered once
     std::vector<const Column*> uniq; std::vector<int> which(t.cols.size());
@@ -261,7 +292,7 @@ std::shared_ptr<Table> gather_rows(Ctx* c, const Table& t, const uint32_t* row_i
         if (f < 0) { f = (int)uniq.size(); uniq.push_back(&t.cols[i]); }
         which[i] = f;
     }
-    auto g = gather_columns(c, uniq, row_ids, nout);
+    auto g = gather_columns(c, uniq, row_ids, nout, miss);
     for (size_t i = 0; i < t.cols.size(); i++) { Column col = g[which[i]]; col.name = t.cols[i].name; r->cols.push_back(col); }
     return r;
 }
@@ -409,6 +440,17 @@ struct LensById {  // row slots: lens[ids[i]]
         }
     }
 };
+struct LensByIdMiss {  // row slots, ids that may be NO_ROW (an empty row): lens[ids[i]] or 0
+    const uint32_t* __restrict__ lens;
+    const uint32_t* __restrict__ ids;
+    __device__ __forceinline__ void load(uint64_t base, uint64_t n, uint32_t (&p)[LS_ITEMS]) const {
+#pragma unroll
+        for (int i = 0; i < LS_ITEMS; i++) {
+            const uint32_t r = base + i < n ? ids[base + i] : NO_ROW;
+            p[i] = r != NO_ROW ? lens[r] : 0u;
+        }
+    }
+};
 struct LensSeq {  // row-carrying hash table: lens[i], written by rowhash_probe_kernel
     const uint32_t* __restrict__ lens;
     __device__ __forceinline__ void load(uint64_t base, uint64_t n, uint32_t (&p)[LS_ITEMS]) const {
@@ -518,11 +560,12 @@ __device__ __forceinline__ void or_value(uint8_t* stage, uint32_t q, const uint8
 // out like the destination (all columns of the group, one 16-byte aligned region each), and the warp writes every
 // column's region in ONE pass of aligned 16-byte stores, the partial first / last vector of a column with a few
 // aligned narrower stores.  No lane loops over the bytes of a value.  A column whose region does not fit the stage
-// any more is copied straight to its destination.  Row i's slot is slots[ids[i]], or slots[i] when ids is null.
+// any more is copied straight to its destination.  Row i's slot is slots[ids[i]], or slots[i] when ids is null; with
+// MISS, an id NO_ROW reads no slot (its lengths, from the offsets, are 0).
 constexpr uint32_t SC_STRIDE_PAD = 12;  // slot stride S + 12 bytes: an odd number of words, and room for or_value's over-read
-template <int NC, int SV>  // SV: 16-byte vectors held per prefetched slot (S <= 16 SV)
-__global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
-                                                                  SlotOut out, uint64_t n) {
+template <int NC, int SV, bool MISS>  // SV: 16-byte vectors held per prefetched slot (S <= 16 SV)
+__device__ __forceinline__ void slot_copy_groups(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
+                                                 SlotOut out, uint64_t n) {
     // (16 bytes ahead of the first slot: or_value may read the word before a value)
     __shared__ __align__(16) uint8_t slot_sm[16 + GW_WARPS * 32 * (RS_MAXS + SC_STRIDE_PAD)];
     __shared__ __align__(16) uint8_t stage_all[GW_WARPS][GW_STAGE];
@@ -539,9 +582,11 @@ __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t*
 #pragma unroll
         for (int c = 0; c < NC; c++) { nd[c] = 0; nlen[c] = 0; }
         if (i < n) {
-            const uint4* sp = reinterpret_cast<const uint4*>(slots + (ids ? (uint64_t)ids[i] : i) * S);
+            if (!MISS || ids[i] != NO_ROW) {
+                const uint4* sp = reinterpret_cast<const uint4*>(slots + (ids ? (uint64_t)ids[i] : i) * S);
 #pragma unroll
-            for (int j = 0; j < SV; j++) if (j < (int)(S / 16)) v[j] = __ldg(sp + j);
+                for (int j = 0; j < SV; j++) if (j < (int)(S / 16)) v[j] = __ldg(sp + j);
+            }
 #pragma unroll
             for (int c = 0; c < NC; c++) { nd[c] = out.off[c][i]; nlen[c] = out.off[c][i + 1] - nd[c]; }
         }
@@ -609,6 +654,16 @@ __global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t*
         __syncwarp();  // the slots and the stage are overwritten by the next round
     }
 }
+template <int NC, int SV>
+__global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_kernel(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
+                                                                  SlotOut out, uint64_t n) {
+    slot_copy_groups<NC, SV, false>(slots, S, ids, out, n);
+}
+template <int NC, int SV>
+__global__ void __launch_bounds__(GW_WARPS * 32) slot_copy_miss_kernel(const uint8_t* __restrict__ slots, uint32_t S, const uint32_t* __restrict__ ids,
+                                                                       SlotOut out, uint64_t n) {
+    slot_copy_groups<NC, SV, true>(slots, S, ids, out, n);
+}
 
 static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& cols, RowOrder order) {
     std::lock_guard<std::mutex> lk(ix.mu);
@@ -651,11 +706,12 @@ static RowSlots& ensure_row_slots(Ctx* c, Index& ix, const std::vector<int>& col
 
 // Columns `names` of n rows from slots of S bytes: the offsets scanned from the packed lengths `src` gives
 // (scan_lens_kernel), ONE host synchronisation for the column totals and *counter (the 64-bit count at counter_dev,
-// when given), then the bytes copied by slot_copy_kernel from slot ids[i] (slot i when ids is null).
+// when given), then the bytes copied by slot_copy_kernel from slot ids[i] (slot i when ids is null; with miss, none
+// for an id NO_ROW, which src gives length 0).
 template <class Src>
 static std::vector<Column> slot_gather(Ctx* c, const std::vector<std::string>& names, uint64_t n, const Src& src, const char* scan_name,
                                        uint64_t scan_bytes, const uint8_t* slots, uint32_t S, const uint32_t* ids,
-                                       const unsigned long long* counter_dev, uint64_t* counter) {
+                                       const unsigned long long* counter_dev, uint64_t* counter, bool miss = false) {
     const int nc = (int)names.size();
     SlotOut so{};
     std::vector<Column> out(nc);
@@ -691,7 +747,8 @@ static std::vector<Column> slot_gather(Ctx* c, const std::vector<std::string>& n
     {
         KernelTimer kt(c, "slot_copy", 2 * all + n * (4 + 4 * (uint64_t)nc));
         const uint32_t gblocks = (uint32_t)std::min<uint64_t>((n + GW_WARPS * 32 - 1) / (GW_WARPS * 32), (uint64_t)c->sm_count * 16);
-#define CPB_SC2(NC, SV) slot_copy_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(slots, S, ids, so, n)
+#define CPB_SC2(NC, SV) (miss ? slot_copy_miss_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(slots, S, ids, so, n) \
+                             : slot_copy_kernel<NC, SV><<<gblocks, GW_WARPS * 32, 0, c->stream>>>(slots, S, ids, so, n))
 #define CPB_SC(NC) (S <= 16 ? CPB_SC2(NC, 1) : S <= 32 ? CPB_SC2(NC, 2) : CPB_SC2(NC, 4))
         switch (nc) { case 1: CPB_SC(1); break; case 2: CPB_SC(2); break; case 3: CPB_SC(3); break; default: CPB_SC(4); break; }
 #undef CPB_SC
@@ -701,7 +758,8 @@ static std::vector<Column> slot_gather(Ctx* c, const std::vector<std::string>& n
     return out;
 }
 
-std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, RowOrder order) {
+std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<int>& cols, const uint32_t* ids, int64_t nout, RowOrder order,
+                                         bool miss) {
     if (cols.empty()) {  // nothing to gather (a join whose index columns are all key columns): no slots, no sorted rows
         auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = ix.schema().first_line;
         return r;
@@ -711,7 +769,7 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
         const Table& st = *keep;
         Table sub; sub.ctx = c; sub.nrows = st.nrows; sub.first_line = st.first_line;
         for (int ci : cols) sub.cols.push_back(st.cols[ci]);
-        return gather_rows(c, sub, ids, nout);
+        return gather_rows(c, sub, ids, nout, miss);
     };
     bool use = ids != nullptr && nout > 0 && cols.size() <= (size_t)RS_MAXC;
     if (use) {
@@ -727,8 +785,12 @@ std::shared_ptr<Table> gather_index_rows(Ctx* c, Index& ix, const std::vector<in
     for (int ci : cols) names.push_back(t.cols[ci].name);
     auto r = std::make_shared<Table>(); r->ctx = c; r->nrows = nout; r->first_line = t.first_line;
     const uint64_t n = (uint64_t)nout;
-    r->cols = slot_gather(c, names, n, LensById{rs.lens->as<uint32_t>(), ids}, "slot_scan_lens", n * (8 + 4 * (uint64_t)cols.size()),
-                          rs.slots->as<uint8_t>(), rs.S, ids, nullptr, nullptr);
+    if (miss)
+        r->cols = slot_gather(c, names, n, LensByIdMiss{rs.lens->as<uint32_t>(), ids}, "slot_scan_lens", n * (8 + 4 * (uint64_t)cols.size()),
+                              rs.slots->as<uint8_t>(), rs.S, ids, nullptr, nullptr, true);
+    else
+        r->cols = slot_gather(c, names, n, LensById{rs.lens->as<uint32_t>(), ids}, "slot_scan_lens", n * (8 + 4 * (uint64_t)cols.size()),
+                              rs.slots->as<uint8_t>(), rs.S, ids, nullptr, nullptr);
     return r;
 }
 

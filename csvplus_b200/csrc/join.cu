@@ -499,7 +499,16 @@ Buf key_flags(Ctx* c, const Table& probe, const std::vector<int>& pidx, Index& i
     return flag;
 }
 
-std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, bool anti) {
+// LeftJoin (mode left) keeps Join's path up to the point where Join drops the probe rows that found nothing; there it keeps
+// them, with every index-only column empty:
+//  * row-carrying table: rowhash_gather's full-length columns are already empty on a miss, so nothing is compacted; the
+//    index key columns Join takes from the probe are gathered from it again with the miss rows' ids NO_ROW;
+//  * run routes: every probe row gives max(cnt, 1) pairs (one more host synchronisation: their total), a miss one pair
+//    whose index id is NO_ROW, and the index side (key columns included) is gathered with empty values for it.
+// Every probe row matching exactly once returns Join's result on Join's kernels; no match at all (an empty index
+// included) returns the probe's columns shared and each index-only column as zeroed offsets, with no gather.
+std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const std::vector<std::string>& cols, JoinMode mode) {
+    const bool anti = mode == JoinMode::anti, left = mode == JoinMode::left;
     const uint64_t np = (uint64_t)probe.nrows, ni = (uint64_t)ix.nrows;
     const int nk = (int)cols.size();
     std::vector<int> pidx;
@@ -516,7 +525,8 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     // the probe value.  icol_key[j] = k takes output column j from probe key column pidx[k]; -1 gathers it from the
     // index (gather_idx: those index columns, in order).  Rows out of key order are searched as the reference does
     // (join_search_kernel): a run there can hold rows whose keys are below the probe's, so every index column is gathered.
-    std::vector<int> icol_key, gather_idx;
+    // (all_idx: every index-only column, key columns included, in order)
+    std::vector<int> icol_key, gather_idx, all_idx;
     const Table& ischema = ix.schema();  // names only: the sorted columns may not be materialised
     if (!anti) for (size_t q = 0; q < ischema.cols.size(); q++) {
         if (probe.find(ischema.cols[q].name) >= 0) continue;
@@ -525,6 +535,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         icols.push_back(&ischema.cols[q]);
         icol_key.push_back(key);
         if (key < 0) gather_idx.push_back((int)q);
+        all_idx.push_back((int)q);
     }
     for (auto& col : probe.cols) pcols.push_back(&col);
 
@@ -557,6 +568,15 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         Buf miss = key_flags(c, probe, pidx, ix, false);
         return flagged_rows(probe, scan_flags(c, miss->as<uint32_t>(), np));
     }
+    // LeftJoin where no probe row matches: the probe's columns shared, each index-only column np empty values
+    auto all_missed = [&]() {
+        Buf zero = dev_alloc(c, (np + 1) * 4), none = dev_alloc(c, 16);
+        CPB_CUDA(cudaMemsetAsync(zero->p, 0, (np + 1) * 4, c->stream));
+        out->nrows = (int64_t)np;
+        for (auto* p : icols) out->cols.push_back(Column{p->name, zero, none, 0});
+        for (auto* p : pcols) out->cols.push_back(*p);
+        return out;
+    };
     if (ix.derived.rowhash.slots && nk == (int)ix.key_cols.size()) {
         // a unique index with a row-carrying table joined on its full key: one random access per probe row
         Buf hit;
@@ -571,11 +591,30 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         } else {
             gi = rowhash_gather(c, ix, probe, pidx, gather_idx, &m);
         }
-        if (m == 0) return empty_result();
+        if (m == 0) return left ? all_missed() : empty_result();
         out->nrows = (int64_t)np;
         put_index_cols(*gi, [&](int k) { return probe.cols[pidx[k]]; });
         for (auto* p : pcols) out->cols.push_back(*p);
         if (m == np) return out;  // every probe row matched: the probe columns are shared as they are
+        if (left) {
+            // the full-length result is LeftJoin's once the key columns taken from the probe are empty on the miss rows
+            std::vector<size_t> keyed;
+            Table kt; kt.ctx = c; kt.nrows = (int64_t)np;
+            for (size_t j = 0; j < icols.size(); j++)
+                if (icol_key[j] >= 0) { keyed.push_back(j); kt.cols.push_back(probe.cols[pidx[icol_key[j]]]); }
+            if (keyed.empty()) return out;
+            if (!hit) hit = rowhash_flags(c, probe, pidx, ix, true);
+            Buf ids = dev_alloc(c, np * 4);
+            {
+                KernelTimer kt_ids(c, "left_ids", np * 8);
+                const uint32_t* h = hit->as<uint32_t>();
+                uint32_t* id = ids->as<uint32_t>();
+                each_row(c, np, [=] __device__(uint64_t i) { id[i] = h[i] ? (uint32_t)i : NO_ROW; });
+            }
+            auto g = gather_rows(c, kt, ids->as<uint32_t>(), (int64_t)np, true);
+            for (size_t x = 0; x < keyed.size(); x++) { Column col = g->cols[x]; col.name = icols[keyed[x]]->name; out->cols[keyed[x]] = col; }
+            return out;
+        }
         // probe rows that found nothing: the full-length result (empty index values there) compacted to the rows that did
         if (!hits.pos) {
             hit = rowhash_flags(c, probe, pidx, ix, true);
@@ -591,7 +630,7 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
     // result ARE the probe columns, in order — share their buffers instead of copying them; no scan of the counts
     const bool probe_identity = ni != 0 && hf[2] == 0 && m == np;
     if (m > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "join result exceeds 2^32-2 rows; probe in smaller batches"};
-    if (m == 0) return empty_result();
+    if (m == 0) return left ? all_missed() : empty_result();
     if (probe_identity) {
         auto gi = gather_index_rows(c, ix, gather_idx, lo->as<uint32_t>(), (int64_t)m, order);  // lo[i] is the single matching index row
         out->nrows = (int64_t)m;
@@ -600,6 +639,38 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
         return out;
     }
     Buf pos = dev_alloc(c, (np + 1) * 4);
+    Table pt; pt.ctx = c; pt.nrows = (int64_t)np;
+    for (auto* p : pcols) pt.cols.push_back(*p);
+    if (left) {
+        // max(cnt[i], 1) pairs per probe row, a miss as one pair (i, NO_ROW); the pair count is read back
+        {
+            KernelTimer kt(c, "left_counts", np * 8);
+            const uint32_t* run_cnt = cnt->as<uint32_t>();
+            uint32_t* at = pos->as<uint32_t>();
+            each_row(c, np, [=] __device__(uint64_t i) { at[i] = run_cnt[i] ? run_cnt[i] : 1u; });
+        }
+        exclusive_scan_u32(c, pos->as<uint32_t>(), pos->as<uint32_t>(), np, flags->as<uint64_t>());
+        const uint64_t ml = read_back<uint64_t>(c, flags->p);
+        if (ml > 0xfffffffeull) throw DataError{CPB_E_TOO_LARGE, -1, 0, false, "join result exceeds 2^32-2 rows; probe in smaller batches"};
+        Buf pid = dev_alloc(c, ml * 4), iid = dev_alloc(c, ml * 4);
+        {
+            KernelTimer kt(c, "join_pairs", np * 12 + ml * 8);
+            const uint32_t *run_lo = lo->as<uint32_t>(), *run_cnt = cnt->as<uint32_t>(), *at = pos->as<uint32_t>();
+            uint32_t *probe_id = pid->as<uint32_t>(), *index_id = iid->as<uint32_t>();
+            each_row(c, np, [=] __device__(uint64_t i) {
+                const uint32_t k = run_cnt[i], p = at[i], l = run_lo[i];
+                if (k == 0) { probe_id[p] = (uint32_t)i; index_id[p] = NO_ROW; }
+                for (uint32_t j = 0; j < k; j++) { probe_id[p + j] = (uint32_t)i; index_id[p + j] = l + j; }
+            });
+        }
+        // every index-only column from the index: a key column taken from the probe would be a value on a miss row
+        auto gi = gather_index_rows(c, ix, all_idx, iid->as<uint32_t>(), (int64_t)ml, order, true);
+        auto gp = gather_rows(c, pt, pid->as<uint32_t>(), (int64_t)ml);
+        out->nrows = (int64_t)ml;
+        for (size_t j = 0; j < icols.size(); j++) { Column col = gi->cols[j]; col.name = icols[j]->name; out->cols.push_back(col); }
+        for (auto& col : gp->cols) out->cols.push_back(col);
+        return out;
+    }
     exclusive_scan_u32(c, cnt->as<uint32_t>(), pos->as<uint32_t>(), np, flags->as<uint64_t>());
     Buf pid = dev_alloc(c, m * 4), iid = dev_alloc(c, m * 4);
     {
@@ -612,8 +683,6 @@ std::shared_ptr<Table> join_tables(Ctx* c, const Table& probe, Index& ix, const 
             for (uint32_t j = 0; j < k; j++) { probe_id[p + j] = (uint32_t)i; index_id[p + j] = l + j; }
         });
     }
-    Table pt; pt.ctx = c; pt.nrows = (int64_t)np;
-    for (auto* p : pcols) pt.cols.push_back(*p);
     auto gi = gather_index_rows(c, ix, gather_idx, iid->as<uint32_t>(), (int64_t)m, order);
     auto gp = gather_rows(c, pt, pid->as<uint32_t>(), (int64_t)m);
     out->nrows = (int64_t)m;

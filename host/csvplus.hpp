@@ -540,7 +540,7 @@ private:
 // ---------------------------------------------------------------- DataSource (csvplus.go:207-608)
 class DataSource {
     struct Op { int kind; Predicate pred; std::vector<std::string> cols; std::shared_ptr<Index> index; uint64_t n = 0; std::function<Row(const Row&)> map; };
-    enum { FILTER, SELECT, DROPCOLS, JOIN, EXCEPT, TOP, DROP, MAP };
+    enum { FILTER, SELECT, DROPCOLS, JOIN, EXCEPT, LEFT_JOIN, TOP, DROP, MAP };
 public:
     explicit DataSource(Reader r) : reader_(new Reader(std::move(r))) {}
     explicit DataSource(Table t) : table_(new Table(std::move(t))) {}
@@ -574,6 +574,12 @@ public:
     DataSource Except(const Index& ix, const std::vector<std::string>& c = {}) const {
         if (c.size() > ix.columns().size()) throw std::logic_error("too many source columns in Except()");
         Op o{EXCEPT}; o.cols = c; o.index.reset(new Index(ix)); return with(std::move(o));
+    }
+    // Join that keeps every row (an extension beyond the reference API, cpb_left_join): a row Join drops is passed on once
+    // with "" in every column only the index contributes.  Columns as Join's.
+    DataSource LeftJoin(const Index& ix, const std::vector<std::string>& c = {}) const {
+        if (c.size() > ix.columns().size()) throw std::logic_error("too many source columns in LeftJoin()");
+        Op o{LEFT_JOIN}; o.cols = c; o.index.reset(new Index(ix)); return with(std::move(o));
     }
     // sinks: each batch of a streamed input is delivered before the next one is parsed
     void operator()(const RowFunc& fn) const {
@@ -771,6 +777,7 @@ private:
                     case DROPCOLS: detail::check(cpb_table_drop(detail::ctx(), t.get(), c.v.data(), (int)o.cols.size(), &out), e); break;
                     case JOIN: detail::check(cpb_join(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
                     case EXCEPT: detail::check(cpb_except(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
+                    case LEFT_JOIN: detail::check(cpb_left_join(detail::ctx(), t.get(), o.index->get(), c.v.data(), (int)o.cols.size(), &out, &e), e); break;
                     case TOP: {  // the reference pulls n + 1 rows then stops (io.EOF): a later error is never met
                         const uint64_t keep = o.n > seen[i] ? std::min(n, o.n - seen[i]) : 0;
                         seen[i] += n;

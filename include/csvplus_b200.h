@@ -293,6 +293,15 @@ int cpb_join(cpb_ctx* ctx, const cpb_table* probe, const cpb_index* ix, const cp
 /* DataSource.Except (csvplus.go:588-608): probe rows whose key is absent from the index */
 int cpb_except(cpb_ctx* ctx, const cpb_table* probe, const cpb_index* ix, const cpb_str* probe_cols, int n,
                cpb_table** out, cpb_error* err);
+/* DataSource.LeftJoin: cpb_join that keeps every probe row.  probe_cols as for cpb_join.  In probe order, a probe row
+ * that cpb_join gives k >= 1 rows gives exactly those rows; any other probe row gives one row: its own values, and ""
+ * in every column only the index contributes (index columns whose names the probe lacks, an index key column named
+ * differently from its probe column included).  The columns are cpb_join's, so the matched rows taken in order are
+ * cpb_join's result.  An empty index gives every probe row; an empty probe an empty table with cpb_join's columns.
+ * Errors are cpb_join's: a missing join column CPB_E_MISSING_COLUMN at row 0; a result above 2^32-2 rows or a column
+ * of 4 GiB or more CPB_E_TOO_LARGE; more probe_cols than index keys CPB_ERR_ARG "too many source columns in LeftJoin()". */
+int cpb_left_join(cpb_ctx* ctx, const cpb_table* probe, const cpb_index* ix, const cpb_str* probe_cols, int n,
+                  cpb_table** out, cpb_error* err);
 
 /* ------------------------------------------------------------------ ToCsv
  * DataSource.ToCsv (csvplus.go:379-406) + encoding/csv.Writer defaults: header line, then one line
