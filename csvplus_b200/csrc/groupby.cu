@@ -92,21 +92,14 @@ __global__ void __launch_bounds__(GB_WARPS * 32) groupby_hash_kernel(const KeyCo
             if (valid) { const uint32_t s = kc.off[k][i]; len = kc.off[k][i + 1] - s; sp += s; }
             const bool is_long = valid && len > LONG_BYTES;
             uint64_t hk = 0;
-            if (valid && !is_long) {
-                uint64_t sum = 0;
-                for (uint32_t w = 0; w * 8 < len; w++) sum += word_mix(word_at(sp, len, w), w);
-                hk = hash_finish(sum, len);
-            }
+            if (valid && !is_long) hk = hash_thread(sp, len);
             for (uint32_t m = __ballot_sync(0xffffffffu, is_long); m; m &= m - 1) {
                 const int l = __ffs(m) - 1;
                 const uint8_t* lp = reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<uintptr_t>(sp), l));
                 const uint32_t ll = __shfl_sync(0xffffffffu, len, l);
-                uint64_t sum = 0;
-                for (uint32_t w = lane; w * 8 < ll; w += 32) sum += word_mix(word_at(lp, ll, w), w);
-                sum = warp_sum_u64(sum);
-                if (lane == l) hk = hash_finish(sum, ll);
+                hk = hash_warp(lp, ll, lane, l, hk);
             }
-            h = fmix64(h + word_mix(hk, (uint32_t)k));
+            h = row_hash_step(h, hk, (uint32_t)k);
         }
         if (valid) hashes[i] = h;
     }

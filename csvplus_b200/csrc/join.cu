@@ -21,13 +21,6 @@ namespace cpb {
 
 constexpr uint32_t EMPTY = 0xffffffffu;
 
-__device__ __forceinline__ uint64_t hash_prefix(const uint64_t* img, uint64_t n, uint64_t r, uint32_t pbytes) {
-    uint32_t full = pbytes >> 3, rem = pbytes & 7;
-    uint64_t h = 0x9E3779B97F4A7C15ull;
-    for (uint32_t w = 0; w < full; w++) h = mix64(h ^ img[(uint64_t)w * n + r]);
-    if (rem) h = mix64(h ^ (img[(uint64_t)full * n + r] & (~0ull << (8 * (8 - rem)))));
-    return h;
-}
 __global__ void hash_insert_kernel(const uint64_t* __restrict__ image, uint64_t n, uint32_t pbytes, const uint32_t* __restrict__ heads,
                                    uint64_t nheads, uint32_t* slots, uint64_t mask) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -1,10 +1,14 @@
 // keyhash.cuh — the byte-value hash and equality of codes.cu and groupby.cu.  The hash of a value is the sum of
 // word_mix(word i, i) over its 8-byte little-endian words (the last one zero-padded), finished with the length
 // (hash_finish).  A sum does not depend on which lane added which word, so one thread or a whole warp computes the same
-// hash.  A value of at most LONG_BYTES is hashed and compared by one thread; a longer one by a whole warp.
+// hash.  A value of at most LONG_BYTES is hashed and compared by one thread; a longer one by a whole warp.  GroupBy
+// chains the hashes hk of a row's key columns k = 0, 1, ... from h = 0 as h = fmix64(h + word_mix(hk, k)) (row_hash_step).
+// tests/hash_ref.py restates every function here, and tests/hash_harness.cu checks that restatement on the device.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "util.cuh"
 
 namespace cpb {
 
@@ -29,6 +33,22 @@ __device__ __forceinline__ uint64_t word_at(const uint8_t* sp, uint32_t len, uin
     if (rem < 8) v &= (1ull << (8 * rem)) - 1;
     return v;
 }
+// the hash of the len bytes at sp, by one thread
+__device__ __forceinline__ uint64_t hash_thread(const uint8_t* sp, uint32_t len) {
+    uint64_t sum = 0;
+    for (uint32_t w = 0; w * 8 < len; w++) sum += word_mix(word_at(sp, len, w), w);
+    return hash_finish(sum, len);
+}
+// the same hash by the whole warp: every lane calls it with the same sp and len; the hash is valid on lane `owner`
+__device__ __forceinline__ uint64_t hash_warp(const uint8_t* sp, uint32_t len, int lane, int owner, uint64_t h) {
+    uint64_t sum = 0;
+    for (uint32_t w = lane; w * 8 < len; w += 32) sum += word_mix(word_at(sp, len, w), w);
+    sum = warp_sum_u64(sum);
+    if (lane == owner) h = hash_finish(sum, len);
+    return h;
+}
+// one key column's hash hk folded into GroupBy's row hash h (column k, counted from 0; h starts at 0)
+__device__ __forceinline__ uint64_t row_hash_step(uint64_t h, uint64_t hk, uint32_t k) { return fmix64(h + word_mix(hk, k)); }
 __device__ __forceinline__ bool equal_thread(const uint8_t* a, const uint8_t* b, uint32_t len) {
     const uint32_t nw = (len + 7) / 8;
     for (uint32_t w = 0; w < nw; w++) if (word_at(a, len, w) != word_at(b, len, w)) return false;

@@ -17,6 +17,15 @@ __device__ __forceinline__ uint64_t hash3(unsigned long long a, unsigned long lo
     return mix64(mix64(mix64(0x9E3779B97F4A7C15ull ^ a) ^ b) ^ c);
 }
 __device__ __forceinline__ uint64_t slot_of(uint64_t h, uint64_t nslots) { return __umul64hi(h, nslots); }
+// the hash of the first pbytes bytes of row r of a key image of n rows (word w at img[w * n + r]): the ordinal probe
+// tables of join.cu (smem, global) start at hash_prefix & (nslots - 1)
+__device__ __forceinline__ uint64_t hash_prefix(const uint64_t* img, uint64_t n, uint64_t r, uint32_t pbytes) {
+    uint32_t full = pbytes >> 3, rem = pbytes & 7;
+    uint64_t h = 0x9E3779B97F4A7C15ull;
+    for (uint32_t w = 0; w < full; w++) h = mix64(h ^ img[(uint64_t)w * n + r]);
+    if (rem) h = mix64(h ^ (img[(uint64_t)full * n + r] & (~0ull << (8 * (8 - rem)))));
+    return h;
+}
 
 __device__ __forceinline__ unsigned long long bswap64(unsigned long long x) {
     return ((unsigned long long)__byte_perm((uint32_t)x, 0, 0x0123) << 32) | __byte_perm((uint32_t)(x >> 32), 0, 0x0123);

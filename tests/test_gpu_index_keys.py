@@ -23,6 +23,7 @@ import pytest
 
 from oracle import oracle as orc
 from tests import gob_oracle as g
+from tests import hash_ref as hr
 from tests import index_ref as ref
 from tests.helpers import assert_table_equals_oracle, gpu_ctx
 
@@ -104,43 +105,16 @@ def _b(rows):
 
 
 # ------------------------------------------------------------------ the probe table a join takes (join.cu)
-def _len_bytes(w):  # the length field after a key column of width w (core.hpp: len_field_bytes)
-    return 1 if w < 255 else 2 if w < 65535 else 4
-
-
-def _image_bytes(widths):
-    return sum(w + _len_bytes(w) for w in widths)
-
-
-def _ordinal_slots(nheads):
-    s = 1
-    while s < max(16, nheads * 2):
-        s <<= 1
-    return s
-
-
-def _probe_kind(nheads, pbytes, nrows):  # join.cu: probe_kind
-    if (_ordinal_slots(nheads) + nheads + 1) * 4 <= 200 * 1024:
-        return "smem"
-    if pbytes <= 12 and nheads == nrows:
-        return "unique16"
-    if pbytes <= 24:
-        return "run32"
-    return "global"
-
-
 def _hash_build_bytes(kind, nheads, pbytes):  # join.cu: ensure_hash's hash_build record
     b = nheads * (pbytes + 8)
-    if kind == "unique16":
-        b += (nheads * 2 + 16) * 16
-    elif kind == "run32":
-        b += (nheads + nheads // 2 + 16) * 32
+    if kind in ("unique16", "run32"):
+        b += hr.probe_slots(kind, nheads) * (16 if kind == "unique16" else 32)
     return b
 
 
 def _rowhash_fits(unique, n, widths, pay_lens):  # sort.cu: build_index, the row-carrying table's limits
     """pay_lens: per row, the lengths of its non-key columns"""
-    return unique and n >= 2 and _image_bytes(widths) <= 12 and len(pay_lens[0]) <= 4 and max(map(sum, pay_lens)) <= 16
+    return unique and n >= 2 and hr.image_bytes(widths) <= 12 and len(pay_lens[0]) <= 4 and max(map(sum, pay_lens)) <= 16
 
 
 def _check_route(st, kind, nheads, pbytes):
@@ -284,13 +258,13 @@ def test_probe_routes(case):
     for nk in [K] + list(range(1, K)):
         pt, op = full if nk == K else part
         nheads = len({r[:nk] for r in rows})
-        pbytes = _image_bytes(case.widths[:nk])
+        pbytes = hr.image_bytes(case.widths[:nk])
         if rowhash and nk == K:
             kind = "rowhash"
         else:
             if case.unique and nk == K:
                 nheads = n  # a unique index probed on its full key: every row is its own run, in source order
-            kind = _probe_kind(nheads, pbytes, n)
+            kind = hr.probe_kind(nheads, pbytes, n)
         if nk == K:
             assert kind == case.route, (case.name, kind, nheads, pbytes)  # the shape lands where the case says
         if case.lead_unique and nk == 1:
@@ -335,7 +309,7 @@ def test_sort_at_scale_and_unique_error():
     cols = _columns({"k0": k0, "k1": k1, "k2": k2, "i": rid})
     t = _device_table(cols)
     ix, st = _with_stats(lambda: t.index_on("k0", "k1", "k2"))
-    words = (_image_bytes([7, 11, 9]) + 7) // 8
+    words = (hr.image_bytes([7, 11, 9]) + 7) // 8
     assert words == 4 and st["sort_hist"]["launches"] == words
     assert st["sort_gather_word"]["launches"] == words - 1
     perm = sorted(range(n), key=lambda i: (k0[i], k1[i], k2[i]))  # index_ref.index_on: a stable sort on the key tuple

@@ -20,8 +20,9 @@ import pytest
 from tests import index_ref as ref
 from tests import left_join_ref as lj
 from tests.helpers import gpu_ctx
-from tests.test_gpu_index_keys import (CASES, _both, _case_data, _check_route, _columns, _device_table, _image_bytes, _load,
-                                       _probe_kind, _resolve_both, _rowhash_fits, _trows, _with_stats)
+from tests.hash_ref import image_bytes, probe_kind
+from tests.test_gpu_index_keys import (CASES, _both, _case_data, _check_route, _columns, _device_table, _load, _resolve_both,
+                                       _rowhash_fits, _trows, _with_stats)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -64,13 +65,13 @@ def test_route_matrix(case):
     for nk in [K] + list(range(1, K)):
         pt = full if nk == K else part
         nheads = len({r[:nk] for r in rows})
-        pbytes = _image_bytes(case.widths[:nk])
+        pbytes = image_bytes(case.widths[:nk])
         if rowhash and nk == K:
             kind = "rowhash"
         else:
             if case.unique and nk == K:
                 nheads = n
-            kind = _probe_kind(nheads, pbytes, n)
+            kind = probe_kind(nheads, pbytes, n)
         # LeftJoin first: its stats hold the probe table's build, as Join's do in test_probe_routes
         _, st = _with_stats(lambda: pt.join(ix, *pnames[:nk], left=True))
         _check_route({**st_build, **st} if nk == K else st, kind, nheads, pbytes)

@@ -1,19 +1,19 @@
 """GPU parity of the region-by-region build of the row-carrying hash table (UniqueIndexOn with a short key and a short
 payload): region counts at and around the region size, keys whose probe sequence wraps inside its region, duplicates,
 and a region that overflows and sends the index to the 16-byte probe table.  Keys aimed at given slots are chosen with a
-numpy restatement of the key image, the hash and the slot / region mapping of rowhash.cuh."""
+restatement of the key image, the hash and the slot mapping of rowhash.cuh (tests/hash_ref.py)."""
 import random
 
 import numpy as np
 import pytest
 
 from oracle import oracle as orc
+from tests.hash_ref import first_slots
 from tests.helpers import assert_table_equals_oracle, gpu_ctx
 
 pytestmark = pytest.mark.gpu
 
 REGION = 1024  # RH_REGION (rowhash.cuh)
-U64 = np.uint64
 
 
 def _layout(n):
@@ -23,26 +23,6 @@ def _layout(n):
     while rs < want and rs < REGION:
         rs *= 2
     return rs, -(-want // rs)
-
-
-def _mix64(h):
-    h = h ^ (h >> U64(33)); h = h * U64(0xff51afd7ed558ccd)
-    h = h ^ (h >> U64(33)); h = h * U64(0xc4ceb9fe1a85ec53)
-    return h ^ (h >> U64(33))
-
-
-def _first_slots(keys, nslots):
-    """first slot of each key (equal-length byte strings of at most 11 bytes) as the one key column of an index: image =
-    the bytes + one length byte, hash3(w0, w1, 0), slot_of = the high 64 bits of hash * nslots"""
-    w = len(keys[0])
-    img = np.zeros((len(keys), 16), np.uint8)
-    img[:, :w] = np.frombuffer(b"".join(keys), np.uint8).reshape(len(keys), w)
-    img[:, w] = w
-    words = img.reshape(len(keys), 2, 8)[:, :, ::-1].copy().view("<u8").reshape(len(keys), 2)  # big-endian words
-    with np.errstate(over="ignore"):
-        h = _mix64(_mix64(_mix64(U64(0x9E3779B97F4A7C15) ^ words[:, 0]) ^ words[:, 1]))
-        lo, hi = h & U64(0xffffffff), h >> U64(32)
-        return (hi * U64(nslots) + ((lo * U64(nslots)) >> U64(32))) >> U64(32)
 
 
 def _parse(data):
@@ -157,7 +137,7 @@ def test_probe_wraps_inside_the_region():
     n = 5000
     rs, nreg = _layout(n)
     cand = [b"%08d" % i for i in range(1_500_000)]
-    slot = _first_slots(cand, rs * nreg)
+    slot = first_slots(cand, rs * nreg)
     by_slot = {}
     for i in np.flatnonzero((slot % rs == rs - 1) | (slot % rs == 0)):
         by_slot.setdefault(int(slot[i]), []).append(cand[i])
@@ -179,7 +159,7 @@ def test_duplicates():
     n = 6000
     rs, nreg = _layout(n)
     cand = [b"%07d" % i for i in range(3 * n)]
-    slot = _first_slots(cand, rs * nreg)
+    slot = first_slots(cand, rs * nreg)
     region0 = [cand[i] for i in np.flatnonzero(slot[n:] // rs == 0) + n]  # keys not in base
     base = cand[:n]
     cases = [
@@ -202,7 +182,7 @@ def test_overflowing_region_takes_the_probe_table():
     n = 20000
     rs, nreg = _layout(n)
     cand = [b"%08d" % i for i in range(600_000)]
-    region = _first_slots(cand, rs * nreg) // rs
+    region = first_slots(cand, rs * nreg) // rs
     crowd = [cand[i] for i in np.flatnonzero(region == 3)][: rs + 50]  # more keys than region 3 can hold
     assert len(crowd) == rs + 50
     others = [cand[i] for i in np.flatnonzero(region != 3)[: n - len(crowd)]]

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 from oracle import oracle as orc
-from tests.test_gpu_rowhash_build import _check, _customers, _first_slots, _index_csv, _layout, _orders, _parse
+from tests.hash_ref import first_slots
+from tests.test_gpu_rowhash_build import _check, _customers, _index_csv, _layout, _orders, _parse
 
 pytestmark = pytest.mark.gpu
 
@@ -32,7 +33,7 @@ def _region_keys(n, ncand):
     the region's first slot) and keys whose first slot is its first"""
     rs, nreg = _layout(n)
     cand = [b"%08d" % i for i in range(ncand)]
-    slot = _first_slots(cand, rs * nreg)
+    slot = first_slots(cand, rs * nreg)
     last, first = {}, {}
     for i in np.flatnonzero(slot % rs == rs - 1):
         last.setdefault(int(slot[i]) // rs, []).append(cand[i])
@@ -88,7 +89,7 @@ def test_overflow_from_rows_of_one_thread():
     n = 20000
     rs, nreg = _layout(n)
     cand = [b"%08d" % i for i in range(600_000)]
-    region = _first_slots(cand, rs * nreg) // rs
+    region = first_slots(cand, rs * nreg) // rs
     crowd = [cand[i] for i in np.flatnonzero(region == 5)][: rs + 3]  # three more keys than region 5 can take
     assert len(crowd) == rs + 3
     others = [cand[i] for i in np.flatnonzero(region != 5)[: n - len(crowd)]]
@@ -102,7 +103,7 @@ def test_region_counts_by_lane():
     n = 6000
     rs, nreg = _layout(n)
     cand = [b"%08d" % i for i in range(400_000)]
-    region = _first_slots(cand, rs * nreg) // rs
+    region = first_slots(cand, rs * nreg) // rs
     full = [cand[i] for i in np.flatnonzero(region == 0)][: rs - 1]
     assert len(full) == rs - 1
     others = [cand[i] for i in np.flatnonzero(region != 0)[: n - len(full)]]
